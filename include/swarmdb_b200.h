@@ -200,7 +200,8 @@ int sdb_free_staged(sdb_handle h, sdb_staged_t s);
 /* ---- dequeue: receive_messages (M:521-601) -> Consumer.poll (M:557-559) ------------------
  * For each listed agent (agent_idx == NULL: every index below the registration watermark)
  * remove up to max_messages pending records and return them, agents in list order, records
- * in delivery order:
+ * in delivery order.  An agent may appear only once in agent_idx (SDB_EINVAL otherwise).
+ * Records are delivered:
  *   flags == 0                 stream (arrival) order - the reference's behaviour;
  *   flags & SDB_RECV_PRIORITY  (priority desc, arrival asc) - the extension of SURVEY
  *                              App. A rule 9; equals stream order when priorities are equal.
@@ -386,7 +387,11 @@ int sdb_queue_stats(sdb_handle h, sdb_queue_summary* out);
  *   mode 1  weighted random (one-item weighted reservoir, Efraimidis-Spirakis exponential
  *           race in integer fixed point): P(b) proportional to weight[b], keyed by
  *           (seed, request index); loads are then incremented atomically.
+ * A handle holds at most SDB_MAX_BACKENDS backends (sdb_create refuses a larger max_backends with SDB_EINVAL).
+ * Weights are in [1, 65535] and initial loads below 2^40; loads then grow with the costs of the picks, and the
+ * compares stay exact for any 64-bit load.
  */
+#define SDB_MAX_BACKENDS 4096u
 int sdb_set_backends(sdb_handle h, uint32_t n, const uint32_t* weight, const uint64_t* load0);
 int sdb_get_backend_loads(sdb_handle h, uint32_t n, uint64_t* load_out);
 int sdb_release_backends(sdb_handle h, uint32_t n, const uint32_t* backend, const uint32_t* cost /* NULL = 1 */);

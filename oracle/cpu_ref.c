@@ -75,6 +75,7 @@ static void build_log2_table(uint32_t* tab) {
   }
   tab[256] = 1u << 24;
 }
+void orc_log2_table(uint32_t* tab257) { build_log2_table(tab257); }
 
 /* ---- per-agent stream digest (definition: include/swarmdb_b200.h, "stream digest") -------------------------
  * rec_hash = sum over the 64-bit little-endian words w_k (k = 0..) of [32-byte header | payload padded to 32 bytes]

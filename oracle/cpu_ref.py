@@ -53,6 +53,7 @@ def lib():
         L.orc_set_backends.argtypes = [vp, u32, vp, vp]
         L.orc_get_backend_loads.argtypes = [vp, vp]
         L.orc_select_backend_batch.argtypes = [vp, u32, vp, u32, u64, vp]
+        L.orc_log2_table.argtypes = [vp]
         L.orc_agent_loads.argtypes = [vp, u32, vp, vp]
         L.orc_digest_enable.argtypes = [vp]
         L.orc_digest_read.argtypes = [vp, u32, vp, vp]
@@ -67,6 +68,13 @@ def _p(a: Optional[np.ndarray]):
 
 def _arr(x, dt) -> np.ndarray:
     return np.ascontiguousarray(x, dtype=dt)
+
+
+def log2_table() -> np.ndarray:
+    """The 257-entry Q24 table of log2(1 + i/256) behind the weighted-random pick (mode 1)."""
+    out = np.zeros(257, np.uint32)
+    lib().orc_log2_table(_p(out))
+    return out
 
 
 class CpuOracle:

@@ -33,6 +33,7 @@ cudaError_t sdb_launch_pull(const sdb_dev_view*, const sdb_pull_view*, const sdb
                             const sdb_batch_base*, uint32_t);
 cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaStream_t, int*, sdb_profiler*, int, uint32_t);
 cudaError_t sdb_recv_prepare_device();
+cudaError_t sdb_balance_prepare_device();
 cudaError_t sdb_launch_receive_small(const sdb_dev_view*, const uint32_t*, uint32_t, uint32_t, uint32_t, uint32_t, uint4*,
                                      uint8_t*, cudaStream_t, sdb_profiler*);
 cudaError_t sdb_launch_digest(const sdb_recv_args*, uint32_t, unsigned long long*, int, cudaStream_t);
@@ -104,7 +105,8 @@ struct sdb_ctx {
   bool memb_dirty = true;
   uint8_t* gexcl_dev = nullptr;          // [max_groups] 1: every member of the group belongs to that group only
   uint32_t n_excl_groups = 0, n_shared_agents = 0;
-  std::vector<uint32_t> rank_cnt;              // per-receiver counters of the point-to-point ranking (all zero between batches)
+  std::vector<uint32_t> rank_cnt;              // per-agent scratch table, all zero between calls: point-to-point ranking, the
+                                               // disjointness check of broadcast lists, the repeated-agent check of receives
   bool shared_cfg = false;                     // SDB_SHARED_PAYLOAD: group sends above the pull threshold share one payload per send
   uint32_t max_lcount = 0;                     // largest local member count of a group (shared payloads need <= 65535)
   std::vector<uint32_t> lp_first;              // broadcast batches: first chunk descriptor of every send
@@ -200,6 +202,13 @@ int fail(sdb_ctx* h, int code, const std::string& msg) {
       return fail(h, SDB_ECUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));            \
   } while (0)
 
+// Host -> device upload ordered on the handle's stream, like every kernel that reads the data, and complete when it
+// returns.  A plain cudaMemcpy runs on the legacy default stream, which the handle's non-blocking stream is not ordered
+// after, and from pageable memory it may return before the data has reached device memory.
+cudaError_t upload(sdb_ctx* h, void* dst, const void* src, size_t bytes) {
+  const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream);
+  return e == cudaSuccess ? cudaStreamSynchronize(h->stream) : e;
+}
 bool is_pow2(uint64_t x) { return x && !(x & (x - 1)); }
 // header + descriptors + group buckets of a wire batch (the part a remote importer copies locally)
 uint64_t wire_meta_bytes(uint32_t max_sends, uint32_t max_groups) {
@@ -516,11 +525,11 @@ int rebuild_inverse(sdb_ctx* h) {
   }
   h->n_excl_groups = n_excl; h->n_shared_agents = n_shared;
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  CUDA_TRY(h, cudaMemcpy(h->gexcl_dev, excl.data(), G, cudaMemcpyHostToDevice));
-  CUDA_TRY(h, cudaMemcpy(h->memb_off_dev, off.data(), off.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, upload(h, h->gexcl_dev, excl.data(), G));
+  CUDA_TRY(h, upload(h, h->memb_off_dev, off.data(), off.size() * sizeof(uint32_t)));
   if (total) {
-    CUDA_TRY(h, cudaMemcpy(h->memb_grp_dev, grp.data(), total * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->memb_pos_dev, pos.data(), total * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, upload(h, h->memb_grp_dev, grp.data(), total * sizeof(uint32_t)));
+    CUDA_TRY(h, upload(h, h->memb_pos_dev, pos.data(), total * sizeof(uint32_t)));
   }
   h->memb_dirty = false;
   return SDB_OK;
@@ -536,8 +545,8 @@ int ensure_ltab(sdb_ctx* h) {
     st[g] = static_cast<uint32_t>(h->gstart[g]); ct[g] = h->gdefined[g] ? h->gcount[g] : 0;
     h->max_lcount = std::max(h->max_lcount, ct[g]);
   }
-  CUDA_TRY(h, cudaMemcpy(h->lstart_dev, st.data(), st.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-  CUDA_TRY(h, cudaMemcpy(h->lcount_dev, ct.data(), ct.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, upload(h, h->lstart_dev, st.data(), st.size() * sizeof(uint32_t)));
+  CUDA_TRY(h, upload(h, h->lcount_dev, ct.data(), ct.size() * sizeof(uint32_t)));
   h->ltab_dirty = false;
   return SDB_OK;
 }
@@ -704,6 +713,7 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
   if (c.max_groups == 0) c.max_groups = 1;
   if (c.member_pool_entries == 0) c.member_pool_entries = 1;
   if (c.max_backends == 0) c.max_backends = 256;
+  if (c.max_backends > SDB_MAX_BACKENDS) return fail(h, SDB_EINVAL, "max_backends must be at most SDB_MAX_BACKENDS (4096)");
   if (c.max_batch_sends == 0) c.max_batch_sends = 65536;
   if (c.max_batch_payload == 0) c.max_batch_payload = static_cast<uint64_t>(c.max_batch_sends) * pad32(std::min(c.max_payload_bytes, 256u));
   if (c.max_recv_records == 0) c.max_recv_records = 1u << 20;
@@ -734,6 +744,7 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
   }
   CUDA_TRY(h, sdb_send_prepare_device());
   CUDA_TRY(h, sdb_recv_prepare_device());
+  CUDA_TRY(h, sdb_balance_prepare_device());
   cudaDeviceProp prop;
   CUDA_TRY(h, cudaGetDeviceProperties(&prop, c.device));
   h->sm_count = prop.multiProcessorCount;
@@ -812,8 +823,8 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
   if (c.shard_id >= c.num_shards || c.num_shards > 255) return fail(h, SDB_EINVAL, "shard_id / num_shards out of range");
   CUDA_TRY(h, dmalloc(&h->member_pos_dev, c.member_pool_entries));
   CUDA_TRY(h, dmalloc(&h->lstart_dev, c.max_groups)); CUDA_TRY(h, dmalloc(&h->lcount_dev, c.max_groups));
-  CUDA_TRY(h, cudaMemset(h->lcount_dev, 0, static_cast<size_t>(c.max_groups) * sizeof(uint32_t)));
-  CUDA_TRY(h, cudaMemset(h->lstart_dev, 0, static_cast<size_t>(c.max_groups) * sizeof(uint32_t)));
+  CUDA_TRY(h, cudaMemsetAsync(h->lcount_dev, 0, static_cast<size_t>(c.max_groups) * sizeof(uint32_t), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->lstart_dev, 0, static_cast<size_t>(c.max_groups) * sizeof(uint32_t), h->stream));
   {
     const uint64_t cap64 = static_cast<uint64_t>(c.num_shards) * c.max_batch_sends;
     if (cap64 > 0x7FFFFFFFull) return fail(h, SDB_EINVAL, "num_shards * max_batch_sends too large");
@@ -830,7 +841,7 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
     CUDA_TRY(h, dmalloc(&h->xs_gs_off_src, G1 * c.num_shards)); CUDA_TRY(h, dmalloc(&h->xs_gs_idx_src, n));
     CUDA_TRY(h, dmalloc(&h->xs_first, SDB_MAX_SRC + 1)); CUDA_TRY(h, dmalloc(&h->xs_lb, sdb_lb_words(static_cast<uint32_t>(n / 256 + 2)) + 4));
     CUDA_TRY(h, dmalloc(&h->cursor_dev, 1)); CUDA_TRY(h, dmalloc(&h->bb_dev, 1)); CUDA_TRY(h, dmalloc(&h->xs_hdrs, SDB_MAX_SRC));
-    CUDA_TRY(h, cudaMemset(h->cursor_dev, 0, sizeof(sdb_cursor))); CUDA_TRY(h, cudaMemset(h->bb_dev, 0, sizeof(sdb_batch_base)));
+    CUDA_TRY(h, cudaMemsetAsync(h->cursor_dev, 0, sizeof(sdb_cursor), h->stream)); CUDA_TRY(h, cudaMemsetAsync(h->bb_dev, 0, sizeof(sdb_batch_base), h->stream));
     {
       auto& S0 = h->xset[0];
       S0.descs = h->xs_descs; S0.gs_off_src = h->xs_gs_off_src; S0.gs_idx_src = h->xs_gs_idx_src; S0.first = h->xs_first;
@@ -843,7 +854,7 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
     h->xs_meta_stride = wire_meta_bytes(c.max_batch_sends, c.max_groups);
     CUDA_TRY(h, dmalloc(&h->xs_meta, h->xs_meta_stride * c.num_shards));
     CUDA_TRY(h, dmalloc(&h->shard_of_dev, c.max_agents));
-    CUDA_TRY(h, cudaMemset(h->shard_of_dev, static_cast<int>(c.shard_id), c.max_agents));
+    CUDA_TRY(h, cudaMemsetAsync(h->shard_of_dev, static_cast<int>(c.shard_id), c.max_agents, h->stream));
     CUDA_TRY(h, cudaHostAlloc(reinterpret_cast<void**>(&h->wire_host), wire_meta_bytes(c.max_batch_sends, c.max_groups), cudaHostAllocDefault));
     CUDA_TRY(h, cudaHostAlloc(reinterpret_cast<void**>(&h->hdrs_host), static_cast<size_t>(c.num_shards) * sizeof(sdb_wire_header), cudaHostAllocDefault));
   }
@@ -1024,8 +1035,8 @@ static int upload_all_groups(sdb_ctx* h) {
     fpos.insert(fpos.end(), h->gpos[k].begin(), h->gpos[k].end());
   }
   if (!flat.empty()) {
-    CUDA_TRY(h, cudaMemcpy(h->members, flat.data(), flat.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->member_pos_dev, fpos.data(), fpos.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, upload(h, h->members, flat.data(), flat.size() * sizeof(uint32_t)));
+    CUDA_TRY(h, upload(h, h->member_pos_dev, fpos.data(), fpos.size() * sizeof(uint32_t)));
   }
   h->member_used = flat.size();
   h->memb_dirty = true; h->ltab_dirty = true;
@@ -1072,12 +1083,12 @@ int sdb_set_agent_shards(sdb_handle h, uint32_t n, const uint8_t* shard_of) {
   h->sharded = h->cfg.num_shards > 1;
   if (h->sharded) h->n_agents = h->cfg.max_agents;   // receivers are named by other ranks: sweeps cover the whole index space
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  CUDA_TRY(h, cudaMemcpy(h->shard_of_dev, h->shard_of.data(), h->cfg.max_agents, cudaMemcpyHostToDevice));
+  CUDA_TRY(h, upload(h, h->shard_of_dev, h->shard_of.data(), h->cfg.max_agents));
   {
     std::vector<uint32_t> owned;
     for (uint32_t i = 0; i < h->cfg.max_agents; ++i) if (h->shard_of[i] == h->cfg.shard_id) owned.push_back(i);
     if (!h->owned_dev) CUDA_TRY(h, dmalloc(&h->owned_dev, h->cfg.max_agents));
-    if (!owned.empty()) CUDA_TRY(h, cudaMemcpy(h->owned_dev, owned.data(), owned.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    if (!owned.empty()) CUDA_TRY(h, upload(h, h->owned_dev, owned.data(), owned.size() * sizeof(uint32_t)));
     h->n_owned = static_cast<uint32_t>(owned.size());
   }
   // groups created earlier are re-filtered against the new ownership map
@@ -1199,7 +1210,8 @@ int sdb_wire_alloc(sdb_handle h, uint64_t bytes, void** dev_out, void* ipc_handl
   if (!h || !dev_out || bytes == 0) return SDB_EINVAL;
   void* p = nullptr;
   CUDA_TRY(h, cudaMalloc(&p, bytes));
-  CUDA_TRY(h, cudaMemset(p, 0, bytes));
+  CUDA_TRY(h, cudaMemsetAsync(p, 0, bytes, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   if (ipc_handle_out) {
     cudaIpcMemHandle_t hd;
     CUDA_TRY(h, cudaIpcGetMemHandle(&hd, p));
@@ -1482,7 +1494,8 @@ int sdb_overflow_log(sdb_handle h, uint32_t cap, uint32_t* agent_out, uint64_t* 
   if (dropped_out) *dropped_out = 0;
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   unsigned long long logged = 0;
-  CUDA_TRY(h, cudaMemcpy(&logged, &h->ctr->ovf_logged, sizeof(logged), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpyAsync(&logged, &h->ctr->ovf_logged, sizeof(logged), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   if (dropped_out) *dropped_out = logged;
   if (logged == 0) return SDB_OK;
   const uint32_t n = static_cast<uint32_t>(std::min<unsigned long long>(std::min<unsigned long long>(logged, SDB_OVF_LOG), cap));
@@ -1553,13 +1566,13 @@ int sdb_stage_batch(sdb_handle h, uint32_t kind, uint32_t n, const uint32_t* sen
     const size_t G1 = static_cast<size_t>(h->cfg.max_groups) + 1;
     e = dmalloc(&s->gs_off_dev, G1);
     if (e == cudaSuccess) e = dmalloc(&s->gs_idx_dev, n_gs ? n_gs : 1);
-    if (e == cudaSuccess) e = cudaMemcpy(s->gs_off_dev, gs.data(), G1 * sizeof(uint32_t), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && n_gs) e = cudaMemcpy(s->gs_idx_dev, gs.data() + G1, static_cast<size_t>(n_gs) * sizeof(uint32_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = upload(h, s->gs_off_dev, gs.data(), G1 * sizeof(uint32_t));
+    if (e == cudaSuccess && n_gs) e = upload(h, s->gs_idx_dev, gs.data() + G1, static_cast<size_t>(n_gs) * sizeof(uint32_t));
   }
   if (e == cudaSuccess) e = dmalloc(&s->payload_dev, payload_bytes + 64);
-  if (e == cudaSuccess) e = cudaMemset(s->payload_dev, 0, payload_bytes + 64);
-  if (e == cudaSuccess) e = cudaMemcpy(s->descs_dev, descs.data(), static_cast<size_t>(n) * sizeof(sdb_send_desc), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && payload_bytes) e = cudaMemcpy(s->payload_dev, payload, payload_bytes, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemsetAsync(s->payload_dev, 0, payload_bytes + 64, h->stream);
+  if (e == cudaSuccess) e = upload(h, s->descs_dev, descs.data(), static_cast<size_t>(n) * sizeof(sdb_send_desc));
+  if (e == cudaSuccess && payload_bytes) e = upload(h, s->payload_dev, payload, payload_bytes);
   if (e != cudaSuccess) {
     if (s->descs_dev) cudaFree(s->descs_dev);
     if (s->payload_dev) cudaFree(s->payload_dev);
@@ -1628,6 +1641,17 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   if (agent_idx) {
     for (uint32_t i = 0; i < n_agents; ++i)
       if (agent_idx[i] >= h->cfg.max_agents) return fail(h, SDB_EINVAL, "agent index out of range");
+    if (n_agents > 1) {
+      // every slot of a listed agent reads the same ring header, so a repeated index would return the same records
+      // twice: refused
+      const size_t A = h->cfg.max_agents;
+      if (h->rank_cnt.size() != A) h->rank_cnt.assign(A, 0u);
+      std::vector<uint32_t>& seen = h->rank_cnt;                            // all zero between calls
+      uint32_t i = 0;
+      for (; i < n_agents && !seen[agent_idx[i]]; ++i) seen[agent_idx[i]] = 1;
+      for (uint32_t k = 0; k < i; ++k) seen[agent_idx[k]] = 0;
+      if (i < n_agents) return fail(h, SDB_EINVAL, "agent index listed twice");
+    }
   }
   // ---- latency path: few agents, host outputs -> one launch, one D2H, one sync
   if (agent_idx && n_agents <= 8 && hdr_out && payload_out &&
@@ -1855,8 +1879,8 @@ int sdb_set_backends(sdb_handle h, uint32_t n, const uint32_t* weight, const uin
     if (load0) { if (load0[i] >= (1ull << 40)) return fail(h, SDB_EINVAL, "backend load must be < 2^40"); l[i] = load0[i]; }
   }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  CUDA_TRY(h, cudaMemcpy(h->be_weight, weight, n * sizeof(uint32_t), cudaMemcpyHostToDevice));
-  CUDA_TRY(h, cudaMemcpy(h->be_load, l.data(), n * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, upload(h, h->be_weight, weight, n * sizeof(uint32_t)));
+  CUDA_TRY(h, upload(h, h->be_load, l.data(), n * sizeof(unsigned long long)));
   h->n_backends = n;
   return SDB_OK;
 }
@@ -1893,7 +1917,7 @@ int sdb_release_backends(sdb_handle h, uint32_t n, const uint32_t* backend, cons
     const unsigned long long c = cost ? cost[i] : 1;
     l[backend[i]] = l[backend[i]] >= c ? l[backend[i]] - c : 0;
   }
-  CUDA_TRY(h, cudaMemcpy(h->be_load, l.data(), h->n_backends * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+  CUDA_TRY(h, upload(h, h->be_load, l.data(), h->n_backends * sizeof(unsigned long long)));
   return SDB_OK;
 }
 

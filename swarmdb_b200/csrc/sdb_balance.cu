@@ -26,7 +26,12 @@
 // Not HBM-bound: the table is < 10 KB (L1/shared-resident); report picks/s (SURVEY 8d).
 #include "sdb_common.cuh"
 
-#define SDB_MAX_BACKENDS_SMEM 4096
+// every pick kernel keeps the backend table in shared memory: at SDB_MAX_BACKENDS (include/swarmdb_b200.h) that is up to
+// 20 x 4096 + 8 bytes, above the 48 KB a launch gets without opting in (sdb_balance_prepare_device)
+static size_t ll_plan_smem(uint32_t B) { return (2 * static_cast<size_t>(B)) * 8 + static_cast<size_t>(B) * 4; }
+static size_t ll_scatter_smem(uint32_t B) { return (2 * static_cast<size_t>(B) + 1) * 8 + static_cast<size_t>(B) * 4; }
+static size_t ll_seq_smem(uint32_t B) { return static_cast<size_t>(B) * 12; }
+static size_t wr_pick_smem(uint32_t B) { return static_cast<size_t>(B) * 12 + 257 * 4; }
 
 // ---- fixed-point -log2 table (host, integer only) --------------------------------------------
 extern "C" void sdb_build_log2_table(uint32_t* tab257) {
@@ -67,26 +72,56 @@ __device__ __forceinline__ uint32_t sdb_neglog2_q24(uint32_t u, const uint32_t* 
 }
 
 // ---- mode 0 -----------------------------------------------------------------------------------
-// number of progression elements of backend bp that precede element (b, j) in pick order
-__device__ __forceinline__ unsigned long long ll_before(unsigned long long Lb_j, uint32_t wb, uint32_t b,
-                                                        unsigned long long Lbp, uint32_t wbp, uint32_t bp) {
-  const unsigned long long X = Lb_j * wbp;
-  const unsigned long long fl = X / wb;
-  if (bp < b) {                       // ties go to the lower index: count (L'+j')*w <= X
-    return fl >= Lbp ? fl - Lbp + 1ull : 0ull;
-  } else {                            // strict: (L'+j')*w < X  <=>  L'+j' <= ceil(X/w) - 1
-    const unsigned long long ce = fl + ((X % wb) ? 1ull : 0ull);
-    return ce > Lbp ? ce - Lbp : 0ull;
-  }
+// Loads are 64-bit and weights up to 2^16, so load x weight needs up to 80 bits: every cross-multiplication below is
+// exact in 128 bits, as in the definition (oracle/cpu_ref.c).  Ranks are only compared with the batch size T < 2^32,
+// so each per-backend count saturates at SDB_RANK_SAT: a sum of B <= 4096 of them cannot wrap, and every rank >= T
+// stays >= T.
+#define SDB_RANK_SAT (1ull << 40)
+
+// a * x < b * y, exactly
+__device__ __forceinline__ bool mul_lt(unsigned long long a, uint32_t x, unsigned long long b, uint32_t y) {
+  const unsigned long long ah = __umul64hi(a, x), bh = __umul64hi(b, y);
+  return ah < bh || (ah == bh && a * x < b * y);
+}
+__device__ __forceinline__ bool mul_eq(unsigned long long a, uint32_t x, unsigned long long b, uint32_t y) {
+  return __umul64hi(a, x) == __umul64hi(b, y) && a * x == b * y;
 }
 
+// number of progression elements of backend bp that precede element (b, j) in pick order (bp == b counts j itself)
+__device__ __forceinline__ unsigned long long ll_before(unsigned long long Lb_j, uint32_t wb, uint32_t b,
+                                                        unsigned long long Lbp, uint32_t wbp, uint32_t bp) {
+  unsigned long long n;
+  if (__umul64hi(Lb_j, wbp) == 0) {
+    const unsigned long long X = Lb_j * wbp;
+    const unsigned long long fl = X / wb;
+    if (bp < b) {                       // ties go to the lower index: count (L'+j')*w <= X
+      const unsigned long long d = fl - Lbp;          // saturated before the + 1: fl - Lbp can be 2^64 - 1
+      n = fl >= Lbp ? (d < SDB_RANK_SAT ? d + 1ull : SDB_RANK_SAT) : 0ull;
+    } else {                            // strict: (L'+j')*w < X  <=>  L'+j' <= ceil(X/w) - 1
+      const unsigned long long ce = fl + ((X % wb) ? 1ull : 0ull);
+      n = ce > Lbp ? ce - Lbp : 0ull;
+    }
+  } else {                              // loads of 2^48 and more: the same in 128 bits
+    const unsigned __int128 X = static_cast<unsigned __int128>(Lb_j) * wbp;
+    const unsigned __int128 fl = X / wb;
+    unsigned __int128 m;
+    if (bp < b) m = fl >= Lbp ? fl - Lbp + 1u : 0u;
+    else {
+      const unsigned __int128 ce = fl + ((X % wb) ? 1u : 0u);
+      m = ce > Lbp ? ce - Lbp : 0u;
+    }
+    n = m < SDB_RANK_SAT ? static_cast<unsigned long long>(m) : SDB_RANK_SAT;
+  }
+  return n < SDB_RANK_SAT ? n : SDB_RANK_SAT;
+}
+
+// global pick-order rank of element (b, j): elements of every progression that precede it, its own included
 __device__ unsigned long long ll_rank(uint32_t b, unsigned long long j, uint32_t B, const unsigned long long* L,
                                       const uint32_t* w) {
-  unsigned long long r = j;
+  unsigned long long r = 0;
   const unsigned long long Lb_j = L[b] + j;
   const uint32_t wb = w[b];
-  for (uint32_t bp = 0; bp < B; ++bp)
-    if (bp != b) r += ll_before(Lb_j, wb, b, L[bp], w[bp], bp);
+  for (uint32_t bp = 0; bp < B; ++bp) r += ll_before(Lb_j, wb, b, L[bp], w[bp], bp);
   return r;
 }
 
@@ -157,8 +192,8 @@ k_ll_seq(uint32_t B, const uint32_t* __restrict__ weight, unsigned long long* __
     unsigned long long bl = ~0ull; uint32_t bw = 1, bi = 0xFFFFFFFFu;
     for (uint32_t b = lane; b < B; b += 32) {
       const unsigned long long l = sL[b]; const uint32_t w = sW[b];
-      // l/w < bl/bw  <=>  l*bw < bl*w   (bl == ~0 means "none yet")
-      if (bi == 0xFFFFFFFFu || l * bw < bl * w) { bl = l; bw = w; bi = b; }
+      // l/w < bl/bw  <=>  l*bw < bl*w   (bi == ~0 means "none yet")
+      if (bi == 0xFFFFFFFFu || mul_lt(l, bw, bl, w)) { bl = l; bw = w; bi = b; }
     }
     for (int o = 16; o; o >>= 1) {
       const unsigned long long ol = __shfl_xor_sync(0xFFFFFFFFu, bl, o);
@@ -167,10 +202,7 @@ k_ll_seq(uint32_t B, const uint32_t* __restrict__ weight, unsigned long long* __
       if (oi != 0xFFFFFFFFu) {
         bool better;
         if (bi == 0xFFFFFFFFu) better = true;
-        else {
-          const unsigned long long a = ol * bw, c = bl * ow;
-          better = (a < c) || (a == c && oi < bi);
-        }
+        else better = mul_lt(ol, bw, bl, ow) || (mul_eq(ol, bw, bl, ow) && oi < bi);
         if (better) { bl = ol; bw = ow; bi = oi; }
       }
     }
@@ -211,26 +243,31 @@ k_wr_pick(uint32_t B, const uint32_t* __restrict__ weight, unsigned long long* _
     if (sH[b]) atomicAdd(&load[b], sH[b]);
 }
 
+extern "C" cudaError_t sdb_balance_prepare_device() {
+  const uint32_t B = SDB_MAX_BACKENDS;
+  cudaError_t e;
+  if ((e = cudaFuncSetAttribute(k_ll_plan, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ll_plan_smem(B)))) != cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(k_ll_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ll_scatter_smem(B)))) != cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(k_ll_seq, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ll_seq_smem(B)))) != cudaSuccess) return e;
+  return cudaFuncSetAttribute(k_wr_pick, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(wr_pick_smem(B)));
+}
+
 extern "C" cudaError_t sdb_launch_pick(int mode, uint32_t B, const uint32_t* weight_dev, unsigned long long* load_dev,
                                        uint32_t n_req, const uint32_t* cost_dev, uint64_t seed, uint32_t* out_dev,
                                        unsigned long long* scratch_dev, const uint32_t* log_tab_dev,
                                        cudaStream_t stream, int* n_launches) {
-  if (B > SDB_MAX_BACKENDS_SMEM) return cudaErrorInvalidValue;
+  if (B > SDB_MAX_BACKENDS) return cudaErrorInvalidValue;
   if (mode == 0) {
     if (cost_dev == nullptr) {
-      const size_t sm1 = (2 * static_cast<size_t>(B)) * 8 + static_cast<size_t>(B) * 4;
-      k_ll_plan<<<1, 1024, sm1, stream>>>(B, weight_dev, load_dev, n_req, scratch_dev);
-      const size_t sm2 = (2 * static_cast<size_t>(B) + 1) * 8 + static_cast<size_t>(B) * 4;
-      k_ll_scatter<<<(n_req + 255) / 256, 256, sm2, stream>>>(B, weight_dev, scratch_dev, n_req, out_dev);
+      k_ll_plan<<<1, 1024, ll_plan_smem(B), stream>>>(B, weight_dev, load_dev, n_req, scratch_dev);
+      k_ll_scatter<<<(n_req + 255) / 256, 256, ll_scatter_smem(B), stream>>>(B, weight_dev, scratch_dev, n_req, out_dev);
       if (n_launches) *n_launches += 2;
     } else {
-      const size_t sm = static_cast<size_t>(B) * 12;
-      k_ll_seq<<<1, 32, sm, stream>>>(B, weight_dev, load_dev, n_req, cost_dev, out_dev);
+      k_ll_seq<<<1, 32, ll_seq_smem(B), stream>>>(B, weight_dev, load_dev, n_req, cost_dev, out_dev);
       if (n_launches) *n_launches += 1;
     }
   } else {
-    const size_t sm = static_cast<size_t>(B) * 12 + 257 * 4;
-    k_wr_pick<<<(n_req + 255) / 256, 256, sm, stream>>>(B, weight_dev, load_dev, n_req, cost_dev, seed, log_tab_dev, out_dev);
+    k_wr_pick<<<(n_req + 255) / 256, 256, wr_pick_smem(B), stream>>>(B, weight_dev, load_dev, n_req, cost_dev, seed, log_tab_dev, out_dev);
     if (n_launches) *n_launches += 1;
   }
   return cudaGetLastError();

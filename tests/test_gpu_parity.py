@@ -521,3 +521,28 @@ def test_broadcast_batches_owner_computes_index_equals_oracle(shape):
         assert prof.get("index", (0, 0))[1] == 0 and prof["commit"][1] == 3          # atomic path + commit sort
     else:
         assert prof["index"][1] == 3 and prof.get("commit", (0, 0))[1] == 0          # owner-computes, nothing to sort
+
+
+def test_receive_list_naming_an_agent_twice_is_refused():
+    """Every slot of a listed agent would read the same ring header and return the same records twice: a receive list
+    with a repeated index is refused with SDB_EINVAL on the small path and on the bulk path, and consumes nothing."""
+    from swarmdb_b200._native import RECV_PEEK, RECV_PRIORITY, SdbError
+    rng = np.random.default_rng(88)
+    A = 300
+    g, c = _pair(A, ring_slots=256)
+    idx = np.arange(A, dtype=np.uint32)
+    g.register(idx); c.register(idx)
+    n = 3000
+    s, r, prio = rng.integers(0, A, n), rng.integers(0, A, n), rng.integers(0, 4, n)
+    lens, off, buf = _mk_payloads(rng, n, 64)
+    g.send_batch(s, r, prio, None, lens, off, buf); c.send_batch(s, r, prio, None, lens, off, buf)
+    bulk = np.concatenate([idx[:200], [17]]).astype(np.uint32)
+    for agents, k in (([5, 9, 5], 4), ([7, 7], 1), (bulk, 50), (np.concatenate([idx[1:], idx[-1:]]), 1000)):
+        for flags in (0, RECV_PRIORITY, RECV_PEEK):
+            with pytest.raises(SdbError) as ei:
+                g.receive_batch(np.asarray(agents, np.uint32), k, flags)
+            assert ei.value.code == -1 and "twice" in str(ei.value)
+    assert g.stats()["delivered"] == 0
+    _same(g.receive_batch([5, 9, 7], 4), c.receive_batch([5, 9, 7], 4))               # the table is clean afterwards
+    _same(g.receive_batch(idx, 1000), c.receive_batch(idx, 1000))
+    g.close(); c.close()
