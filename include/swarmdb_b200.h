@@ -208,9 +208,16 @@ int sdb_free_staged(sdb_handle h, sdb_staged_t s);
  * Outputs (host pointers, each nullable to skip the copy): count_out[n_agents];
  * hdr_out[total]; payload_out = payloads back to back, each padded to SDB_GRANULE, in the
  * same order (offset of record r = sum of pad32(hdr_out[0..r).len)).  *total_out /
- * *payload_bytes_out receive the totals.  Capacity: hdr_cap records / payload_cap bytes;
- * agents that would exceed max_recv_records are truncated (their remaining records stay
- * queued), never dropped.
+ * *payload_bytes_out receive the totals.
+ * Capacity: one call returns at most rec_cap = min(max_recv_records,
+ * max_recv_payload / P, hdr_cap, payload_cap / P) records, P = pad32(max_payload_bytes)
+ * (hdr_cap / payload_cap count only when the pointer is given), so that rec_cap records of
+ * the largest size always fit.  The rule is the same on every path (bulk, few-agent and
+ * latency server): records are laid out agent by agent in list order; if an agent's records
+ * do not all fit, that agent and every later agent are truncated and stay queued, never
+ * dropped.  The only exception is an agent that is first in the output (nothing placed
+ * before it): it gets its first rec_cap records, in the call's delivery order, and keeps
+ * the rest queued.  So every call on a non-empty queue makes progress.
  */
 #define SDB_RECV_PRIORITY 1u
 #define SDB_RECV_PEEK 2u                /* return what a receive would deliver, retire nothing (history snapshots, M:852-892) */
@@ -230,7 +237,9 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
  * sdb_receive_batch calls naming exactly one agent with host outputs (what the Python surface's receive_messages makes)
  * then post a request there and read the answer - count, headers and payloads - from pinned host memory the kernel wrote
  * directly: no kernel launch, no cudaStreamSynchronize, no cudaMemcpy on the path.  Results are identical to the
- * ordinary path (same selection code).  enable = 0 stops it (also done by sdb_destroy).  While it runs the handle
+ * ordinary path (same selection code).  Starting it first loads every kernel of the library (under lazy module loading
+ * a kernel's first launch would otherwise wait for the server, which never ends; needs a CUDA 12.4 or later driver).
+ * enable = 0 stops it (also done by sdb_destroy).  While it runs the handle
  * stops it around its own calls that free device memory (cudaFree waits for running kernels) and restarts it on the
  * next single-agent receive; callers must likewise not call cudaDeviceSynchronize / cudaFree from outside while it runs. */
 int sdb_latency_server(sdb_handle h, int enable);

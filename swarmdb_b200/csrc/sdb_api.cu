@@ -4,6 +4,7 @@
 // sequence counter, arena space accounting (tail / floor / reclaim), pinned staging for
 // per-send descriptors, and the launch sequence of every entry point.  No CPU data path:
 // every routed byte goes through the kernels in sdb_send.cu / sdb_recv.cu / sdb_balance.cu.
+#include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -39,6 +40,10 @@ cudaError_t sdb_launch_receive_small(const sdb_dev_view*, const uint32_t*, uint3
 cudaError_t sdb_launch_digest(const sdb_recv_args*, uint32_t, unsigned long long*, int, cudaStream_t);
 cudaError_t sdb_launch_arena_floor(const sdb_dev_view*, uint32_t, uint32_t, unsigned long long*, cudaStream_t);
 cudaError_t sdb_launch_latency_server(const sdb_dev_view*, sdb_ls_mailbox*, uint8_t*, uint32_t, uint4*, cudaStream_t);
+const void* sdb_send_kernel_anchor();
+const void* sdb_recv_kernel_anchor();
+const void* sdb_balance_kernel_anchor();
+const void* sdb_xshard_kernel_anchor();
 cudaError_t sdb_launch_pick(int mode, uint32_t n_backends, const uint32_t* weight_dev, unsigned long long* load_dev,
                             uint32_t n_req, const uint32_t* cost_dev, uint64_t seed, uint32_t* out_dev,
                             unsigned long long* scratch_dev, const uint32_t* log_tab_dev,
@@ -229,8 +234,41 @@ int ls_stop(sdb_ctx* h) {
   h->ls_running = false;
   return SDB_OK;
 }
+// Under lazy module loading (the CUDA 12 default) the first launch of a kernel loads its code into the context, and that
+// load waits for the kernels running there: with the persistent latency server running it would wait forever.  So every
+// kernel of the library is loaded before the server starts.  The driver functions come through the runtime's entry
+// point query; cuModuleEnumerateFunctions and cuFuncLoad need a CUDA 12.4 driver.
+cudaError_t load_all_kernels() {
+  using get_module_t = CUresult (*)(CUmodule*, CUfunction);
+  using count_t = CUresult (*)(unsigned int*, CUmodule);
+  using enumerate_t = CUresult (*)(CUfunction*, unsigned int, CUmodule);
+  using load_t = CUresult (*)(CUfunction);
+  void *gm = nullptr, *cn = nullptr, *en = nullptr, *ld = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  for (auto [name, fp] : {std::pair<const char*, void**>{"cuFuncGetModule", &gm}, {"cuModuleGetFunctionCount", &cn},
+                          {"cuModuleEnumerateFunctions", &en}, {"cuFuncLoad", &ld}}) {
+    const cudaError_t e = cudaGetDriverEntryPoint(name, fp, cudaEnableDefault, &q);
+    if (e != cudaSuccess) return e;
+    if (q != cudaDriverEntryPointSuccess || !*fp) return cudaErrorNotSupported;
+  }
+  for (const void* anchor : {sdb_send_kernel_anchor(), sdb_recv_kernel_anchor(), sdb_balance_kernel_anchor(), sdb_xshard_kernel_anchor()}) {
+    cudaFunction_t f = nullptr;
+    cudaError_t e = cudaGetFuncBySymbol(&f, anchor);
+    if (e != cudaSuccess) return e;
+    CUmodule mod = nullptr;
+    unsigned int n = 0;
+    if (reinterpret_cast<get_module_t>(gm)(&mod, reinterpret_cast<CUfunction>(f)) != CUDA_SUCCESS ||
+        reinterpret_cast<count_t>(cn)(&n, mod) != CUDA_SUCCESS) return cudaErrorUnknown;
+    std::vector<CUfunction> fs(n);
+    if (n && reinterpret_cast<enumerate_t>(en)(fs.data(), n, mod) != CUDA_SUCCESS) return cudaErrorUnknown;
+    for (CUfunction fn : fs) if (reinterpret_cast<load_t>(ld)(fn) != CUDA_SUCCESS) return cudaErrorUnknown;
+  }
+  return cudaSuccess;
+}
+
 int ls_start(sdb_ctx* h) {
   if (h->ls_running) return SDB_OK;
+  CUDA_TRY(h, load_all_kernels());
   if (!h->ls_mbox) {
     h->ls_out_cap = 64u + 1024u * 64u;                                       // k_recv_small's block: 64-byte head + records
     const uint64_t need = 64ull + 1024ull * (32ull + pad32(h->cfg.max_payload_bytes));
@@ -1653,12 +1691,17 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
       if (i < n_agents) return fail(h, SDB_EINVAL, "agent index listed twice");
     }
   }
+  // record capacity of the call, the same on every path: the device buffers and the caller's buffers must each hold
+  // rec_cap records of the maximum size (what does not fit stays queued: include/swarmdb_b200.h)
+  const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
+  uint64_t rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
+  if (hdr_out) rec_cap = std::min<uint64_t>(rec_cap, hdr_cap);
+  if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
+  if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
   // ---- latency path: few agents, host outputs -> one launch, one D2H, one sync
   if (agent_idx && n_agents <= 8 && hdr_out && payload_out &&
       static_cast<uint64_t>(n_agents) * max_messages <= 1024) {
-    const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
-    uint64_t rec_cap = std::min<uint64_t>(1024, std::min<uint64_t>(hdr_cap, payload_cap / max_rec_bytes));
-    if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+    rec_cap = std::min<uint64_t>(rec_cap, 1024);
     h->last_rx_valid = false;
     bool served = false;
     if (h->ls_wanted && n_agents == 1) {
@@ -1711,12 +1754,6 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   r.rec_off = h->rx_rec_off; r.plan = h->rx_plan; r.lb = h->rx_lb;
   r.plan_tops = h->rx_plan_tops; r.totals = h->rx_totals; r.big_list = h->rx_big_list; r.big_count = h->rx_big_count;
   r.count_out = h->rx_count; r.hdr_out = h->rx_hdr; r.payload_out = h->rx_payload;
-  // record capacity: bounded so that even maximum-size payloads fit the payload buffers
-  const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
-  uint64_t rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
-  if (hdr_out) rec_cap = std::min<uint64_t>(rec_cap, hdr_cap);
-  if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
-  if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
   r.rec_cap = rec_cap;
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes));

@@ -153,7 +153,8 @@ k_recv_count(sdb_dev_view v, sdb_recv_args r) {
 // one at a time by the whole warp (window scans with ballots).  For every selected record the
 // plan (arena handle, payload granules) is written at its output index, the ring entry is
 // retired (head advanced / tombstoned), and count_out is final.  Agents that would overflow
-// the record capacity are left untouched (whole-agent truncation: nothing is ever lost).
+// the record capacity are left untouched (whole-agent truncation: nothing is ever lost),
+// except the first agent in the output (roff == 0), which takes its first rec_cap records.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t lane_prefix(uint32_t ballot, uint32_t lane) {
   return __popc(ballot & ((1u << lane) - 1u));
@@ -278,9 +279,10 @@ k_recv_select(sdb_dev_view v, sdb_recv_args r) {
     a = r.agent_idx ? r.agent_idx[q] : q;
     cnt = r.cnt[q];
     roff = r.rec_local[q] + r.rec_tops[q / SDB_SCAN_TILE];
-    if (cnt && static_cast<uint64_t>(roff) + cnt > r.rec_cap) {      // does not fit: stays queued
-      atomicMin(r.totals, static_cast<unsigned long long>(roff));
-      cnt = 0;
+    if (cnt && static_cast<uint64_t>(roff) + cnt > r.rec_cap) {      // does not fit: stays queued ...
+      if (roff == 0) cnt = static_cast<uint32_t>(r.rec_cap);          // ... unless first in the output: its first rec_cap records
+      else cnt = 0;
+      atomicMin(r.totals, static_cast<unsigned long long>(roff) + cnt);
     }
     r.count_out[q] = cnt;
     r.rec_off[q] = roff;
@@ -466,7 +468,8 @@ k_scan_plan(uint4* __restrict__ plan, uint32_t* __restrict__ tops, const unsigne
 // record's output index and its payload offset come out of the same pass.
 // Agents whose window holds consumed entries (holes left by earlier priority receives) are walked by their warp.
 // Capacity: an agent whose records would run past rec_cap is left untouched together with every agent after it
-// (whole-agent truncation, nothing is ever lost); the totals are lowered with an atomic min on the packed pair.
+// (whole-agent truncation, nothing is ever lost), except an agent first in the output (exclusive prefix 0), which takes
+// its first rec_cap records; the totals are lowered with an atomic min on the packed pair.
 //   r.lb               look-back scratch (layout in sdb_common.cuh, zeroed by the launcher), then the tile ticket, then
 //                      ~(records << 32 | granules) of the call, maintained with atomicMax (= min of the value)
 // ------------------------------------------------------------------------------------------
@@ -489,8 +492,9 @@ __device__ __forceinline__ uint32_t holey_sum_warp(const uint2* rs, uint32_t mas
   for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xFFFFFFFFu, sum, o);
   return sum;
 }
-// payload offsets of C freshly planned records [RO, RO + C): running sum of .z from g0, whole warp
-__device__ __forceinline__ void fill_offsets_warp(uint4* plan, uint32_t RO, uint32_t C, uint32_t g0, uint32_t lane) {
+// payload offsets of C freshly planned records [RO, RO + C): running sum of .z from g0, whole warp; returns the offset
+// after the last one
+__device__ __forceinline__ uint32_t fill_offsets_warp(uint4* plan, uint32_t RO, uint32_t C, uint32_t g0, uint32_t lane) {
   uint32_t run = g0;
   for (uint32_t j0 = 0; j0 < C; j0 += 32) {
     const uint32_t j = j0 + lane;
@@ -501,9 +505,12 @@ __device__ __forceinline__ void fill_offsets_warp(uint4* plan, uint32_t RO, uint
     if (j < C) plan[RO + j].y = run + incl - g;
     run += __shfl_sync(0xFFFFFFFFu, incl, 31);
   }
+  return run;
 }
 
-__global__ void __launch_bounds__(SDB_PLAN_TILE)
+// at most 64 registers (4 CTAs per SM, the shared-memory limit allows 5): with 80, which the compiler picks otherwise,
+// the c2 plan ran 13 % slower on an H100 (400 W power limit)
+__global__ void __launch_bounds__(SDB_PLAN_TILE, 4)
 k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) {
   __shared__ uint32_t s_tile;
   __shared__ unsigned long long s_wr[SDB_PLAN_WARPS], s_wg[SDB_PLAN_WARPS];
@@ -537,11 +544,12 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
   }
   const bool holey = cnt && nt != 0;
   const bool simple = cnt && !holey;
+  const bool in_regs = simple && cnt <= KEEP;       // entries held in ev[] (decided before any capacity truncation)
   const uint2* rs = sdb_ring_of(v, valid && a < v.max_agents ? a : 0u);
   uint64_t ev[KEEP];
   uint32_t gsum = 0;
   if (simple) {
-    if (cnt <= KEEP) {
+    if (in_regs) {
 #pragma unroll
       for (uint32_t j = 0; j < KEEP; ++j)
         if (j < cnt) ev[j] = sdb_ld_u64_pol(reinterpret_cast<const uint64_t*>(rs + ((head + j) & mask)), pol);
@@ -593,12 +601,16 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
   const unsigned long long pr = s_br + s_wr[warp] + ir - cnt, pg = s_bg + s_wg[warp] + ig - gsum;   // exclusive prefix of this slot
   const uint32_t roff = static_cast<uint32_t>(min(pr, 0xFFFFFFFFull));
   const uint32_t goff = static_cast<uint32_t>(min(pg, 0xFFFFFFFFull));
-  if (cnt && pr + cnt > r.rec_cap) {                                            // does not fit: stays queued
+  const bool over = cnt && pr + cnt > r.rec_cap;                                // does not fit: stays queued ...
+  const bool lead = over && pr == 0;                                            // ... unless first in the output: then it
+  if (lead) cnt = static_cast<uint32_t>(r.rec_cap);                             // takes its first rec_cap records (their
+  else if (over) {                                                              // granules are summed while they are planned)
     atomicMax(r.lb + totals_at, ~((static_cast<unsigned long long>(roff) << 32) | goff));
     cnt = 0;
   }
   if (valid) { r.count_out[q] = cnt; r.rec_off[q] = roff; }
 
+  uint32_t gend = goff;                                                         // payload granule offset after this slot
   // ---- plan entries of the warp's simple agents: staged in shared memory, written as whole 32-byte sectors
   // (per-thread 16-byte stores to scattered places would make the L2 fetch every sector before merging it)
   {
@@ -616,7 +628,7 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
       if (mycnt) {
         for (uint32_t j = 0; j < mycnt; ++j) {
           uint64_t e;
-          if (cnt <= KEEP) {
+          if (in_regs) {
             e = ev[0];
 #pragma unroll
             for (uint32_t u = 1; u < KEEP; ++u) if (j == u) e = ev[u];
@@ -631,6 +643,7 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
           }
           g0 += g;
         }
+        gend = g0;
       }
       __syncwarp();
       const uint32_t nst = min(SDB_PLAN_STAGE, wtotal - c0);
@@ -650,8 +663,10 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
     select_agent_warp(v, r.plan, Q_, false, A_, H_, T_, N_, C_, RO_, lane, retire);
     __threadfence_block();
     __syncwarp();
-    fill_offsets_warp(r.plan, RO_, C_, G_, lane);
+    const uint32_t end = fill_offsets_warp(r.plan, RO_, C_, G_, lane);
+    if (lane == src) gend = end;
   }
+  if (lead) atomicMax(r.lb + totals_at, ~((static_cast<unsigned long long>(cnt) << 32) | gend));
   uint32_t n_deliv = retire ? cnt : 0u;
   for (int o = 16; o; o >>= 1) n_deliv += __shfl_xor_sync(0xFFFFFFFFu, n_deliv, o);
   if (lane == 0 && n_deliv) atomicAdd(&v.ctr->delivered, static_cast<unsigned long long>(n_deliv));
@@ -937,7 +952,9 @@ k_recv_small(sdb_dev_view v, sdb_small_agents ag, uint32_t n, uint32_t max_messa
     for (uint32_t w = 0; w < SDB_SMALL_AGENTS; ++w) {
       s_roff[w] = acc;
       const uint32_t c = s_cnt[w];
-      if (open && acc + c <= rec_cap) total = acc + c; else { open = false; s_cnt[w] = 0; }   // whole-agent truncation
+      if (open && acc + c <= rec_cap) total = acc + c;
+      else if (open && acc == 0) { open = false; s_cnt[w] = rec_cap; total = rec_cap; }      // first in the output: its first rec_cap
+      else { open = false; s_cnt[w] = 0; }                                                    // whole-agent truncation
       acc += c;
     }
     s_total = total;
@@ -1263,3 +1280,6 @@ extern "C" cudaError_t sdb_launch_arena_floor(const sdb_dev_view* v, uint32_t n_
   if (n_agents) k_arena_floor<<<(n_agents + 255) / 256, 256, 0, stream>>>(*v, n_agents, tail32, max_dist_dev);
   return cudaGetLastError();
 }
+
+// any kernel of this file: its module is loaded as a whole before the latency server starts (sdb_api.cu)
+extern "C" const void* sdb_recv_kernel_anchor() { return reinterpret_cast<const void*>(&k_scan_local); }

@@ -1552,3 +1552,6 @@ extern "C" cudaError_t sdb_launch_commit(const sdb_dev_view* v, uint32_t n_agent
   sdb_prof_end(prof, pi, stream);
   return cudaGetLastError();
 }
+
+// any kernel of this file: its module is loaded as a whole before the latency server starts (sdb_api.cu)
+extern "C" const void* sdb_send_kernel_anchor() { return reinterpret_cast<const void*>(&k_commit_ranked_sweep); }

@@ -105,6 +105,46 @@ def test_c2_full_batch_matches_oracle(variant, fixed):
     gpu.close(); cpu.close()
 
 
+def test_c2_full_batch_priority_receive_matches_oracle():
+    """The c2 construction (1M agents, two batches of 65,536 group sends to groups of 64) drained in PRIORITY order
+    with k = 5, then k = 100.  The record bound min(n k, capacity) is above 4 x 2^20, so the payload scan's k_scan_tops
+    sweeps more than 1024 tiles of 4096 records, and k_recv_select_big selects for every one of the 1M agents."""
+    from bench import Workload
+    from oracle.cpu_ref import CpuOracle
+    from swarmdb_b200._native import RECV_PRIORITY, Shard
+    wl = Workload()
+    cap = wl.S * wl.F * 2 + (1 << 16)
+    assert min(wl.A * 5, cap) > 1024 * 4096                       # tiles of 4096 records, 1024 tiles per sweep
+    gpu = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 32, max_payload_bytes=wl.L, max_groups=1 << 14,
+                member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                max_recv_records=cap, max_recv_payload=cap * wl.L)
+    cpu = CpuOracle(wl.A, wl.G)
+    gpu.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        gpu.create_group(g, wl.members(g)); cpu.create_group(g, wl.members(g))
+    cpu.digest_enable(); gpu.digest_reset()
+    rng = np.random.default_rng(9)
+    for _ in range(2):
+        snd, grp, prio, typ, lens, off, payload = wl.batch()
+        prio = rng.integers(0, 4, wl.S).astype(np.uint8)                  # four levels: the selection has work to do
+        lens = rng.integers(1, wl.L + 1, wl.S).astype(np.uint16)
+        assert gpu.send_group_batch(snd, grp, prio, typ, lens, off, payload) == \
+            cpu.send_group_batch(snd, grp, prio, typ, lens, off, payload)[0]
+    gpu.profile(True)
+    for k in (5, 100):
+        _, total, _ = gpu.receive_batch(None, k, RECV_PRIORITY, copy_out=False)
+        assert gpu.profile_read()["recv_count"][1] == 1                    # the priority pipeline served it
+        gpu.digest_fold()
+        _, ctotal = cpu.receive_counts(None, k, RECV_PRIORITY)
+        assert total == ctotal
+    st = gpu.stats()
+    assert st["ring_overflow"] == 0 and st["delivered"] == 2 * wl.S * wl.F
+    dg, dc = gpu.digest_read(), cpu.digest_read()
+    assert int((dc != 0).sum()) > 0.99 * wl.A
+    assert not _mismatch(dg, dc), _mismatch(dg, dc)
+    gpu.close(); cpu.close()
+
+
 @pytest.mark.parametrize("priority", [True, False])
 def test_c4_sweeps_until_empty_match_oracle(priority):
     """BASELINE config 4 shape: ~10k agents, 2,048 pending records each, 4 priority levels; receive 100 per agent

@@ -22,6 +22,7 @@ pytestmark = pytest.mark.gpu
 ROOT = Path(__file__).resolve().parents[1]
 PARITY = "tests/test_gpu_parity.py"
 SHARED = "tests/test_gpu_shared_layout.py"
+PATHS = "tests/test_gpu_receive_paths.py"
 
 MATRIX = {
     "SDB_SHARED_PAYLOAD=0": [SHARED + "::test_shared_records_through_the_small_receive_path",
@@ -41,7 +42,8 @@ MATRIX = {
                       PARITY + "::test_many_records_for_one_agent_in_one_batch"],
     "SDB_PLAN_TICKET=0": [PARITY + "::test_p2p_then_drain",
                           PARITY + "::test_receive_capacity_truncates_by_whole_agents_without_loss",
-                          SHARED + "::test_shared_records_through_the_bulk_gathers"],
+                          SHARED + "::test_shared_records_through_the_bulk_gathers",
+                          PATHS + "::test_plan_warps_mix_empty_simple_holey_and_truncated_agents"],
     "SDB_OVERLAP_INDEX=1": [SHARED + "::test_shared_records_through_the_bulk_gathers",
                             SHARED + "::test_shared_batches_wrap_a_small_arena",
                             PARITY + "::test_group_fanout_parity"],
