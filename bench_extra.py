@@ -5,6 +5,7 @@
   c4  priority dequeue: 10k agents x 10k pending 256-byte messages, 4 levels, receive_batch(all, 100)
   c5  backend balancer: 1M requests over 256 backends (weighted least-load, weighted random)
   k1  point-to-point enqueue kernel roofline (1M records x 256 B)
+  compact  the c2 step with host buffers out: full receive format against the compact format (sdb_receive_compact)
 
 bench.py remains the contract benchmark (c2/c3); this file only feeds DESIGN.md.
 """
@@ -185,6 +186,121 @@ def bcast(n_agents=1_000_000, n_sends=16):
             "roofline": {"bound": "hbm", "algorithmic_bytes": alg, "achieved": alg / (send_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                          "frac": alg / (send_ms * 1e-3) / 1e9 / peak, "peak_source": src,
                          "note": "fan-out kernel only; the call's wall time adds host validation and 64 MB of recipient indices over PCIe"}}
+
+
+def _gpu_card(index=0):
+    """Name and enforced power limit of the card (NVML reads only)."""
+    import torch
+    out = {"gpu": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        h = pynvml.nvmlDeviceGetHandleByIndex(index)
+        out["power_limit_w"] = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
+    except Exception as e:  # pragma: no cover
+        out["power_limit_error"] = repr(e)
+    return out
+
+
+def compact(rounds=3, block=8):
+    """The c2 step with host buffers out (bench.py's e2e step: send_group_batch from pinned inputs, then a receive of
+    every agent into pinned outputs), full format against the compact format (sdb_receive_compact), alternated in
+    blocks in one process.  D2H bytes per step come from the returned totals."""
+    import torch
+    from bench import ClockSampler, Workload
+    from swarmdb_b200._native import ENTRY_DTYPE, HDR_DTYPE, RECV_PEEK, SEND_DTYPE, Shard, expand_compact
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py compact: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    stream = torch.cuda.Stream()
+    shard = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+    shard.set_stream(stream.cuda_stream)
+    shard.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        shard.create_group(g, wl.members(g))
+    shard.sync()
+
+    def pinned(nbytes):
+        return torch.empty(nbytes, dtype=torch.uint8, pin_memory=True).numpy()
+
+    pinned_in = []
+    for _ in range(4):
+        b = wl.batch()
+        t = pinned(b[6].nbytes); t[:] = b[6]
+        pinned_in.append(b[:6] + (t,))
+    pin_hdr, pin_pay = pinned(rec_cap * 32).view(HDR_DTYPE), pinned(rec_cap * wl.L)
+    pin_ent, pin_snd, pin_cpay = pinned(rec_cap * 16).view(ENTRY_DTYPE), pinned(rec_cap * 32).view(SEND_DTYPE), pinned(rec_cap * wl.L)
+
+    def full_step(i):
+        shard.send_group_batch(*pinned_in[i % len(pinned_in)])
+        cnt, hdr, pay = shard.receive_batch(None, 100, 0, copy_out=True, out_hdr=pin_hdr, out_payload=pin_pay)
+        assert len(hdr) == per_step
+        return len(cnt) * 4 + len(hdr) * 32 + len(pay) + 16                   # counts + headers + payloads + totals
+
+    def compact_step(i):
+        shard.send_group_batch(*pinned_in[i % len(pinned_in)])
+        cnt, ent, snd, pay = shard.receive_compact(None, 100, 0, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_cpay)
+        assert len(ent) == per_step
+        return len(cnt) * 4 + len(ent) * 16 + len(snd) * 32 + len(pay) + 24     # counts + entries + rows + payloads + totals
+
+    def timed(step, i0):
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t = time.perf_counter()
+        e0.record(stream)
+        nbytes = [step(i0 + i) for i in range(block)]
+        e1.record(stream)
+        torch.cuda.synchronize()
+        ms = max(e0.elapsed_time(e1), (time.perf_counter() - t) * 1e3)         # host work between calls counts too
+        return ms / block, nbytes[-1]
+
+    res = {"full": [], "compact": []}
+    d2h = {}
+    with torch.cuda.stream(stream):
+        for i in range(2):
+            full_step(i); compact_step(i)
+        # outside the timed region: one compact step equals a full receive of the same records
+        shard.send_group_batch(*pinned_in[0])
+        cnt, ent, snd, pay = shard.receive_compact(None, 100, RECV_PEEK)
+        hdr_c, pay_c = expand_compact(ent, snd, pay)
+        cnt = cnt.copy()
+        cg, hg, pg = shard.receive_batch(None, 100, 0)
+        assert np.array_equal(cnt, cg) and hdr_c.tobytes() == hg.tobytes() and pay_c.tobytes() == pg.tobytes()
+        assert len(snd) == wl.S
+        del hdr_c, pay_c
+        clocks = ClockSampler(0); clocks.start()
+        for r in range(rounds):
+            for name, step in (("full", full_step), ("compact", compact_step)):
+                ms, d2h[name] = timed(step, r * block)
+                res[name].append(ms)
+        clk = clocks.stop()
+        kern = {}
+        for name, step in (("full", full_step), ("compact", compact_step)):
+            shard.profile(True)
+            for i in range(block):
+                step(i)
+            prof = shard.profile_read()
+            shard.profile(False)
+            kern[name] = {k: v[0] / block for k, v in prof.items() if v[1]}
+    st = shard.stats()
+    assert st["ring_overflow"] == 0 and st["delivered"] == st["enqueued"]
+    shard.close()
+    out = {"config": f"c2 e2e: {wl.A} agents, {wl.S} group sends x {wl.F} members, {wl.L}-B payloads; pinned host "
+                     f"buffers in and out; {rounds} rounds of {block} full-format steps, then {block} compact steps"}
+    for name in ("full", "compact"):
+        ms = float(np.median(res[name]))
+        recv_k = kern[name].get("recv_select", 0.0) + kern[name].get("recv_gather" if name == "full" else "recv_compact", 0.0)
+        out[name] = {"ms_per_step_blocks": res[name], "ms_per_step": ms, "msgs_per_s": per_step / (ms * 1e-3),
+                     "d2h_bytes_per_step": d2h[name], "receive_kernels_ms_per_step": recv_k,
+                     "kernel_ms_per_step": kern[name]}
+    out["speedup"] = out["full"]["ms_per_step"] / out["compact"]["ms_per_step"]
+    out.update(_gpu_card(0))
+    out["clocks"] = clk
+    return out
 
 
 def main():

@@ -129,7 +129,8 @@ int sdb_advance_seq(sdb_handle h, uint64_t next_seq);
 /* Per-kernel device timing (CUDA events on the handle's stream), used by bench.py for the
  * roofline: enable, run, then read accumulated milliseconds and launch counts per kernel class. */
 enum { SDB_PK_P2P = 0, SDB_PK_FANOUT, SDB_PK_COMMIT, SDB_PK_RECV_COUNT, SDB_PK_RECV_SCAN, SDB_PK_RECV_SELECT,
-       SDB_PK_RECV_GATHER, SDB_PK_ARENA_FLOOR, SDB_PK_PICK, SDB_PK_XSHARD, SDB_PK_INDEX, SDB_PK_XWAIT, SDB_PK_N = 16 };
+       SDB_PK_RECV_GATHER, SDB_PK_ARENA_FLOOR, SDB_PK_PICK, SDB_PK_XSHARD, SDB_PK_INDEX, SDB_PK_XWAIT,
+       SDB_PK_RECV_COMPACT = 12, SDB_PK_N = 16 };
 int sdb_profile(sdb_handle h, int enable);
 int sdb_profile_read(sdb_handle h, double* ms_out /* [SDB_PK_N] */, uint64_t* count_out /* [SDB_PK_N] */);
 
@@ -232,6 +233,51 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
                       uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
                       uint8_t* payload_out, uint64_t payload_cap,
                       uint64_t* total_out, uint64_t* payload_bytes_out);
+/* Compact receive: the records sdb_receive_batch would select and retire, with each distinct payload image
+ * returned once.  For host consumers, whose cost is the bytes that cross PCIe: a group send's m records share one
+ * payload in the arena (shared layout), and the full format copies that payload out m times.
+ *   count_out[n_agents]  as in sdb_receive_batch;
+ *   entry_out[total]     one 16-byte entry per record, in sdb_receive_batch's header order (agent by agent,
+ *                        delivery order);
+ *   send_out[n_sends]    one 32-byte row per distinct payload image;
+ *   payload_out          the distinct payloads back to back, each padded to SDB_GRANULE, in row order.
+ * Contract:
+ *   1. Expansion equals the full receive byte for byte.  With row = send_out[entry.send], record r's header is
+ *      {entry.seq, row.timestamp, row.sender, entry.receiver, row.group, row.len, row.prio, row.type} and its padded
+ *      payload is payload_out[row.payload_off, row.payload_off + pad32(row.len)), pad bytes included.
+ *   2. Records whose ring entries point at the same arena payload (shared layout: one group send) share one row;
+ *      every other record (point-to-point, broadcast copies, SDB_SHARED_PAYLOAD=0) has its own.  A send with only
+ *      some of its records in the call still gets exactly one row.  Zero-length payloads of different sends never
+ *      share a row.
+ *   3. Rows are in order of first appearance in entry_out: the first occurrences of entry.send read 0, 1, 2, ..
+ *      and payload_off is the running sum of pad32(len) over the rows.  The result depends neither on timing nor
+ *      on the grid.
+ *   4. Capacity as in sdb_receive_batch, with rec_cap = min(max_recv_records, max_recv_payload / P, entry_cap,
+ *      send_cap, payload_cap / P) (each caller cap counts only when its pointer is given), P = pad32(max_payload_bytes).
+ *      The unshared worst case always fits, so which records a call takes never depends on how much they share.
+ *   5. SDB_RECV_PRIORITY, SDB_RECV_PEEK and SDB_RECV_OWNED as in sdb_receive_batch; SDB_RECV_ASYNC is refused
+ *      (SDB_EINVAL).  The call always runs the bulk plan (never the few-agent or latency-server paths).  It leaves no
+ *      full-format device results: sdb_digest_fold after it returns SDB_EINVAL until the next sdb_receive_batch.
+ * *total_out, *n_sends_out and *payload_bytes_out (each nullable) receive the totals. */
+typedef struct sdb_recv_entry {
+  uint64_t seq;        /* header.seq of this record */
+  uint32_t send;       /* row of send_out holding the rest of its header and its payload */
+  uint32_t receiver;   /* header.receiver of this record */
+} sdb_recv_entry;
+typedef struct sdb_recv_send {
+  double   timestamp;
+  uint64_t payload_off; /* byte offset of the padded payload in payload_out */
+  uint32_t sender;
+  uint32_t group;
+  uint16_t len;
+  uint8_t  prio;
+  uint8_t  type;
+  uint32_t reserved;    /* 0 */
+} sdb_recv_send;
+int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                        uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                        sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                        uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
 /* Low-latency dequeue server (opt-in): receive_messages (M:521-601) for ONE agent in a few microseconds.
  * enable = 1 starts a persistent single-CTA kernel on its own stream that polls a mailbox in mapped pinned host memory;
  * sdb_receive_batch calls naming exactly one agent with host outputs (what the Python surface's receive_messages makes)

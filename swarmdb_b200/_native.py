@@ -23,6 +23,11 @@ QSTATS_FIELDS = ["agents_with_pending", "pending", "p0", "p1", "p2", "p3", "pend
 HDR_DTYPE = np.dtype([("seq", "<u8"), ("timestamp", "<f8"), ("sender", "<u4"), ("receiver", "<u4"),
                       ("group", "<u4"), ("len", "<u2"), ("prio", "u1"), ("type", "u1")])
 assert HDR_DTYPE.itemsize == 32
+# compact receive format (sdb_recv_entry / sdb_recv_send): one entry per record, one row per distinct payload image
+ENTRY_DTYPE = np.dtype([("seq", "<u8"), ("send", "<u4"), ("receiver", "<u4")])
+SEND_DTYPE = np.dtype([("timestamp", "<f8"), ("payload_off", "<u8"), ("sender", "<u4"), ("group", "<u4"),
+                       ("len", "<u2"), ("prio", "u1"), ("type", "u1"), ("reserved", "<u4")])
+assert ENTRY_DTYPE.itemsize == 16 and SEND_DTYPE.itemsize == 32
 
 NO_GROUP = 0xFFFFFFFF
 NO_RECEIVER = 0xFFFFFFFF
@@ -68,7 +73,7 @@ class SdbStats(C.Structure):
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
-           "sdb_receive_batch", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
+           "sdb_receive_batch", "sdb_receive_compact", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
@@ -113,6 +118,8 @@ def load_library() -> C.CDLL:
     L.sdb_free_staged.restype = i32; L.sdb_free_staged.argtypes = [vp, vp]
     L.sdb_receive_batch.restype = i32
     L.sdb_receive_batch.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, vp]
+    L.sdb_receive_compact.restype = i32
+    L.sdb_receive_compact.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_latency_server.restype = i32; L.sdb_latency_server.argtypes = [vp, i32]
     L.sdb_last_receive_dev.restype = i32; L.sdb_last_receive_dev.argtypes = [vp, vp, vp, vp]
     L.sdb_last_receive_totals.restype = i32; L.sdb_last_receive_totals.argtypes = [vp, vp, vp]
@@ -242,7 +249,7 @@ class Shard:
         self._check(self._L.sdb_advance_seq(self._h, next_seq))
 
     PROFILE_KINDS = ["p2p", "fanout", "commit", "recv_count", "recv_scan", "recv_select", "recv_gather",
-                     "arena_floor", "pick", "xshard", "index", "xwait"]
+                     "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact"]
 
     def profile(self, enable: bool) -> None:
         self._check(self._L.sdb_profile(self._h, 1 if enable else 0))
@@ -476,6 +483,36 @@ class Shard:
             counts = counts[: self.n_owned if owned else self.stats_n_agents()]
         return counts, hdr[: total.value], pay[: pbytes.value]
 
+    def receive_compact(self, agents, max_messages: int, flags: int = 0, out_entries: Optional[np.ndarray] = None,
+                        out_sends: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+        """The records receive_batch would return, in the compact format (include/swarmdb_b200.h:
+        sdb_receive_compact): (counts[n_agents], entries[total] ENTRY_DTYPE, sends[n_sends] SEND_DTYPE, payload bytes),
+        each distinct payload once.  Views into reusable buffers unless explicit (e.g. pinned) arrays are given;
+        expand_compact() turns them into receive_batch's (headers, payload)."""
+        if agents is None:
+            a, n = None, 0
+            counts = np.zeros(self.max_agents, np.uint32)
+        else:
+            a = _arr(agents, np.uint32)
+            n = len(a)
+            counts = np.zeros(n, np.uint32)
+        if out_entries is None or out_sends is None:
+            cur = getattr(self, "_out_ent", None)
+            if cur is None or len(cur[0]) < self.max_recv_records:
+                self._out_ent = (np.zeros(self.max_recv_records, ENTRY_DTYPE), np.zeros(self.max_recv_records, SEND_DTYPE))
+        ent = out_entries if out_entries is not None else self._out_ent[0]
+        snd = out_sends if out_sends is not None else self._out_ent[1]
+        pay = out_payload if out_payload is not None else self._grow_pay()
+        total, n_sends, pbytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_receive_compact(self._h, n, _p(a), max_messages, flags, _p(counts), _p(ent), len(ent),
+                                                _p(snd), len(snd), _p(pay), pay.nbytes,
+                                                C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
+                                                C.cast(C.byref(pbytes), C.c_void_p)))
+        if agents is None:
+            owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
+            counts = counts[: self.n_owned if owned else self.stats_n_agents()]
+        return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
+
     def latency_server(self, enable: bool) -> None:
         """Start / stop the persistent low-latency dequeue server (single-agent receives then skip launch, sync and D2H)."""
         self._check(self._L.sdb_latency_server(self._h, 1 if enable else 0))
@@ -593,6 +630,31 @@ class Shard:
         out = np.zeros(n_req, np.uint32)
         self._check(self._L.sdb_select_backend_batch(self._h, n_req, _p(c), mode, seed, _p(out)))
         return out
+
+
+def expand_compact(entries: np.ndarray, sends: np.ndarray, payload: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
+    """(headers, payload) in receive_batch's format from a compact receive's (entries, sends, payload): record r takes
+    seq and receiver from its entry, every other header field and its padded payload from row sends[entry.send]."""
+    entries = np.asarray(entries, ENTRY_DTYPE)
+    sends = np.asarray(sends, SEND_DTYPE)
+    payload = np.asarray(payload, np.uint8)
+    row = sends[entries["send"].astype(np.int64)]
+    hdr = np.empty(len(entries), HDR_DTYPE)
+    hdr["seq"], hdr["receiver"] = entries["seq"], entries["receiver"]
+    for f in ("timestamp", "sender", "group", "len", "prio", "type"):
+        hdr[f] = row[f]
+    # padded payloads are whole 32-byte granules: granule k of record r is granule row.payload_off / 32 + k of the
+    # compact payload, so one gather over granules builds the full stream
+    glen = pad32(row["len"].astype(np.int64)) >> 5
+    total = int(glen.sum())
+    out = np.empty(total * 32, np.uint8)
+    if total:
+        dst_start = np.zeros(len(glen), np.int64)
+        np.cumsum(glen[:-1], out=dst_start[1:])
+        src = np.repeat((row["payload_off"].astype(np.int64) >> 5) - dst_start, glen) + np.arange(total, dtype=np.int64)
+        gran = np.ascontiguousarray(payload[: len(payload) & ~31]).view("V32")
+        out.view("V32")[:] = gran[src]
+    return hdr, out
 
 
 def payload_offsets(hdr: np.ndarray) -> np.ndarray:

@@ -738,6 +738,13 @@ class SwarmsDB:
         pr = self.gpu_config.priority_dequeue if priority is None else priority
         return self.shard.receive_batch(agent_idx, max_messages, RECV_PRIORITY if pr else 0, **kw)
 
+    def receive_batch_compact(self, agent_idx=None, max_messages: int = 100, priority: Optional[bool] = None, **kw):
+        """receive_batch's records in the compact format: (counts, entries, sends, payload) with each distinct
+        payload once (Shard.receive_compact; _native.expand_compact gives receive_batch's (headers, payload))."""
+        self.flush()
+        pr = self.gpu_config.priority_dequeue if priority is None else priority
+        return self.shard.receive_compact(agent_idx, max_messages, RECV_PRIORITY if pr else 0, **kw)
+
     # ------------------------------------------------------------------ LLM backends (M:1281-1325 + real balancer)
     def set_llm_load_balancing(self, enabled: bool = True) -> None:
         self.llm_load_balancing = enabled

@@ -32,7 +32,8 @@ cudaError_t sdb_launch_commit(const sdb_dev_view*, uint32_t, uint32_t, uint32_t*
 cudaError_t sdb_launch_pull(const sdb_dev_view*, const sdb_pull_view*, const sdb_send_desc*, uint32_t, uint32_t, const uint8_t*,
                             uint32_t, uint32_t, const uint32_t*, const uint32_t*, uint64_t, int, cudaStream_t, sdb_profiler*, int*,
                             const sdb_batch_base*, uint32_t);
-cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaStream_t, int*, sdb_profiler*, int, uint32_t);
+cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaStream_t, int*, sdb_profiler*, int, uint32_t,
+                               const sdb_compact_args*);
 cudaError_t sdb_recv_prepare_device();
 cudaError_t sdb_balance_prepare_device();
 cudaError_t sdb_launch_receive_small(const sdb_dev_view*, const uint32_t*, uint32_t, uint32_t, uint32_t, uint32_t, uint4*,
@@ -172,6 +173,8 @@ struct sdb_ctx {
   cudaStream_t ls_stream = nullptr; bool ls_wanted = false, ls_running = false; uint32_t ls_seq = 0;
   bool stream_busy = false;                    // work was enqueued on `stream` since the last synchronisation
   sdb_recv_args last_rx{}; bool last_rx_valid = false;   // the last bulk receive (sdb_digest_fold reads its device results)
+  bool last_rx_compact = false;                          // the last receive was compact: no full-format device results
+  sdb_compact_args cx{};                                 // compact receive scratch + outputs, allocated on first use
   unsigned long long* digest = nullptr;                  // [max_agents] stream digests, allocated on first use
   // backends
   uint32_t* be_weight = nullptr; unsigned long long* be_load = nullptr; uint32_t n_backends = 0;
@@ -931,7 +934,9 @@ int sdb_destroy(sdb_handle h) {
                  h->xs_lw_tops, h->xs_tab, h->xs_meta, h->shard_of_dev, h->rx_agent, h->rx_cnt,
                  h->rx_rec_local, h->rx_rec_tops, h->rx_plan, h->rx_plan_tops,
                  h->rx_totals, h->rx_big_list, h->rx_big_count, h->rx_count, h->rx_hdr, h->rx_payload,
-                 h->be_weight, h->be_load, h->be_scratch, h->be_logtab, h->be_req_cost, h->be_out, h->digest};
+                 h->be_weight, h->be_load, h->be_scratch, h->be_logtab, h->be_req_cost, h->be_out, h->digest,
+                 h->cx.table, h->cx.rec_slot, h->cx.head, h->cx.head_local, h->cx.head_tops, h->cx.gran, h->cx.gran_local,
+                 h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out};
   for (void* p : dev) if (p) cudaFree(p);
   if (h->descs_host) cudaFreeHost(h->descs_host);
   if (h->list_host) cudaFreeHost(h->list_host);
@@ -1666,15 +1671,8 @@ static void unpack_small(const uint8_t* block, uint32_t n_agents, uint32_t* coun
   if (payload_bytes_out) *payload_bytes_out = poff;
 }
 
-int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
-                      uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
-                      uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
-  if (!h) return SDB_EINVAL;
-  if (total_out) *total_out = 0;
-  if (payload_bytes_out) *payload_bytes_out = 0;
-  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
-  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
-  if (n_agents == 0 || max_messages == 0) return SDB_OK;
+// agent list of a receive: within the index space, and no agent twice
+static int check_recv_agents(sdb_ctx* h, uint32_t n_agents, const uint32_t* agent_idx) {
   if (n_agents > h->cfg.max_agents) return fail(h, SDB_EINVAL, "n_agents > max_agents");
   if (agent_idx) {
     for (uint32_t i = 0; i < n_agents; ++i)
@@ -1691,6 +1689,19 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
       if (i < n_agents) return fail(h, SDB_EINVAL, "agent index listed twice");
     }
   }
+  return SDB_OK;
+}
+
+int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                      uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
+                      uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
+  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
+  if (n_agents == 0 || max_messages == 0) return SDB_OK;
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
   // record capacity of the call, the same on every path: the device buffers and the caller's buffers must each hold
   // rec_cap records of the maximum size (what does not fit stays queued: include/swarmdb_b200.h)
   const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
@@ -1702,7 +1713,7 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   if (agent_idx && n_agents <= 8 && hdr_out && payload_out &&
       static_cast<uint64_t>(n_agents) * max_messages <= 1024) {
     rec_cap = std::min<uint64_t>(rec_cap, 1024);
-    h->last_rx_valid = false;
+    h->last_rx_valid = false; h->last_rx_compact = false;
     bool served = false;
     if (h->ls_wanted && n_agents == 1) {
       { int rcl = ls_start(h); if (rcl != SDB_OK) return rcl; }
@@ -1756,10 +1767,11 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   r.count_out = h->rx_count; r.hdr_out = h->rx_hdr; r.payload_out = h->rx_payload;
   r.rec_cap = rec_cap;
   int nl = 0;
-  cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes));
+  cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
+                                     nullptr);
   h->launches += nl;
   if (!(r.flags & SDB_RECV_PRIORITY)) r.plan_tops = nullptr;       // single-pass path: plan offsets are absolute
-  h->last_rx = r; h->last_rx_valid = (e == cudaSuccess);
+  h->last_rx = r; h->last_rx_valid = (e == cudaSuccess); h->last_rx_compact = false;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("receive launch: ") + cudaGetErrorString(e));
   h->stream_busy = async;
   if (async) return SDB_OK;          // the caller consumes on the device (stream order) or asks sdb_last_receive_totals later
@@ -1774,6 +1786,89 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
     if (hdr_out) CUDA_TRY(h, cudaMemcpyAsync(hdr_out, h->rx_hdr, total * sizeof(sdb_msg_header), cudaMemcpyDeviceToHost, h->stream));
     if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->rx_payload, pbytes, cudaMemcpyDeviceToHost, h->stream));
     if (hdr_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return SDB_OK;
+}
+
+// compact receive scratch and outputs, sized for max_recv_records; allocated once, on the first compact call
+static int compact_ensure(sdb_ctx* h) {
+  sdb_compact_args& c = h->cx;
+  if (c.table) return SDB_OK;
+  { int rcl = ls_stop(h); if (rcl != SDB_OK) return rcl; }      // the allocations below may wait for running kernels
+  const size_t R = h->cfg.max_recv_records, tiles = (R + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE + 1;
+  uint32_t tbits = 10;
+  while ((1ull << tbits) < 2 * R) ++tbits;
+  const bool ok = dmalloc(&c.rec_slot, R) == cudaSuccess && dmalloc(&c.head, R) == cudaSuccess &&
+                  dmalloc(&c.head_local, R) == cudaSuccess && dmalloc(&c.head_tops, tiles) == cudaSuccess &&
+                  dmalloc(&c.gran, R) == cudaSuccess && dmalloc(&c.gran_local, R) == cudaSuccess &&
+                  dmalloc(&c.gran_tops, tiles) == cudaSuccess && dmalloc(&c.totals, 2) == cudaSuccess &&
+                  dmalloc(&c.entry_out, R) == cudaSuccess && dmalloc(&c.send_out, R) == cudaSuccess &&
+                  dmalloc(&c.payload_out, h->pay_cap_gran * SDB_GRANULE) == cudaSuccess &&
+                  dmalloc(&c.table, static_cast<size_t>(1) << tbits) == cudaSuccess;   // last: marks the set complete
+  if (!ok) {
+    void* p[] = {c.table, c.rec_slot, c.head, c.head_local, c.head_tops, c.gran, c.gran_local, c.gran_tops, c.totals,
+                 c.entry_out, c.send_out, c.payload_out};
+    for (void* q : p) if (q) cudaFree(q);
+    c = sdb_compact_args{};
+    cudaGetLastError();
+    return fail(h, SDB_ENOMEM, "compact receive: device allocation failed");
+  }
+  return SDB_OK;
+}
+
+int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                        uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                        sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                        uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_compact returns host results: SDB_RECV_ASYNC is not accepted");
+  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
+  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
+  if (n_agents == 0 || max_messages == 0) return SDB_OK;
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
+  // the same record capacity as sdb_receive_batch: rec_cap unshared records of the maximum size fit every buffer
+  const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
+  uint64_t rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
+  if (entry_out) rec_cap = std::min<uint64_t>(rec_cap, entry_cap);
+  if (send_out) rec_cap = std::min<uint64_t>(rec_cap, send_cap);
+  if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
+  if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  if (agent_idx) {
+    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  }
+  sdb_recv_args r{};
+  r.agent_idx = agent_idx ? h->rx_agent : (owned ? h->owned_dev : nullptr); r.n = n_agents; r.max_messages = max_messages;
+  r.flags = flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK);
+  r.cnt = h->rx_cnt; r.rec_local = h->rx_rec_local; r.rec_tops = h->rx_rec_tops;
+  r.rec_off = h->rx_rec_off; r.plan = h->rx_plan; r.lb = h->rx_lb;
+  r.plan_tops = h->rx_plan_tops; r.totals = h->rx_totals; r.big_list = h->rx_big_list; r.big_count = h->rx_big_count;
+  r.count_out = h->rx_count; r.hdr_out = h->rx_hdr; r.payload_out = h->rx_payload;
+  r.rec_cap = rec_cap;
+  int nl = 0;
+  cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
+                                     &h->cx);
+  h->launches += nl;
+  h->last_rx_valid = false; h->last_rx_compact = true;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("compact receive launch: ") + cudaGetErrorString(e));
+  h->stream_busy = false;
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host + 6, h->cx.totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  if (count_out)
+    CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  const uint64_t total = h->totals_host[0], n_sends = h->totals_host[6], pbytes = h->totals_host[7] * SDB_GRANULE;
+  if (total_out) *total_out = total;
+  if (n_sends_out) *n_sends_out = n_sends;
+  if (payload_bytes_out) *payload_bytes_out = pbytes;
+  if (total) {
+    if (entry_out) CUDA_TRY(h, cudaMemcpyAsync(entry_out, h->cx.entry_out, total * sizeof(sdb_recv_entry), cudaMemcpyDeviceToHost, h->stream));
+    if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
+    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
+    if (entry_out || send_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
   return SDB_OK;
 }
@@ -1876,6 +1971,7 @@ int sdb_digest_reset(sdb_handle h) {
 
 int sdb_digest_fold(sdb_handle h) {
   if (!h) return SDB_EINVAL;
+  if (h->last_rx_compact) return fail(h, SDB_EINVAL, "sdb_digest_fold: the last receive was compact (sdb_receive_compact writes no full-format device results)");
   if (!h->last_rx_valid) return fail(h, SDB_EINVAL, "sdb_digest_fold: no bulk receive to fold (the <= 8-agent latency path keeps no device results)");
   int rc = digest_ensure(h);
   if (rc != SDB_OK) return rc;

@@ -58,6 +58,7 @@ struct __align__(16) sdb_send_desc {
 };
 static_assert(sizeof(sdb_send_desc) == 64, "desc must be 64 bytes");
 static_assert(sizeof(sdb_msg_header) == 32, "header must be 32 bytes");
+static_assert(sizeof(sdb_recv_entry) == 16 && sizeof(sdb_recv_send) == 32, "compact receive entries must be 16 and 32 bytes");
 
 #define SDB_DESC_SKIP_SENDER 1u   // group send: member == sender is skipped (M:1268)
 #define SDB_DESC_SHARED_SEQ 2u    // broadcast: every copy carries the same seq (one Message)
@@ -163,6 +164,23 @@ struct sdb_recv_args {
   sdb_msg_header* hdr_out;     // [rec_cap]
   uint8_t* payload_out;        // [rec_cap * pad32(max_payload)]
   uint64_t rec_cap;
+};
+
+// scratch + outputs of a compact receive (sdb_receive_compact), all indexed by output record number unless noted
+struct sdb_compact_args {
+  unsigned long long* table;   // [2^tbits] open addressing: payload position p << 32 | smallest record naming it; ~0 = empty
+  uint32_t tbits;
+  uint32_t* rec_slot;          // table slot of each record, then (k_compact_heads) the record that owns its image
+  uint32_t* head;              // 1 where a record owns its image (first appearance)
+  uint32_t* head_local;        // exclusive scan of head = row index (block-local part) ...
+  uint32_t* head_tops;         // ... and per-tile part
+  uint32_t* gran;              // payload granules of the image at its owner, 0 elsewhere
+  uint32_t* gran_local;        // exclusive scan of gran = payload offset in granules (block-local part) ...
+  uint32_t* gran_tops;         // ... and per-tile part
+  unsigned long long* totals;  // [0] rows, [1] payload granules
+  sdb_recv_entry* entry_out;   // [rec_cap]
+  sdb_recv_send* send_out;     // [rec_cap]
+  uint8_t* payload_out;        // [rec_cap * pad32(max_payload)]
 };
 
 // ---- asynchronous import (sdb_import_wire_ptrs_async): everything the host used to learn through a sync lives on

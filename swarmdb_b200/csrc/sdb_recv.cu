@@ -24,6 +24,8 @@
 //                                          the selected ring positions in (prio desc, arrival);
 //   scan            pay_off  = exclusive scan of payload granules over the planned RECORDS
 //   k_recv_gather   flat over records: copy header + payload from the arena to the packed output
+// A compact receive (sdb_receive_compact) runs either plan and replaces the gather with the compact kernels (below):
+// 16-byte entries per record and one row + payload per distinct payload image.
 //
 // Roofline: HBM-bound.  Algorithmic bytes per agent-call: P*1 priority bytes scanned (we scan
 // 2-byte ring_meta entries) + 2*k*(L+H) gather+emit (SURVEY 8d).
@@ -869,6 +871,120 @@ k_recv_gather_cpa(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
 }
 
 // ------------------------------------------------------------------------------------------
+// compact receive (sdb_receive_compact): the same plan, then one 16-byte entry per record and one row + payload per
+// distinct payload image.  A record's image is identified by its payload position p = handle + 1 + dm1 (mod 2^32):
+// the records of one shared-layout group send all point at the same p, every other record has its own (pending
+// images never overlap and the arena holds fewer than 2^32 granules).  Rows are numbered in order of first appearance:
+//   k_compact_owner   one thread per record: insert p into an open-addressing table, keep the smallest record naming
+//                     it (slot = p << 32 | record; one CAS claims an empty slot, an atomicMin on the same key lowers
+//                     the record)
+//   k_compact_heads   head flag where a record owns its image, and the image's payload granules at its owner
+//   scans             exclusive scans of both (k_scan_local + k_scan_tops): row index and payload offset
+//   k_compact_emit    every record writes its entry; owners write the row and copy the payload once
+// Record counts come from the plan's totals on the device (as the gathers read them): no host round trip.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_compact_owner(sdb_recv_args r, const unsigned long long* __restrict__ packed_inv, sdb_compact_args c) {
+  const uint32_t total = gather_total(r, packed_inv);
+  const uint32_t tmask = (1u << c.tbits) - 1u;
+  for (uint32_t rec = blockIdx.x * blockDim.x + threadIdx.x; rec < total; rec += gridDim.x * blockDim.x) {
+    const uint4 pe = __ldg(r.plan + rec);
+    const uint32_t p = pe.x + 1u + sdb_entry_dm1(pe.z);
+    const unsigned long long mine = (static_cast<unsigned long long>(p) << 32) | rec;
+    uint32_t s = (p * 0x9E3779B1u) >> (32u - c.tbits);            // Fibonacci hash: strided positions spread evenly
+    for (;;) {
+      unsigned long long cur = __ldcg(c.table + s);
+      if (cur == ~0ull) {
+        cur = atomicCAS(c.table + s, ~0ull, mine);
+        if (cur == ~0ull) break;
+      }
+      if ((cur >> 32) == p) {                                     // same key: min over the record half only
+        if (static_cast<uint32_t>(cur) > rec) atomicMin(c.table + s, mine);
+        break;
+      }
+      s = (s + 1u) & tmask;
+    }
+    c.rec_slot[rec] = s;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_compact_heads(sdb_recv_args r, sdb_compact_args c, uint32_t bound) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= bound) return;
+  const uint32_t total = static_cast<uint32_t>(r.totals[0]);
+  uint32_t h = 0, g = 0;
+  if (i < total) {
+    const uint32_t own = static_cast<uint32_t>(c.table[c.rec_slot[i]]);
+    c.rec_slot[i] = own;
+    h = own == i;
+    if (h) g = r.plan[i].z & 0xFFFFu;
+  }
+  c.head[i] = h;
+  c.gran[i] = g;
+}
+
+// 8 lanes per record, 4 records per warp step: lane 0 reads the 32-byte header and writes the entry (and, at an owner,
+// the row); an owner's 8 lanes copy its padded payload in 16-byte chunks
+__global__ void __launch_bounds__(256)
+k_compact_emit(sdb_dev_view v, sdb_recv_args r, sdb_compact_args c) {
+  const uint32_t total = static_cast<uint32_t>(r.totals[0]);
+  const uint32_t lane = threadIdx.x & 31, sub = lane >> 3, l8 = lane & 7;
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t nw = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t r0 = gw * 4u; r0 < total; r0 += nw * 4u) {
+    const uint32_t rec = r0 + sub;
+    if (rec >= total) continue;
+    const uint4 pe = __ldg(r.plan + rec);
+    const uint32_t own = c.rec_slot[rec];
+    const bool head = own == rec;
+    const uint64_t po = head ? (static_cast<uint64_t>(c.gran_local[rec]) + c.gran_tops[rec / SDB_SCAN_TILE]) << 5 : 0u;
+    if (l8 == 0) {
+      const uint8_t* src = v.arena + ((static_cast<uint64_t>(pe.x) & v.gmask) << 5);
+      const uint4 lo = sdb_ld_stream(src), hi = sdb_ld_stream(src + 16);    // {seq, timestamp}, {sender, receiver, group, len|prio|type}
+      const uint32_t row = c.head_local[own] + c.head_tops[own / SDB_SCAN_TILE];
+      sdb_st_stream(c.entry_out + rec, make_uint4(lo.x, lo.y, row, hi.y));
+      if (head) {
+        uint4* dst = reinterpret_cast<uint4*>(c.send_out + row);
+        sdb_st_stream(dst, make_uint4(lo.z, lo.w, static_cast<uint32_t>(po), static_cast<uint32_t>(po >> 32)));
+        sdb_st_stream(dst + 1, make_uint4(hi.x, hi.z, hi.w, 0u));
+      }
+    }
+    if (head) {
+      const uint32_t nchunk = (pe.z & 0xFFFFu) << 1;
+      const uint8_t* psrc = sdb_payload_of(v, pe.x, sdb_entry_dm1(pe.z));
+      uint8_t* pdst = c.payload_out + po;
+      for (uint32_t k = l8; k < nchunk; k += 8) sdb_st_stream(pdst + (k << 4), sdb_ld_stream(psrc + (k << 4)));
+    }
+  }
+}
+
+static cudaError_t launch_compact(const sdb_dev_view* v, const sdb_recv_args* r, const sdb_compact_args* c0,
+                                  const unsigned long long* packed_inv, uint64_t bound, int sm_count, cudaStream_t stream,
+                                  sdb_profiler* prof, int* n_launches) {
+  sdb_compact_args c = *c0;
+  uint32_t tbits = 10;                                         // at least twice as many slots as records: load <= 1/2
+  while ((1ull << tbits) < 2 * bound) ++tbits;
+  c.tbits = tbits;
+  const uint32_t n = static_cast<uint32_t>(bound), tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
+  uint64_t grid = (bound + 255) / 256;
+  const uint64_t cap = static_cast<uint64_t>(sm_count) * 8;
+  const int pi = sdb_prof_begin(prof, SDB_PK_RECV_COMPACT, stream);
+  cudaMemsetAsync(c.table, 0xFF, (1ull << tbits) * sizeof(unsigned long long), stream);
+  k_compact_owner<<<static_cast<uint32_t>(grid < cap ? grid : cap), 256, 0, stream>>>(*r, packed_inv, c);
+  k_compact_heads<<<static_cast<uint32_t>(grid), 256, 0, stream>>>(*r, c, n);
+  k_scan_local<<<tiles, 1024, 0, stream>>>(c.head, 0xFFFFFFFFu, c.head_local, c.head_tops, n);
+  k_scan_tops<<<1, 1024, 0, stream>>>(c.head_tops, tiles, c.totals);
+  k_scan_local<<<tiles, 1024, 0, stream>>>(c.gran, 0xFFFFFFFFu, c.gran_local, c.gran_tops, n);
+  k_scan_tops<<<1, 1024, 0, stream>>>(c.gran_tops, tiles, c.totals + 1);
+  const uint64_t ewarps = (bound + 3) / 4, eblocks = (ewarps + 7) / 8, ecap = static_cast<uint64_t>(sm_count) * 8 * 4;
+  k_compact_emit<<<static_cast<uint32_t>(eblocks < ecap ? eblocks : ecap), 256, 0, stream>>>(*v, *r, c);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += 7;
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------
 // stream digests (definition in include/swarmdb_b200.h): one warp per request slot folds the records the last
 // receive delivered to that agent, in delivery order, into digest[agent].  Lanes hash the 64-bit words of a
 // record in parallel (the per-word terms are position-keyed and summed), lane 0 chains the records.
@@ -1181,8 +1297,10 @@ extern "C" cudaError_t sdb_recv_prepare_device() {
   return cudaFuncSetAttribute(k_recv_gather_tma<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2 * 32 * 544);
 }
 
+// ca != nullptr: a compact receive (the same plan; the compact kernels replace the gather)
 extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_args* r0, cudaStream_t stream,
-                                          int* n_launches, sdb_profiler* prof, int sm_count, uint32_t max_rec_bytes) {
+                                          int* n_launches, sdb_profiler* prof, int sm_count, uint32_t max_rec_bytes,
+                                          const sdb_compact_args* ca) {
   if (r0->n == 0) return cudaSuccess;
   sdb_recv_args ra = *r0;
   sdb_recv_args* r = &ra;
@@ -1201,6 +1319,7 @@ extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_
     k_recv_plan<<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, ticketed);
     sdb_prof_end(prof, pi, stream);
     if (n_launches) *n_launches += 1;
+    if (ca) return launch_compact(v, r, ca, r->lb + sdb_lb_words(tiles) - 1, bound, sm_count, stream, prof, n_launches);
     return launch_gather(v, r, r->lb + sdb_lb_words(tiles) - 1, bound, max_rec_bytes, sm_count, stream, prof, n_launches);
   }
   const uint32_t tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
@@ -1227,6 +1346,7 @@ extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_
   k_scan_tops<<<1, 1024, 0, stream>>>(r->plan_tops, rtiles, r->totals + 1);    // totals[1] = payload granules
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += 7;
+  if (ca) return launch_compact(v, r, ca, nullptr, bound, sm_count, stream, prof, n_launches);
   return launch_gather(v, r, nullptr, bound, max_rec_bytes, sm_count, stream, prof, n_launches);
 }
 
