@@ -6,6 +6,7 @@
   c5  backend balancer: 1M requests over 256 backends (weighted least-load, weighted random)
   k1  point-to-point enqueue kernel roofline (1M records x 256 B)
   compact  the c2 step with host buffers out: full receive format against the compact format (sdb_receive_compact)
+  expire   retention on the c2 backlog (sdb_expire): drop mode at the median cutoff, SDB_EXPIRE_ALL, archive mode
 
 bench.py remains the contract benchmark (c2/c3); this file only feeds DESIGN.md.
 """
@@ -298,6 +299,126 @@ def compact(rounds=3, block=8):
                      "d2h_bytes_per_step": d2h[name], "receive_kernels_ms_per_step": recv_k,
                      "kernel_ms_per_step": kern[name]}
     out["speedup"] = out["full"]["ms_per_step"] / out["compact"]["ms_per_step"]
+    out.update(_gpu_card(0))
+    out["clocks"] = clk
+    return out
+
+
+def expire(rounds=3, block=4):
+    """sdb_expire on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 pending records, a seeded uniform
+    timestamp per send): drop mode at the median cutoff, SDB_EXPIRE_ALL, and archive mode into pinned host buffers,
+    alternated in blocks in one process.  Every timed call starts from a fresh backlog (drain + resend, untimed).
+    Outside the timed region the drop-mode result is drained through the digests and checked against an oracle that was
+    only ever sent the surviving sends."""
+    import torch
+    from bench import ClockSampler, Workload
+    from oracle.cpu_ref import CpuOracle
+    from swarmdb_b200._native import ENTRY_DTYPE, EXPIRE_ALL, SEND_DTYPE, Shard
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py expire: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    stream = torch.cuda.Stream()
+    shard = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+    shard.set_stream(stream.cuda_stream)
+    shard.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        shard.create_group(g, wl.members(g))
+    batch = wl.batch()
+    ts = np.random.default_rng(4242).uniform(0.0, 1.0, wl.S)
+    cut = float(np.median(ts))
+
+    def pinned(nbytes):
+        return torch.empty(nbytes, dtype=torch.uint8, pin_memory=True).numpy()
+    pin_ent, pin_snd, pin_pay = pinned(rec_cap * 16).view(ENTRY_DTYPE), pinned(rec_cap * 32).view(SEND_DTYPE), pinned(rec_cap * wl.L)
+
+    seq_base = [0]
+
+    def backlog():
+        while shard.receive_batch(None, 1 << 10, copy_out=False)[1]:
+            pass
+        seq_base[0] = shard.send_group_batch(*batch, ts=ts)
+        shard.sync()
+
+    calls = {"drop_median": lambda: shard.expire(None, cut, archive=False)[1],
+             "expire_all": lambda: shard.expire(None, 0.0, EXPIRE_ALL, archive=False)[1],
+             "archive_median": lambda: len(shard.expire(None, cut, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_pay)[1])}
+
+    def timed(fn):
+        backlog()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        t = time.perf_counter()
+        n = fn()                                         # synchronises: it returns totals
+        wall = (time.perf_counter() - t) * 1e3
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return wall, e0.elapsed_time(e1), n
+
+    res = {k: {"call_ms": [], "event_ms": []} for k in calls}
+    expired = {}
+    with torch.cuda.stream(stream):
+        for fn in calls.values():                        # warm-up: every shape once
+            timed(fn)
+        # outside the timed region: drop at the median, drain through the digests, compare with the oracle's own expiry
+        backlog()
+        n_drop = calls["drop_median"]()
+        shard.digest_reset()
+        while True:
+            _, t, _ = shard.receive_batch(None, 100, copy_out=False)
+            if not t:
+                break
+            shard.digest_fold()
+        o = CpuOracle(wl.A, wl.G)
+        o.register(np.arange(wl.A))
+        for g in range(wl.G):
+            o.create_group(g, wl.members(g))
+        # the oracle is sent only the surviving sends, with the device's sequence numbers (send i numbers its F members
+        # from seq_base + F i: every group has F members and no sender is in its own group)
+        keep = ~(ts < cut)
+        snd, grp, prio, typ, lens, off, pay = batch
+        o.send_group_seq(snd[keep], grp[keep], prio[keep], typ[keep], lens[keep], off[keep], pay,
+                         seq_base[0] + wl.F * np.nonzero(keep)[0].astype(np.uint64), ts[keep])
+        assert n_drop == wl.F * int((~keep).sum())
+        o.digest_enable()
+        o.receive_counts(None, 100)
+        digests_ok = bool(np.array_equal(shard.digest_read(), o.digest_read()))
+        o.close()
+        assert digests_ok, "digests after expiry differ from the oracle's"
+        clocks = ClockSampler(0); clocks.start()
+        for _ in range(rounds):
+            for name, fn in calls.items():
+                for _ in range(block):
+                    wall, ev, n = timed(fn)
+                    res[name]["call_ms"].append(wall); res[name]["event_ms"].append(ev)
+                    expired[name] = n
+        clk = clocks.stop()
+        kern = {}
+        for name, fn in calls.items():
+            backlog()
+            shard.profile(True)
+            fn()
+            prof = shard.profile_read()
+            shard.profile(False)
+            kern[name] = {k: v[0] for k, v in prof.items() if v[1]}
+    shard.close()
+    out = {"config": f"c2 backlog: {wl.A} agents, {wl.S} group sends x {wl.F} members = {per_step} pending records, "
+                     f"{wl.L}-B payloads, timestamps U[0,1) per send; {rounds} rounds of {block} calls per mode, each on a "
+                     f"fresh backlog", "digests_match_oracle": digests_ok}
+    for name in calls:
+        ms = float(np.median(res[name]["call_ms"]))
+        n = expired[name]
+        # algorithmic bytes: 16-B ring header per agent, then per pending record its 8-B entry and one 32-B timestamp
+        # sector, plus an 8-B tombstone per expired record; SDB_EXPIRE_ALL reads no entries (header read + write)
+        nbytes = 16 * wl.A * 2 if name == "expire_all" else 16 * wl.A + 40 * per_step + 8 * n
+        kms = sum(kern[name].values())
+        out[name] = {"records_expired": n, "ms_per_call": ms, "event_ms_per_call": float(np.median(res[name]["event_ms"])),
+                     "records_per_s": n / (ms * 1e-3), "kernel_ms": kern[name], "kernel_ms_total": kms,
+                     "algorithmic_bytes": nbytes, "algorithmic_gb_per_s_kernel": nbytes / (kms * 1e-3) / 1e9 if kms else None,
+                     "call_ms_blocks": res[name]["call_ms"]}
     out.update(_gpu_card(0))
     out["clocks"] = clk
     return out

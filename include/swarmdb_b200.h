@@ -130,7 +130,7 @@ int sdb_advance_seq(sdb_handle h, uint64_t next_seq);
  * roofline: enable, run, then read accumulated milliseconds and launch counts per kernel class. */
 enum { SDB_PK_P2P = 0, SDB_PK_FANOUT, SDB_PK_COMMIT, SDB_PK_RECV_COUNT, SDB_PK_RECV_SCAN, SDB_PK_RECV_SELECT,
        SDB_PK_RECV_GATHER, SDB_PK_ARENA_FLOOR, SDB_PK_PICK, SDB_PK_XSHARD, SDB_PK_INDEX, SDB_PK_XWAIT,
-       SDB_PK_RECV_COMPACT = 12, SDB_PK_N = 16 };
+       SDB_PK_RECV_COMPACT = 12, SDB_PK_EXPIRE = 13, SDB_PK_N = 16 };
 int sdb_profile(sdb_handle h, int enable);
 int sdb_profile_read(sdb_handle h, double* ms_out /* [SDB_PK_N] */, uint64_t* count_out /* [SDB_PK_N] */);
 
@@ -431,6 +431,37 @@ typedef struct sdb_queue_summary {
 } sdb_queue_summary;
 int sdb_agent_loads(sdb_handle h, uint32_t n, const uint32_t* agent_idx, sdb_agent_load* out);
 int sdb_queue_stats(sdb_handle h, sdb_queue_summary* out);
+
+/* ---- retention: flush_old_messages (M:1159-1206), retention.ms (M:123, M:254) --------------------------------------
+ * The arena is a log: space is reclaimed only behind the oldest pending record of any ring, so an agent that never
+ * receives (crashed, deregistered - deregistration keeps the ring - or idle) pins the whole log until sends fail with
+ * SDB_EARENA_FULL.  sdb_expire retires pending records on the device without delivering them.
+ *   Selection  for each listed agent (agent_idx == NULL: every index below the watermark, or the owned agents with
+ *              SDB_RECV_OWNED), every pending record whose header timestamp < older_than (the strict compare of M:1179:
+ *              a NaN timestamp or cutoff never expires anything).  Records sent with timestamp == NULL carry 0.0, so any
+ *              positive cutoff expires them.  SDB_EXPIRE_ALL: every pending record of the listed agents, timestamps not
+ *              read (purge).  An agent may appear only once in agent_idx (SDB_EINVAL otherwise).
+ *   Retire     the selected ring entries are tombstoned; the remaining records keep their order, and every later receive
+ *              (any order, any path) delivers what it would have delivered had the expired records never been enqueued.
+ *              sdb_stats does not move (expired records are neither delivered nor un-enqueued); in sdb_agent_loads
+ *              `pending` and `pending_granules` fall and `received` stays.  The arena floor is not moved by the call:
+ *              the next send that needs room recomputes it and finds the space.
+ *   Archive    (any of entry_out / send_out / payload_out given) the expired records are returned in the compact receive
+ *   mode       format with its contract and capacity rule (sdb_receive_compact, points 1-4): agents in list order, stream
+ *              order within an agent, one row per distinct payload image.  What does not fit stays queued: loop until
+ *              *total_out == 0.  No usable output capacity: SDB_EOUTPUT.
+ *   Drop mode  (all three output pointers NULL) no capacity limit and no copy-out: count_out[n_agents] (nullable) and
+ *              *total_out are filled, *n_sends_out and *payload_bytes_out read 0.  The at-scale path.
+ *   Flags      SDB_RECV_PEEK (dry run: select and report, retire nothing), SDB_RECV_OWNED, SDB_EXPIRE_ALL; any other bit
+ *              is refused (SDB_EINVAL).
+ *   Ordering   stream-ordered on the handle's stream; synchronises (it returns totals).  It touches rings only, so it
+ *              may sit between sdb_import_prefetch(step) and sdb_import_wire_ptrs_async(step): the prefetch stream reads
+ *              the wire batches and writes its own buffers, never a ring. */
+#define SDB_EXPIRE_ALL 16u              /* every pending record of the listed agents, timestamps not read (purge) */
+int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, double older_than, uint32_t flags,
+               uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+               sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+               uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
 
 /* ---- LLM backend balancer: set_llm_load_balancing / assign_llm_backend / get_llm_backend
  * (M:1281-1325).  The reference stores a flag and a dict and has NO pick algorithm

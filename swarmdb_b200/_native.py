@@ -35,6 +35,7 @@ RECV_PRIORITY = 1
 RECV_PEEK = 2
 RECV_ASYNC = 4
 RECV_OWNED = 8
+EXPIRE_ALL = 16
 TYPEF_JSON = 0x08
 TYPEF_EXTRAS = 0x10
 TYPE_MASK = 0x07
@@ -73,7 +74,7 @@ class SdbStats(C.Structure):
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
-           "sdb_receive_batch", "sdb_receive_compact", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
+           "sdb_receive_batch", "sdb_receive_compact", "sdb_expire", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
@@ -120,6 +121,8 @@ def load_library() -> C.CDLL:
     L.sdb_receive_batch.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, vp]
     L.sdb_receive_compact.restype = i32
     L.sdb_receive_compact.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    L.sdb_expire.restype = i32
+    L.sdb_expire.argtypes = [vp, u32, vp, C.c_double, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_latency_server.restype = i32; L.sdb_latency_server.argtypes = [vp, i32]
     L.sdb_last_receive_dev.restype = i32; L.sdb_last_receive_dev.argtypes = [vp, vp, vp, vp]
     L.sdb_last_receive_totals.restype = i32; L.sdb_last_receive_totals.argtypes = [vp, vp, vp]
@@ -249,7 +252,7 @@ class Shard:
         self._check(self._L.sdb_advance_seq(self._h, next_seq))
 
     PROFILE_KINDS = ["p2p", "fanout", "commit", "recv_count", "recv_scan", "recv_select", "recv_gather",
-                     "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact"]
+                     "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact", "expire"]
 
     def profile(self, enable: bool) -> None:
         self._check(self._L.sdb_profile(self._h, 1 if enable else 0))
@@ -511,6 +514,42 @@ class Shard:
         if agents is None:
             owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
             counts = counts[: self.n_owned if owned else self.stats_n_agents()]
+        return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
+
+    def expire(self, agents, older_than: float, flags: int = 0, archive: bool = True,
+               out_entries: Optional[np.ndarray] = None, out_sends: Optional[np.ndarray] = None,
+               out_payload: Optional[np.ndarray] = None):
+        """Retire pending records older than `older_than` (every pending record with EXPIRE_ALL) without delivering them
+        (include/swarmdb_b200.h: sdb_expire).  archive=True returns the expired records in receive_compact's shape,
+        (counts, entries, sends, payload) - what does not fit stays queued, so loop until no entry comes back;
+        archive=False drops them on the device and returns (counts, total)."""
+        if agents is None:
+            a, n = None, 0
+            counts = np.zeros(self.max_agents, np.uint32)
+        else:
+            a = _arr(agents, np.uint32)
+            n = len(a)
+            counts = np.zeros(n, np.uint32)
+        total, n_sends, pbytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        ent = snd = pay = None
+        if archive:
+            if out_entries is None or out_sends is None:
+                cur = getattr(self, "_out_ent", None)
+                if cur is None or len(cur[0]) < self.max_recv_records:
+                    self._out_ent = (np.zeros(self.max_recv_records, ENTRY_DTYPE), np.zeros(self.max_recv_records, SEND_DTYPE))
+            ent = out_entries if out_entries is not None else self._out_ent[0]
+            snd = out_sends if out_sends is not None else self._out_ent[1]
+            pay = out_payload if out_payload is not None else self._grow_pay()
+        self._check(self._L.sdb_expire(self._h, n, _p(a), float(older_than), flags, _p(counts),
+                                       _p(ent), 0 if ent is None else len(ent), _p(snd), 0 if snd is None else len(snd),
+                                       _p(pay), 0 if pay is None else pay.nbytes,
+                                       C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
+                                       C.cast(C.byref(pbytes), C.c_void_p)))
+        if agents is None:
+            owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
+            counts = counts[: self.n_owned if owned else self.stats_n_agents()]
+        if not archive:
+            return counts, int(total.value)
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
 
     def latency_server(self, enable: bool) -> None:

@@ -38,7 +38,7 @@ import numpy as np
 from pydantic import BaseModel, Field
 
 from . import _native
-from ._native import NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON, SdbError, Shard, pad32
+from ._native import EXPIRE_ALL, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON, SdbError, Shard, pad32
 
 
 class RingOverflow(SdbError):
@@ -129,7 +129,7 @@ class KafkaConfig:
     auto_offset_reset: str = "earliest"
     num_partitions: int = 3
     replication_factor: int = 1
-    retention_ms: int = 604800000
+    retention_ms: int = 604800000          # default cutoff of expire_pending()
     max_poll_interval_ms: int = 300000
     session_timeout_ms: int = 30000
     heartbeat_interval_ms: int = 10000
@@ -367,12 +367,19 @@ class SwarmsDB:
             self.shard.register(idx)
         return idx
 
-    def deregister_agent(self, agent_id: str) -> None:
+    def deregister_agent(self, agent_id: str, purge: bool = False) -> None:
+        """purge=True also drops every message still queued for the agent on the device, so that a departed agent
+        stops pinning the message arena (the ring itself is kept, like the Kafka consumer-group offset)."""
         if agent_id not in self.registered_agents:
             logger.warning(f"Agent {agent_id} not registered")
             return
         self.registered_agents.remove(agent_id)
         self.shard.deregister(self._index(agent_id))
+        if purge:
+            agents, flags = self._expire_scope([agent_id])
+            if len(agents):
+                self._pre_read()
+                self.shard.expire(agents, 0.0, flags | EXPIRE_ALL, archive=False)
 
     # ------------------------------------------------------------------ send
     def send_message(
@@ -920,16 +927,59 @@ class SwarmsDB:
                 inbox.remove(message_id)
         return True
 
-    def flush_old_messages(self, older_than: Optional[float] = None) -> int:
+    def flush_old_messages(self, older_than: Optional[float] = None, include_device: bool = False) -> int:
+        """Archive every message older than the cutoff to archives/archive_{ts}.json and delete it (M:1159-1206).
+        include_device=True also expires the messages still queued on the device (device-only traffic included) and
+        archives them with the rest: a host record wins over its device copy, a broadcast is one entry.  Returns the
+        number of distinct messages archived."""
         cutoff = older_than if older_than is not None else time.time() - 7 * 24 * 3600
         old = [mid for mid, m in self.messages.items() if m.timestamp < cutoff]
-        if old:
+        archived = {mid: self.messages[mid].to_dict() for mid in old}
+        if include_device:
+            for m in self._expire_device_archive(cutoff):
+                if m.id not in archived:
+                    host = self.messages.get(m.id)
+                    archived[m.id] = (host if host is not None else m).to_dict()
+        if archived:
             path = self.save_dir / "archives" / f"archive_{int(time.time())}.json"
             path.parent.mkdir(parents=True, exist_ok=True)
-            path.write_text(json.dumps({mid: self.messages[mid].to_dict() for mid in old}))
-            for mid in old:
+            path.write_text(json.dumps(archived))
+            for mid in archived:
                 self.delete_message(mid)
-        return len(old)
+        return len(archived)
+
+    # ------------------------------------------------------------------ retention (sdb_expire)
+    def _expire_scope(self, agent_ids: Optional[Iterable[str]]):
+        """(agent indices or None = every agent below the watermark, flags) an expiry acts on.  Unknown agents have
+        nothing queued and are left out, as are repeats (the device refuses an agent listed twice)."""
+        if agent_ids is None:
+            return None, 0
+        idx = dict.fromkeys(self._agent_idx[a] for a in agent_ids if a in self._agent_idx)
+        return np.fromiter(idx, dtype=np.uint32, count=len(idx)), 0
+
+    def expire_pending(self, older_than: Optional[float] = None, agent_ids: Optional[Iterable[str]] = None) -> int:
+        """Drop the device-queued messages whose timestamp is older than the cutoff (default: now - retention_ms)
+        without delivering them, and return how many records went.  Messages sent without a timestamp (bulk sends)
+        carry 0.0 and go with any positive cutoff.  Host records are not touched (flush_old_messages archives those)."""
+        self._pre_read()
+        cutoff = older_than if older_than is not None else time.time() - self.config.retention_ms / 1000.0
+        agents, flags = self._expire_scope(agent_ids)
+        if agents is not None and len(agents) == 0:
+            return 0
+        return self.shard.expire(agents, cutoff, flags, archive=False)[1]
+
+    def _expire_device_archive(self, cutoff: float) -> List[Message]:
+        """Expire the device-queued records older than the cutoff in archive mode, call after call until none is left,
+        and decode them (one Message per record: the copies of a broadcast share one id)."""
+        self._pre_read()
+        agents, flags = self._expire_scope(None)
+        out: List[Message] = []
+        while True:
+            _, ent, snd, pay = self.shard.expire(agents, cutoff, flags, archive=True)
+            if len(ent) == 0:
+                return out
+            hdr, p = _native.expand_compact(ent, snd, pay)
+            out.extend(self._decode(hdr, p, "", record=False, status=MessageStatus.DELIVERED))
 
     # ------------------------------------------------------------------ history (schema of M:878-884)
     def _history(self, include_device: bool = False) -> Dict[str, Any]:

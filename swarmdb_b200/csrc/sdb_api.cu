@@ -34,6 +34,8 @@ cudaError_t sdb_launch_pull(const sdb_dev_view*, const sdb_pull_view*, const sdb
                             const sdb_batch_base*, uint32_t);
 cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaStream_t, int*, sdb_profiler*, int, uint32_t,
                                const sdb_compact_args*);
+cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double, uint32_t, const sdb_compact_args*, cudaStream_t,
+                              int*, sdb_profiler*, int);
 cudaError_t sdb_recv_prepare_device();
 cudaError_t sdb_balance_prepare_device();
 cudaError_t sdb_launch_receive_small(const sdb_dev_view*, const uint32_t*, uint32_t, uint32_t, uint32_t, uint32_t, uint4*,
@@ -1869,6 +1871,69 @@ int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
     if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
     if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
     if (entry_out || send_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return SDB_OK;
+}
+
+int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, double older_than, uint32_t flags,
+               uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+               sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+               uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (flags & ~(SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_EXPIRE_ALL))
+    return fail(h, SDB_EINVAL, "sdb_expire accepts SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_EXPIRE_ALL only");
+  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
+  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
+  const bool archive = entry_out || send_out || payload_out;
+  uint64_t rec_cap = 0;
+  if (archive) {
+    // the capacity rule of sdb_receive_compact: rec_cap unshared records of the maximum size fit every buffer
+    const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
+    rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
+    if (entry_out) rec_cap = std::min<uint64_t>(rec_cap, entry_cap);
+    if (send_out) rec_cap = std::min<uint64_t>(rec_cap, send_cap);
+    if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
+    if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  }
+  if (n_agents == 0) return SDB_OK;
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
+  if (archive) { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  if (agent_idx) {
+    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  }
+  sdb_recv_args r{};
+  r.agent_idx = agent_idx ? h->rx_agent : (owned ? h->owned_dev : nullptr); r.n = n_agents;
+  r.flags = flags & SDB_RECV_PEEK;
+  r.cnt = h->rx_cnt; r.rec_local = h->rx_rec_local; r.rec_tops = h->rx_rec_tops;
+  r.plan = h->rx_plan; r.totals = h->rx_totals;
+  r.count_out = (archive || count_out) ? h->rx_count : nullptr;
+  r.rec_cap = rec_cap;
+  int nl = 0;
+  cudaError_t e = sdb_launch_expire(&h->view, &r, older_than, (flags & SDB_EXPIRE_ALL) ? 1u : 0u, archive ? &h->cx : nullptr,
+                                    h->stream, &nl, &h->prof, h->sm_count);
+  h->launches += nl;
+  h->last_rx_valid = false; h->last_rx_compact = false;       // the receive scratch was reused: nothing left to fold
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("expire launch: ") + cudaGetErrorString(e));
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  if (archive)
+    CUDA_TRY(h, cudaMemcpyAsync(h->totals_host + 6, h->cx.totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  if (count_out)
+    CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  const uint64_t total = h->totals_host[0];
+  const uint64_t n_sends = archive ? h->totals_host[6] : 0, pbytes = archive ? h->totals_host[7] * SDB_GRANULE : 0;
+  if (total_out) *total_out = total;
+  if (n_sends_out) *n_sends_out = n_sends;
+  if (payload_bytes_out) *payload_bytes_out = pbytes;
+  if (archive && total) {
+    if (entry_out) CUDA_TRY(h, cudaMemcpyAsync(entry_out, h->cx.entry_out, total * sizeof(sdb_recv_entry), cudaMemcpyDeviceToHost, h->stream));
+    if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
+    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
   return SDB_OK;
 }

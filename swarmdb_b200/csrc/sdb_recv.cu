@@ -1351,6 +1351,136 @@ extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_
 }
 
 // ------------------------------------------------------------------------------------------
+// expiry (sdb_expire): retire the pending records of the listed agents whose header timestamp is < older_than (every
+// pending record with SDB_EXPIRE_ALL) as if they had never been enqueued.  8 lanes per request slot, 4 slots per warp:
+// the 16-byte ring header once, the window's 8-byte entries coalesced, then one header-timestamp load per live entry
+// (arena granule of the handle + 8 bytes: one random 32-byte sector per record, the kernel's whole cost), 4 entries per
+// lane in flight.  Matches are tombstoned, the head moves to the first live entry left and ntomb stays exact (the rule of
+// select_agent_warp); an agent without a match gets no store at all.  Modes:
+//   EXP_DROP    every match; count_out[q] (nullable) and totals[0] += matches (one atomic per warp)
+//   EXP_COUNT   cnt[q] = matches, nothing retired (archive mode, before the scan of cnt)
+//   EXP_SELECT  capacity cut of k_recv_select on the scanned counts, then the first count_out[q] matches are planned in
+//               stream order at their output index {handle, 0, plan z, slot} and retired; the compact back end follows
+// With SDB_EXPIRE_ALL, EXP_DROP and EXP_COUNT read no entries: the count is tail - head - ntomb, the ring is emptied.
+// ------------------------------------------------------------------------------------------
+enum { SDB_EXP_DROP = 0, SDB_EXP_COUNT = 1, SDB_EXP_SELECT = 2 };
+#define SDB_EXP_G 8u     // lanes per request slot
+#define SDB_EXP_U 4u     // entries per lane in flight
+
+template <int MODE>
+__global__ void __launch_bounds__(256)
+k_expire(sdb_dev_view v, sdb_recv_args r, double older_than, uint32_t all) {
+  const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_EXP_G - 1), gsh = lane & ~(SDB_EXP_G - 1);
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1;
+  const bool retire = MODE != SDB_EXP_COUNT && !(r.flags & SDB_RECV_PEEK);
+  constexpr uint32_t SPW = 32u / SDB_EXP_G;                     // request slots per warp
+  unsigned long long wsum = 0;
+  for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
+    const uint32_t q = qb + lane / SDB_EXP_G;
+    const bool valid = q < r.n;
+    uint32_t a = 0, H = 0, T = 0, NT = 0;
+    if (valid) {
+      a = r.agent_idx ? r.agent_idx[q] : q;
+      const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);     // one address for the slot's 8 lanes
+      H = h.x; T = h.y; NT = h.w;
+    }
+    const uint32_t live = T - H - NT;
+    uint32_t limit = 0xFFFFFFFFu, RO = 0;
+    if (MODE == SDB_EXP_SELECT && valid) {
+      uint32_t c = r.cnt[q];
+      RO = r.rec_local[q] + r.rec_tops[q / SDB_SCAN_TILE];
+      if (c && static_cast<uint64_t>(RO) + c > r.rec_cap) {     // does not fit: stays queued ...
+        c = RO == 0 ? static_cast<uint32_t>(r.rec_cap) : 0u;    // ... unless first in the output: its first rec_cap matches
+        if (l8 == 0) atomicMin(r.totals, static_cast<unsigned long long>(RO) + c);
+      }
+      if (l8 == 0) r.count_out[q] = c;
+      limit = c;
+    }
+    // entries are walked unless ALL makes the count alone enough (a selection always needs the handles)
+    const bool walk = valid && live && (MODE == SDB_EXP_SELECT ? limit != 0 : !all);
+    const uint32_t W = walk ? T - H : 0u;
+    const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
+    uint32_t got = walk ? 0u : (valid && MODE != SDB_EXP_SELECT ? live : 0u);
+    uint32_t nh = walk ? T : (got ? T : H);
+    uint2* rs = sdb_ring_of(v, a);
+    for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_EXP_G * SDB_EXP_U) {
+      uint2 e[SDB_EXP_U];
+      double ts[SDB_EXP_U];
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t j = j0 + u * SDB_EXP_G + l8;
+        e[u] = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+      }
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u)               // independent random loads, all issued before any use
+        ts[u] = (!all && sdb_meta(e[u]) != SDB_META_TOMB)
+                    ? __ldg(reinterpret_cast<const double*>(v.arena + ((static_cast<uint64_t>(e[u].x) & v.gmask) << 5) + 8))
+                    : 0.0;
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t j = j0 + u * SDB_EXP_G + l8;
+        const bool lv = sdb_meta(e[u]) != SDB_META_TOMB;
+        const bool match = lv && (all || ts[u] < older_than);           // NaN never compares below: never expires
+        const uint32_t bm = (__ballot_sync(0xFFFFFFFFu, match) >> gsh) & 0xFFu;
+        const uint32_t k = got + __popc(bm & ((1u << l8) - 1u));
+        const bool sel = match && k < limit;
+        if (sel) {
+          if (MODE == SDB_EXP_SELECT) r.plan[RO + k] = make_uint4(e[u].x, 0u, sdb_plan_z(e[u].y), q);
+          if (retire) rs[(H + j) & mask].y = SDB_META_TOMB;
+        }
+        const uint32_t bs = (__ballot_sync(0xFFFFFFFFu, sel) >> gsh) & 0xFFu;
+        const uint32_t bk = (__ballot_sync(0xFFFFFFFFu, lv && !sel) >> gsh) & 0xFFu;
+        got += __popc(bs);
+        if (bk && nh == T) nh = H + j0 + u * SDB_EXP_G + (__ffs(bk) - 1);
+      }
+    }
+    if (l8 == 0 && valid) {
+      if (retire && got) {                                      // the ring header, once
+        v.ring_hdr[a].head = nh;
+        v.ring_hdr[a].ntomb = NT + got - (nh - H);
+      }
+      if (MODE == SDB_EXP_COUNT) r.cnt[q] = got;
+      if (MODE == SDB_EXP_DROP) { if (r.count_out) r.count_out[q] = got; wsum += got; }
+    }
+  }
+  if (MODE == SDB_EXP_DROP) {
+    for (int o = 16; o; o >>= 1) wsum += __shfl_xor_sync(0xFFFFFFFFu, wsum, o);
+    if (lane == 0 && wsum) atomicAdd(r.totals, wsum);
+  }
+}
+
+// drop mode (ca == nullptr): one launch; totals[0] = records expired.  Archive mode: count, scan, select, then the compact
+// back end exactly as a compact receive runs it (totals as there).
+extern "C" cudaError_t sdb_launch_expire(const sdb_dev_view* v, const sdb_recv_args* r, double older_than, uint32_t all,
+                                         const sdb_compact_args* ca, cudaStream_t stream, int* n_launches, sdb_profiler* prof,
+                                         int sm_count) {
+  if (r->n == 0) return cudaSuccess;
+  const uint32_t n = r->n;
+  uint64_t blocks = (static_cast<uint64_t>(n) + 31) / 32;                    // 4 slots per warp, 8 warps per block
+  const uint64_t bcap = static_cast<uint64_t>(sm_count) * 8 * 4;             // grid-stride beyond ~4 waves
+  if (blocks > bcap) blocks = bcap;
+  const int pi = sdb_prof_begin(prof, SDB_PK_EXPIRE, stream);
+  if (!ca) {
+    cudaMemsetAsync(r->totals, 0, sizeof(unsigned long long), stream);
+    k_expire<SDB_EXP_DROP><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, older_than, all);
+    sdb_prof_end(prof, pi, stream);
+    if (n_launches) *n_launches += 1;
+    return cudaGetLastError();
+  }
+  const uint32_t tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
+  k_expire<SDB_EXP_COUNT><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, older_than, all);
+  k_scan_local<<<tiles, 1024, 0, stream>>>(r->cnt, 0xFFFFFFFFu, r->rec_local, r->rec_tops, n);
+  k_scan_tops<<<1, 1024, 0, stream>>>(r->rec_tops, tiles, r->totals);       // totals[0] = matches; the cut may lower it
+  k_expire<SDB_EXP_SELECT><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, older_than, all);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += 4;
+  uint64_t bound = static_cast<uint64_t>(n) * v->ring_slots;               // upper bound on the records planned
+  if (bound > r->rec_cap) bound = r->rec_cap;
+  return launch_compact(v, r, ca, nullptr, bound, sm_count, stream, prof, n_launches);
+}
+
+// ------------------------------------------------------------------------------------------
 // arena floor: smallest arena position still referenced by a pending ring entry.
 // One thread per agent; distance below the current arena tail is maximised with atomicMax.
 // ------------------------------------------------------------------------------------------

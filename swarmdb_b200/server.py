@@ -362,8 +362,10 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
         return {"status": "success", "timestamp": time.time()}
 
     @app.post("/admin/flush")
-    def flush_old(older_than: Optional[float] = None, _: str = Depends(admin)):
-        return {"status": "success", "flushed_count": guarded("flush old messages", lambda: db.flush_old_messages(older_than))}
+    def flush_old(older_than: Optional[float] = None, include_device: bool = False, _: str = Depends(admin)):
+        # include_device: also archive and expire the device-queued messages older than the cutoff
+        return {"status": "success", "flushed_count": guarded("flush old messages",
+                                                              lambda: db.flush_old_messages(older_than, include_device))}
 
     @app.post("/admin/resend_failed")
     def resend_failed(_: str = Depends(admin)):

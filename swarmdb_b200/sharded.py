@@ -13,7 +13,7 @@ from typing import Iterable
 
 import numpy as np
 
-from ._native import SdbError
+from ._native import RECV_OWNED, SdbError
 from .core import GpuConfig, MessagePriority, MessageStatus, MessageType, SwarmsDB
 
 FNV_OFFSET = 0xCBF29CE484222325
@@ -700,9 +700,17 @@ class ShardedSwarmsDB(SwarmsDB):
             return []
         return super().peek_messages(agent_id, max_messages)
 
-    def deregister_agent(self, agent_id: str) -> None:
-        """REPLICATED, like register_agent (the registry must agree on every rank)."""
-        super().deregister_agent(agent_id)
+    def deregister_agent(self, agent_id: str, purge: bool = False) -> None:
+        """REPLICATED, like register_agent (the registry must agree on every rank); purge=True drops the agent's
+        queued messages on the rank that owns it (the other ranks hold none)."""
+        super().deregister_agent(agent_id, purge)
+
+    # ---- retention is LOCAL: each rank expires (and archives) what its own agents hold, no collective
+    def _expire_scope(self, agent_ids):
+        self._push_shard_map()
+        if agent_ids is None:
+            return None, RECV_OWNED
+        return super()._expire_scope([a for a in agent_ids if self.owner(a) == self.rank])
 
     def close(self) -> None:
         """Collective like flush(): every rank closes.  Buffered sends are NOT flushed here (a flush is a collective
