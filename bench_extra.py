@@ -7,6 +7,8 @@
   k1  point-to-point enqueue kernel roofline (1M records x 256 B)
   compact  the c2 step with host buffers out: full receive format against the compact format (sdb_receive_compact)
   expire   retention on the c2 backlog (sdb_expire): drop mode at the median cutoff, SDB_EXPIRE_ALL, archive mode
+  where    filtered receive on the c2 backlog (sdb_receive_where): header-clause and keyword PEEKs, a take of one group's
+           records, and keyword counts over deep queues
 
 bench.py remains the contract benchmark (c2/c3); this file only feeds DESIGN.md.
 """
@@ -419,6 +421,166 @@ def expire(rounds=3, block=4):
                      "records_per_s": n / (ms * 1e-3), "kernel_ms": kern[name], "kernel_ms_total": kms,
                      "algorithmic_bytes": nbytes, "algorithmic_gb_per_s_kernel": nbytes / (kms * 1e-3) / 1e9 if kms else None,
                      "call_ms_blocks": res[name]["call_ms"]}
+    out.update(_gpu_card(0))
+    out["clocks"] = clk
+    return out
+
+
+def where(rounds=3, block=4):
+    """sdb_receive_where on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 pending records): a
+    header-clause PEEK over every agent, an ASCII-folded 8-byte keyword PEEK, and a take-mode filtered receive of one
+    group's records (each take on a fresh backlog, rebuilt untimed); then a deep queue (10,000 agents x 1,000 pending
+    64-byte records) for the keyword kernel's work distribution (DROP | PEEK: counted, nothing copied out), and the
+    latency of a one-agent call.  Outside the timed region the c2 PEEK results are checked against the oracle's PEEK of
+    the whole queue, filtered in numpy."""
+    import torch
+    from bench import ALNUM, ClockSampler, Workload
+    from oracle.cpu_ref import CpuOracle
+    from swarmdb_b200._native import HDR_DTYPE, RECV_PEEK, WHERE_DROP, Shard, make_filter, payload_offsets
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py where: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    stream = torch.cuda.Stream()
+    shard = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+    shard.set_stream(stream.cuda_stream)
+    shard.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        shard.create_group(g, wl.members(g))
+    batch = wl.batch()
+    snd, grp, prio, typ, lens, off, pay = batch
+    g0 = int(grp[0])
+    k0 = int(np.nonzero(grp != g0)[0][0])                 # the keyword's send is not among the records the take consumes
+    kw = pay[int(off[k0]) + 20:int(off[k0]) + 28].tobytes().swapcase()
+
+    def pinned(nbytes):
+        return torch.empty(nbytes, dtype=torch.uint8, pin_memory=True).numpy()
+    pin_hdr, pin_pay = pinned(rec_cap * 32).view(HDR_DTYPE), pinned(rec_cap * wl.L)
+
+    def backlog():
+        while shard.receive_batch(None, 1 << 10, copy_out=False)[1]:
+            pass
+        shard.send_group_batch(*batch)
+        shard.sync()
+
+    f_hdr, f_kw, f_grp = make_filter(prios=[3]), make_filter(keyword=kw, icase=True), make_filter(group=g0)
+    calls = {"header_peek": (False, lambda: shard.receive_where(None, 100, RECV_PEEK, f_hdr, out_hdr=pin_hdr, out_payload=pin_pay)),
+             "keyword_peek": (False, lambda: shard.receive_where(None, 100, RECV_PEEK, f_kw, out_hdr=pin_hdr, out_payload=pin_pay)),
+             "take_group": (True, lambda: shard.receive_where(None, 100, 0, f_grp, out_hdr=pin_hdr, out_payload=pin_pay))}
+
+    def timed(fn, fresh):
+        if fresh:
+            backlog()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        t = time.perf_counter()
+        n = len(fn()[1])                                 # synchronises: it returns totals
+        wall = (time.perf_counter() - t) * 1e3
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return wall, e0.elapsed_time(e1), n
+
+    res = {k: {"call_ms": [], "event_ms": []} for k in calls}
+    got = {}
+    with torch.cuda.stream(stream):
+        backlog()
+        # outside the timed region: the PEEK queries against the oracle's PEEK of the whole queue, filtered in numpy
+        o = CpuOracle(wl.A, wl.G)
+        o.register(np.arange(wl.A))
+        for g in range(wl.G):
+            o.create_group(g, wl.members(g))
+        o.send_group_batch(*batch)
+        cc, hc, pc = o.receive_batch(np.arange(wl.A), 100, RECV_PEEK, rec_cap=per_step, pay_cap=per_step * wl.L)
+        o.close()
+        owner = np.repeat(np.arange(wl.A), cc.astype(np.int64))
+        per_send = np.array([kw.lower() in pay[int(off[i]):int(off[i]) + int(lens[i])].tobytes().lower() for i in range(wl.S)])
+        sel_kw = per_send[(hc["seq"].astype(np.int64) - int(hc["seq"].min())) // wl.F]
+        checks = {}
+        for name, keep in (("header_peek", hc["prio"] == 3), ("keyword_peek", sel_kw), ("take_group", hc["group"] == g0)):
+            c, h, _ = shard.receive_where(None, 100, RECV_PEEK, {"header_peek": f_hdr, "keyword_peek": f_kw, "take_group": f_grp}[name])
+            checks[name] = bool(np.array_equal(c, np.bincount(owner[keep], minlength=wl.A)[: len(c)]) and
+                                h.tobytes() == hc[keep].tobytes())
+        assert all(checks.values()), checks
+        del hc, pc
+        for fresh, fn in calls.values():                  # warm-up: every shape once
+            timed(fn, fresh)
+        backlog()
+        clocks = ClockSampler(0); clocks.start()
+        for _ in range(rounds):
+            for name, (fresh, fn) in calls.items():
+                for _ in range(block):
+                    wall, ev, n = timed(fn, fresh)
+                    res[name]["call_ms"].append(wall); res[name]["event_ms"].append(ev)
+                    got[name] = n
+        clk = clocks.stop()
+        kern = {}
+        for name, (fresh, fn) in calls.items():
+            backlog()
+            shard.profile(True)
+            fn()
+            prof = shard.profile_read()
+            shard.profile(False)
+            kern[name] = {k: v[0] for k, v in prof.items() if v[1]}
+        # one agent, header clause, PEEK: the small-call latency (several launches even for one agent)
+        one = np.array([int(wl.members(g0)[0])], np.uint32)
+        for _ in range(20):
+            shard.receive_where(one, 100, RECV_PEEK, f_grp)
+        t = time.perf_counter()
+        for _ in range(500):
+            shard.receive_where(one, 100, RECV_PEEK, f_grp)
+        one_us = (time.perf_counter() - t) / 500 * 1e6
+    shard.close()
+    # deep queues: 10,000 agents x 1,000 pending 64-byte records, keyword DROP | PEEK
+    A2, D, L2 = 10_000, 1_000, 64
+    deep = Shard(max_agents=A2, ring_slots=1024, arena_bytes=1 << 31, max_payload_bytes=L2, max_batch_sends=1 << 20,
+                 max_batch_payload=(1 << 20) * L2)
+    deep.register(np.arange(A2, dtype=np.uint32))
+    rng = np.random.default_rng(5)
+    n_all = A2 * D
+    for b0 in range(0, n_all, 1 << 20):
+        n = min(1 << 20, n_all - b0)
+        r = (np.arange(b0, b0 + n) % A2).astype(np.uint32)
+        dpay = ALNUM[rng.integers(0, 62, n * L2)]
+        deep.send_batch(r, r, None, None, np.full(n, L2, np.uint16), np.arange(n, dtype=np.uint64) * L2, dpay)
+    assert deep.queue_stats()["pending"] == n_all and deep.stats()["ring_overflow"] == 0
+    dkw = dpay[:8].tobytes().swapcase()
+    f_deep = make_filter(keyword=dkw, icase=True)
+    deep_ms = []
+    deep.receive_where(None, D, RECV_PEEK, f_deep, drop=True)
+    for _ in range(rounds * block):
+        t = time.perf_counter()
+        _, deep_hits = deep.receive_where(None, D, RECV_PEEK, f_deep, drop=True)
+        deep_ms.append((time.perf_counter() - t) * 1e3)
+    deep.profile(True)
+    deep.receive_where(None, D, RECV_PEEK, f_deep, drop=True)
+    deep_kern = {k: v[0] for k, v in deep.profile_read().items() if v[1]}
+    deep.close()
+
+    peak = 3.35e12                                        # H100 SXM data sheet, HBM3
+    out = {"config": f"c2 backlog: {wl.A} agents, {wl.S} group sends x {wl.F} members = {per_step} pending records, "
+                     f"{wl.L}-B payloads; {rounds} rounds of {block} calls per query, takes on a fresh backlog; pinned "
+                     f"host outputs", "oracle_checks": checks,
+           "verdict_bitmap_bytes_c2": wl.A * ((64 + 31) // 32) * 4, "one_agent_peek_us": one_us}
+    for name in calls:
+        ms = float(np.median(res[name]["call_ms"]))
+        kms = kern[name].get("where", 0.0)
+        # algorithmic bytes of the selection kernels: 16-B ring header per agent and, per pending record, its 8-B entry
+        # and 32-B header sector (the keyword pass also reads the 256-B payload of every record it searches)
+        nbytes = 16 * wl.A + per_step * (40 + (wl.L if name == "keyword_peek" else 0))
+        out[name] = {"records": got[name], "ms_per_call": ms, "event_ms_per_call": float(np.median(res[name]["event_ms"])),
+                     "records_per_s_scanned": per_step / (ms * 1e-3), "kernel_ms": kern[name], "where_kernel_ms": kms,
+                     "algorithmic_bytes": nbytes, "where_gb_per_s": nbytes / (kms * 1e-3) / 1e9 if kms else None,
+                     "frac_of_3.35TB_s": nbytes / (kms * 1e-3) / peak if kms else None, "call_ms_blocks": res[name]["call_ms"]}
+    dk = deep_kern.get("where", 0.0)
+    dbytes = 16 * A2 + n_all * (40 + L2)
+    out["deep_keyword_count"] = {"agents": A2, "pending_per_agent": D, "hits": deep_hits, "ms_per_call": float(np.median(deep_ms)),
+                                 "records_per_s_scanned": n_all / (float(np.median(deep_ms)) * 1e-3), "where_kernel_ms": dk,
+                                 "algorithmic_bytes": dbytes, "where_gb_per_s": dbytes / (dk * 1e-3) / 1e9 if dk else None,
+                                 "frac_of_3.35TB_s": dbytes / (dk * 1e-3) / peak if dk else None}
     out.update(_gpu_card(0))
     out["clocks"] = clk
     return out

@@ -130,7 +130,7 @@ int sdb_advance_seq(sdb_handle h, uint64_t next_seq);
  * roofline: enable, run, then read accumulated milliseconds and launch counts per kernel class. */
 enum { SDB_PK_P2P = 0, SDB_PK_FANOUT, SDB_PK_COMMIT, SDB_PK_RECV_COUNT, SDB_PK_RECV_SCAN, SDB_PK_RECV_SELECT,
        SDB_PK_RECV_GATHER, SDB_PK_ARENA_FLOOR, SDB_PK_PICK, SDB_PK_XSHARD, SDB_PK_INDEX, SDB_PK_XWAIT,
-       SDB_PK_RECV_COMPACT = 12, SDB_PK_EXPIRE = 13, SDB_PK_N = 16 };
+       SDB_PK_RECV_COMPACT = 12, SDB_PK_EXPIRE = 13, SDB_PK_WHERE = 14, SDB_PK_N = 16 };
 int sdb_profile(sdb_handle h, int enable);
 int sdb_profile_read(sdb_handle h, double* ms_out /* [SDB_PK_N] */, uint64_t* count_out /* [SDB_PK_N] */);
 
@@ -462,6 +462,65 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
                uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
                sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
+
+/* ---- filtered receive: query_messages / search_messages / get_conversation / delete_message (M:671-808, M:1132-1157)
+ * on the device queue itself, and selective receives ("my COMMAND messages", "what the coordinator sent me").
+ * sdb_receive_where takes, for each listed agent (agent_idx == NULL: as in sdb_receive_batch), the first max_messages
+ * pending records that match `filter`, in the call's delivery order (stream, or SDB_RECV_PRIORITY), and leaves every
+ * other record queued in its order.
+ *   Filter     the SDB_FILTER_* clauses named in `fields` are ANDed; fields == 0 matches every pending record.
+ *   Keyword    matched against a record's content bytes: payload [0, len), or with SDB_TYPEF_EXTRAS the slice
+ *              [4, 4 + clen), clen = the little-endian u32 at the payload's start clamped to len - 4 (empty when
+ *              len < 4).  A keyword in the JSON extras, or across content and extras, does not match.  For JSON content
+ *              the bytes are json.dumps(content).  SDB_FILTER_ICASE folds ASCII A-Z/a-z only; every other byte is
+ *              compared exactly.  keyword_len == 0 matches every record.  Cost: up to len x keyword_len byte compares
+ *              per record that passes the header clauses (a first-byte test skips most start positions).
+ *   Contract   1. The result equals, byte for byte, what sdb_receive_batch returns on a queue holding only the matching
+ *                 records, in its full format (count_out, 32-byte headers, payloads padded to SDB_GRANULE).
+ *              2. Without SDB_RECV_PEEK the returned records are retired: every later receive (any path, any order)
+ *                 delivers what it would have delivered had they been received.
+ *              3. stats.delivered grows by the records returned; in sdb_agent_loads `pending` falls, `received` stays.
+ *              4. Capacity: sdb_receive_batch's rule (lead-agent exception included) applies to the matches; loop
+ *                 until *total_out == 0 to drain.
+ *              5. Flags: SDB_RECV_PRIORITY, SDB_RECV_PEEK (a query: nothing retired), SDB_RECV_OWNED, SDB_WHERE_DROP.
+ *              6. SDB_WHERE_DROP retires the matches without returning them: every output pointer but count_out must be
+ *                 NULL, there is no capacity limit (max_messages still applies), stats do not move (as in sdb_expire's
+ *                 drop mode) and *payload_bytes_out reads 0.  DROP | PEEK is a dry-run count.
+ *              7. SDB_EINVAL: a NULL filter or a wrong struct_bytes, unknown bits in fields or flags, SDB_RECV_ASYNC, a
+ *                 NULL keyword with keyword_len > 0, keyword_len > SDB_FILTER_MAX_KEYWORD, drop mode with output
+ *                 buffers, an agent listed twice or out of range.  SDB_EOUTPUT as in sdb_receive_batch.
+ *              8. The call always runs the bulk kernels (never the few-agent or latency-server paths); sdb_digest_fold
+ *                 after it returns SDB_EINVAL until the next sdb_receive_batch.
+ *   Memory     one verdict bit per ring slot (max_agents x ring_slots bits) and a 256-byte keyword buffer, allocated on
+ *              the first call. */
+#define SDB_FILTER_SENDER   1u          /* header.sender == sender */
+#define SDB_FILTER_RECEIVER 2u          /* header.receiver == receiver (SDB_NO_RECEIVER: broadcast copies) */
+#define SDB_FILTER_GROUP    4u          /* header.group == group (SDB_NO_GROUP: non-group sends) */
+#define SDB_FILTER_TYPE     8u          /* bit (header.type & SDB_TYPE_MASK) of type_mask set */
+#define SDB_FILTER_PRIO     16u         /* bit header.prio of prio_mask set */
+#define SDB_FILTER_TIME     32u         /* after < timestamp < before, both strict: a NaN never matches */
+#define SDB_FILTER_SEQ      64u         /* seq_lo <= seq < seq_hi */
+#define SDB_FILTER_KEYWORD  128u        /* keyword occurs in the content bytes */
+#define SDB_FILTER_ICASE    256u        /* keyword compare folds ASCII A-Z/a-z only; every other byte is compared exactly */
+#define SDB_FILTER_MAX_KEYWORD 256u
+#define SDB_WHERE_DROP 32u              /* flag: retire the matches without returning them */
+typedef struct sdb_filter {
+  uint32_t struct_bytes;    /* sizeof(sdb_filter) */
+  uint32_t fields;          /* SDB_FILTER_* clauses that apply (ANDed); 0 matches every pending record */
+  uint32_t sender;          /* SDB_FILTER_SENDER */
+  uint32_t receiver;        /* SDB_FILTER_RECEIVER */
+  uint32_t group;           /* SDB_FILTER_GROUP */
+  uint8_t  type_mask;       /* SDB_FILTER_TYPE */
+  uint8_t  prio_mask;       /* SDB_FILTER_PRIO */
+  uint16_t keyword_len;     /* SDB_FILTER_KEYWORD: 0 .. SDB_FILTER_MAX_KEYWORD */
+  double   after, before;   /* SDB_FILTER_TIME */
+  uint64_t seq_lo, seq_hi;  /* SDB_FILTER_SEQ */
+  const uint8_t* keyword;   /* host pointer */
+} sdb_filter;
+int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                      const sdb_filter* filter,
+                      uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
+                      uint8_t* payload_out, uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out);
 
 /* ---- LLM backend balancer: set_llm_load_balancing / assign_llm_backend / get_llm_backend
  * (M:1281-1325).  The reference stores a flag and a dict and has NO pick algorithm

@@ -36,6 +36,10 @@ RECV_PEEK = 2
 RECV_ASYNC = 4
 RECV_OWNED = 8
 EXPIRE_ALL = 16
+WHERE_DROP = 32
+FILTER_SENDER, FILTER_RECEIVER, FILTER_GROUP, FILTER_TYPE = 1, 2, 4, 8
+FILTER_PRIO, FILTER_TIME, FILTER_SEQ, FILTER_KEYWORD, FILTER_ICASE = 16, 32, 64, 128, 256
+FILTER_MAX_KEYWORD = 256
 TYPEF_JSON = 0x08
 TYPEF_EXTRAS = 0x10
 TYPE_MASK = 0x07
@@ -65,6 +69,52 @@ class SdbConfig(C.Structure):
                 ("list_pool_entries", C.c_uint64), ("fanout_variant", C.c_uint32), ("flags", C.c_uint32)]
 
 
+class SdbFilter(C.Structure):
+    """sdb_filter (include/swarmdb_b200.h): the clauses named in `fields` are ANDed; make_filter() builds one."""
+    _fields_ = [("struct_bytes", C.c_uint32), ("fields", C.c_uint32), ("sender", C.c_uint32), ("receiver", C.c_uint32),
+                ("group", C.c_uint32), ("type_mask", C.c_uint8), ("prio_mask", C.c_uint8), ("keyword_len", C.c_uint16),
+                ("after", C.c_double), ("before", C.c_double), ("seq_lo", C.c_uint64), ("seq_hi", C.c_uint64),
+                ("keyword", C.c_void_p)]
+
+
+def make_filter(sender=None, receiver=None, group=None, types=None, prios=None, after=None, before=None, seq=None,
+                keyword=None, icase=False) -> SdbFilter:
+    """A filter for Shard.receive_where.  Each argument that is not None adds its clause: sender / receiver / group are
+    indices (NO_RECEIVER selects broadcast copies, NO_GROUP non-group sends); types / prios are iterables of type codes
+    (0..7) and priorities (0..3); after / before bound the timestamp strictly (either may be None: unbounded); seq is a
+    half-open range (lo, hi); keyword (bytes or str, UTF-8) must occur in the content bytes, ASCII case folded with
+    icase.  The keyword bytes are kept alive by the returned object."""
+    f = SdbFilter()
+    f.struct_bytes = C.sizeof(SdbFilter)
+    fields = 0
+    if sender is not None:
+        fields |= FILTER_SENDER; f.sender = int(sender)
+    if receiver is not None:
+        fields |= FILTER_RECEIVER; f.receiver = int(receiver)
+    if group is not None:
+        fields |= FILTER_GROUP; f.group = int(group)
+    if types is not None:
+        fields |= FILTER_TYPE; f.type_mask = sum(1 << (int(t) & TYPE_MASK) for t in set(types))
+    if prios is not None:
+        fields |= FILTER_PRIO; f.prio_mask = sum(1 << int(p) for p in set(prios))
+    if after is not None or before is not None:
+        fields |= FILTER_TIME
+        f.after = float("-inf") if after is None else float(after)
+        f.before = float("inf") if before is None else float(before)
+    if seq is not None:
+        fields |= FILTER_SEQ; f.seq_lo, f.seq_hi = int(seq[0]), int(seq[1])
+    if keyword is not None:
+        kw = keyword.encode("utf-8") if isinstance(keyword, str) else bytes(keyword)
+        fields |= FILTER_KEYWORD
+        f._kw = C.create_string_buffer(kw, max(len(kw), 1))
+        f.keyword = C.cast(f._kw, C.c_void_p)
+        f.keyword_len = len(kw) if len(kw) <= 0xFFFF else 0xFFFF
+    if icase:
+        fields |= FILTER_ICASE
+    f.fields = fields
+    return f
+
+
 class SdbStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("next_seq", "enqueued", "delivered", "ring_overflow", "skipped_sender",
                                           "arena_tail_bytes", "arena_floor_bytes", "n_agents", "kernel_launches",
@@ -74,7 +124,7 @@ class SdbStats(C.Structure):
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
-           "sdb_receive_batch", "sdb_receive_compact", "sdb_expire", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
+           "sdb_receive_batch", "sdb_receive_compact", "sdb_expire", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
@@ -123,6 +173,8 @@ def load_library() -> C.CDLL:
     L.sdb_receive_compact.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_expire.restype = i32
     L.sdb_expire.argtypes = [vp, u32, vp, C.c_double, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    L.sdb_receive_where.restype = i32
+    L.sdb_receive_where.argtypes = [vp, u32, vp, u32, u32, C.POINTER(SdbFilter), vp, vp, u64, vp, u64, vp, vp]
     L.sdb_latency_server.restype = i32; L.sdb_latency_server.argtypes = [vp, i32]
     L.sdb_last_receive_dev.restype = i32; L.sdb_last_receive_dev.argtypes = [vp, vp, vp, vp]
     L.sdb_last_receive_totals.restype = i32; L.sdb_last_receive_totals.argtypes = [vp, vp, vp]
@@ -252,7 +304,7 @@ class Shard:
         self._check(self._L.sdb_advance_seq(self._h, next_seq))
 
     PROFILE_KINDS = ["p2p", "fanout", "commit", "recv_count", "recv_scan", "recv_select", "recv_gather",
-                     "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact", "expire"]
+                     "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact", "expire", "where"]
 
     def profile(self, enable: bool) -> None:
         self._check(self._L.sdb_profile(self._h, 1 if enable else 0))
@@ -551,6 +603,38 @@ class Shard:
         if not archive:
             return counts, int(total.value)
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
+
+    def receive_where(self, agents, max_messages: int, flags: int = 0, filt: Optional[SdbFilter] = None,
+                      drop: bool = False, out_hdr: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+        """Take (or with RECV_PEEK, only look at) the first max_messages pending records per agent that match `filt`
+        (make_filter(); None matches every record), in delivery order (include/swarmdb_b200.h: sdb_receive_where).
+        Returns receive_batch's (counts, headers, payload); what does not fit stays queued, so loop until nothing
+        comes back.  drop=True retires the matches on the device without returning them: (counts, total)."""
+        if filt is None:
+            filt = make_filter()
+        if agents is None:
+            a, n = None, 0
+            counts = np.zeros(self.max_agents, np.uint32)
+        else:
+            a = _arr(agents, np.uint32)
+            n = len(a)
+            counts = np.zeros(n, np.uint32)
+        total, pbytes = C.c_uint64(0), C.c_uint64(0)
+        hdr = pay = None
+        if drop:
+            flags |= WHERE_DROP
+        else:
+            hdr = out_hdr if out_hdr is not None else self._grow_hdr()
+            pay = out_payload if out_payload is not None else self._grow_pay()
+        self._check(self._L.sdb_receive_where(self._h, n, _p(a), max_messages, flags, C.byref(filt), _p(counts), _p(hdr),
+                                              0 if hdr is None else len(hdr), _p(pay), 0 if pay is None else pay.nbytes,
+                                              C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(pbytes), C.c_void_p)))
+        if agents is None:
+            owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
+            counts = counts[: self.n_owned if owned else self.stats_n_agents()]
+        if drop:
+            return counts, int(total.value)
+        return counts, hdr[: total.value], pay[: pbytes.value]
 
     def latency_server(self, enable: bool) -> None:
         """Start / stop the persistent low-latency dequeue server (single-agent receives then skip launch, sync and D2H)."""

@@ -38,7 +38,8 @@ import numpy as np
 from pydantic import BaseModel, Field
 
 from . import _native
-from ._native import EXPIRE_ALL, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON, SdbError, Shard, pad32
+from ._native import (EXPIRE_ALL, FILTER_MAX_KEYWORD, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON,
+                      SdbError, Shard, make_filter, pad32)
 
 
 class RingOverflow(SdbError):
@@ -614,11 +615,17 @@ class SwarmsDB:
         """Pop up to `max_messages` pending messages for `agent_id` in stream order (or priority
         order with GpuConfig.priority_dequeue).  Never blocks: `timeout` is accepted for
         compatibility (the reference spins up to `timeout` when fewer are available, M:553-556)."""
+        self._prepare_receive(agent_id)
+        return self._receive_local(agent_id, max_messages)
+
+    def _prepare_receive(self, agent_id: str) -> bool:
+        """Before a receive for `agent_id`: register it if needed and push buffered sends (a sharded front-end checks
+        ownership instead).  False when the agent can have nothing queued."""
         if agent_id not in self.registered_agents:
             logger.warning(f"Agent {agent_id} not registered, registering now")
             self.register_agent(agent_id)
         self.flush()
-        return self._receive_local(agent_id, max_messages)
+        return True
 
     def _receive_local(self, agent_id: str, max_messages: int) -> List[Message]:
         if max_messages <= 0:
@@ -649,6 +656,95 @@ class SwarmsDB:
         hdr, pay, _ = self.shard.receive_one(self._index(agent_id), max_messages, flags)
         return self._decode(hdr, pay, agent_id, record=False, status=MessageStatus.DELIVERED)
 
+    def _where_filter(self, sender_id=None, receiver_idx=None, message_type=None, min_priority=None, group_name=None,
+                      after_timestamp=None, before_timestamp=None, keyword=None, case_sensitive=True):
+        """The device filter (make_filter) for these host-level clauses, or None when an unknown sender or group makes
+        it match nothing."""
+        kw = {}
+        if sender_id is not None:
+            if sender_id not in self._agent_idx:
+                return None
+            kw["sender"] = self._agent_idx[sender_id]
+        if receiver_idx is not None:
+            kw["receiver"] = receiver_idx
+        if message_type is not None:
+            kw["types"] = [_TYPE_CODE[MessageType(message_type)]]
+        if min_priority is not None:
+            kw["prios"] = range(int(MessagePriority(min_priority)), 4)
+        if group_name is not None:
+            if group_name not in self._group_idx:
+                return None
+            kw["group"] = self._group_idx[group_name]
+        if after_timestamp is not None or before_timestamp is not None:
+            kw["after"], kw["before"] = after_timestamp, before_timestamp
+        if keyword is not None:
+            kw["keyword"], kw["icase"] = keyword, not case_sensitive
+        return make_filter(**kw)
+
+    def receive_matching(self, agent_id: str, max_messages: int = 100, *, sender_id: Optional[str] = None,
+                         message_type: Optional[MessageType] = None, min_priority: Optional[MessagePriority] = None,
+                         group_name: Optional[str] = None, after_timestamp: Optional[float] = None,
+                         before_timestamp: Optional[float] = None, keyword: Optional[str] = None,
+                         case_sensitive: bool = False) -> List[Message]:
+        """A selective receive_messages: pop up to `max_messages` of the agent's pending messages that match every
+        given clause, in stream order (priority order with GpuConfig.priority_dequeue), with receive_messages'
+        bookkeeping; the other messages stay queued in their order.  The timestamp bounds are strict.  `keyword` must
+        occur in the message content (its UTF-8 text; JSON content as json.dumps gives it), at most 256 bytes; the
+        case-insensitive compare folds ASCII letters only."""
+        if keyword is not None and len(keyword.encode("utf-8")) > FILTER_MAX_KEYWORD:
+            raise ValueError(f"keyword longer than {FILTER_MAX_KEYWORD} bytes")     # taken records cannot be re-checked
+        if not self._prepare_receive(agent_id):
+            return []
+        filt = self._where_filter(sender_id, None, message_type, min_priority, group_name, after_timestamp,
+                                  before_timestamp, keyword, case_sensitive)
+        if max_messages <= 0 or filt is None:
+            return []
+        flags = RECV_PRIORITY if self.gpu_config.priority_dequeue else 0
+        out: List[Message] = []
+        a = np.array([self._index(agent_id)], np.uint32)
+        while len(out) < max_messages:
+            _, hdr, pay = self.shard.receive_where(a, max_messages - len(out), flags, filt)
+            if len(hdr) == 0:
+                break
+            out.extend(self._decode(hdr, pay, agent_id))
+        return out
+
+    def _device_agents(self) -> np.ndarray:
+        """Indices of the agents whose device queues this instance reads (a sharded rank: the ones it owns)."""
+        agents, _ = self._expire_scope(self._agent_name)
+        return agents
+
+    def _device_matches(self, filt, need: int, accept: Callable[[Message], bool],
+                        agents: Optional[np.ndarray] = None) -> List[Message]:
+        """The newest (highest sequence number) `need` device-pending messages that match `filt` (PEEK receives: nothing
+        is consumed), pass `accept` and have no host record (a host record wins over its device copy), one per id (the
+        copies of a broadcast share one).  Each call's records are decoded newest first and only until `need` of them
+        are taken: a message among the overall newest `need` is also among the newest `need` taken from its own call,
+        so the Python work is bounded by `need` and the rejected candidates, not by the number of matches."""
+        self._pre_read()
+        if filt is None or need <= 0:
+            return []
+        found: Dict[int, Message] = {}
+        seen = set()
+        for part, cap in self._pending_chunks(self._device_agents() if agents is None else agents, 1 << 31):
+            _, hdr, pay = self.shard.receive_where(part, cap, RECV_PEEK, filt)
+            offs = _native.payload_offsets(hdr)
+            seqs = hdr["seq"]
+            taken = 0
+            for i in np.argsort(seqs, kind="stable")[::-1].tolist():
+                seq = int(seqs[i])
+                if seq in seen:
+                    continue
+                seen.add(seq)
+                m = self._decode(hdr[i:i + 1], pay[int(offs[i]):], "", record=False, status=MessageStatus.DELIVERED)[0]
+                if m.id in self.messages or not accept(m):
+                    continue
+                found[seq] = m
+                taken += 1
+                if taken >= need:
+                    break
+        return [found[k] for k in sorted(found, reverse=True)[:need]]
+
     def pending_snapshot(self, per_agent: int = 1024) -> Dict[str, List[Message]]:
         """Every message still queued on the device, per agent, in delivery order (non-destructive).
         This is the D2H ring dump behind `save_message_history(include_device=True)`."""
@@ -657,24 +753,8 @@ class SwarmsDB:
         out: Dict[str, List[Message]] = {}
         if n == 0:
             return out
-        g = self.gpu_config
-        flags = RECV_PEEK | (RECV_PRIORITY if g.priority_dequeue else 0)
-        # A receive call holds min(max_recv_records, max_recv_payload / padded payload) records and leaves out whole
-        # agents beyond that; a PEEK consumes nothing, so a fixed chunking would silently skip them.  Chunks are packed
-        # from the agents' pending counts instead (one device query), so that every chunk fits.
-        max_recv_payload = g.max_recv_payload or g.max_recv_records * 256
-        cap = max(1, min(g.max_recv_records, max_recv_payload // pad32(g.max_payload_bytes)))
-        pending = np.minimum(self.shard.agent_loads(None, n)["pending"][:n].astype(np.int64), per_agent)
-        busy = np.nonzero(pending)[0]
-        b = 0
-        while b < len(busy):
-            e, room = b, cap
-            while e < len(busy) and (pending[busy[e]] <= room or e == b):
-                room -= int(pending[busy[e]]); e += 1
-            part = busy[b:e].astype(np.uint32)
-            if e == b + 1 and pending[busy[b]] > cap:
-                logger.warning(f"pending_snapshot: agent {self._agent_name[int(busy[b])]} has more pending messages than one "
-                               f"receive call holds ({cap}); the snapshot keeps the first {cap}")
+        flags = RECV_PEEK | (RECV_PRIORITY if self.gpu_config.priority_dequeue else 0)
+        for part, cap in self._pending_chunks(np.arange(n, dtype=np.uint32), per_agent):
             counts, hdr, pay = self.shard.receive_batch(part, min(per_agent, cap), flags)
             offs = _native.payload_offsets(hdr)
             pos = 0
@@ -685,8 +765,30 @@ class SwarmsDB:
                     sub_pay = pay[int(offs[pos]):] if pos < len(offs) else pay[:0]
                     out[name] = self._decode(hdr[pos:pos + c], sub_pay, name, record=False, status=MessageStatus.DELIVERED)
                 pos += c
-            b = e
         return out
+
+    def _pending_chunks(self, agents: np.ndarray, per_agent: int):
+        """Yield (agent list, record capacity): consecutive parts of `agents` whose pending messages (at most per_agent
+        each) fit one receive call.  A call holds min(max_recv_records, max_recv_payload / padded payload) records and
+        leaves out whole agents beyond that; a PEEK consumes nothing, so a fixed chunking would silently skip them.  The
+        parts are packed from the agents' pending counts instead (one device query)."""
+        g = self.gpu_config
+        max_recv_payload = g.max_recv_payload or g.max_recv_records * 256
+        cap = max(1, min(g.max_recv_records, max_recv_payload // pad32(g.max_payload_bytes)))
+        if len(agents) == 0:
+            return
+        pending = np.minimum(self.shard.agent_loads(agents)["pending"][: len(agents)].astype(np.int64), per_agent)
+        busy = np.nonzero(pending)[0]
+        b = 0
+        while b < len(busy):
+            e, room = b, cap
+            while e < len(busy) and (pending[busy[e]] <= room or e == b):
+                room -= int(pending[busy[e]]); e += 1
+            if e == b + 1 and pending[busy[b]] > cap:
+                logger.warning(f"agent {self._agent_name[int(agents[busy[b]])]} has more pending messages than one receive "
+                               f"call holds ({cap}); only the first {cap} are read")
+            yield agents[busy[b:e]].astype(np.uint32), cap
+            b = e
 
     def _decode(self, hdr: np.ndarray, pay: np.ndarray, agent_id: str, record: bool = True,
                 status: MessageStatus = MessageStatus.READ) -> List[Message]:
@@ -831,7 +933,11 @@ class SwarmsDB:
     def query_messages(self, sender_id: Optional[str] = None, receiver_id: Optional[str] = None,
                        message_type: Optional[MessageType] = None, status: Optional[MessageStatus] = None,
                        after_timestamp: Optional[float] = None, before_timestamp: Optional[float] = None,
-                       limit: int = 100) -> List[Message]:
+                       limit: int = 100, include_device: bool = False) -> List[Message]:
+        """Host records that match, newest first (M:671-700).  include_device=True adds the matching messages still
+        queued on the device that have no host record (bulk sends, other ranks' traffic, messages sent before a
+        load_message_history), newest first, after the host hits; they read as DELIVERED, so a `status` other than
+        DELIVERED adds none.  receiver_id reads that agent's queue and, as the host rule does, leaves broadcasts out."""
         def keep(m: Message) -> bool:
             return ((sender_id is None or m.sender_id == sender_id)
                     and (receiver_id is None or m.receiver_id == receiver_id)
@@ -845,23 +951,47 @@ class SwarmsDB:
                 break
             if keep(m):
                 hits.append(m)
+        if include_device and len(hits) < limit and status in (None, MessageStatus.DELIVERED):
+            agents = None
+            if receiver_id is not None:
+                owned = self._expire_scope([receiver_id])[0] if receiver_id in self._agent_idx else []
+                if len(owned) == 0:
+                    return hits
+                agents = owned
+            filt = self._where_filter(sender_id, None if agents is None else int(agents[0]), message_type, None, None,
+                                      after_timestamp, before_timestamp)
+            hits += self._device_matches(filt, limit - len(hits), keep, agents)
         return hits
 
-    def search_messages(self, keyword: str, case_sensitive: bool = False, limit: int = 100) -> List[Message]:
+    def search_messages(self, keyword: str, case_sensitive: bool = False, limit: int = 100,
+                        include_device: bool = False) -> List[Message]:
+        """Host records whose content contains `keyword`, newest first (M:702-740).  include_device=True adds the
+        matching device-queued messages without a host record, newest first, after the host hits.  On the device the
+        content bytes are searched for the keyword's first 256 UTF-8 bytes with ASCII-only case folding, then every
+        candidate is checked with the host rule; a message that matches only under Unicode case folding beyond ASCII
+        (e.g. the Kelvin sign against "k") is not found on the device."""
         needle = keyword if case_sensitive else keyword.lower()
+
+        def keep(m: Message) -> bool:
+            text = json.dumps(m.content) if isinstance(m.content, (dict, list)) else str(m.content)
+            return needle in (text if case_sensitive else text.lower())
         hits: List[Message] = []
         for m in reversed(list(self.messages.values())):
             if len(hits) >= limit:
                 break
-            text = json.dumps(m.content) if isinstance(m.content, (dict, list)) else str(m.content)
-            if needle in (text if case_sensitive else text.lower()):
+            if keep(m):
                 hits.append(m)
+        if include_device and len(hits) < limit:
+            kw = keyword.encode("utf-8")[:FILTER_MAX_KEYWORD]
+            filt = make_filter(keyword=kw, icase=not case_sensitive)
+            hits += self._device_matches(filt, limit - len(hits), keep)
         return hits
 
-    def get_conversation(self, agent_id_1: str, agent_id_2: str, limit: int = 100) -> List[Message]:
+    def get_conversation(self, agent_id_1: str, agent_id_2: str, limit: int = 100,
+                         include_device: bool = False) -> List[Message]:
         half = limit // 2
-        return (self.query_messages(sender_id=agent_id_1, receiver_id=agent_id_2, limit=half)
-                + self.query_messages(sender_id=agent_id_2, receiver_id=agent_id_1, limit=half))
+        return (self.query_messages(sender_id=agent_id_1, receiver_id=agent_id_2, limit=half, include_device=include_device)
+                + self.query_messages(sender_id=agent_id_2, receiver_id=agent_id_1, limit=half, include_device=include_device))
 
     def get_unread_message_count(self, agent_id: str) -> int:
         return sum(1 for mid in self.agent_inbox.get(agent_id, [])
@@ -919,13 +1049,32 @@ class SwarmsDB:
             resent.append(new_id)
         return resent
 
-    def delete_message(self, message_id: str) -> bool:
-        if self.messages.pop(message_id, None) is None:
-            return False
-        for inbox in self.agent_inbox.values():
-            if message_id in inbox:
-                inbox.remove(message_id)
-        return True
+    def delete_message(self, message_id: str, include_device: bool = False) -> bool:
+        """Delete the host record (M:1132-1157).  include_device=True also drops every device-queued copy of the
+        message (all copies of a broadcast), so it is never delivered; only ids this instance issued are looked up
+        there.  True when anything was deleted."""
+        found = self.messages.pop(message_id, None) is not None
+        if found:
+            for inbox in self.agent_inbox.values():
+                if message_id in inbox:
+                    inbox.remove(message_id)
+        if include_device:
+            seq = self._seq_of_id(message_id)
+            if seq is not None:
+                self._pre_read()
+                agents, flags = self._expire_scope(None)
+                _, n = self.shard.receive_where(agents, 1, flags, make_filter(seq=(seq, seq + 1)), drop=True)
+                found = found or n > 0
+        return found
+
+    def _seq_of_id(self, message_id: str) -> Optional[int]:
+        """The sequence number behind an id this instance issued (_make_id), else None."""
+        try:
+            v = int(message_id.replace("-", ""), 16)
+        except ValueError:
+            return None
+        seq = v & ((1 << 64) - 1)
+        return seq if (v ^ seq) == self._id_hi and 0 < seq and self._make_id(seq) == message_id else None
 
     def flush_old_messages(self, older_than: Optional[float] = None, include_device: bool = False) -> int:
         """Archive every message older than the cutoff to archives/archive_{ts}.json and delete it (M:1159-1206).

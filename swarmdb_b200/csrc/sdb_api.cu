@@ -36,6 +36,8 @@ cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaSt
                                const sdb_compact_args*);
 cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double, uint32_t, const sdb_compact_args*, cudaStream_t,
                               int*, sdb_profiler*, int);
+cudaError_t sdb_launch_where(const sdb_dev_view*, const sdb_recv_args*, const sdb_where_args*, int, uint32_t, cudaStream_t, int*,
+                             sdb_profiler*, int);
 cudaError_t sdb_recv_prepare_device();
 cudaError_t sdb_balance_prepare_device();
 cudaError_t sdb_launch_receive_small(const sdb_dev_view*, const uint32_t*, uint32_t, uint32_t, uint32_t, uint32_t, uint4*,
@@ -177,6 +179,8 @@ struct sdb_ctx {
   sdb_recv_args last_rx{}; bool last_rx_valid = false;   // the last bulk receive (sdb_digest_fold reads its device results)
   bool last_rx_compact = false;                          // the last receive was compact: no full-format device results
   sdb_compact_args cx{};                                 // compact receive scratch + outputs, allocated on first use
+  uint32_t* where_bits = nullptr;                        // filtered receive: verdict bitmap [max_agents][ceil(R / 32)] ...
+  uint8_t* where_kw = nullptr;                           // ... and the keyword [SDB_FILTER_MAX_KEYWORD], allocated on first use
   unsigned long long* digest = nullptr;                  // [max_agents] stream digests, allocated on first use
   // backends
   uint32_t* be_weight = nullptr; unsigned long long* be_load = nullptr; uint32_t n_backends = 0;
@@ -938,7 +942,7 @@ int sdb_destroy(sdb_handle h) {
                  h->rx_totals, h->rx_big_list, h->rx_big_count, h->rx_count, h->rx_hdr, h->rx_payload,
                  h->be_weight, h->be_load, h->be_scratch, h->be_logtab, h->be_req_cost, h->be_out, h->digest,
                  h->cx.table, h->cx.rec_slot, h->cx.head, h->cx.head_local, h->cx.head_tops, h->cx.gran, h->cx.gran_local,
-                 h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out};
+                 h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out, h->where_bits, h->where_kw};
   for (void* p : dev) if (p) cudaFree(p);
   if (h->descs_host) cudaFreeHost(h->descs_host);
   if (h->list_host) cudaFreeHost(h->list_host);
@@ -1934,6 +1938,91 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
     if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
     if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return SDB_OK;
+}
+
+int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                      const sdb_filter* filter, uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
+                      uint8_t* payload_out, uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  constexpr uint32_t all_fields = SDB_FILTER_SENDER | SDB_FILTER_RECEIVER | SDB_FILTER_GROUP | SDB_FILTER_TYPE | SDB_FILTER_PRIO |
+                                  SDB_FILTER_TIME | SDB_FILTER_SEQ | SDB_FILTER_KEYWORD | SDB_FILTER_ICASE;
+  if (!filter || filter->struct_bytes != sizeof(sdb_filter)) return fail(h, SDB_EINVAL, "sdb_receive_where: struct_bytes != sizeof(sdb_filter)");
+  if (filter->fields & ~all_fields) return fail(h, SDB_EINVAL, "sdb_receive_where: unknown filter fields");
+  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_where returns host results: SDB_RECV_ASYNC is not accepted");
+  if (flags & ~(SDB_RECV_PRIORITY | SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_WHERE_DROP))
+    return fail(h, SDB_EINVAL, "sdb_receive_where accepts SDB_RECV_PRIORITY, SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_WHERE_DROP only");
+  const bool use_kw = (filter->fields & SDB_FILTER_KEYWORD) && filter->keyword_len;
+  if (filter->fields & SDB_FILTER_KEYWORD) {
+    if (filter->keyword_len > SDB_FILTER_MAX_KEYWORD) return fail(h, SDB_EINVAL, "sdb_receive_where: keyword_len > SDB_FILTER_MAX_KEYWORD");
+    if (filter->keyword_len && !filter->keyword) return fail(h, SDB_EINVAL, "sdb_receive_where: NULL keyword");
+  }
+  const bool drop = (flags & SDB_WHERE_DROP) != 0;
+  if (drop && (hdr_out || payload_out)) return fail(h, SDB_EINVAL, "sdb_receive_where: drop mode takes no output buffers but count_out");
+  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
+  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
+  if (n_agents == 0 || max_messages == 0) return SDB_OK;
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
+  uint64_t rec_cap = ~0ull;
+  if (!drop) {
+    // sdb_receive_batch's record capacity: rec_cap records of the maximum size fit the device and the caller's buffers
+    const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
+    rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
+    if (hdr_out) rec_cap = std::min<uint64_t>(rec_cap, hdr_cap);
+    if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
+    if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  }
+  const uint32_t stride = (h->cfg.ring_slots + 31) / 32;
+  if (!h->where_bits) {
+    { int rcl = ls_stop(h); if (rcl != SDB_OK) return rcl; }      // the allocations below may wait for running kernels
+    uint32_t* bits = nullptr; uint8_t* kw = nullptr;
+    if (dmalloc(&bits, static_cast<size_t>(h->cfg.max_agents) * stride) != cudaSuccess ||
+        dmalloc(&kw, SDB_FILTER_MAX_KEYWORD) != cudaSuccess) {
+      if (bits) cudaFree(bits);
+      cudaGetLastError();
+      return fail(h, SDB_ENOMEM, "filtered receive: device allocation failed");
+    }
+    h->where_bits = bits; h->where_kw = kw;
+  }
+  if (agent_idx) {
+    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  }
+  if (use_kw) CUDA_TRY(h, cudaMemcpyAsync(h->where_kw, filter->keyword, filter->keyword_len, cudaMemcpyHostToDevice, h->stream));
+  sdb_where_args f{};
+  f.fields = use_kw ? filter->fields : (filter->fields & ~SDB_FILTER_KEYWORD);
+  f.sender = filter->sender; f.receiver = filter->receiver; f.group = filter->group;
+  f.type_mask = filter->type_mask; f.prio_mask = filter->prio_mask; f.kw_len = use_kw ? filter->keyword_len : 0u;
+  f.after = filter->after; f.before = filter->before; f.seq_lo = filter->seq_lo; f.seq_hi = filter->seq_hi;
+  f.kw = h->where_kw; f.bits = h->where_bits; f.stride = stride;
+  sdb_recv_args r{};
+  r.agent_idx = agent_idx ? h->rx_agent : (owned ? h->owned_dev : nullptr); r.n = n_agents; r.max_messages = max_messages;
+  r.flags = flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK);
+  r.cnt = h->rx_cnt; r.rec_local = h->rx_rec_local; r.rec_tops = h->rx_rec_tops;
+  r.rec_off = h->rx_rec_off; r.plan = h->rx_plan; r.lb = h->rx_lb;
+  r.plan_tops = h->rx_plan_tops; r.totals = h->rx_totals; r.big_list = h->rx_big_list; r.big_count = h->rx_big_count;
+  r.count_out = h->rx_count; r.hdr_out = h->rx_hdr; r.payload_out = h->rx_payload;
+  r.rec_cap = rec_cap;
+  int nl = 0;
+  cudaError_t e = sdb_launch_where(&h->view, &r, &f, drop ? 1 : 0, 32u + pad32(h->cfg.max_payload_bytes), h->stream, &nl,
+                                   &h->prof, h->sm_count);
+  h->launches += nl;
+  h->last_rx_valid = false; h->last_rx_compact = false;       // no full receive to fold: the plan belongs to a filtered call
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("filtered receive launch: ") + cudaGetErrorString(e));
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  if (count_out)
+    CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  const uint64_t total = h->totals_host[0], pbytes = drop ? 0 : h->totals_host[1] * SDB_GRANULE;
+  if (total_out) *total_out = total;
+  if (payload_bytes_out) *payload_bytes_out = pbytes;
+  if (!drop && total) {
+    if (hdr_out) CUDA_TRY(h, cudaMemcpyAsync(hdr_out, h->rx_hdr, total * sizeof(sdb_msg_header), cudaMemcpyDeviceToHost, h->stream));
+    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->rx_payload, pbytes, cudaMemcpyDeviceToHost, h->stream));
+    if (hdr_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
   return SDB_OK;
 }

@@ -183,6 +183,18 @@ struct sdb_compact_args {
   uint8_t* payload_out;        // [rec_cap * pad32(max_payload)]
 };
 
+// filter of a filtered receive (sdb_receive_where) as the kernels read it, plus the verdict bitmap
+struct sdb_where_args {
+  uint32_t fields;             // SDB_FILTER_* (KEYWORD only with kw_len > 0)
+  uint32_t sender, receiver, group;
+  uint32_t type_mask, prio_mask, kw_len;
+  double after, before;
+  unsigned long long seq_lo, seq_hi;
+  const uint8_t* kw;           // [kw_len] device copy of the keyword (unfolded)
+  uint32_t* bits;              // [max_agents][stride] bit j of agent a: the record at head + j matches
+  uint32_t stride;             // words per agent = ceil(ring_slots / 32)
+};
+
 // ---- asynchronous import (sdb_import_wire_ptrs_async): everything the host used to learn through a sync lives on
 // the device.  `sdb_cursor` is the device-resident twin of the host's arena / sequence counters (whoever advanced
 // them last marks the other side stale); `sdb_batch_base` carries one import's placement from the kernel that

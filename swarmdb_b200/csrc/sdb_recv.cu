@@ -1481,6 +1481,312 @@ extern "C" cudaError_t sdb_launch_expire(const sdb_dev_view* v, const sdb_recv_a
 }
 
 // ------------------------------------------------------------------------------------------
+// filtered receive (sdb_receive_where): the predicate is evaluated once per pending record and kept as one verdict bit
+// per ring slot (f.bits, agent a, offset j from the head); the selection then reads bits and ring entries only.
+//   k_where_eval    header clauses only, k_expire's shape: 8 lanes per request slot, the ring header once, the window's
+//                   entries coalesced, the 32-byte header sector of every live entry with 4 loads per lane in flight
+//   k_where_kw      with a keyword: one warp per request slot, a lane per entry for the header clauses, then every
+//                   record that passes gets a warp-cooperative substring search of its content bytes
+//   both            write the verdict words and cnt[q] = min(matches, max_messages)
+//   scan            k_scan_local / k_scan_tops over cnt (take mode)
+//   k_where_select  capacity cut of k_recv_select, then the first count_out[q] set bits in delivery order (priority
+//                   order: one walk per level 3..0 over the entries' meta) are planned {handle, -, plan z, slot} and
+//                   tombstoned; head / ntomb by select_agent_warp's rule, the ring header stored at most once.  Take
+//                   mode adds to `delivered` with one atomic per warp; drop mode adds to totals[0] instead and stops
+//   back end        k_scan_plan + k_scan_tops, then the receive gather unchanged
+// ------------------------------------------------------------------------------------------
+#define SDB_WHERE_HDR_FIELDS (SDB_FILTER_SENDER | SDB_FILTER_RECEIVER | SDB_FILTER_GROUP | SDB_FILTER_TYPE | SDB_FILTER_PRIO | \
+                              SDB_FILTER_TIME | SDB_FILTER_SEQ)
+#define SDB_WHERE_STAGE 1024u     // content bytes staged per warp and step of the keyword search
+
+// lo = {seq lo, seq hi, timestamp lo, timestamp hi}, hi = {sender, receiver, group, len | prio << 16 | type << 24}
+__device__ __forceinline__ bool where_header(const sdb_where_args& f, const uint4& lo, const uint4& hi) {
+  const uint32_t fl = f.fields;
+  bool ok = true;
+  if (fl & SDB_FILTER_SENDER) ok = ok && hi.x == f.sender;
+  if (fl & SDB_FILTER_RECEIVER) ok = ok && hi.y == f.receiver;
+  if (fl & SDB_FILTER_GROUP) ok = ok && hi.z == f.group;
+  if (fl & SDB_FILTER_TYPE) ok = ok && ((f.type_mask >> ((hi.w >> 24) & SDB_TYPE_MASK)) & 1u);
+  if (fl & SDB_FILTER_PRIO) { const uint32_t p = (hi.w >> 16) & 0xFFu; ok = ok && p < 8u && ((f.prio_mask >> p) & 1u); }
+  if (fl & SDB_FILTER_TIME) {
+    const double ts = __hiloint2double(static_cast<int>(lo.w), static_cast<int>(lo.z));
+    ok = ok && ts > f.after && ts < f.before;                 // strict: a NaN never matches
+  }
+  if (fl & SDB_FILTER_SEQ) {
+    const unsigned long long s = (static_cast<unsigned long long>(lo.y) << 32) | lo.x;
+    ok = ok && s >= f.seq_lo && s < f.seq_hi;
+  }
+  return ok;
+}
+
+__device__ __forceinline__ uint32_t where_fold(uint32_t c, bool icase) { return (icase && c - 65u < 26u) ? c + 32u : c; }
+
+__global__ void __launch_bounds__(256)
+k_where_eval(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
+  const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_EXP_G - 1), gsh = lane & ~(SDB_EXP_G - 1);
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1;
+  const bool need_hdr = (f.fields & SDB_WHERE_HDR_FIELDS) != 0;
+  constexpr uint32_t SPW = 32u / SDB_EXP_G;
+  for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
+    const uint32_t q = qb + lane / SDB_EXP_G;
+    const bool valid = q < r.n;
+    uint32_t a = 0, H = 0, T = 0, NT = 0;
+    if (valid) {
+      a = r.agent_idx ? r.agent_idx[q] : q;
+      const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);
+      H = h.x; T = h.y; NT = h.w;
+    }
+    const uint32_t W = (valid && T - H - NT) ? T - H : 0u;
+    const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
+    const uint2* rs = sdb_ring_of(v, a);
+    uint32_t* bits = f.bits + static_cast<size_t>(a) * f.stride;
+    uint32_t got = 0;
+    for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_EXP_G * SDB_EXP_U) {
+      uint2 e[SDB_EXP_U];
+      uint4 lo[SDB_EXP_U], hi[SDB_EXP_U];
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t j = j0 + u * SDB_EXP_G + l8;
+        e[u] = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+      }
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {              // independent random loads, all issued before any use
+        lo[u] = hi[u] = make_uint4(0u, 0u, 0u, 0u);
+        if (need_hdr && sdb_meta(e[u]) != SDB_META_TOMB) {
+          const uint4* src = reinterpret_cast<const uint4*>(v.arena + ((static_cast<uint64_t>(e[u].x) & v.gmask) << 5));
+          lo[u] = __ldg(src); hi[u] = __ldg(src + 1);
+        }
+      }
+      uint32_t word = 0;
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const bool match = sdb_meta(e[u]) != SDB_META_TOMB && (!need_hdr || where_header(f, lo[u], hi[u]));
+        word |= ((__ballot_sync(0xFFFFFFFFu, match) >> gsh) & 0xFFu) << (u * SDB_EXP_G);
+      }
+      if (l8 == 0 && j0 < W) bits[j0 >> 5] = word;
+      got += __popc(word);
+    }
+    if (l8 == 0 && valid) r.cnt[q] = min(got, r.max_messages);
+  }
+}
+
+// does kw[0, K) (folded) occur in the bytes [cs, ce) of the padded payload p[0, plen)?  Whole warp; the content is staged
+// through `buf` in chunks that overlap by K - 1 bytes, 16-byte loads; lanes test start positions, first byte first.
+__device__ __forceinline__ bool where_find(const uint8_t* p, uint32_t plen, uint32_t cs, uint32_t ce, const uint8_t* kw,
+                                           uint32_t K, bool icase, uint8_t* buf, uint32_t lane) {
+  if (ce < cs + K) return false;
+  const uint32_t last = ce - K;                               // last start position
+  const uint32_t k0 = kw[0];
+  uint32_t s = cs;                                            // first start position not tested yet
+  for (;;) {
+    const uint32_t c0 = s & ~15u;                             // staged: payload bytes [c0, min(c0 + STAGE, plen))
+    const uint32_t end = min(c0 + SDB_WHERE_STAGE, plen);
+    __syncwarp();
+    for (uint32_t b = lane << 4; c0 + b < end; b += 512)
+      *reinterpret_cast<uint4*>(buf + b) = __ldg(reinterpret_cast<const uint4*>(p + c0 + b));
+    __syncwarp();
+    const uint32_t hi = min(last, c0 + SDB_WHERE_STAGE - K);  // last start whose K bytes are staged
+    for (uint32_t t0 = s; t0 <= hi; t0 += 32) {               // warp-uniform
+      const uint32_t t = t0 + lane;
+      bool hit = false;
+      if (t <= hi) {
+        const uint8_t* x = buf + (t - c0);
+        if (where_fold(x[0], icase) == k0) {
+          uint32_t i = 1;
+          while (i < K && where_fold(x[i], icase) == kw[i]) ++i;
+          hit = i == K;
+        }
+      }
+      if (__any_sync(0xFFFFFFFFu, hit)) return true;
+    }
+    if (hi >= last) return false;
+    s = hi + 1;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_where_kw(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
+  __shared__ uint8_t s_kw[SDB_FILTER_MAX_KEYWORD];
+  __shared__ __align__(16) uint8_t s_buf[8][SDB_WHERE_STAGE];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1, K = f.kw_len;
+  const bool icase = (f.fields & SDB_FILTER_ICASE) != 0;
+  for (uint32_t i = threadIdx.x; i < K; i += blockDim.x) s_kw[i] = static_cast<uint8_t>(where_fold(f.kw[i], icase));
+  __syncthreads();
+  for (uint32_t q = gw; q < r.n; q += nw) {                   // warp-uniform: one request slot per warp
+    const uint32_t a = r.agent_idx ? r.agent_idx[q] : q;
+    const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);
+    const uint32_t H = h.x, T = h.y, NT = h.w;
+    const uint32_t W = T - H - NT ? T - H : 0u;
+    const uint2* rs = sdb_ring_of(v, a);
+    uint32_t* bits = f.bits + static_cast<size_t>(a) * f.stride;
+    uint32_t got = 0;
+    for (uint32_t j0 = 0; j0 < W; j0 += 32) {
+      const uint32_t j = j0 + lane;
+      const uint2 e = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+      const bool lv = sdb_meta(e) != SDB_META_TOMB;
+      uint4 lo = make_uint4(0u, 0u, 0u, 0u), hi = lo;
+      if (lv) {
+        const uint4* src = reinterpret_cast<const uint4*>(v.arena + ((static_cast<uint64_t>(e.x) & v.gmask) << 5));
+        lo = __ldg(src); hi = __ldg(src + 1);
+      }
+      uint32_t word = __ballot_sync(0xFFFFFFFFu, lv && where_header(f, lo, hi));
+      for (uint32_t c = word; c; c &= c - 1) {
+        const uint32_t src = __ffs(c) - 1;
+        const uint32_t hx = __shfl_sync(0xFFFFFFFFu, e.x, src), hy = __shfl_sync(0xFFFFFFFFu, e.y, src);
+        const uint32_t hw = __shfl_sync(0xFFFFFFFFu, hi.w, src);
+        const uint32_t len = hw & 0xFFFFu;
+        const uint8_t* p = sdb_payload_of(v, hx, sdb_entry_dm1(hy));      // shared-layout images: handle + 1 + dm1
+        uint32_t cs = 0, ce = len;
+        if ((hw >> 24) & SDB_TYPEF_EXTRAS) {                               // u32 content length | content | extras
+          cs = 4;
+          ce = len < 4 ? 4u : 4u + min(__ldg(reinterpret_cast<const uint32_t*>(p)), len - 4u);
+        }
+        if (!where_find(p, (len + 31u) & ~31u, cs, ce, s_kw, K, icase, s_buf[warp], lane)) word &= ~(1u << src);
+      }
+      if (lane == 0) bits[j0 >> 5] = word;
+      got += __popc(word);
+    }
+    if (lane == 0) r.cnt[q] = min(got, r.max_messages);
+  }
+}
+
+template <bool PLAN>
+__global__ void __launch_bounds__(256)
+k_where_select(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
+  const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_EXP_G - 1), gsh = lane & ~(SDB_EXP_G - 1);
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1;
+  const bool retire = !(r.flags & SDB_RECV_PEEK);
+  const int top = (r.flags & SDB_RECV_PRIORITY) ? 3 : -1;      // -1: one walk, every level (stream order)
+  constexpr uint32_t SPW = 32u / SDB_EXP_G;
+  unsigned long long wsum = 0;
+  for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
+    const uint32_t q = qb + lane / SDB_EXP_G;
+    const bool valid = q < r.n;
+    uint32_t a = 0, H = 0, T = 0, NT = 0, c = 0, RO = 0;
+    if (valid) {
+      a = r.agent_idx ? r.agent_idx[q] : q;
+      c = r.cnt[q];
+      if (PLAN) {
+        RO = r.rec_local[q] + r.rec_tops[q / SDB_SCAN_TILE];
+        if (c && static_cast<uint64_t>(RO) + c > r.rec_cap) {   // does not fit: stays queued ...
+          c = RO == 0 ? static_cast<uint32_t>(r.rec_cap) : 0u;  // ... unless first in the output: its first rec_cap matches
+          if (l8 == 0) atomicMin(r.totals, static_cast<unsigned long long>(RO) + c);
+        }
+      }
+      if (l8 == 0) r.count_out[q] = c;
+      if (c) {
+        const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);
+        H = h.x; T = h.y; NT = h.w;
+      }
+    }
+    const uint32_t W = c ? T - H : 0u;
+    const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
+    uint2* rs = sdb_ring_of(v, a);
+    const uint32_t* bits = f.bits + static_cast<size_t>(a) * f.stride;
+    uint32_t seen = 0;                                          // matches met so far in delivery order
+    for (int L = top;; --L) {
+      for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_EXP_G * SDB_EXP_U) {
+        if (__all_sync(0xFFFFFFFFu, seen >= c)) break;
+        const uint32_t word = (j0 < W && seen < c) ? bits[j0 >> 5] : 0u;
+        uint2 e[SDB_EXP_U];
+#pragma unroll
+        for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+          const uint32_t j = j0 + u * SDB_EXP_G + l8;
+          e[u] = ((word >> (u * SDB_EXP_G + l8)) & 1u) ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+        }
+#pragma unroll
+        for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+          const uint32_t m = sdb_meta(e[u]);
+          const bool match = m != SDB_META_TOMB && (L < 0 || (m >> 14) == static_cast<uint32_t>(L));
+          const uint32_t bm = (__ballot_sync(0xFFFFFFFFu, match) >> gsh) & 0xFFu;
+          const uint32_t k = seen + __popc(bm & ((1u << l8) - 1u));
+          if (match && k < c) {
+            if (PLAN) r.plan[RO + k] = make_uint4(e[u].x, 0u, sdb_plan_z(e[u].y), q);
+            if (retire) rs[(H + j0 + u * SDB_EXP_G + l8) & mask].y = SDB_META_TOMB;
+          }
+          seen += __popc(bm);
+        }
+      }
+      if (L <= 0) break;
+    }
+    // new head: the first live entry left (each lane re-reads only the slots it may have tombstoned itself)
+    const uint32_t took = min(seen, c);
+    const bool fix = retire && took;
+    const uint32_t W2 = fix ? W : 0u;
+    const uint32_t wmax2 = __reduce_max_sync(0xFFFFFFFFu, W2);
+    uint32_t nh = T;
+    bool found = false;
+    for (uint32_t j0 = 0; j0 < wmax2; j0 += SDB_EXP_G * SDB_EXP_U) {
+      if (__all_sync(0xFFFFFFFFu, !fix || found)) break;
+      uint32_t m[SDB_EXP_U];
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t j = j0 + u * SDB_EXP_G + l8;
+        m[u] = (j < W2 && !found) ? sdb_meta(rs[(H + j) & mask]) : SDB_META_TOMB;
+      }
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t b = (__ballot_sync(0xFFFFFFFFu, m[u] != SDB_META_TOMB) >> gsh) & 0xFFu;
+        if (b && !found) { nh = H + j0 + u * SDB_EXP_G + (__ffs(b) - 1); found = true; }
+      }
+    }
+    if (l8 == 0 && valid) {
+      if (fix) {                                                // the ring header, once
+        v.ring_hdr[a].head = nh;
+        v.ring_hdr[a].ntomb = NT + took - (nh - H);
+      }
+      if (!PLAN || retire) wsum += took;
+    }
+  }
+  for (int o = 16; o; o >>= 1) wsum += __shfl_xor_sync(0xFFFFFFFFu, wsum, o);
+  if (lane == 0 && wsum) atomicAdd(PLAN ? &v.ctr->delivered : r.totals, wsum);
+}
+
+// drop mode: eval + select, totals[0] = records selected.  Take mode: eval, scan, select, plan scan, then the receive
+// gather exactly as the priority pipeline runs it (totals[0] records, totals[1] payload granules)
+extern "C" cudaError_t sdb_launch_where(const sdb_dev_view* v, const sdb_recv_args* r, const sdb_where_args* f, int drop,
+                                        uint32_t max_rec_bytes, cudaStream_t stream, int* n_launches, sdb_profiler* prof,
+                                        int sm_count) {
+  if (r->n == 0) return cudaSuccess;
+  const uint32_t n = r->n;
+  uint64_t blocks = (static_cast<uint64_t>(n) + 31) / 32;                    // 4 slots per warp, 8 warps per block
+  const uint64_t bcap = static_cast<uint64_t>(sm_count) * 8 * 4;             // grid-stride beyond ~4 waves
+  if (blocks > bcap) blocks = bcap;
+  const int pi = sdb_prof_begin(prof, SDB_PK_WHERE, stream);
+  if (f->fields & SDB_FILTER_KEYWORD) {
+    uint64_t kb = (static_cast<uint64_t>(n) + 7) / 8;                        // a warp per slot, 8 warps per block
+    const uint64_t kcap = static_cast<uint64_t>(sm_count) * 8;
+    if (kb > kcap) kb = kcap;
+    k_where_kw<<<static_cast<uint32_t>(kb), 256, 0, stream>>>(*v, *r, *f);
+  } else {
+    k_where_eval<<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, *f);
+  }
+  if (drop) {
+    cudaMemsetAsync(r->totals, 0, 2 * sizeof(unsigned long long), stream);
+    k_where_select<false><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, *f);
+    sdb_prof_end(prof, pi, stream);
+    if (n_launches) *n_launches += 2;
+    return cudaGetLastError();
+  }
+  const uint32_t tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
+  k_scan_local<<<tiles, 1024, 0, stream>>>(r->cnt, 0xFFFFFFFFu, r->rec_local, r->rec_tops, n);
+  k_scan_tops<<<1, 1024, 0, stream>>>(r->rec_tops, tiles, r->totals);       // totals[0] = matches; the cut may lower it
+  k_where_select<true><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, *f);
+  uint64_t bound = static_cast<uint64_t>(n) * (r->max_messages < v->ring_slots ? r->max_messages : v->ring_slots);   // records planned, at most
+  if (bound > r->rec_cap) bound = r->rec_cap;
+  const uint32_t rtiles = static_cast<uint32_t>((bound + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE);
+  k_scan_plan<<<rtiles, 1024, 0, stream>>>(r->plan, r->plan_tops, r->totals);
+  k_scan_tops<<<1, 1024, 0, stream>>>(r->plan_tops, rtiles, r->totals + 1);  // totals[1] = payload granules
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += 6;
+  return launch_gather(v, r, nullptr, bound, max_rec_bytes, sm_count, stream, prof, n_launches);
+}
+
+// ------------------------------------------------------------------------------------------
 // arena floor: smallest arena position still referenced by a pending ring entry.
 // One thread per agent; distance below the current arena tail is maximised with atomicMax.
 // ------------------------------------------------------------------------------------------

@@ -298,13 +298,19 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
     @app.get("/messages", response_model=List[MessageOut])
     def query(sender_id: Optional[str] = None, receiver_id: Optional[str] = None, message_type: Optional[MessageType] = None,
               status_filter: Optional[MessageStatus] = Query(None, alias="status"), after_timestamp: Optional[float] = None,
-              before_timestamp: Optional[float] = None, limit: int = 100, who: str = Depends(caller)):
+              before_timestamp: Optional[float] = None, limit: int = 100, include_device: bool = False,
+              who: str = Depends(caller)):
         if who != "admin" and sender_id and sender_id != who and receiver_id != who:
             raise HTTPException(status_code=http.HTTP_403_FORBIDDEN,
                                 detail="You can only query messages you sent or received")
+        if include_device and who != "admin" and receiver_id != who:
+            # the device queues hold every agent's undelivered messages: a caller may read its own queue only
+            raise HTTPException(status_code=http.HTTP_403_FORBIDDEN,
+                                detail="include_device needs receiver_id set to yourself or admin privileges")
         found = guarded("query messages", lambda: db.query_messages(
             sender_id=sender_id, receiver_id=receiver_id, message_type=message_type, status=status_filter,
-            after_timestamp=after_timestamp, before_timestamp=before_timestamp, limit=limit))
+            after_timestamp=after_timestamp, before_timestamp=before_timestamp, limit=limit,
+            include_device=include_device))                  # include_device: also the matching device-queued messages
         return [MessageOut.of(m) for m in found]
 
     @app.get("/agents/{agent_id}/messages", response_model=List[MessageOut])

@@ -690,6 +690,12 @@ class ShardedSwarmsDB(SwarmsDB):
             return []
         return self._receive_local(agent_id, max_messages)
 
+    def _prepare_receive(self, agent_id: str) -> bool:
+        """receive_matching runs on the owner rank, locally (no collective), like receive_messages."""
+        if self.owner(agent_id) != self.rank:
+            raise ValueError(f"agent {agent_id!r} lives on shard {self.owner(agent_id)}, not on rank {self.rank}")
+        return agent_id in self._agent_idx
+
     def _pre_read(self) -> None:
         return None                              # reads see what earlier collective flushes delivered
 
