@@ -9,6 +9,7 @@
   expire   retention on the c2 backlog (sdb_expire): drop mode at the median cutoff, SDB_EXPIRE_ALL, archive mode
   where    filtered receive on the c2 backlog (sdb_receive_where): header-clause and keyword PEEKs, a take of one group's
            records, and keyword counts over deep queues
+  restore  restore on the c2 backlog (sdb_restore_compact): snapshot, restore into a fresh handle, requeue
 
 bench.py remains the contract benchmark (c2/c3); this file only feeds DESIGN.md.
 """
@@ -583,6 +584,119 @@ def where(rounds=3, block=4):
                                  "frac_of_3.35TB_s": dbytes / (dk * 1e-3) / peak if dk else None}
     out.update(_gpu_card(0))
     out["clocks"] = clk
+    return out
+
+
+def restore(rounds=3):
+    """sdb_restore_compact on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 pending records): a
+    snapshot (PEEK compact receive into pinned host buffers), its restore into a fresh handle from those buffers, and the
+    requeue of one full compact receive (rows renumbered by smallest seq, then restored behind an empty queue), each
+    timed per call (wall clock around a synchronising call) with the restore kernels' time from the profiler.  Outside
+    the timed region the restored handle's full drain is checked, by digests, against the original handle's, and the
+    arena granules the restore took against those the original send took."""
+    import torch
+    from bench import ClockSampler, Workload
+    from swarmdb_b200._native import ENTRY_DTYPE, RECV_PEEK, SEND_DTYPE, Shard
+    from swarmdb_b200.core import _renumber_rows
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py restore: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+
+    def handle():
+        s = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+        s.register(np.arange(wl.A, dtype=np.uint32))
+        for g in range(wl.G):
+            s.create_group(g, wl.members(g))
+        return s
+
+    def pinned(nbytes):
+        return torch.empty(nbytes, dtype=torch.uint8, pin_memory=True).numpy()
+
+    def drain(s, digest=False):
+        if digest:
+            s.digest_reset()
+        while True:
+            _, total, _ = s.receive_batch(None, 1 << 10, copy_out=False)
+            if digest:
+                s.digest_fold()
+            if not total:
+                break
+        return s.digest_read() if digest else None
+
+    src, dst = handle(), handle()
+    agents = np.arange(wl.A, dtype=np.uint32)
+    pin_ent, pin_snd, pin_pay = pinned(rec_cap * 16).view(ENTRY_DTYPE), pinned(rec_cap * 32).view(SEND_DTYPE), pinned(rec_cap * wl.L)
+    t0 = src.stats()["arena_tail_bytes"]
+    src.send_group_batch(*wl.batch())
+    sent_bytes = src.stats()["arena_tail_bytes"] - t0
+
+    def snapshot():
+        return src.receive_compact(None, 1 << 10, RECV_PEEK, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_pay)
+
+    cnt, ent, snd, pay = snapshot()
+    ent2, snd2 = _renumber_rows(ent, snd)
+    pin_ent2, pin_snd2 = pinned(len(ent2) * 16).view(ENTRY_DTYPE), pinned(len(snd2) * 32).view(SEND_DTYPE)
+    pin_ent2[:], pin_snd2[:] = ent2, snd2
+    cnt = cnt.copy()
+    n_rec, n_rows = len(ent2), len(snd2)
+
+    def timed(fn, before=None):
+        res = {"wall_ms": [], "kernel_ms": []}
+        for _ in range(rounds):
+            if before:
+                before()
+            for s in (src, dst):
+                s.sync(); s.profile(True)
+            t = time.perf_counter()
+            part = fn()
+            res["wall_ms"].append((time.perf_counter() - t) * 1e3)
+            if isinstance(part, float):                      # the part of the call the step times itself
+                res.setdefault("part_ms", []).append(part)
+            k = 0.0
+            for s in (src, dst):
+                prof = s.profile_read(); s.profile(False)
+                k += prof["restore"][0] + prof["recv_compact"][0] + sum(prof[x][0] for x in ("recv_count", "recv_scan", "recv_select"))
+            res["kernel_ms"].append(k)
+        return {k: float(np.median(v)) for k, v in res.items()} | {"per_round": res}
+
+    clocks = ClockSampler(0); clocks.start()
+    out = {"snapshot": timed(snapshot)}
+    out["restore"] = timed(lambda: dst.restore_compact(agents, cnt, pin_ent2, pin_snd2, pin_pay[: len(pay)]),
+                           before=lambda: drain(dst))
+    # outside the timed region: the restored queue drains to the original's digests, in the original's arena bytes
+    drain(dst)
+    t1 = dst.stats()["arena_tail_bytes"]
+    dst.restore_compact(agents, cnt, pin_ent2, pin_snd2, pin_pay[: len(pay)])
+    restored_bytes = dst.stats()["arena_tail_bytes"] - t1
+    same = bool(np.array_equal(drain(dst, True), drain(src, True)))
+
+    def requeue():
+        c, e, s, p = src.receive_compact(None, 1 << 10, 0, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_pay)
+        t = time.perf_counter()
+        e, s = _renumber_rows(e, s)
+        src.restore_compact(agents, c, e, s, p)
+        return (time.perf_counter() - t) * 1e3
+
+    def refill():
+        drain(src)
+        src.send_group_batch(*wl.batch())
+    out["requeue_receive_plus_restore"] = timed(requeue, before=refill)
+    clk = clocks.stop()
+    src.close(); dst.close()
+    rk = out["restore"]["kernel_ms"]
+    alg = n_rec * (16 + 32 + 8) + n_rows * (32 + 2 * ((wl.L + 31) & ~31))
+    out.update({"config": f"c2 backlog: {wl.A} agents, {wl.S} group sends x {wl.F} members = {per_step} pending records, "
+                          f"{wl.L}-B payloads; pinned host buffers; {rounds} calls each",
+                "records": n_rec, "rows": n_rows, "h2d_bytes": n_rec * 16 + n_rows * 32 + len(pay),
+                "restore_alg_bytes": alg, "restore_kernel_gbps": alg / (rk * 1e-3) / 1e9,
+                "restore_floor_us_at_3.35TBps": alg / 3.35e12 * 1e6,
+                "drain_digests_equal": same, "arena_bytes_sent": sent_bytes, "arena_bytes_restored": restored_bytes,
+                "clocks": clk})
+    out.update(_gpu_card(0))
     return out
 
 

@@ -130,7 +130,7 @@ int sdb_advance_seq(sdb_handle h, uint64_t next_seq);
  * roofline: enable, run, then read accumulated milliseconds and launch counts per kernel class. */
 enum { SDB_PK_P2P = 0, SDB_PK_FANOUT, SDB_PK_COMMIT, SDB_PK_RECV_COUNT, SDB_PK_RECV_SCAN, SDB_PK_RECV_SELECT,
        SDB_PK_RECV_GATHER, SDB_PK_ARENA_FLOOR, SDB_PK_PICK, SDB_PK_XSHARD, SDB_PK_INDEX, SDB_PK_XWAIT,
-       SDB_PK_RECV_COMPACT = 12, SDB_PK_EXPIRE = 13, SDB_PK_WHERE = 14, SDB_PK_N = 16 };
+       SDB_PK_RECV_COMPACT = 12, SDB_PK_EXPIRE = 13, SDB_PK_WHERE = 14, SDB_PK_RESTORE = 15, SDB_PK_N = 16 };
 int sdb_profile(sdb_handle h, int enable);
 int sdb_profile_read(sdb_handle h, double* ms_out /* [SDB_PK_N] */, uint64_t* count_out /* [SDB_PK_N] */);
 
@@ -278,6 +278,47 @@ int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
                         uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
                         sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                         uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
+/* Restore: put records in the compact format back on the device - a queue snapshot (a PEEK compact receive) after a
+ * restart, or what a compact receive just took when its consumer failed (requeue).  Input in exactly the shape
+ * sdb_receive_compact and sdb_expire's archive mode return: listed agent i owns the next count[i] entries.
+ *   1. Effect     each listed agent gets its records appended behind whatever it has pending, in the given order.  Record
+ *                 r has the header of entry r and its row (contract point 1 of sdb_receive_compact: seq, timestamp,
+ *                 sender, receiver, group, len, prio, type) and the padded payload bytes.  Every later receive (any path,
+ *                 any order, digests) delivers what it would deliver had those records been sent in that position.
+ *                 Sequence numbers are kept: message ids do not change.
+ *   2. Counters   next_seq = max(next_seq, largest restored seq + 1); stats.enqueued += records, delivered stays; in
+ *                 sdb_agent_loads `received`, `pending`, `pending_by_prio` and `pending_granules` grow as if the records
+ *                 had been sent; the registration watermark covers every listed agent.
+ *   3. Arena      rows in row-index order, each as its headers in entry order followed by ONE payload (shared layout; a
+ *                 row with more than 65535 records takes consecutive blocks of at most 65535 headers, each with its own
+ *                 payload copy).  From an agent's first entry that names a lower row than its previous entry on, that
+ *                 agent's entries are private images (header + payload) in a tail region after all rows, in entry order.
+ *                 With SDB_SHARED_PAYLOAD=0 every record is a private image.  Rows no restored entry names take no space.
+ *                 Arena positions strictly increase along every ring, and the layout is deterministic.  Rows numbered by
+ *                 their smallest seq in a stream-order snapshot give no private images.
+ *   4. All or nothing: the call validates and plans on the device, synchronises once, then writes.  On any error rings,
+ *                 arena, stats and digests are unchanged:
+ *                   SDB_ERING_OVERFLOW  some agent's tail - head + count[i] exceeds ring_slots (tombstones count);
+ *                   SDB_EARENA_FULL     the region does not fit after a floor reclaim;
+ *                   SDB_ECAPACITY       more than one compact receive holds: n_entries or n_sends above rec_cap, or
+ *                                       payload_bytes above rec_cap x pad32(max_payload_bytes) (rec_cap of
+ *                                       sdb_receive_compact without caller caps) - a chunk one compact receive
+ *                                       returned always restores in one call;
+ *                   SDB_EINVAL          agent_idx NULL with n_agents > 0, an agent listed twice or >= max_agents,
+ *                                       sum(count) != n_entries, entry.send >= n_sends, entry.receiver neither the
+ *                                       listed agent nor SDB_NO_RECEIVER, row len > max_payload_bytes or prio > 3,
+ *                                       payload_off not 16-byte aligned or payload_off + pad32(len) > payload_bytes,
+ *                                       unknown flag bits.
+ *                 Every row is checked, whether an entry names it or not.
+ *   5. Flags      SDB_RECV_OWNED on a sharded handle skips the entries of agents this shard does not own (unchecked), so
+ *                 every rank can be given the whole snapshot: a snapshot of N shards restores onto M.
+ *   6. Ordering   stream-ordered on the handle's stream; synchronises.  Works while the latency server runs.  The last
+ *                 receive's device results are left alone (sdb_digest_fold is unaffected).
+ * *restored_out (nullable) = records enqueued, *seq_end_out (nullable) = next_seq after the call. */
+int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, const uint32_t* count,
+                        const sdb_recv_entry* entries, uint64_t n_entries, const sdb_recv_send* sends, uint64_t n_sends,
+                        const uint8_t* payload, uint64_t payload_bytes, uint32_t flags, uint64_t* restored_out,
+                        uint64_t* seq_end_out);
 /* Low-latency dequeue server (opt-in): receive_messages (M:521-601) for ONE agent in a few microseconds.
  * enable = 1 starts a persistent single-CTA kernel on its own stream that polls a mailbox in mapped pinned host memory;
  * sdb_receive_batch calls naming exactly one agent with host outputs (what the Python surface's receive_messages makes)

@@ -124,7 +124,7 @@ class SdbStats(C.Structure):
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
-           "sdb_receive_batch", "sdb_receive_compact", "sdb_expire", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
+           "sdb_receive_batch", "sdb_receive_compact", "sdb_restore_compact", "sdb_expire", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
@@ -171,6 +171,8 @@ def load_library() -> C.CDLL:
     L.sdb_receive_batch.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, vp]
     L.sdb_receive_compact.restype = i32
     L.sdb_receive_compact.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    L.sdb_restore_compact.restype = i32
+    L.sdb_restore_compact.argtypes = [vp, u32, vp, vp, vp, u64, vp, u64, vp, u64, u32, vp, vp]
     L.sdb_expire.restype = i32
     L.sdb_expire.argtypes = [vp, u32, vp, C.c_double, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_receive_where.restype = i32
@@ -304,7 +306,7 @@ class Shard:
         self._check(self._L.sdb_advance_seq(self._h, next_seq))
 
     PROFILE_KINDS = ["p2p", "fanout", "commit", "recv_count", "recv_scan", "recv_select", "recv_gather",
-                     "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact", "expire", "where"]
+                     "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact", "expire", "where", "restore"]
 
     def profile(self, enable: bool) -> None:
         self._check(self._L.sdb_profile(self._h, 1 if enable else 0))
@@ -567,6 +569,21 @@ class Shard:
             owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
             counts = counts[: self.n_owned if owned else self.stats_n_agents()]
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
+
+    def restore_compact(self, agents, counts, entries, sends, payload, flags: int = 0) -> Tuple[int, int]:
+        """Append records in the compact receive format behind what each listed agent has pending, with their own
+        sequence numbers (include/swarmdb_b200.h: sdb_restore_compact): agent i takes the next counts[i] entries.  All
+        or nothing.  Returns (records restored, next sequence number)."""
+        a, c = _arr(agents, np.uint32), _arr(counts, np.uint32)
+        if len(a) != len(c):
+            raise ValueError("agents and counts differ in length")
+        ent, snd = np.ascontiguousarray(entries, ENTRY_DTYPE), np.ascontiguousarray(sends, SEND_DTYPE)
+        pay = np.ascontiguousarray(payload, np.uint8)
+        restored, seq_end = C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_restore_compact(self._h, len(a), _p(a), _p(c), _p(ent), len(ent), _p(snd), len(snd),
+                                                _p(pay), pay.nbytes, flags, C.cast(C.byref(restored), C.c_void_p),
+                                                C.cast(C.byref(seq_end), C.c_void_p)))
+        return int(restored.value), int(seq_end.value)
 
     def expire(self, agents, older_than: float, flags: int = 0, archive: bool = True,
                out_entries: Optional[np.ndarray] = None, out_sends: Optional[np.ndarray] = None,

@@ -32,7 +32,7 @@ import uuid
 from dataclasses import dataclass
 from enum import Enum
 from pathlib import Path
-from typing import Any, Callable, Dict, Iterable, List, Optional, Set, Union
+from typing import Any, Callable, Dict, Iterable, List, Optional, Set, Tuple, Union
 
 import numpy as np
 from pydantic import BaseModel, Field
@@ -164,6 +164,38 @@ def _encode_content(content: Any) -> (bytes, int):
     if isinstance(content, str):
         return content.encode("utf-8"), 0
     return json.dumps(content).encode("utf-8"), TYPEF_JSON
+
+
+def _renumber_rows(entries, sends) -> Tuple[np.ndarray, np.ndarray]:
+    """Rows of a compact-format result reordered by their smallest seq (unreferenced rows last), entries remapped.  A
+    restore lays rows out in row order, so records restored in stream order then take the arena positions, and share the
+    payloads, they had when they were sent."""
+    ent = np.array(entries, _native.ENTRY_DTYPE)
+    snd = np.asarray(sends, _native.SEND_DTYPE)
+    rows = np.ascontiguousarray(ent["send"])                       # contiguous: ufunc.at over strided fields is ~20x slower
+    smallest = np.full(len(snd), np.iinfo(np.uint64).max, np.uint64)
+    np.minimum.at(smallest, rows, np.ascontiguousarray(ent["seq"]))
+    order = np.argsort(smallest, kind="stable")
+    inv = np.empty(len(order), np.uint32)
+    inv[order] = np.arange(len(order), dtype=np.uint32)
+    ent["send"] = inv[rows]
+    return ent, snd[order]
+
+
+def _compact_rows(entries, sends, payload) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """Only the rows `entries` name, in row order, with their padded payloads packed back to back."""
+    ent = np.array(entries, _native.ENTRY_DTYPE)
+    used, inv = np.unique(ent["send"].astype(np.int64), return_inverse=True)
+    ent["send"] = inv.astype(np.uint32)
+    snd = np.array(sends[used], _native.SEND_DTYPE)
+    glen = pad32(snd["len"].astype(np.int64)) >> 5
+    start = np.zeros(len(snd), np.int64)
+    if len(snd) > 1:
+        np.cumsum(glen[:-1], out=start[1:])
+    src = np.repeat((snd["payload_off"].astype(np.int64) >> 5) - start, glen) + np.arange(int(glen.sum()), dtype=np.int64)
+    pay = np.ascontiguousarray(payload[: len(payload) & ~31]).view("V32")[src].view(np.uint8).copy()
+    snd["payload_off"] = (start << 5).astype(np.uint64)
+    return ent, snd, pay
 
 
 class _TransportAdmin:
@@ -853,6 +885,139 @@ class SwarmsDB:
         self.flush()
         pr = self.gpu_config.priority_dequeue if priority is None else priority
         return self.shard.receive_compact(agent_idx, max_messages, RECV_PRIORITY if pr else 0, **kw)
+
+    def requeue_batch_compact(self, counts, entries, sends, payload, agent_idx) -> int:
+        """The nack of receive_batch_compact: put what a compact receive took (or any input of that shape: agent_idx[i]
+        owns the next counts[i] entries) back behind what each agent has pending, with the original message ids.  Rows are
+        renumbered by their smallest seq first, so records requeued in stream order share payloads as they did.
+        All or nothing (Shard.restore_compact).  Returns the records requeued."""
+        self.flush()
+        ent, snd = _renumber_rows(entries, sends)
+        n, seq_end = self.shard.restore_compact(agent_idx, counts, ent, snd, payload)
+        self._next_seq = max(self._next_seq, seq_end); self._b_first_seq = self._next_seq
+        return n
+
+    # ------------------------------------------------------------------ queue snapshots (restart persistence)
+    SNAPSHOT_VERSION = 1
+
+    def save_queue_snapshot(self, path: Union[str, Path]) -> Path:
+        """Write every message pending on the device to one .npz file (no pickle) that load_queue_snapshot puts back
+        into a fresh instance: the agent and group tables in index order, the id nonce, the sequence counter and the
+        pending records as PEEK compact receives in stream order (rows renumbered by smallest seq).  Nothing is
+        consumed.  An agent with more pending records than one receive call holds raises: a snapshot is complete or it
+        is not written."""
+        self.flush()
+        g = self.gpu_config
+        cap = max(1, min(g.max_recv_records, (g.max_recv_payload or g.max_recv_records * 256) // pad32(g.max_payload_bytes)))
+        agents = np.arange(len(self._agent_name), dtype=np.uint32)
+        parts: List[Tuple[np.ndarray, ...]] = []
+        if len(agents):
+            pending = self.shard.agent_loads(agents)["pending"][: len(agents)].astype(np.int64)
+            deep = np.nonzero(pending > cap)[0]
+            if len(deep):
+                raise RuntimeError(f"agent {self._agent_name[int(agents[deep[0]])]} has {int(pending[deep[0]])} pending "
+                                   f"messages, more than one receive call holds ({cap}): no snapshot written")
+            for part, _ in self._pending_chunks(agents, cap):
+                cnt, ent, snd, pay = self.shard.receive_compact(part, cap, RECV_PEEK)
+                ent, snd = _renumber_rows(ent, snd)
+                parts.append((part, cnt.astype(np.uint32), ent, snd, pay.copy()))
+        off = np.zeros((len(parts) + 1, 4), np.uint64)          # chunk k: agents, entries, rows, payload bytes
+        for k, (a, _, e, s, p) in enumerate(parts):
+            off[k + 1] = off[k] + [len(a), len(e), len(s), len(p)]
+        snd_all = np.concatenate([s for *_, s, _ in parts]) if parts else np.zeros(0, _native.SEND_DTYPE)
+        ent_all = np.concatenate([e for _, _, e, _, _ in parts]) if parts else np.zeros(0, _native.ENTRY_DTYPE)
+        if parts:                 # entries index the whole row table, rows the whole payload: add each chunk's offsets
+            snd_all["payload_off"] += np.repeat(off[:-1, 3], [len(s) for *_, s, _ in parts])
+            ent_all["send"] += np.repeat(off[:-1, 2], [len(e) for _, _, e, _, _ in parts]).astype(np.uint32)
+        members = [[self._agent_idx[a] for a in (self._group_snapshot[k] or [])] for k in range(len(self._group_name))]
+        moff = np.zeros(len(members) + 1, np.uint64)
+        moff[1:] = np.cumsum([len(m) for m in members]) if members else []
+        path = Path(path)
+        with open(path, "wb") as f:
+            np.savez(f, version=np.uint32(self.SNAPSHOT_VERSION),
+                     shard=np.array([g.shard_id, max(1, g.num_shards)], np.uint32),
+                     id_nonce=np.uint64(self._id_hi >> 64), next_seq=np.uint64(self._next_seq),
+                     agent_names=np.array(self._agent_name, dtype=np.str_),
+                     registered=np.array([a in self.registered_agents for a in self._agent_name], bool),
+                     group_names=np.array(self._group_name, dtype=np.str_), group_off=moff,
+                     group_members=np.array([x for m in members for x in m], np.uint32),
+                     chunk_off=off,
+                     agents=np.concatenate([p[0] for p in parts]).astype(np.uint32) if parts else np.zeros(0, np.uint32),
+                     counts=np.concatenate([p[1] for p in parts]) if parts else np.zeros(0, np.uint32),
+                     entries=ent_all,
+                     sends=snd_all,
+                     payload=np.concatenate([p[4] for p in parts]) if parts else np.zeros(0, np.uint8))
+        return path
+
+    @staticmethod
+    def _read_snapshot(path: Union[str, Path]) -> Dict[str, np.ndarray]:
+        with np.load(Path(path), allow_pickle=False) as z:
+            snap = {k: z[k] for k in z.files}
+        if int(snap["version"]) != SwarmsDB.SNAPSHOT_VERSION:
+            raise ValueError(f"{path}: queue snapshot format {int(snap['version'])}, expected {SwarmsDB.SNAPSHOT_VERSION}")
+        return snap
+
+    def _check_fresh(self) -> None:
+        st = self.shard.stats()
+        if self._agent_name or self._group_name or len(self._b_sender) or st["enqueued"] or st["next_seq"] != 1:
+            raise RuntimeError("load_queue_snapshot needs a fresh instance (no agent, group or send yet)")
+
+    def _adopt_tables(self, snap: Dict[str, np.ndarray]) -> None:
+        """Agents and groups in the snapshot's index order (indices keep their meaning: payloads of long visible_to
+        lists hold dense agent indices), the id nonce and the sequence counter."""
+        nonce = int(snap["id_nonce"])
+        g = self.gpu_config
+        if not g.deterministic_ids:
+            if g.id_nonce is not None and (g.id_nonce & ((1 << 63) - 1)) != nonce:
+                raise ValueError(f"GpuConfig.id_nonce={g.id_nonce:#x} differs from the snapshot's id nonce {nonce:#x}")
+            self._id_hi = nonce << 64
+        names = [str(x) for x in snap["agent_names"]]
+        for a in names:
+            self._index(a)
+        reg = [a for a, r in zip(names, snap["registered"].tolist()) if r]
+        if reg:
+            self.register_agents(reg)
+        moff, mem = snap["group_off"].astype(np.int64), snap["group_members"]
+        for k, gname in enumerate(str(x) for x in snap["group_names"]):
+            self.add_agent_group(gname, [names[int(i)] for i in mem[moff[k]:moff[k + 1]]])
+        nxt = int(snap["next_seq"])
+        self.shard.advance_seq(nxt)
+        self._next_seq = max(self._next_seq, nxt); self._b_first_seq = self._next_seq
+
+    def _restore_chunks(self, snap: Dict[str, np.ndarray]) -> int:
+        """Restore every chunk of a snapshot, split by whole agents where this instance's receive capacity is smaller;
+        returns the largest sequence number + 1 seen."""
+        g = self.gpu_config
+        cap = max(1, min(g.max_recv_records, (g.max_recv_payload or g.max_recv_records * 256) // pad32(g.max_payload_bytes)))
+        off = snap["chunk_off"].astype(np.int64)
+        agents, counts, ent, snd, pay = snap["agents"], snap["counts"], snap["entries"], snap["sends"], snap["payload"]
+        seq_end = self._next_seq
+        for k in range(len(off) - 1):
+            a0, a1, e0 = off[k, 0], off[k + 1, 0], off[k, 1]
+            ca = counts[a0:a1].astype(np.int64)
+            if len(ca) and ca.max() > cap:
+                raise RuntimeError(f"snapshot agent with {int(ca.max())} records does not fit one restore call ({cap})")
+            first = e0 + np.concatenate([[0], np.cumsum(ca)])
+            i = 0
+            while i < len(ca):
+                j = i
+                while j < len(ca) and first[j + 1] - first[i] <= cap:
+                    j += 1
+                part_ent, part_snd, part_pay = _compact_rows(ent[first[i]:first[j]], snd, pay)
+                _, se = self.shard.restore_compact(agents[a0 + i:a0 + j], ca[i:j], part_ent, part_snd, part_pay)
+                seq_end = max(seq_end, se)
+                i = j
+        return seq_end
+
+    def load_queue_snapshot(self, path: Union[str, Path]) -> None:
+        """Put a snapshot written by save_queue_snapshot back into this instance, which must be fresh: the agents and
+        groups are re-created in the snapshot's index order, its id nonce is adopted (GpuConfig.id_nonce, when set, must
+        equal it) and every pending record is restored with its id, to be delivered as if it had never left."""
+        self._check_fresh()
+        snap = self._read_snapshot(path)
+        self._adopt_tables(snap)
+        seq_end = self._restore_chunks(snap)
+        self._next_seq = max(self._next_seq, seq_end); self._b_first_seq = self._next_seq
 
     # ------------------------------------------------------------------ LLM backends (M:1281-1325 + real balancer)
     def set_llm_load_balancing(self, enabled: bool = True) -> None:

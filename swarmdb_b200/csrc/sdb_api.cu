@@ -65,6 +65,10 @@ cudaError_t sdb_launch_wire_set(uint32_t*, uint32_t, cudaStream_t);
 cudaError_t sdb_launch_import_fused(const sdb_import2_args*, cudaStream_t, sdb_profiler*, int*);
 cudaError_t sdb_launch_import_place(const sdb_import_totals*, sdb_cursor*, sdb_batch_base*, unsigned long long, uint32_t, uint32_t*, cudaStream_t);
 cudaError_t sdb_launch_arena_floor_cur(const sdb_dev_view*, uint32_t, sdb_cursor*, cudaStream_t);
+cudaError_t sdb_launch_restore_plan(const sdb_dev_view*, const sdb_restore_args*, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_restore_write(const sdb_dev_view*, const sdb_restore_args*, unsigned long long, uint32_t, cudaStream_t,
+                                     sdb_profiler*, int*, int);
+const void* sdb_restore_kernel_anchor();
 }
 
 #define SDB_SCAN_TILE 4096u
@@ -182,6 +186,9 @@ struct sdb_ctx {
   uint32_t* where_bits = nullptr;                        // filtered receive: verdict bitmap [max_agents][ceil(R / 32)] ...
   uint8_t* where_kw = nullptr;                           // ... and the keyword [SDB_FILTER_MAX_KEYWORD], allocated on first use
   unsigned long long* digest = nullptr;                  // [max_agents] stream digests, allocated on first use
+  uint32_t* rs_agent = nullptr;                          // restore: per-agent tables [6][max_agents] + scan tops, allocated
+  unsigned long long* rs_tot = nullptr;                  // on first use; totals [8]
+  uint32_t* rs_sort = nullptr;                           // restore: radix-sort keys / values [4][max_recv_records] + digit tables
   // backends
   uint32_t* be_weight = nullptr; unsigned long long* be_load = nullptr; uint32_t n_backends = 0;
   uint32_t* be_req_cost = nullptr; uint32_t* be_out = nullptr; unsigned long long* be_scratch = nullptr;
@@ -260,7 +267,8 @@ cudaError_t load_all_kernels() {
     if (e != cudaSuccess) return e;
     if (q != cudaDriverEntryPointSuccess || !*fp) return cudaErrorNotSupported;
   }
-  for (const void* anchor : {sdb_send_kernel_anchor(), sdb_recv_kernel_anchor(), sdb_balance_kernel_anchor(), sdb_xshard_kernel_anchor()}) {
+  for (const void* anchor : {sdb_send_kernel_anchor(), sdb_recv_kernel_anchor(), sdb_balance_kernel_anchor(), sdb_xshard_kernel_anchor(),
+                              sdb_restore_kernel_anchor()}) {
     cudaFunction_t f = nullptr;
     cudaError_t e = cudaGetFuncBySymbol(&f, anchor);
     if (e != cudaSuccess) return e;
@@ -942,7 +950,8 @@ int sdb_destroy(sdb_handle h) {
                  h->rx_totals, h->rx_big_list, h->rx_big_count, h->rx_count, h->rx_hdr, h->rx_payload,
                  h->be_weight, h->be_load, h->be_scratch, h->be_logtab, h->be_req_cost, h->be_out, h->digest,
                  h->cx.table, h->cx.rec_slot, h->cx.head, h->cx.head_local, h->cx.head_tops, h->cx.gran, h->cx.gran_local,
-                 h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out, h->where_bits, h->where_kw};
+                 h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out, h->where_bits, h->where_kw,
+                 h->rs_agent, h->rs_tot, h->rs_sort};
   for (void* p : dev) if (p) cudaFree(p);
   if (h->descs_host) cudaFreeHost(h->descs_host);
   if (h->list_host) cudaFreeHost(h->list_host);
@@ -1939,6 +1948,106 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
     if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
+  return SDB_OK;
+}
+
+int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, const uint32_t* count,
+                        const sdb_recv_entry* entries, uint64_t n_entries, const sdb_recv_send* sends, uint64_t n_sends,
+                        const uint8_t* payload, uint64_t payload_bytes, uint32_t flags, uint64_t* restored_out,
+                        uint64_t* seq_end_out) {
+  if (!h) return SDB_EINVAL;
+  if (restored_out) *restored_out = 0;
+  { int rcc = cursor_to_host(h); if (rcc != SDB_OK) return rcc; }      // a host-placed write, like a send
+  if (seq_end_out) *seq_end_out = h->next_seq;
+  if (flags & ~SDB_RECV_OWNED) return fail(h, SDB_EINVAL, "sdb_restore_compact accepts SDB_RECV_OWNED only");
+  if (n_agents && (!agent_idx || !count)) return fail(h, SDB_EINVAL, "sdb_restore_compact: agent_idx and count are required");
+  if ((n_entries && !entries) || (n_sends && !sends) || (payload_bytes && !payload))
+    return fail(h, SDB_EINVAL, "sdb_restore_compact: null input array");
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
+  uint64_t sum = 0;
+  for (uint32_t i = 0; i < n_agents; ++i) sum += count[i];
+  if (sum != n_entries) return fail(h, SDB_EINVAL, "sdb_restore_compact: sum(count) != n_entries");
+  // one compact receive's capacity: the input is staged in its device buffers
+  const uint64_t P = pad32(h->cfg.max_payload_bytes);
+  const uint64_t rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / P);
+  if (n_entries > rec_cap || n_sends > rec_cap || payload_bytes > rec_cap * P)
+    return fail(h, SDB_ECAPACITY, "sdb_restore_compact: input larger than one compact receive's capacity");
+  if (n_agents == 0) return SDB_OK;
+  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  const size_t A = h->cfg.max_agents, tiles = A / SDB_SCAN_TILE + 2;
+  if (!h->rs_agent) {
+    { int rcl = ls_stop(h); if (rcl != SDB_OK) return rcl; }      // the allocations below may wait for running kernels
+    const size_t R = h->cfg.max_recv_records, H = 256 * (R / 1024 + 1);
+    if (dmalloc(&h->rs_sort, 4 * R + 2 * H + H / SDB_SCAN_TILE + 2) != cudaSuccess || dmalloc(&h->rs_tot, 8) != cudaSuccess ||
+        dmalloc(&h->rs_agent, 6 * A + tiles) != cudaSuccess) {
+      for (void* p : {static_cast<void*>(h->rs_sort), static_cast<void*>(h->rs_tot), static_cast<void*>(h->rs_agent)}) if (p) cudaFree(p);
+      h->rs_agent = nullptr; h->rs_sort = nullptr; h->rs_tot = nullptr;
+      cudaGetLastError();
+      return fail(h, SDB_ENOMEM, "restore: device allocation failed");
+    }
+  }
+  std::vector<uint32_t> first(n_agents);
+  { uint32_t run = 0; for (uint32_t i = 0; i < n_agents; ++i) { first[i] = run; run += count[i]; } }
+  sdb_restore_args r{};
+  uint32_t* t = h->rs_agent;
+  r.agent = t; r.count = t + A; r.first = t + 2 * A; r.nsh = t + 3 * A; r.pgran = t + 4 * A; r.p_local = t + 5 * A; r.p_tops = t + 6 * A;
+  const size_t n = n_agents;
+  CUDA_TRY(h, cudaMemcpyAsync(t, agent_idx, n * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(t + A, count, n * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(t + 2 * A, first.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  sdb_compact_args& c = h->cx;
+  if (n_entries) CUDA_TRY(h, cudaMemcpyAsync(c.entry_out, entries, n_entries * sizeof(sdb_recv_entry), cudaMemcpyHostToDevice, h->stream));
+  if (n_sends) CUDA_TRY(h, cudaMemcpyAsync(c.send_out, sends, n_sends * sizeof(sdb_recv_send), cudaMemcpyHostToDevice, h->stream));
+  if (payload_bytes) CUDA_TRY(h, cudaMemcpyAsync(c.payload_out, payload, payload_bytes, cudaMemcpyHostToDevice, h->stream));
+  r.ent = c.entry_out; r.snd = c.send_out; r.payload = c.payload_out; r.payload_bytes = payload_bytes;
+  r.n = n_agents; r.n_entries = static_cast<uint32_t>(n_entries); r.n_sends = static_cast<uint32_t>(n_sends);
+  r.max_payload = h->cfg.max_payload_bytes;
+  r.shared = h->shared_cfg ? 1u : 0u;
+  r.owned = (flags & SDB_RECV_OWNED) && h->sharded ? 1u : 0u; r.shard_id = h->cfg.shard_id; r.shard_of = h->shard_of_dev;
+  // scratch of the compact receive (max_recv_records entries each; the hash table holds >= 4 x that many words) and of
+  // the restore's radix sort
+  const size_t R = h->cfg.max_recv_records;
+  uint32_t* tw = reinterpret_cast<uint32_t*>(c.table);
+  r.e_row = c.rec_slot;
+  r.row_cnt = c.head; r.rc_local = c.head_local; r.rc_tops = c.head_tops;
+  r.row_gran = c.gran; r.rg_local = c.gran_local; r.rg_tops = c.gran_tops;
+  r.e_handle = tw; r.e_y = tw + R;
+  {
+    uint32_t* q = h->rs_sort;
+    const size_t H = 256 * (R / 1024 + 1);
+    r.key_a = q; r.key_b = q + R; r.val_a = q + 2 * R; r.val_b = q + 3 * R;
+    r.hist = q + 4 * R; r.h_local = q + 4 * R + H; r.h_tops = q + 4 * R + 2 * H;
+  }
+  r.tot = h->rs_tot;
+  int nl = 0;
+  cudaError_t e = sdb_launch_restore_plan(&h->view, &r, h->stream, &h->prof, &nl, h->sm_count);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("restore plan launch: ") + cudaGetErrorString(e));
+  unsigned long long tot[6];
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rs_tot, sizeof(tot), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  std::memcpy(tot, h->totals_host, sizeof(tot));
+  if (tot[3] & SDB_RS_EINVAL)
+    return fail(h, SDB_EINVAL, "sdb_restore_compact: bad entry (send index, receiver) or row (len, prio, payload_off)");
+  if (tot[3] & SDB_RS_ERING) return fail(h, SDB_ERING_OVERFLOW, "sdb_restore_compact: a ring cannot take the agent's records");
+  const uint64_t records = tot[4], need = tot[0] + tot[1];
+  if (records) {
+    uint64_t base = 0;
+    { const int rc = arena_reserve(h, need, &base); if (rc != SDB_OK) return rc; }
+    r.base = base;
+    nl = 0;
+    e = sdb_launch_restore_write(&h->view, &r, tot[0], static_cast<uint32_t>(tot[5]), h->stream, &h->prof, &nl, h->sm_count);
+    h->launches += nl;
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("restore write launch: ") + cudaGetErrorString(e));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    h->arena_tail = base + need;
+    if (tot[2] + 1 > h->next_seq) h->next_seq = tot[2] + 1;
+    h->dev_stale = true;
+  }
+  for (uint32_t i = 0; i < n_agents; ++i) h->n_agents = std::max(h->n_agents, agent_idx[i] + 1);
+  h->stream_busy = false;
+  if (restored_out) *restored_out = records;
+  if (seq_end_out) *seq_end_out = h->next_seq;
   return SDB_OK;
 }
 

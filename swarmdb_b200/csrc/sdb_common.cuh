@@ -195,6 +195,40 @@ struct sdb_where_args {
   uint32_t stride;             // words per agent = ceil(ring_slots / 32)
 };
 
+// arguments of one restore (sdb_restore_compact): the compact-format input staged in the compact receive's buffers, the
+// per-agent tables uploaded by the host, and scratch carved out of the compact receive's scratch (sdb_api.cu)
+struct sdb_restore_args {
+  const uint32_t* agent;           // [n] listed agents
+  const uint32_t* count;           // [n] entries of each
+  const uint32_t* first;           // [n] index of the agent's first entry (exclusive scan of count)
+  const sdb_recv_entry* ent;       // [n_entries]
+  const sdb_recv_send* snd;        // [n_sends]
+  const uint8_t* payload;          // [payload_bytes]
+  uint64_t payload_bytes;
+  uint32_t n, n_entries, n_sends, max_payload;
+  uint32_t shared;                 // 1: rows take the shared layout (headers + one payload); 0: every record is a private image
+  uint32_t owned, shard_id;        // owned: skip the agents whose shard_of[] is not shard_id
+  const uint8_t* shard_of;
+  uint32_t* nsh;                   // [n] entries in the agent's shared prefix (before its first row descent)
+  uint32_t* pgran;                 // [n] granules of the agent's private images, then its scan (p_local / p_tops)
+  uint32_t* p_local; uint32_t* p_tops;
+  uint32_t* e_row;                 // [n_entries] row of a shared entry, ~0 for private / skipped entries
+  uint32_t* row_cnt;               // [n_sends] shared entries per row, then its scan (rc_local / rc_tops): bucket base
+  uint32_t* rc_local; uint32_t* rc_tops;
+  uint32_t* row_gran;              // [n_sends] granules of the row's region, then its scan (rg_local / rg_tops): arena offset
+  uint32_t* rg_local; uint32_t* rg_tops;
+  uint32_t* key_a; uint32_t* key_b;  // [n_entries] stable radix sort of the entries by row (non-shared entries key n_sends) ...
+  uint32_t* val_a; uint32_t* val_b;  // ... carrying entry indices: afterwards row r's shared entries sit, in entry order, at
+                                     // [rc_local/rc_tops scan of r, + row_cnt[r])
+  uint32_t* hist; uint32_t* h_local; uint32_t* h_tops;   // [256 x sort tiles] digit counts per tile (digit-major) and scan
+  uint32_t* e_handle;              // [n_entries] arena handle of each shared entry's header ...
+  uint32_t* e_y;                   // ... and its ring entry's .y (meta | dm1 << 16)
+  unsigned long long* tot;         // [0] row granules [1] private granules [2] largest seq [3] error bits [4] records [5] shared
+  unsigned long long base;         // arena position of the region (write phase)
+};
+#define SDB_RS_EINVAL 1ull         // tot[3]: a bad entry or row
+#define SDB_RS_ERING 2ull          // tot[3]: some agent's ring cannot take its records
+
 // ---- asynchronous import (sdb_import_wire_ptrs_async): everything the host used to learn through a sync lives on
 // the device.  `sdb_cursor` is the device-resident twin of the host's arena / sequence counters (whoever advanced
 // them last marks the other side stale); `sdb_batch_base` carries one import's placement from the kernel that

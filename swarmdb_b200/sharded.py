@@ -718,6 +718,19 @@ class ShardedSwarmsDB(SwarmsDB):
             return None, RECV_OWNED
         return super()._expire_scope([a for a in agent_ids if self.owner(a) == self.rank])
 
+    # ---- queue snapshots and requeue: a sharded deployment needs per-rank files, owned-agent restores and the composite
+    # round moved past the restored ids; until that exists these refuse instead of restoring every agent on every rank
+    def save_queue_snapshot(self, path):
+        raise NotImplementedError("ShardedSwarmsDB does not write queue snapshots yet; a rank can restore its share of a "
+                                  "single-shard snapshot with Shard.restore_compact(..., RECV_OWNED)")
+
+    def load_queue_snapshot(self, path):
+        raise NotImplementedError("ShardedSwarmsDB does not load queue snapshots yet (see save_queue_snapshot)")
+
+    def requeue_batch_compact(self, counts, entries, sends, payload, agent_idx):
+        raise NotImplementedError("ShardedSwarmsDB does not requeue yet: restored ids must stay below the composite "
+                                  "sequence numbers of later rounds")
+
     def close(self) -> None:
         """Collective like flush(): every rank closes.  Buffered sends are NOT flushed here (a flush is a collective
         the caller schedules); the exchange's buffers are released only after their last reader is done."""
