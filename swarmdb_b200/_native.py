@@ -232,6 +232,14 @@ def pad32(n):
     return (n + 31) & ~31
 
 
+def recv_capacity(cfg) -> int:
+    """Records of the maximum size one receive call takes under `cfg` (a GpuConfig or SdbConfig):
+    min(max_recv_records, max_recv_payload / pad32(max_payload_bytes)), at least 1.  The library divides
+    max_recv_payload rounded up to 32 bytes, so it may allow a call more records than this, never fewer."""
+    payload = int(cfg.max_recv_payload) or int(cfg.max_recv_records) * 256
+    return max(1, min(int(cfg.max_recv_records), payload // pad32(int(cfg.max_payload_bytes))))
+
+
 # kernel variant used when the caller does not choose one (SDB_FANOUT_VARIANT overrides, for A/B runs)
 DEFAULT_FANOUT_VARIANT = int(os.environ.get("SDB_FANOUT_VARIANT", "2"))
 
@@ -514,13 +522,7 @@ class Shard:
             if copy_out:
                 raise ValueError("wait=False needs copy_out=False")
             flags |= RECV_ASYNC
-        if agents is None:
-            a, n = None, 0
-            counts = np.zeros(self.max_agents, np.uint32) if copy_out else None
-        else:
-            a = _arr(agents, np.uint32)
-            n = len(a)
-            counts = np.zeros(n, np.uint32) if copy_out else None
+        a, n, counts = self._agents_arg(agents, copy_out)
         total, pbytes = C.c_uint64(0), C.c_uint64(0)
         hdr = pay = None
         hdr_cap = pay_cap = 0
@@ -536,8 +538,7 @@ class Shard:
         if not copy_out:
             return None, total.value, pbytes.value
         if agents is None:
-            owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
-            counts = counts[: self.n_owned if owned else self.stats_n_agents()]
+            counts = self._served_counts(counts, flags)
         return counts, hdr[: total.value], pay[: pbytes.value]
 
     def receive_compact(self, agents, max_messages: int, flags: int = 0, out_entries: Optional[np.ndarray] = None,
@@ -546,28 +547,15 @@ class Shard:
         sdb_receive_compact): (counts[n_agents], entries[total] ENTRY_DTYPE, sends[n_sends] SEND_DTYPE, payload bytes),
         each distinct payload once.  Views into reusable buffers unless explicit (e.g. pinned) arrays are given;
         expand_compact() turns them into receive_batch's (headers, payload)."""
-        if agents is None:
-            a, n = None, 0
-            counts = np.zeros(self.max_agents, np.uint32)
-        else:
-            a = _arr(agents, np.uint32)
-            n = len(a)
-            counts = np.zeros(n, np.uint32)
-        if out_entries is None or out_sends is None:
-            cur = getattr(self, "_out_ent", None)
-            if cur is None or len(cur[0]) < self.max_recv_records:
-                self._out_ent = (np.zeros(self.max_recv_records, ENTRY_DTYPE), np.zeros(self.max_recv_records, SEND_DTYPE))
-        ent = out_entries if out_entries is not None else self._out_ent[0]
-        snd = out_sends if out_sends is not None else self._out_ent[1]
-        pay = out_payload if out_payload is not None else self._grow_pay()
+        a, n, counts = self._agents_arg(agents)
+        ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
         total, n_sends, pbytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
         self._check(self._L.sdb_receive_compact(self._h, n, _p(a), max_messages, flags, _p(counts), _p(ent), len(ent),
                                                 _p(snd), len(snd), _p(pay), pay.nbytes,
                                                 C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
                                                 C.cast(C.byref(pbytes), C.c_void_p)))
         if agents is None:
-            owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
-            counts = counts[: self.n_owned if owned else self.stats_n_agents()]
+            counts = self._served_counts(counts, flags)
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
 
     def restore_compact(self, agents, counts, entries, sends, payload, flags: int = 0) -> Tuple[int, int]:
@@ -592,31 +580,18 @@ class Shard:
         (include/swarmdb_b200.h: sdb_expire).  archive=True returns the expired records in receive_compact's shape,
         (counts, entries, sends, payload) - what does not fit stays queued, so loop until no entry comes back;
         archive=False drops them on the device and returns (counts, total)."""
-        if agents is None:
-            a, n = None, 0
-            counts = np.zeros(self.max_agents, np.uint32)
-        else:
-            a = _arr(agents, np.uint32)
-            n = len(a)
-            counts = np.zeros(n, np.uint32)
+        a, n, counts = self._agents_arg(agents)
         total, n_sends, pbytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
         ent = snd = pay = None
         if archive:
-            if out_entries is None or out_sends is None:
-                cur = getattr(self, "_out_ent", None)
-                if cur is None or len(cur[0]) < self.max_recv_records:
-                    self._out_ent = (np.zeros(self.max_recv_records, ENTRY_DTYPE), np.zeros(self.max_recv_records, SEND_DTYPE))
-            ent = out_entries if out_entries is not None else self._out_ent[0]
-            snd = out_sends if out_sends is not None else self._out_ent[1]
-            pay = out_payload if out_payload is not None else self._grow_pay()
+            ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
         self._check(self._L.sdb_expire(self._h, n, _p(a), float(older_than), flags, _p(counts),
                                        _p(ent), 0 if ent is None else len(ent), _p(snd), 0 if snd is None else len(snd),
                                        _p(pay), 0 if pay is None else pay.nbytes,
                                        C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
                                        C.cast(C.byref(pbytes), C.c_void_p)))
         if agents is None:
-            owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
-            counts = counts[: self.n_owned if owned else self.stats_n_agents()]
+            counts = self._served_counts(counts, flags)
         if not archive:
             return counts, int(total.value)
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
@@ -629,13 +604,7 @@ class Shard:
         comes back.  drop=True retires the matches on the device without returning them: (counts, total)."""
         if filt is None:
             filt = make_filter()
-        if agents is None:
-            a, n = None, 0
-            counts = np.zeros(self.max_agents, np.uint32)
-        else:
-            a = _arr(agents, np.uint32)
-            n = len(a)
-            counts = np.zeros(n, np.uint32)
+        a, n, counts = self._agents_arg(agents)
         total, pbytes = C.c_uint64(0), C.c_uint64(0)
         hdr = pay = None
         if drop:
@@ -647,8 +616,7 @@ class Shard:
                                               0 if hdr is None else len(hdr), _p(pay), 0 if pay is None else pay.nbytes,
                                               C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(pbytes), C.c_void_p)))
         if agents is None:
-            owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
-            counts = counts[: self.n_owned if owned else self.stats_n_agents()]
+            counts = self._served_counts(counts, flags)
         if drop:
             return counts, int(total.value)
         return counts, hdr[: total.value], pay[: pbytes.value]
@@ -715,6 +683,29 @@ class Shard:
         if self._out_pay.nbytes < need:
             self._out_pay = np.zeros(need, np.uint8)
         return self._out_pay
+
+    def _compact_outputs(self, out_entries, out_sends, out_payload):
+        """(entries, sends, payload) output arrays of a compact-format call: the caller's, else reusable buffers."""
+        if out_entries is None or out_sends is None:
+            cur = getattr(self, "_out_ent", None)
+            if cur is None or len(cur[0]) < self.max_recv_records:
+                self._out_ent = (np.zeros(self.max_recv_records, ENTRY_DTYPE), np.zeros(self.max_recv_records, SEND_DTYPE))
+        return (out_entries if out_entries is not None else self._out_ent[0],
+                out_sends if out_sends is not None else self._out_ent[1],
+                out_payload if out_payload is not None else self._grow_pay())
+
+    def _agents_arg(self, agents, with_counts: bool = True):
+        """(agent array or None, n_agents, zeroed counts) of a receive-family call; None means every agent."""
+        if agents is None:
+            return None, 0, np.zeros(self.max_agents, np.uint32) if with_counts else None
+        a = _arr(agents, np.uint32)
+        return a, len(a), np.zeros(len(a), np.uint32) if with_counts else None
+
+    def _served_counts(self, counts, flags: int):
+        """counts of a call without an agent list, cut to the agents it served: this shard's own with RECV_OWNED on a
+        sharded handle, else every agent below the registration watermark."""
+        owned = (flags & RECV_OWNED) and getattr(self, "n_owned", None) is not None
+        return counts[: self.n_owned if owned else self.stats_n_agents()]
 
     def last_receive_dev(self) -> Tuple[int, int, int]:
         c, h, p = C.c_void_p(), C.c_void_p(), C.c_void_p()

@@ -39,7 +39,7 @@ from pydantic import BaseModel, Field
 
 from . import _native
 from ._native import (EXPIRE_ALL, FILTER_MAX_KEYWORD, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON,
-                      SdbError, Shard, make_filter, pad32)
+                      SdbError, Shard, make_filter, pad32, recv_capacity)
 
 
 class RingOverflow(SdbError):
@@ -804,9 +804,7 @@ class SwarmsDB:
         each) fit one receive call.  A call holds min(max_recv_records, max_recv_payload / padded payload) records and
         leaves out whole agents beyond that; a PEEK consumes nothing, so a fixed chunking would silently skip them.  The
         parts are packed from the agents' pending counts instead (one device query)."""
-        g = self.gpu_config
-        max_recv_payload = g.max_recv_payload or g.max_recv_records * 256
-        cap = max(1, min(g.max_recv_records, max_recv_payload // pad32(g.max_payload_bytes)))
+        cap = recv_capacity(self.gpu_config)
         if len(agents) == 0:
             return
         pending = np.minimum(self.shard.agent_loads(agents)["pending"][: len(agents)].astype(np.int64), per_agent)
@@ -908,7 +906,7 @@ class SwarmsDB:
         is not written."""
         self.flush()
         g = self.gpu_config
-        cap = max(1, min(g.max_recv_records, (g.max_recv_payload or g.max_recv_records * 256) // pad32(g.max_payload_bytes)))
+        cap = recv_capacity(g)
         agents = np.arange(len(self._agent_name), dtype=np.uint32)
         parts: List[Tuple[np.ndarray, ...]] = []
         if len(agents):
@@ -987,8 +985,7 @@ class SwarmsDB:
     def _restore_chunks(self, snap: Dict[str, np.ndarray]) -> int:
         """Restore every chunk of a snapshot, split by whole agents where this instance's receive capacity is smaller;
         returns the largest sequence number + 1 seen."""
-        g = self.gpu_config
-        cap = max(1, min(g.max_recv_records, (g.max_recv_payload or g.max_recv_records * 256) // pad32(g.max_payload_bytes)))
+        cap = recv_capacity(self.gpu_config)
         off = snap["chunk_off"].astype(np.int64)
         agents, counts, ent, snd, pay = snap["agents"], snap["counts"], snap["entries"], snap["sends"], snap["payload"]
         seq_end = self._next_seq

@@ -96,6 +96,18 @@ struct sdb_staged {
 // group batches at least this large build ring entries with the agent-parallel pull kernel
 static const uint64_t SDB_PULL_THRESHOLD = 16384;
 
+// slots of the receive totals: rx_totals on the device and its pinned host mirror totals_host
+enum : uint32_t {
+  TOT_RECORDS = 0,            // records delivered
+  TOT_GRANULES = 1,           // payload granules delivered
+  TOT_FLOOR = 2,              // arena reclaim: granules from the oldest pending record to the tail
+  TOT_IMPORT_GRANULES = 4,    // import: arena granules of the batch
+  TOT_IMPORT_OWNED = 5,       // import: recipients this shard owns
+  TOT_CX_SENDS = 6,           // compact receive: rows (host mirror of cx.totals[0])
+  TOT_CX_GRANULES = 7,        // compact receive: payload granules (host mirror of cx.totals[1])
+  TOT_SLOTS = 8
+};
+
 struct sdb_ctx {
   sdb_config cfg{};
   int sm_count = 132;
@@ -171,7 +183,7 @@ struct sdb_ctx {
   uint32_t* rx_plan_tops = nullptr; unsigned long long* rx_totals = nullptr;
   uint32_t* rx_big_list = nullptr; uint32_t* rx_big_count = nullptr;
   uint32_t* rx_count = nullptr; sdb_msg_header* rx_hdr = nullptr; uint8_t* rx_payload = nullptr;
-  unsigned long long* totals_host = nullptr;   // pinned [4]
+  unsigned long long* totals_host = nullptr;   // pinned [TOT_SLOTS]
   uint8_t* rx_small = nullptr;                 // device output block of the latency path
   uint8_t* small_host = nullptr;               // pinned mirror
   uint64_t small_bytes = 0;
@@ -249,6 +261,22 @@ int ls_stop(sdb_ctx* h) {
   CUDA_TRY(h, cudaStreamSynchronize(h->ls_stream));
   h->ls_running = false;
   return SDB_OK;
+}
+// one device buffer of a set allocated on first use: where its pointer goes and how many elements it holds
+struct dbuf {
+  void** p; size_t bytes;
+  template <typename T> dbuf(T** q, size_t n) : p(reinterpret_cast<void**>(q)), bytes(n * sizeof(T)) {}
+};
+// Allocates a set of device buffers on first use, in order.  The latency server is stopped first (an allocation may wait
+// for the kernels running on the device), and a set that cannot be allocated whole is freed again: SDB_ENOMEM, `what`.
+int dmalloc_set(sdb_ctx* h, std::initializer_list<dbuf> set, const char* what) {
+  { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }
+  bool ok = true;
+  for (const dbuf& b : set) ok = ok && cudaMalloc(b.p, b.bytes) == cudaSuccess;
+  if (ok) return SDB_OK;
+  for (const dbuf& b : set) { if (*b.p) cudaFree(*b.p); *b.p = nullptr; }
+  cudaGetLastError();
+  return fail(h, SDB_ENOMEM, what);
 }
 // Under lazy module loading (the CUDA 12 default) the first launch of a kernel loads its code into the context, and that
 // load waits for the kernels running there: with the persistent latency server running it would wait forever.  So every
@@ -344,13 +372,13 @@ int arena_reserve(sdb_ctx* h, uint64_t need, uint64_t* base_out) {
   if (tail + need - h->arena_floor > G) {
     // reclaim: recompute the floor from the oldest pending record of every ring
     cudaError_t e = sdb_launch_arena_floor(&h->view, h->n_agents, static_cast<uint32_t>(h->arena_tail),
-                                           h->rx_totals + 2, h->stream);
+                                           h->rx_totals + TOT_FLOOR, h->stream);
     h->launches += 1;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h->totals_host + 2, h->rx_totals + 2, sizeof(unsigned long long),
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->totals_host + TOT_FLOOR, h->rx_totals + TOT_FLOOR, sizeof(unsigned long long),
                                              cudaMemcpyDeviceToHost, h->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
     if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("arena floor: ") + cudaGetErrorString(e));
-    h->arena_floor = h->arena_tail - h->totals_host[2];
+    h->arena_floor = h->arena_tail - h->totals_host[TOT_FLOOR];
     if (tail + need - h->arena_floor > G)
       return fail(h, SDB_EARENA_FULL, "message arena full: unconsumed messages pin the log (receive or enlarge arena_bytes)");
   }
@@ -847,14 +875,14 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
   CUDA_TRY(h, dmalloc(&h->rx_plan, c.max_recv_records + 4)); CUDA_TRY(h, dmalloc(&h->rx_rec_off, A));
   CUDA_TRY(h, dmalloc(&h->rx_plan_tops, rtiles));
   CUDA_TRY(h, dmalloc(&h->rx_lb, sdb_lb_words(static_cast<uint32_t>(A / 64 + 2)) + 4));
-  CUDA_TRY(h, dmalloc(&h->rx_totals, 8));
+  CUDA_TRY(h, dmalloc(&h->rx_totals, TOT_SLOTS));
   CUDA_TRY(h, dmalloc(&h->rx_big_list, A)); CUDA_TRY(h, dmalloc(&h->rx_big_count, 4));
   CUDA_TRY(h, dmalloc(&h->rx_count, A));
   CUDA_TRY(h, dmalloc(&h->rx_hdr, c.max_recv_records));
   h->pay_cap_gran = (c.max_recv_payload + SDB_GRANULE - 1) / SDB_GRANULE;
   if (h->pay_cap_gran >= 0x7FFFFFF0ull) return fail(h, SDB_EINVAL, "max_recv_payload too large (< 64 GiB per call)");
   CUDA_TRY(h, dmalloc(&h->rx_payload, h->pay_cap_gran * SDB_GRANULE));
-  CUDA_TRY(h, cudaHostAlloc(reinterpret_cast<void**>(&h->totals_host), 8 * sizeof(unsigned long long), cudaHostAllocDefault));
+  CUDA_TRY(h, cudaHostAlloc(reinterpret_cast<void**>(&h->totals_host), TOT_SLOTS * sizeof(unsigned long long), cudaHostAllocDefault));
   h->small_bytes = 64 + 1024ull * (32 + pad32(c.max_payload_bytes));
   CUDA_TRY(h, dmalloc(&h->rx_small, h->small_bytes));
   CUDA_TRY(h, cudaHostAlloc(reinterpret_cast<void**>(&h->small_host), h->small_bytes, cudaHostAllocDefault));
@@ -1334,15 +1362,16 @@ int sdb_import_wire_ptrs(sdb_handle h, uint32_t n_src, const void* const* wire_p
   a.tmp_list = h->scratch.list_dev; a.list_cap = static_cast<uint32_t>(std::min<uint64_t>(h->cfg.list_pool_entries, 0xFFFFFFFFull));
   int nl = 0;
   cudaError_t e = sdb_launch_import_measure(&a, n_cap, h->xs_w_local, h->xs_w_tops, h->xs_gs_local, h->xs_gs_tops,
-                                            h->xs_gs_cur /* goff */, h->xs_lw_local, h->xs_lw_tops, h->rx_totals + 4, h->stream, &h->prof, &nl);
+                                            h->xs_gs_cur /* goff */, h->xs_lw_local, h->xs_lw_tops, h->rx_totals + TOT_IMPORT_GRANULES, h->stream, &h->prof, &nl);
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("import measure: ") + cudaGetErrorString(e));
   // the host needs the arena footprint and the sequence numbers consumed: one small sync
-  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host + 4, h->rx_totals + 4, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host + TOT_IMPORT_GRANULES, h->rx_totals + TOT_IMPORT_GRANULES, 2 * sizeof(unsigned long long),
+                              cudaMemcpyDeviceToHost, h->stream));
   for (uint32_t k = 0; k < n_src; ++k)
     CUDA_TRY(h, cudaMemcpyAsync(h->hdrs_host + k, wire_ptrs[k], sizeof(sdb_wire_header), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   uint64_t total_recs = 0, n_other = 0, explicit_end = 0; uint32_t max_padlen = 0;
-  if (h->totals_host[5] > a.list_cap) return fail(h, SDB_ECAPACITY, "owned recipients of this import exceed list_pool_entries");
+  if (h->totals_host[TOT_IMPORT_OWNED] > a.list_cap) return fail(h, SDB_ECAPACITY, "owned recipients of this import exceed list_pool_entries");
   for (uint32_t s = 0; s < n_src; ++s) {
     const sdb_wire_header& wh = h->hdrs_host[s];
     n_other += wh.n_other;
@@ -1351,7 +1380,7 @@ int sdb_import_wire_ptrs(sdb_handle h, uint32_t n_src, const void* const* wire_p
     if (wh.n_sends > h->cfg.max_batch_sends) return fail(h, SDB_ECAPACITY, "wire batch larger than max_batch_sends");
     total_recs += wh.total_recs; max_padlen = std::max(max_padlen, wh.max_padlen);
   }
-  const uint64_t total_grans = h->totals_host[4];
+  const uint64_t total_grans = h->totals_host[TOT_IMPORT_GRANULES];
   uint64_t base = 0;
   int rc = arena_reserve(h, total_grans, &base);
   if (rc != SDB_OK) return rc;
@@ -1707,23 +1736,102 @@ static int check_recv_agents(sdb_ctx* h, uint32_t n_agents, const uint32_t* agen
   return SDB_OK;
 }
 
+// Without a list a receive serves every agent below the registration watermark, or, with SDB_RECV_OWNED on a sharded
+// handle, the agents this shard owns; returns whether it serves the owned agents.
+static bool recv_agents(const sdb_ctx* h, uint32_t flags, const uint32_t* agent_idx, uint32_t* n_agents) {
+  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
+  if (!agent_idx) *n_agents = owned ? h->n_owned : h->n_agents;
+  return owned;
+}
+
+// Record capacity of one receive call, the same on every path: the device buffers hold this many records of the maximum
+// size (what does not fit stays queued: include/swarmdb_b200.h).
+static uint64_t recv_rec_cap(const sdb_ctx* h) {
+  return std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / pad32(h->cfg.max_payload_bytes));
+}
+// room of an optional caller buffer: no bound when it is not given
+static uint64_t room(const void* buf, uint64_t cap) { return buf ? cap : ~0ull; }
+// ... and bounded by the caller's buffers: `rec_room` records in each record array, `payload_room` payload bytes
+static int out_rec_cap(sdb_ctx* h, uint64_t rec_room, uint64_t payload_room, uint64_t* rec_cap) {
+  *rec_cap = std::min({recv_rec_cap(h), rec_room, payload_room / pad32(h->cfg.max_payload_bytes)});
+  if (*rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  return SDB_OK;
+}
+
+// The arguments of a receive over the handle's receive scratch and device outputs, after the agent list (if any) is
+// uploaded to rx_agent.  Callers override what their call uses differently.
+static int recv_args(sdb_ctx* h, uint32_t n_agents, const uint32_t* agent_idx, bool owned, uint32_t max_messages,
+                     uint32_t flags, uint64_t rec_cap, sdb_recv_args* out) {
+  if (agent_idx) {
+    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  }
+  sdb_recv_args r{};
+  r.agent_idx = agent_idx ? h->rx_agent : (owned ? h->owned_dev : nullptr); r.n = n_agents; r.max_messages = max_messages;
+  r.flags = flags;
+  r.cnt = h->rx_cnt; r.rec_local = h->rx_rec_local; r.rec_tops = h->rx_rec_tops;
+  r.rec_off = h->rx_rec_off; r.plan = h->rx_plan; r.lb = h->rx_lb;
+  r.plan_tops = h->rx_plan_tops; r.totals = h->rx_totals; r.big_list = h->rx_big_list; r.big_count = h->rx_big_count;
+  r.count_out = h->rx_count; r.hdr_out = h->rx_hdr; r.payload_out = h->rx_payload;
+  r.rec_cap = rec_cap;
+  *out = r;
+  return SDB_OK;
+}
+
+// Full-format results to the caller: totals and counts, one synchronisation, then headers and payload and, if any was
+// asked for, a second one.
+static int copy_full(sdb_ctx* h, uint32_t n_agents, uint32_t* count_out, sdb_msg_header* hdr_out, uint8_t* payload_out,
+                     uint64_t* total_out, uint64_t* payload_bytes_out) {
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  if (count_out)
+    CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  const uint64_t total = h->totals_host[TOT_RECORDS], pbytes = h->totals_host[TOT_GRANULES] * SDB_GRANULE;
+  if (total_out) *total_out = total;
+  if (payload_bytes_out) *payload_bytes_out = pbytes;
+  if (total) {
+    if (hdr_out) CUDA_TRY(h, cudaMemcpyAsync(hdr_out, h->rx_hdr, total * sizeof(sdb_msg_header), cudaMemcpyDeviceToHost, h->stream));
+    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->rx_payload, pbytes, cudaMemcpyDeviceToHost, h->stream));
+    if (hdr_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return SDB_OK;
+}
+
+// Compact-format results to the caller: totals, the compact totals and counts, one synchronisation, then entries, sends
+// and payload and, if any was asked for, a second one.
+static int copy_compact(sdb_ctx* h, uint32_t n_agents, uint32_t* count_out, sdb_recv_entry* entry_out, sdb_recv_send* send_out,
+                        uint8_t* payload_out, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host + TOT_CX_SENDS, h->cx.totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  if (count_out)
+    CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  const uint64_t total = h->totals_host[TOT_RECORDS], n_sends = h->totals_host[TOT_CX_SENDS];
+  const uint64_t pbytes = h->totals_host[TOT_CX_GRANULES] * SDB_GRANULE;
+  if (total_out) *total_out = total;
+  if (n_sends_out) *n_sends_out = n_sends;
+  if (payload_bytes_out) *payload_bytes_out = pbytes;
+  if (total) {
+    if (entry_out) CUDA_TRY(h, cudaMemcpyAsync(entry_out, h->cx.entry_out, total * sizeof(sdb_recv_entry), cudaMemcpyDeviceToHost, h->stream));
+    if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
+    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
+    if (entry_out || send_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return SDB_OK;
+}
+
 int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
                       uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
                       uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
   if (!h) return SDB_EINVAL;
   if (total_out) *total_out = 0;
   if (payload_bytes_out) *payload_bytes_out = 0;
-  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
-  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
+  const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
   if (n_agents == 0 || max_messages == 0) return SDB_OK;
   { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
-  // record capacity of the call, the same on every path: the device buffers and the caller's buffers must each hold
-  // rec_cap records of the maximum size (what does not fit stays queued: include/swarmdb_b200.h)
-  const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
-  uint64_t rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
-  if (hdr_out) rec_cap = std::min<uint64_t>(rec_cap, hdr_cap);
-  if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
-  if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  uint64_t rec_cap = 0;
+  { const int rc = out_rec_cap(h, room(hdr_out, hdr_cap), room(payload_out, payload_cap), &rec_cap); if (rc != SDB_OK) return rc; }
   // ---- latency path: few agents, host outputs -> one launch, one D2H, one sync
   if (agent_idx && n_agents <= 8 && hdr_out && payload_out &&
       static_cast<uint64_t>(n_agents) * max_messages <= 1024) {
@@ -1733,7 +1841,7 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
     if (h->ls_wanted && n_agents == 1) {
       { int rcl = ls_start(h); if (rcl != SDB_OK) return rcl; }
       const uint64_t want = std::min<uint64_t>(max_messages, rec_cap);
-      served = 64ull + want * (32 + max_rec_bytes) <= h->ls_out_cap;      // the whole answer must fit the pinned block
+      served = 64ull + want * (32 + pad32(h->cfg.max_payload_bytes)) <= h->ls_out_cap;   // the whole answer must fit the pinned block
     }
     if (served) {
       // ---- the persistent server: post the request in mapped pinned memory, read the answer from pinned memory
@@ -1768,19 +1876,11 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
     (void)total;
     return SDB_OK;
   }
-  if (agent_idx) {
-    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
-  }
+  sdb_recv_args r{};
+  { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK), rec_cap, &r);
+    if (rc != SDB_OK) return rc; }
   const bool async = (flags & SDB_RECV_ASYNC) != 0;
   if (async && (count_out || hdr_out || payload_out)) return fail(h, SDB_EINVAL, "SDB_RECV_ASYNC takes no host output buffers");
-  sdb_recv_args r{};
-  r.agent_idx = agent_idx ? h->rx_agent : (owned ? h->owned_dev : nullptr); r.n = n_agents; r.max_messages = max_messages;
-  r.flags = flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK);
-  r.cnt = h->rx_cnt; r.rec_local = h->rx_rec_local; r.rec_tops = h->rx_rec_tops;
-  r.rec_off = h->rx_rec_off; r.plan = h->rx_plan; r.lb = h->rx_lb;
-  r.plan_tops = h->rx_plan_tops; r.totals = h->rx_totals; r.big_list = h->rx_big_list; r.big_count = h->rx_big_count;
-  r.count_out = h->rx_count; r.hdr_out = h->rx_hdr; r.payload_out = h->rx_payload;
-  r.rec_cap = rec_cap;
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
                                      nullptr);
@@ -1788,47 +1888,22 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   if (!(r.flags & SDB_RECV_PRIORITY)) r.plan_tops = nullptr;       // single-pass path: plan offsets are absolute
   h->last_rx = r; h->last_rx_valid = (e == cudaSuccess); h->last_rx_compact = false;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("receive launch: ") + cudaGetErrorString(e));
-  h->stream_busy = async;
-  if (async) return SDB_OK;          // the caller consumes on the device (stream order) or asks sdb_last_receive_totals later
-  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
-  if (count_out)
-    CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  const uint64_t total = h->totals_host[0], pbytes = h->totals_host[1] * SDB_GRANULE;
-  if (total_out) *total_out = total;
-  if (payload_bytes_out) *payload_bytes_out = pbytes;
-  if (total) {
-    if (hdr_out) CUDA_TRY(h, cudaMemcpyAsync(hdr_out, h->rx_hdr, total * sizeof(sdb_msg_header), cudaMemcpyDeviceToHost, h->stream));
-    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->rx_payload, pbytes, cudaMemcpyDeviceToHost, h->stream));
-    if (hdr_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  }
-  return SDB_OK;
+  if (async) { h->stream_busy = true; return SDB_OK; }   // the caller consumes on the device (stream order) or asks sdb_last_receive_totals later
+  return copy_full(h, n_agents, count_out, hdr_out, payload_out, total_out, payload_bytes_out);
 }
 
 // compact receive scratch and outputs, sized for max_recv_records; allocated once, on the first compact call
 static int compact_ensure(sdb_ctx* h) {
   sdb_compact_args& c = h->cx;
   if (c.table) return SDB_OK;
-  { int rcl = ls_stop(h); if (rcl != SDB_OK) return rcl; }      // the allocations below may wait for running kernels
   const size_t R = h->cfg.max_recv_records, tiles = (R + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE + 1;
   uint32_t tbits = 10;
   while ((1ull << tbits) < 2 * R) ++tbits;
-  const bool ok = dmalloc(&c.rec_slot, R) == cudaSuccess && dmalloc(&c.head, R) == cudaSuccess &&
-                  dmalloc(&c.head_local, R) == cudaSuccess && dmalloc(&c.head_tops, tiles) == cudaSuccess &&
-                  dmalloc(&c.gran, R) == cudaSuccess && dmalloc(&c.gran_local, R) == cudaSuccess &&
-                  dmalloc(&c.gran_tops, tiles) == cudaSuccess && dmalloc(&c.totals, 2) == cudaSuccess &&
-                  dmalloc(&c.entry_out, R) == cudaSuccess && dmalloc(&c.send_out, R) == cudaSuccess &&
-                  dmalloc(&c.payload_out, h->pay_cap_gran * SDB_GRANULE) == cudaSuccess &&
-                  dmalloc(&c.table, static_cast<size_t>(1) << tbits) == cudaSuccess;   // last: marks the set complete
-  if (!ok) {
-    void* p[] = {c.table, c.rec_slot, c.head, c.head_local, c.head_tops, c.gran, c.gran_local, c.gran_tops, c.totals,
-                 c.entry_out, c.send_out, c.payload_out};
-    for (void* q : p) if (q) cudaFree(q);
-    c = sdb_compact_args{};
-    cudaGetLastError();
-    return fail(h, SDB_ENOMEM, "compact receive: device allocation failed");
-  }
-  return SDB_OK;
+  return dmalloc_set(h, {{&c.rec_slot, R}, {&c.head, R}, {&c.head_local, R}, {&c.head_tops, tiles}, {&c.gran, R},
+                         {&c.gran_local, R}, {&c.gran_tops, tiles}, {&c.totals, 2}, {&c.entry_out, R}, {&c.send_out, R},
+                         {&c.payload_out, h->pay_cap_gran * SDB_GRANULE},
+                         {&c.table, static_cast<size_t>(1) << tbits}},          // last: marks the set complete
+                     "compact receive: device allocation failed");
 }
 
 int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
@@ -1840,52 +1915,24 @@ int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
   if (n_sends_out) *n_sends_out = 0;
   if (payload_bytes_out) *payload_bytes_out = 0;
   if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_compact returns host results: SDB_RECV_ASYNC is not accepted");
-  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
-  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
+  const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
   if (n_agents == 0 || max_messages == 0) return SDB_OK;
   { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
-  // the same record capacity as sdb_receive_batch: rec_cap unshared records of the maximum size fit every buffer
-  const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
-  uint64_t rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
-  if (entry_out) rec_cap = std::min<uint64_t>(rec_cap, entry_cap);
-  if (send_out) rec_cap = std::min<uint64_t>(rec_cap, send_cap);
-  if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
-  if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  // sdb_receive_batch's capacity: rec_cap unshared records of the maximum size fit every buffer
+  uint64_t rec_cap = 0;
+  { const int rc = out_rec_cap(h, std::min(room(entry_out, entry_cap), room(send_out, send_cap)), room(payload_out, payload_cap), &rec_cap);
+    if (rc != SDB_OK) return rc; }
   { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
-  if (agent_idx) {
-    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
-  }
   sdb_recv_args r{};
-  r.agent_idx = agent_idx ? h->rx_agent : (owned ? h->owned_dev : nullptr); r.n = n_agents; r.max_messages = max_messages;
-  r.flags = flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK);
-  r.cnt = h->rx_cnt; r.rec_local = h->rx_rec_local; r.rec_tops = h->rx_rec_tops;
-  r.rec_off = h->rx_rec_off; r.plan = h->rx_plan; r.lb = h->rx_lb;
-  r.plan_tops = h->rx_plan_tops; r.totals = h->rx_totals; r.big_list = h->rx_big_list; r.big_count = h->rx_big_count;
-  r.count_out = h->rx_count; r.hdr_out = h->rx_hdr; r.payload_out = h->rx_payload;
-  r.rec_cap = rec_cap;
+  { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK), rec_cap, &r);
+    if (rc != SDB_OK) return rc; }
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
                                      &h->cx);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = true;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("compact receive launch: ") + cudaGetErrorString(e));
-  h->stream_busy = false;
-  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host + 6, h->cx.totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
-  if (count_out)
-    CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  const uint64_t total = h->totals_host[0], n_sends = h->totals_host[6], pbytes = h->totals_host[7] * SDB_GRANULE;
-  if (total_out) *total_out = total;
-  if (n_sends_out) *n_sends_out = n_sends;
-  if (payload_bytes_out) *payload_bytes_out = pbytes;
-  if (total) {
-    if (entry_out) CUDA_TRY(h, cudaMemcpyAsync(entry_out, h->cx.entry_out, total * sizeof(sdb_recv_entry), cudaMemcpyDeviceToHost, h->stream));
-    if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
-    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
-    if (entry_out || send_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  }
-  return SDB_OK;
+  return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
 }
 
 int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, double older_than, uint32_t flags,
@@ -1898,56 +1945,33 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
   if (payload_bytes_out) *payload_bytes_out = 0;
   if (flags & ~(SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_EXPIRE_ALL))
     return fail(h, SDB_EINVAL, "sdb_expire accepts SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_EXPIRE_ALL only");
-  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
-  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
+  const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
   const bool archive = entry_out || send_out || payload_out;
   uint64_t rec_cap = 0;
-  if (archive) {
-    // the capacity rule of sdb_receive_compact: rec_cap unshared records of the maximum size fit every buffer
-    const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
-    rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
-    if (entry_out) rec_cap = std::min<uint64_t>(rec_cap, entry_cap);
-    if (send_out) rec_cap = std::min<uint64_t>(rec_cap, send_cap);
-    if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
-    if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  if (archive) {      // sdb_receive_compact's capacity rule
+    const int rc = out_rec_cap(h, std::min(room(entry_out, entry_cap), room(send_out, send_cap)), room(payload_out, payload_cap), &rec_cap);
+    if (rc != SDB_OK) return rc;
   }
   if (n_agents == 0) return SDB_OK;
   { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
   if (archive) { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
-  if (agent_idx) {
-    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
-  }
   sdb_recv_args r{};
-  r.agent_idx = agent_idx ? h->rx_agent : (owned ? h->owned_dev : nullptr); r.n = n_agents;
-  r.flags = flags & SDB_RECV_PEEK;
-  r.cnt = h->rx_cnt; r.rec_local = h->rx_rec_local; r.rec_tops = h->rx_rec_tops;
-  r.plan = h->rx_plan; r.totals = h->rx_totals;
-  r.count_out = (archive || count_out) ? h->rx_count : nullptr;
-  r.rec_cap = rec_cap;
+  { const int rc = recv_args(h, n_agents, agent_idx, owned, 0, flags & SDB_RECV_PEEK, rec_cap, &r); if (rc != SDB_OK) return rc; }
+  if (!archive && !count_out) r.count_out = nullptr;           // nobody reads the counts
   int nl = 0;
   cudaError_t e = sdb_launch_expire(&h->view, &r, older_than, (flags & SDB_EXPIRE_ALL) ? 1u : 0u, archive ? &h->cx : nullptr,
                                     h->stream, &nl, &h->prof, h->sm_count);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = false;       // the receive scratch was reused: nothing left to fold
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("expire launch: ") + cudaGetErrorString(e));
+  if (archive) return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
+  // drop mode: the number of records expired and the counts
   CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
-  if (archive)
-    CUDA_TRY(h, cudaMemcpyAsync(h->totals_host + 6, h->cx.totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
   if (count_out)
     CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   h->stream_busy = false;
-  const uint64_t total = h->totals_host[0];
-  const uint64_t n_sends = archive ? h->totals_host[6] : 0, pbytes = archive ? h->totals_host[7] * SDB_GRANULE : 0;
-  if (total_out) *total_out = total;
-  if (n_sends_out) *n_sends_out = n_sends;
-  if (payload_bytes_out) *payload_bytes_out = pbytes;
-  if (archive && total) {
-    if (entry_out) CUDA_TRY(h, cudaMemcpyAsync(entry_out, h->cx.entry_out, total * sizeof(sdb_recv_entry), cudaMemcpyDeviceToHost, h->stream));
-    if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
-    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  }
+  if (total_out) *total_out = h->totals_host[TOT_RECORDS];
   return SDB_OK;
 }
 
@@ -1968,23 +1992,17 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
   for (uint32_t i = 0; i < n_agents; ++i) sum += count[i];
   if (sum != n_entries) return fail(h, SDB_EINVAL, "sdb_restore_compact: sum(count) != n_entries");
   // one compact receive's capacity: the input is staged in its device buffers
-  const uint64_t P = pad32(h->cfg.max_payload_bytes);
-  const uint64_t rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / P);
-  if (n_entries > rec_cap || n_sends > rec_cap || payload_bytes > rec_cap * P)
+  const uint64_t rec_cap = recv_rec_cap(h);
+  if (n_entries > rec_cap || n_sends > rec_cap || payload_bytes > rec_cap * pad32(h->cfg.max_payload_bytes))
     return fail(h, SDB_ECAPACITY, "sdb_restore_compact: input larger than one compact receive's capacity");
   if (n_agents == 0) return SDB_OK;
   { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
   const size_t A = h->cfg.max_agents, tiles = A / SDB_SCAN_TILE + 2;
+  const size_t R = h->cfg.max_recv_records, H = 256 * (R / 1024 + 1);
   if (!h->rs_agent) {
-    { int rcl = ls_stop(h); if (rcl != SDB_OK) return rcl; }      // the allocations below may wait for running kernels
-    const size_t R = h->cfg.max_recv_records, H = 256 * (R / 1024 + 1);
-    if (dmalloc(&h->rs_sort, 4 * R + 2 * H + H / SDB_SCAN_TILE + 2) != cudaSuccess || dmalloc(&h->rs_tot, 8) != cudaSuccess ||
-        dmalloc(&h->rs_agent, 6 * A + tiles) != cudaSuccess) {
-      for (void* p : {static_cast<void*>(h->rs_sort), static_cast<void*>(h->rs_tot), static_cast<void*>(h->rs_agent)}) if (p) cudaFree(p);
-      h->rs_agent = nullptr; h->rs_sort = nullptr; h->rs_tot = nullptr;
-      cudaGetLastError();
-      return fail(h, SDB_ENOMEM, "restore: device allocation failed");
-    }
+    const int rc = dmalloc_set(h, {{&h->rs_sort, 4 * R + 2 * H + H / SDB_SCAN_TILE + 2}, {&h->rs_tot, 8}, {&h->rs_agent, 6 * A + tiles}},
+                               "restore: device allocation failed");
+    if (rc != SDB_OK) return rc;
   }
   std::vector<uint32_t> first(n_agents);
   { uint32_t run = 0; for (uint32_t i = 0; i < n_agents; ++i) { first[i] = run; run += count[i]; } }
@@ -2006,7 +2024,6 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
   r.owned = (flags & SDB_RECV_OWNED) && h->sharded ? 1u : 0u; r.shard_id = h->cfg.shard_id; r.shard_of = h->shard_of_dev;
   // scratch of the compact receive (max_recv_records entries each; the hash table holds >= 4 x that many words) and of
   // the restore's radix sort
-  const size_t R = h->cfg.max_recv_records;
   uint32_t* tw = reinterpret_cast<uint32_t*>(c.table);
   r.e_row = c.rec_slot;
   r.row_cnt = c.head; r.rc_local = c.head_local; r.rc_tops = c.head_tops;
@@ -2014,7 +2031,6 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
   r.e_handle = tw; r.e_y = tw + R;
   {
     uint32_t* q = h->rs_sort;
-    const size_t H = 256 * (R / 1024 + 1);
     r.key_a = q; r.key_b = q + R; r.val_a = q + 2 * R; r.val_b = q + 3 * R;
     r.hist = q + 4 * R; r.h_local = q + 4 * R + H; r.h_tops = q + 4 * R + 2 * H;
   }
@@ -2023,7 +2039,9 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
   cudaError_t e = sdb_launch_restore_plan(&h->view, &r, h->stream, &h->prof, &nl, h->sm_count);
   h->launches += nl;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("restore plan launch: ") + cudaGetErrorString(e));
+  // the plan's totals come back through totals_host and are kept apart: arena_reserve reuses its TOT_FLOOR slot
   unsigned long long tot[6];
+  static_assert(sizeof(tot) <= TOT_SLOTS * sizeof(unsigned long long), "totals_host holds the restore plan's totals");
   CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rs_tot, sizeof(tot), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   std::memcpy(tot, h->totals_host, sizeof(tot));
@@ -2071,34 +2089,23 @@ int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   }
   const bool drop = (flags & SDB_WHERE_DROP) != 0;
   if (drop && (hdr_out || payload_out)) return fail(h, SDB_EINVAL, "sdb_receive_where: drop mode takes no output buffers but count_out");
-  const bool owned = (flags & SDB_RECV_OWNED) && !agent_idx && h->sharded && h->owned_dev;
-  if (!agent_idx) n_agents = owned ? h->n_owned : h->n_agents;
+  const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
   if (n_agents == 0 || max_messages == 0) return SDB_OK;
   { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
   uint64_t rec_cap = ~0ull;
-  if (!drop) {
-    // sdb_receive_batch's record capacity: rec_cap records of the maximum size fit the device and the caller's buffers
-    const uint64_t max_rec_bytes = pad32(h->cfg.max_payload_bytes);
-    rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, h->pay_cap_gran * SDB_GRANULE / max_rec_bytes);
-    if (hdr_out) rec_cap = std::min<uint64_t>(rec_cap, hdr_cap);
-    if (payload_out) rec_cap = std::min<uint64_t>(rec_cap, payload_cap / max_rec_bytes);
-    if (rec_cap == 0) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  if (!drop) {        // sdb_receive_batch's capacity rule
+    const int rc = out_rec_cap(h, room(hdr_out, hdr_cap), room(payload_out, payload_cap), &rec_cap);
+    if (rc != SDB_OK) return rc;
   }
   const uint32_t stride = (h->cfg.ring_slots + 31) / 32;
   if (!h->where_bits) {
-    { int rcl = ls_stop(h); if (rcl != SDB_OK) return rcl; }      // the allocations below may wait for running kernels
-    uint32_t* bits = nullptr; uint8_t* kw = nullptr;
-    if (dmalloc(&bits, static_cast<size_t>(h->cfg.max_agents) * stride) != cudaSuccess ||
-        dmalloc(&kw, SDB_FILTER_MAX_KEYWORD) != cudaSuccess) {
-      if (bits) cudaFree(bits);
-      cudaGetLastError();
-      return fail(h, SDB_ENOMEM, "filtered receive: device allocation failed");
-    }
-    h->where_bits = bits; h->where_kw = kw;
+    const int rc = dmalloc_set(h, {{&h->where_bits, static_cast<size_t>(h->cfg.max_agents) * stride}, {&h->where_kw, SDB_FILTER_MAX_KEYWORD}},
+                               "filtered receive: device allocation failed");
+    if (rc != SDB_OK) return rc;
   }
-  if (agent_idx) {
-    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
-  }
+  sdb_recv_args r{};
+  { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK), rec_cap, &r);
+    if (rc != SDB_OK) return rc; }
   if (use_kw) CUDA_TRY(h, cudaMemcpyAsync(h->where_kw, filter->keyword, filter->keyword_len, cudaMemcpyHostToDevice, h->stream));
   sdb_where_args f{};
   f.fields = use_kw ? filter->fields : (filter->fields & ~SDB_FILTER_KEYWORD);
@@ -2106,34 +2113,14 @@ int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   f.type_mask = filter->type_mask; f.prio_mask = filter->prio_mask; f.kw_len = use_kw ? filter->keyword_len : 0u;
   f.after = filter->after; f.before = filter->before; f.seq_lo = filter->seq_lo; f.seq_hi = filter->seq_hi;
   f.kw = h->where_kw; f.bits = h->where_bits; f.stride = stride;
-  sdb_recv_args r{};
-  r.agent_idx = agent_idx ? h->rx_agent : (owned ? h->owned_dev : nullptr); r.n = n_agents; r.max_messages = max_messages;
-  r.flags = flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK);
-  r.cnt = h->rx_cnt; r.rec_local = h->rx_rec_local; r.rec_tops = h->rx_rec_tops;
-  r.rec_off = h->rx_rec_off; r.plan = h->rx_plan; r.lb = h->rx_lb;
-  r.plan_tops = h->rx_plan_tops; r.totals = h->rx_totals; r.big_list = h->rx_big_list; r.big_count = h->rx_big_count;
-  r.count_out = h->rx_count; r.hdr_out = h->rx_hdr; r.payload_out = h->rx_payload;
-  r.rec_cap = rec_cap;
   int nl = 0;
   cudaError_t e = sdb_launch_where(&h->view, &r, &f, drop ? 1 : 0, 32u + pad32(h->cfg.max_payload_bytes), h->stream, &nl,
                                    &h->prof, h->sm_count);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = false;       // no full receive to fold: the plan belongs to a filtered call
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("filtered receive launch: ") + cudaGetErrorString(e));
-  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
-  if (count_out)
-    CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  h->stream_busy = false;
-  const uint64_t total = h->totals_host[0], pbytes = drop ? 0 : h->totals_host[1] * SDB_GRANULE;
-  if (total_out) *total_out = total;
-  if (payload_bytes_out) *payload_bytes_out = pbytes;
-  if (!drop && total) {
-    if (hdr_out) CUDA_TRY(h, cudaMemcpyAsync(hdr_out, h->rx_hdr, total * sizeof(sdb_msg_header), cudaMemcpyDeviceToHost, h->stream));
-    if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->rx_payload, pbytes, cudaMemcpyDeviceToHost, h->stream));
-    if (hdr_out || payload_out) CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  }
-  return SDB_OK;
+  // drop mode has no output buffers, and its payload byte count stays 0
+  return copy_full(h, n_agents, count_out, hdr_out, payload_out, total_out, drop ? nullptr : payload_bytes_out);
 }
 
 int sdb_last_receive_dev(sdb_handle h, const uint32_t** count_dev, const sdb_msg_header** hdr_dev, const uint8_t** payload_dev) {
@@ -2148,8 +2135,8 @@ int sdb_last_receive_totals(sdb_handle h, uint64_t* total_out, uint64_t* payload
   if (!h) return SDB_EINVAL;
   CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  if (total_out) *total_out = h->totals_host[0];
-  if (payload_bytes_out) *payload_bytes_out = h->totals_host[1] * SDB_GRANULE;
+  if (total_out) *total_out = h->totals_host[TOT_RECORDS];
+  if (payload_bytes_out) *payload_bytes_out = h->totals_host[TOT_GRANULES] * SDB_GRANULE;
   return SDB_OK;
 }
 
@@ -2219,7 +2206,7 @@ int sdb_backend_loads_from_queues(sdb_handle h) {
 // ---- stream digests -------------------------------------------------------------------------
 static int digest_ensure(sdb_ctx* h) {
   if (h->digest) return SDB_OK;
-  CUDA_TRY(h, dmalloc(&h->digest, h->cfg.max_agents));
+  { const int rc = dmalloc_set(h, {{&h->digest, h->cfg.max_agents}}, "stream digests: device allocation failed"); if (rc != SDB_OK) return rc; }
   CUDA_TRY(h, cudaMemsetAsync(h->digest, 0, static_cast<size_t>(h->cfg.max_agents) * sizeof(unsigned long long), h->stream));
   return SDB_OK;
 }
