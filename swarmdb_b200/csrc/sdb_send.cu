@@ -934,6 +934,49 @@ k_commit_ranked(sdb_dev_view v, const sdb_send_desc* __restrict__ descs, uint32_
 //   k_pull_index        four lanes per agent, for agents with several memberships (merged by (send, position)) or
 //                       in groups that are not exclusive.
 // ------------------------------------------------------------------------------------------
+
+// Whole-sector appends.  A quad of lanes appends one agent's new entries in slot order, up to four per step.  A
+// partial-sector store into rings far larger than L2 makes L2 fetch the sector before it merges the write
+// (scripts/ubench/stores.cu), so when no live entry shares the sectors the entries land in - the tail is
+// sector-aligned, or the ring is drained (head == tail) - and the rounded-up end stays within R of head, the quad
+// assembles each 32-byte sector in its four lanes and stores it whole.  Slots of a sector that get no entry take a
+// consumed filler (SDB_META_TOMB): they lie outside [head, tail), which is all any reader of a ring looks at.  Otherwise
+// (live entries left by a partial drain, tombstoned windows, a ring about to fill, rings of 2 slots) the caller stores
+// each entry where it belongs.  Nothing overflows on the fast path: n_max bounds the entries the agent can take.
+struct sdb_sector_append {
+  uint32_t S;      // first slot of the open sector
+  uint64_t cur;    // this lane's slot S + sub of the open sector
+  bool fast;
+  __device__ __forceinline__ sdb_sector_append(bool ok, uint32_t R, uint32_t head, uint32_t tail, uint32_t n_max)
+      : S(tail & ~3u), cur(static_cast<uint64_t>(SDB_META_TOMB) << 32),
+        fast(ok && R >= 4u && ((tail & 3u) == 0u || head == tail) && ((tail + n_max + 3u) & ~3u) - head <= R) {}
+  // one step: the quad's lanes set in `qbits` hold (in lane order) the entries for slots [p, p + popc(qbits)); e is
+  // this lane's.  Every sector the step completes is stored.  Whole warp (shuffles).
+  __device__ __forceinline__ void step(uint2* rs, uint32_t mask, uint32_t p, uint32_t qbits, uint64_t e,
+                                       uint32_t sub, uint32_t qb, uint64_t pol) {
+    const uint32_t cnt = __popc(qbits);
+    const uint32_t j = (sub - p) & 3u;                   // the step's entry that falls on a slot = sub (mod 4), if any
+    uint32_t m = qbits;                                  // its lane: the j-th set bit of qbits
+    if (j > 0) m &= m - 1u;
+    if (j > 1) m &= m - 1u;
+    if (j > 2) m &= m - 1u;
+    const uint64_t x = __shfl_sync(0xFFFFFFFFu, e, qb + (m ? __ffs(m) - 1u : 0u));
+    if (!fast) return;
+    const bool has = j < cnt;
+    const uint32_t s = p + j;
+    if (has && s - S < 4u) cur = x;
+    if (p + cnt - S >= 4u) {                             // sector S is complete (quad-uniform)
+      sdb_st_u64_pol(reinterpret_cast<uint64_t*>(rs + ((S + sub) & mask)), cur, pol);
+      S += 4u;
+      cur = (has && s - S < 4u) ? x : static_cast<uint64_t>(SDB_META_TOMB) << 32;
+    }
+  }
+  // the open sector, filled up with filler; p = the agent's new tail
+  __device__ __forceinline__ void finish(uint2* rs, uint32_t mask, uint32_t p, uint32_t sub, uint64_t pol) {
+    if (fast && p != S) sdb_st_u64_pol(reinterpret_cast<uint64_t*>(rs + ((S + sub) & mask)), cur, pol);
+  }
+};
+
 __global__ void __launch_bounds__(128)
 k_pull_index_group(sdb_dev_view v, sdb_pull_view pv, const sdb_send_desc* __restrict__ descs, uint32_t n_groups,
                    const uint8_t* __restrict__ gexcl, const uint32_t* __restrict__ lstart, const uint32_t* __restrict__ lcount,
@@ -989,10 +1032,9 @@ k_pull_index_group(sdb_dev_view v, sdb_pull_view pv, const sdb_send_desc* __rest
         if (ok0) hd0 = *reinterpret_cast<const uint4*>(v.ring_hdr + a0);                     // head, tail, ctail, ntomb
         if (ok1) hd1 = *reinterpret_cast<const uint4*>(v.ring_hdr + a1);
         uint32_t t0 = hd0.y, t1 = hd1.y;
-        // Stores: a QUAD of lanes writes up to four consecutive entries of ONE member in one instruction, so the
-        // memory system sees one or two sector writes per member instead of one partial-sector write per entry
-        // (scattered partial-sector stores into a table far larger than L2 cost several times a full sector).  Per warp step:
-        // 8 members x 4 sends; the members' ids / heads / tails travel by shuffle from the lanes that loaded them.
+        // Stores: a QUAD of lanes appends ONE member's entries, four sends per step, in whole sectors where the ring
+        // allows it (sdb_sector_append), else up to four consecutive entries in one instruction.  Eight members per
+        // warp step; the members' ids / heads / tails travel by shuffle from the lanes that loaded them.
         const uint32_t quad = lane >> 2, sub = lane & 3u, qb = lane & ~3u;
         for (uint32_t k0 = 0; k0 < total; k0 += 32) {
           if (k0) {                                                                          // buckets deeper than 32 sends
@@ -1001,40 +1043,41 @@ k_pull_index_group(sdb_dev_view v, sdb_pull_view pv, const sdb_send_desc* __rest
             if (sidx != 0xFFFFFFFFu) q1 = __ldg(reinterpret_cast<const uint4*>(descs + sidx) + 1);
           }
           const uint32_t nk = min(32u, total - k0);
-          for (uint32_t c0 = 0; c0 < nk; c0 += 4) {                                          // four sends per step
-            const uint32_t t = c0 + sub;
-            const uint32_t gran0 = __shfl_sync(0xFFFFFFFFu, q1.x, t & 31u), sender = __shfl_sync(0xFFFFFFFFu, q1.y, t & 31u);
-            const uint32_t rgran = __shfl_sync(0xFFFFFFFFu, q1.z, t & 31u), lpt = __shfl_sync(0xFFFFFFFFu, q1.w, t & 31u);
-            const bool have_send = t < nk;
-            for (uint32_t mb = 0; mb < 64; mb += 8) {                                        // eight members per step
-              const uint32_t mi = mb + quad;                                                 // member slot 0..63 of this block of 64
-              const uint32_t srcl = mi & 31u;
-              const uint32_t am = __shfl_sync(0xFFFFFFFFu, mi < 32 ? a0 : a1, srcl);
-              const uint32_t hm = __shfl_sync(0xFFFFFFFFu, mi < 32 ? hd0.x : hd1.x, srcl);
-              const uint32_t tm = __shfl_sync(0xFFFFFFFFu, mi < 32 ? t0 : t1, srcl);
-              const bool okm = am < v.max_agents;
-              const bool keep = have_send && okm && sender != am;                            // member == sender (M:1268)
-              const uint32_t bal = __ballot_sync(0xFFFFFFFFu, keep);
-              const uint32_t qbits = (bal >> qb) & 0xFu;
-              const uint32_t pos = tm + __popc(qbits & ((1u << sub) - 1u));
+          for (uint32_t mb = 0; mb < 64; mb += 8) {                                          // eight members per step
+            const uint32_t mi = mb + quad;                                                   // member slot 0..63 of this block of 64
+            const uint32_t srcl = mi & 31u;
+            const uint32_t am = __shfl_sync(0xFFFFFFFFu, mi < 32 ? a0 : a1, srcl);
+            const uint32_t hm = __shfl_sync(0xFFFFFFFFu, mi < 32 ? hd0.x : hd1.x, srcl);
+            const uint32_t tm = __shfl_sync(0xFFFFFFFFu, mi < 32 ? t0 : t1, srcl);
+            const bool okm = am < v.max_agents;
+            uint2* rs = sdb_ring_of(v, okm ? am : 0u);
+            // record slot jm of the send's region: a whole record, or (shared payloads) its header, the one payload
+            // sitting behind the region's mcount headers
+            const uint32_t jm = m0 + mi;
+            sdb_sector_append sa(okm, R, hm, tm, nk);
+            uint32_t p = tm;                                                                 // the member's running tail
+            for (uint32_t c0 = 0; c0 < nk; c0 += 4) {                                        // four sends per step
+              const uint32_t t = c0 + sub;
+              const uint32_t gran0 = __shfl_sync(0xFFFFFFFFu, q1.x, t & 31u), sender = __shfl_sync(0xFFFFFFFFu, q1.y, t & 31u);
+              const uint32_t rgran = __shfl_sync(0xFFFFFFFFu, q1.z, t & 31u), lpt = __shfl_sync(0xFFFFFFFFu, q1.w, t & 31u);
+              const bool keep = t < nk && okm && sender != am;                               // member == sender (M:1268)
+              const uint32_t qbits = (__ballot_sync(0xFFFFFFFFu, keep) >> qb) & 0xFu;
+              const uint32_t pos = p + __popc(qbits & ((1u << sub) - 1u));
+              const uint32_t handle = static_cast<uint32_t>(arena_base + gran0 + (shared ? static_cast<uint64_t>(jm) : static_cast<uint64_t>(jm) * rgran));
+              const uint64_t meta_hi = static_cast<uint64_t>((((lpt >> 16) & 0xFFu) << 14) | rgran | (shared ? (mcount - 1u - jm) << 16 : 0u)) << 32;
               if (keep) {
-                // record slot jm of the send's region: a whole record, or (shared payloads) its header, the one payload
-                // sitting behind the region's mcount headers
-                const uint32_t jm = m0 + mi;
-                const uint32_t handle = static_cast<uint32_t>(arena_base + gran0 + (shared ? static_cast<uint64_t>(jm) : static_cast<uint64_t>(jm) * rgran));
-                if (pos - hm >= R) { ++n_ovf; sdb_note_overflow(v, am, handle); }
-                else {
-                  const uint64_t meta_hi = static_cast<uint64_t>((((lpt >> 16) & 0xFFu) << 14) | rgran | (shared ? (mcount - 1u - jm) << 16 : 0u)) << 32;
-                  sdb_st_u64_pol(reinterpret_cast<uint64_t*>(sdb_ring_of(v, am) + (pos & mask)), meta_hi | handle, pol);
-                  ++n_enq;
-                }
+                if (sa.fast) ++n_enq;
+                else if (pos - hm >= R) { ++n_ovf; sdb_note_overflow(v, am, handle); }
+                else { sdb_st_u64_pol(reinterpret_cast<uint64_t*>(rs + (pos & mask)), meta_hi | handle, pol); ++n_enq; }
               }
-              // the lane that owns this member advances its tail by the quad's kept entries
-              const uint32_t add_lo = __popc((bal >> ((lane & 7u) << 2)) & 0xFu);             // quad (lane & 7) of THIS step
-              // member slot handled by quad q in this step is mb + q: its owner lane is (mb + q) & 31, in half (mb + q) >> 5
-              if ((lane >> 3) == ((mb >> 3) & 3u) ) {                                        // lanes [mb & 31, (mb & 31) + 8) own the 8 members
-                if (mb < 32) t0 += add_lo; else t1 += add_lo;
-              }
+              sa.step(rs, mask, p, qbits, meta_hi | handle, sub, qb, pol);
+              p += __popc(qbits);
+            }
+            sa.finish(rs, mask, p, sub, pol);
+            // member slot mb + q (quad q) is owned by lane (mb + q) & 31, in half (mb + q) >> 5: it takes the new tail
+            const uint32_t pq = __shfl_sync(0xFFFFFFFFu, p, (lane & 7u) << 2);
+            if ((lane >> 3) == ((mb >> 3) & 3u)) {                                           // lanes [mb & 31, (mb & 31) + 8) own the 8 members
+              if (mb < 32) t0 = pq; else t1 = pq;
             }
           }
         }
@@ -1090,35 +1133,36 @@ k_list_index(sdb_dev_view v, sdb_list_view lv, const sdb_send_desc* __restrict__
     if (ok0) hd0 = *reinterpret_cast<const uint4*>(v.ring_hdr + a0);                       // head, tail, ctail, ntomb
     if (ok1) hd1 = *reinterpret_cast<const uint4*>(v.ring_hdr + a1);
     uint32_t t0 = hd0.y, t1 = hd1.y;
-    const uint32_t quad = lane >> 2, sub = lane & 3u;
+    const uint32_t quad = lane >> 2, sub = lane & 3u, qb = lane & ~3u;
     for (uint32_t k0 = 0; k0 < total; k0 += 32) {
       uint4 q1 = make_uint4(0, 0, 0, 0);
       if (k0 + lane < total) q1 = __ldg(reinterpret_cast<const uint4*>(descs + __ldg(lv.idx + b0 + k0 + lane)) + 1);   // gran0, sender, rgran, len|prio|type
       const uint32_t nk = min(32u, total - k0);
-      for (uint32_t c0 = 0; c0 < nk; c0 += 4) {                                            // four sends per step
-        const uint32_t t = c0 + sub;
-        const uint32_t gran0 = __shfl_sync(0xFFFFFFFFu, q1.x, t & 31u);
-        const uint32_t rgran = __shfl_sync(0xFFFFFFFFu, q1.z, t & 31u), lpt = __shfl_sync(0xFFFFFFFFu, q1.w, t & 31u);
-        const bool have_send = t < nk;
-        const uint32_t nsend = min(4u, nk - c0);                                           // every member takes all of them
-        for (uint32_t mb = 0; mb < 64; mb += 8) {                                          // eight members per step
-          const uint32_t mi = mb + quad, srcl = mi & 31u;
-          const uint32_t am = __shfl_sync(0xFFFFFFFFu, mi < 32 ? a0 : a1, srcl);
-          const uint32_t hm = __shfl_sync(0xFFFFFFFFu, mi < 32 ? hd0.x : hd1.x, srcl);
-          const uint32_t tm = __shfl_sync(0xFFFFFFFFu, mi < 32 ? t0 : t1, srcl);
-          if (have_send && am < v.max_agents) {
-            const uint32_t pos = tm + sub;
-            if (pos - hm >= R) { ++n_ovf; sdb_note_overflow(v, am, static_cast<uint32_t>(arena_base + gran0 + static_cast<uint64_t>(m0 + mi) * rgran)); }
-            else {
-              const uint64_t meta_hi = static_cast<uint64_t>((((lpt >> 16) & 0xFFu) << 14) | rgran) << 32;
-              sdb_st_u64_pol(reinterpret_cast<uint64_t*>(sdb_ring_of(v, am) + (pos & mask)),
-                             meta_hi | static_cast<uint32_t>(arena_base + gran0 + static_cast<uint64_t>(m0 + mi) * rgran), pol);
-              ++n_enq;
-            }
+      for (uint32_t mb = 0; mb < 64; mb += 8) {                                            // eight members per step
+        const uint32_t mi = mb + quad, srcl = mi & 31u;
+        const uint32_t am = __shfl_sync(0xFFFFFFFFu, mi < 32 ? a0 : a1, srcl);
+        const uint32_t hm = __shfl_sync(0xFFFFFFFFu, mi < 32 ? hd0.x : hd1.x, srcl);
+        const uint32_t tm = __shfl_sync(0xFFFFFFFFu, mi < 32 ? t0 : t1, srcl);
+        const bool okm = am < v.max_agents;
+        uint2* rs = sdb_ring_of(v, okm ? am : 0u);
+        sdb_sector_append sa(okm, R, hm, tm, nk);
+        for (uint32_t c0 = 0; c0 < nk; c0 += 4) {                                          // four sends per step
+          const uint32_t t = c0 + sub;
+          const uint32_t gran0 = __shfl_sync(0xFFFFFFFFu, q1.x, t & 31u);
+          const uint32_t rgran = __shfl_sync(0xFFFFFFFFu, q1.z, t & 31u), lpt = __shfl_sync(0xFFFFFFFFu, q1.w, t & 31u);
+          const uint32_t pos = tm + c0 + sub;                                              // every member takes every send
+          const uint32_t handle = static_cast<uint32_t>(arena_base + gran0 + static_cast<uint64_t>(m0 + mi) * rgran);
+          const uint64_t meta_hi = static_cast<uint64_t>((((lpt >> 16) & 0xFFu) << 14) | rgran) << 32;
+          if (t < nk && okm) {
+            if (sa.fast) ++n_enq;
+            else if (pos - hm >= R) { ++n_ovf; sdb_note_overflow(v, am, handle); }
+            else { sdb_st_u64_pol(reinterpret_cast<uint64_t*>(rs + (pos & mask)), meta_hi | handle, pol); ++n_enq; }
           }
+          sa.step(rs, mask, tm + c0, okm ? (1u << min(4u, nk - c0)) - 1u : 0u, meta_hi | handle, sub, qb, pol);
         }
-        t0 += nsend; t1 += nsend;                                                          // (members that do not exist never store their tail)
+        sa.finish(rs, mask, tm + nk, sub, pol);
       }
+      t0 += nk; t1 += nk;                                                                  // (members that do not exist never store their tail)
     }
     if (ok0) { if (t0 - hd0.x > R) t0 = hd0.x + R; hd0.y = t0; hd0.z = t0; *reinterpret_cast<uint4*>(v.ring_hdr + a0) = hd0; }
     if (ok1) { if (t1 - hd1.x > R) t1 = hd1.x + R; hd1.y = t1; hd1.z = t1; *reinterpret_cast<uint4*>(v.ring_hdr + a1) = hd1; }
