@@ -700,6 +700,125 @@ def restore(rounds=3):
     return out
 
 
+def lease(rounds=3):
+    """Leased receives on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 pending records): a leased
+    receive of the whole backlog against a plain compact receive of it (alternated, each after a fresh send), the settle
+    of the acks of every other record (2,097,152 ids), the sweep that redelivers the other half, and, for comparison, the
+    host requeue of the same half (requeue_batch_compact: rows renumbered on the host, then restored from host memory).
+    Per call: wall clock around the synchronising call, and the `lease` kernel time from the profiler (the sweep's
+    restore phases are reported apart).  Outside the timed region the redelivered half is checked by digests against
+    the same half requeued on a twin handle."""
+    import torch
+    from bench import ClockSampler, Workload
+    from swarmdb_b200._native import ENTRY_DTYPE, LEASE_ACK, LEASE_ALL, SEND_DTYPE, Shard, pad32
+    from swarmdb_b200.core import _renumber_rows
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py lease: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+
+    def handle():
+        s = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+        s.register(np.arange(wl.A, dtype=np.uint32))
+        for g in range(wl.G):
+            s.create_group(g, wl.members(g))
+        return s
+
+    def pinned(nbytes):
+        return torch.empty(nbytes, dtype=torch.uint8, pin_memory=True).numpy()
+
+    def drain(s, digest=False):
+        if digest:
+            s.digest_reset()
+        while True:
+            _, total, _ = s.receive_batch(None, 1 << 10, copy_out=False)
+            if digest:
+                s.digest_fold()
+            if not total:
+                break
+        return s.digest_read() if digest else None
+
+    src, twin = handle(), handle()
+    src.lease_reserve(rec_cap, rec_cap * pad32(wl.L))
+    agents = np.arange(wl.A, dtype=np.uint32)
+    pin_ent, pin_snd, pin_pay = pinned(rec_cap * 16).view(ENTRY_DTYPE), pinned(rec_cap * 32).view(SEND_DTYPE), pinned(rec_cap * wl.L)
+    batch = wl.batch()
+
+    def call(fn):
+        src.sync(); src.profile(True)
+        t = time.perf_counter()
+        r = fn()
+        wall = (time.perf_counter() - t) * 1e3
+        prof = src.profile_read(); src.profile(False)
+        recv = prof["recv_compact"][0] + sum(prof[x][0] for x in ("recv_count", "recv_scan", "recv_select"))
+        return r, {"wall_ms": wall, "lease_kernel_ms": prof["lease"][0], "restore_kernel_ms": prof["restore"][0],
+                   "receive_kernel_ms": recv}
+
+    def med(rows):
+        return {k: float(np.median([r[k] for r in rows])) for k in rows[0]} | {"per_round": rows}
+
+    clocks = ClockSampler(0); clocks.start()
+    plain, leased, settle, sweep, requeue = [], [], [], [], []
+    for _ in range(rounds):
+        for kind in ("plain", "leased"):
+            drain(src)
+            if src.lease_stats()["live"]:
+                src.lease_sweep(0.0, LEASE_ALL); drain(src)
+            src.send_group_batch(*batch)
+            if kind == "plain":
+                res, t = call(lambda: src.receive_compact(None, 1 << 10, 0, out_entries=pin_ent, out_sends=pin_snd,
+                                                          out_payload=pin_pay))
+                assert len(res[1]) == per_step
+                plain.append(t)
+            else:
+                res, t = call(lambda: src.receive_leased(None, 1 << 10, 1.0, 0, out_entries=pin_ent, out_sends=pin_snd,
+                                                         out_payload=pin_pay))
+                assert len(res[1]) == per_step
+                leased.append(t)
+                base = res[4]
+                half = np.arange(base, base + per_step, 2, dtype=np.uint64)
+                (_, n_acked), t = call(lambda: src.lease_settle(half, LEASE_ACK))
+                assert n_acked == len(half)
+                settle.append(t)
+                (red, blocked, left), t = call(lambda: src.lease_sweep(2.0))
+                assert red == per_step - len(half) and blocked == 0 and left == 0
+                sweep.append(t)
+    # the host requeue of the same half (rows renumbered by smallest seq, restored from host memory), and the digest check
+    drain(src)
+    src.send_group_batch(*batch)
+    c, e, s, p, base = src.receive_leased(None, 1 << 10, 1.0, 0, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_pay)
+    keep = np.zeros(len(e), bool); keep[1::2] = True                  # the unacked half, as the sweep redelivers it
+    who = np.repeat(np.arange(len(c)), c.astype(np.int64))
+    cnt_half = np.bincount(who[keep], minlength=len(c)).astype(np.uint32)
+    e_half = e[keep].copy(); s_all = s.copy(); p_all = p.copy()
+    src.lease_settle(np.arange(base, base + len(e), 2, dtype=np.uint64), LEASE_ACK)
+    src.lease_sweep(2.0)
+    want = drain(src, True)
+    for _ in range(rounds):
+        drain(twin)
+        twin.send_group_batch(*batch)
+        twin.receive_compact(None, 1 << 10, 0, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_pay)
+        twin.sync()
+        t0 = time.perf_counter()
+        ent2, snd2 = _renumber_rows(e_half, s_all)
+        twin.restore_compact(agents, cnt_half, ent2, snd2, p_all)
+        requeue.append({"wall_ms": (time.perf_counter() - t0) * 1e3})
+    same = bool(np.array_equal(drain(twin, True), want))
+    clk = clocks.stop()
+    src.close(); twin.close()
+    out = {"receive_compact": med(plain), "receive_leased": med(leased), "settle_acks": med(settle),
+           "sweep_redeliver_half": med(sweep), "requeue_batch_compact_same_half": med(requeue),
+           "config": f"c2 backlog: {wl.A} agents, {wl.S} group sends x {wl.F} members = {per_step} records, {wl.L}-B "
+                     f"payloads; pinned host buffers; leased and plain receives alternated, {rounds} rounds",
+           "records": per_step, "acked": per_step // 2, "redelivered": per_step - per_step // 2,
+           "redelivered_digests_equal_requeue": same, "clocks": clk}
+    out.update(_gpu_card(0))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", nargs="*", default=["c1", "c4", "c5", "k1", "bcast"])

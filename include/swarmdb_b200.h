@@ -130,9 +130,15 @@ int sdb_advance_seq(sdb_handle h, uint64_t next_seq);
  * roofline: enable, run, then read accumulated milliseconds and launch counts per kernel class. */
 enum { SDB_PK_P2P = 0, SDB_PK_FANOUT, SDB_PK_COMMIT, SDB_PK_RECV_COUNT, SDB_PK_RECV_SCAN, SDB_PK_RECV_SELECT,
        SDB_PK_RECV_GATHER, SDB_PK_ARENA_FLOOR, SDB_PK_PICK, SDB_PK_XSHARD, SDB_PK_INDEX, SDB_PK_XWAIT,
-       SDB_PK_RECV_COMPACT = 12, SDB_PK_EXPIRE = 13, SDB_PK_WHERE = 14, SDB_PK_RESTORE = 15, SDB_PK_N = 16 };
+       SDB_PK_RECV_COMPACT = 12, SDB_PK_EXPIRE = 13, SDB_PK_WHERE = 14, SDB_PK_RESTORE = 15, SDB_PK_N = 16,
+       /* classes past SDB_PK_N: sdb_profile_read fills SDB_PK_N entries (the array size of every ABI-1 caller), so
+          these are read with sdb_profile_read_n only */
+       SDB_PK_LEASE = 16, SDB_PK_ALL = 17 };
 int sdb_profile(sdb_handle h, int enable);
 int sdb_profile_read(sdb_handle h, double* ms_out /* [SDB_PK_N] */, uint64_t* count_out /* [SDB_PK_N] */);
+/* The same for the first min(n, SDB_PK_ALL) classes (entries from there to n are zeroed); like sdb_profile_read it
+ * consumes the recorded intervals. */
+int sdb_profile_read_n(sdb_handle h, uint32_t n, double* ms_out /* [n] */, uint64_t* count_out /* [n] */);
 
 /* ---- registry: register_agent (M:314-349) / deregister_agent (M:351-372) ------------------
  * Rings exist for every index < max_agents; registration only moves the watermark that
@@ -319,6 +325,59 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
                         const sdb_recv_entry* entries, uint64_t n_entries, const sdb_recv_send* sends, uint64_t n_sends,
                         const uint8_t* payload, uint64_t payload_bytes, uint32_t flags, uint64_t* restored_out,
                         uint64_t* seq_end_out);
+/* ---- leased receive: at-least-once delivery (mark_message_as_processed, M:654-669; MessageStatus READ / PROCESSED,
+ * M:44-51).  A lease store in device memory keeps a copy of every record a leased receive hands out, in the compact format,
+ * until the record is acknowledged or redelivered.  Redelivery puts it back behind what its agent has pending.
+ *   sdb_lease_reserve   allocates the store: max_records entries (and rows) and max_payload_bytes (rounded up to
+ *                       SDB_GRANULE) of payload, double-buffered for compaction.  max_records == 0 frees it.  Refused
+ *                       (SDB_EINVAL) while the store holds live leases.  Nobody who does not call it pays the memory.
+ *   sdb_receive_leased  selects, retires and returns exactly what sdb_receive_compact would with the same arguments (its
+ *                       contract points 1-4), and appends each returned record to the store with `deadline`.  Record r of
+ *                       the call, in entry_out order, gets lease id *lease_base_out + r; ids are monotonic per handle.
+ *                       Capacity: rec_cap = min(sdb_receive_compact's rec_cap, free store entries, free store payload / P),
+ *                       so a call never overfills the store; no room for one maximum-size record: SDB_ECAPACITY ("lease
+ *                       store full: settle or sweep").  Flags: SDB_RECV_PRIORITY and SDB_RECV_OWNED; SDB_RECV_PEEK,
+ *                       SDB_RECV_ASYNC and other bits are refused (SDB_EINVAL), as is a call without a reserved store.
+ *   sdb_lease_settle    op SDB_LEASE_ACK marks live leases done; SDB_LEASE_RENEW sets their deadline (a later one extends,
+ *                       -INFINITY makes them due at the next sweep: a nack).  settled_out[i] (nullable) is 1 when lease
+ *                       lease_id[i] was live before the call, else 0 (unknown, already acked, already redelivered: a late
+ *                       ack after redelivery is visible, not an error); an id repeated in one call reads 1 each time and is
+ *                       settled once.  *n_settled_out = requests that read 1.  Acks free no space: the next sweep does.
+ *   sdb_lease_sweep     redelivery.  Due: every live lease with deadline <= now (a NaN deadline or NaN `now` makes nothing
+ *                       due); with SDB_LEASE_ALL every live lease, deadlines not read.  One call takes at most one compact
+ *                       receive's capacity of due records, in lease-id order (*due_left_out = due records beyond it: loop
+ *                       until it reads 0).  Each agent's records are appended behind what it has pending, in lease-id
+ *                       order - the original delivery order - with sdb_restore_compact's effect (its points 1-3: seq,
+ *                       ids and headers kept; enqueued and agent loads move as for a restore).  Rows are numbered by
+ *                       their smallest redelivered seq, so a stream-order lease comes back in its sends' arena layout.  An
+ *                       agent whose ring cannot take all of its records of the call (tail - head + records > ring_slots,
+ *                       tombstones count) keeps them in the store and is counted in *blocked_out; every other agent is
+ *                       served.  SDB_EARENA_FULL (after a floor reclaim) fails the call whole: store, rings and stats
+ *                       unchanged.  Afterwards the store is compacted: acked and redelivered entries and the rows and
+ *                       payloads no live entry names are dropped, in a stable order (lease ids stay ascending).
+ *   sdb_lease_stats     host bookkeeping of the store (no synchronisation).
+ * All but sdb_lease_stats are stream-ordered on the handle's stream and synchronise. */
+#define SDB_LEASE_ACK 0u
+#define SDB_LEASE_RENEW 1u
+#define SDB_LEASE_ALL 1u                /* sdb_lease_sweep flag: every live lease is due */
+typedef struct sdb_lease_summary {
+  uint64_t live;                /* leases neither acked nor redelivered */
+  uint64_t acked_unreclaimed;   /* acked entries the next sweep drops */
+  uint64_t redelivered_total;   /* records redelivered so far */
+  uint64_t acked_total;         /* leases acked so far */
+  uint64_t entries_used, entries_reserved;
+  uint64_t payload_used, payload_reserved;   /* bytes */
+} sdb_lease_summary;
+int sdb_lease_reserve(sdb_handle h, uint64_t max_records, uint64_t max_payload_bytes);
+int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                       double deadline, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                       sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                       uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out, uint64_t* lease_base_out);
+int sdb_lease_settle(sdb_handle h, uint64_t n, const uint64_t* lease_id, uint32_t op, double deadline, uint8_t* settled_out,
+                     uint64_t* n_settled_out);
+int sdb_lease_sweep(sdb_handle h, double now, uint32_t flags, uint64_t* redelivered_out, uint64_t* blocked_out,
+                    uint64_t* due_left_out);
+int sdb_lease_stats(sdb_handle h, sdb_lease_summary* out);
 /* Low-latency dequeue server (opt-in): receive_messages (M:521-601) for ONE agent in a few microseconds.
  * enable = 1 starts a persistent single-CTA kernel on its own stream that polls a mailbox in mapped pinned host memory;
  * sdb_receive_batch calls naming exactly one agent with host outputs (what the Python surface's receive_messages makes)

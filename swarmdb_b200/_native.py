@@ -37,6 +37,9 @@ RECV_ASYNC = 4
 RECV_OWNED = 8
 EXPIRE_ALL = 16
 WHERE_DROP = 32
+LEASE_ACK = 0                   # sdb_lease_settle ops
+LEASE_RENEW = 1
+LEASE_ALL = 1                   # sdb_lease_sweep flag: every live lease is due
 FILTER_SENDER, FILTER_RECEIVER, FILTER_GROUP, FILTER_TYPE = 1, 2, 4, 8
 FILTER_PRIO, FILTER_TIME, FILTER_SEQ, FILTER_KEYWORD, FILTER_ICASE = 16, 32, 64, 128, 256
 FILTER_MAX_KEYWORD = 256
@@ -121,15 +124,21 @@ class SdbStats(C.Structure):
                                           "backend_picks")]
 
 
+class SdbLeaseSummary(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("live", "acked_unreclaimed", "redelivered_total", "acked_total", "entries_used",
+                                          "entries_reserved", "payload_used", "payload_reserved")]
+
+
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
-           "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
+           "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_profile_read_n", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
            "sdb_receive_batch", "sdb_receive_compact", "sdb_restore_compact", "sdb_expire", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
            "sdb_release_backends", "sdb_select_backend_batch", "sdb_agent_loads", "sdb_queue_stats",
-           "sdb_assign_agent_backends", "sdb_backend_loads_from_queues"]
+           "sdb_assign_agent_backends", "sdb_backend_loads_from_queues", "sdb_lease_reserve", "sdb_receive_leased",
+           "sdb_lease_settle", "sdb_lease_sweep", "sdb_lease_stats"]
 
 _lib = None
 
@@ -156,6 +165,7 @@ def load_library() -> C.CDLL:
     L.sdb_advance_seq.restype = i32; L.sdb_advance_seq.argtypes = [vp, u64]
     L.sdb_profile.restype = i32; L.sdb_profile.argtypes = [vp, i32]
     L.sdb_profile_read.restype = i32; L.sdb_profile_read.argtypes = [vp, vp, vp]
+    L.sdb_profile_read_n.restype = i32; L.sdb_profile_read_n.argtypes = [vp, u32, vp, vp]
     L.sdb_register_agents.restype = i32; L.sdb_register_agents.argtypes = [vp, u32, vp]
     L.sdb_deregister_agents.restype = i32; L.sdb_deregister_agents.argtypes = [vp, u32, vp]
     L.sdb_create_group.restype = i32; L.sdb_create_group.argtypes = [vp, u32, u32, vp]
@@ -173,6 +183,12 @@ def load_library() -> C.CDLL:
     L.sdb_receive_compact.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_restore_compact.restype = i32
     L.sdb_restore_compact.argtypes = [vp, u32, vp, vp, vp, u64, vp, u64, vp, u64, u32, vp, vp]
+    L.sdb_lease_reserve.restype = i32; L.sdb_lease_reserve.argtypes = [vp, u64, u64]
+    L.sdb_receive_leased.restype = i32
+    L.sdb_receive_leased.argtypes = [vp, u32, vp, u32, u32, C.c_double, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp, vp]
+    L.sdb_lease_settle.restype = i32; L.sdb_lease_settle.argtypes = [vp, u64, vp, u32, C.c_double, vp, vp]
+    L.sdb_lease_sweep.restype = i32; L.sdb_lease_sweep.argtypes = [vp, C.c_double, u32, vp, vp, vp]
+    L.sdb_lease_stats.restype = i32; L.sdb_lease_stats.argtypes = [vp, C.POINTER(SdbLeaseSummary)]
     L.sdb_expire.restype = i32
     L.sdb_expire.argtypes = [vp, u32, vp, C.c_double, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_receive_where.restype = i32
@@ -313,18 +329,21 @@ class Shard:
         """Move the handle's sequence counter forward (ids of a refused batch are never reissued)."""
         self._check(self._L.sdb_advance_seq(self._h, next_seq))
 
+    # the SDB_PK_N classes sdb_profile_read fills, then the classes only sdb_profile_read_n reports (SDB_PK_ALL in all)
     PROFILE_KINDS = ["p2p", "fanout", "commit", "recv_count", "recv_scan", "recv_select", "recv_gather",
                      "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact", "expire", "where", "restore"]
+    PROFILE_KINDS_ALL = PROFILE_KINDS + ["lease"]
 
     def profile(self, enable: bool) -> None:
         self._check(self._L.sdb_profile(self._h, 1 if enable else 0))
 
     def profile_read(self) -> dict:
-        """{kernel class: (total ms, launches)} measured with CUDA events on the launching stream."""
-        ms = np.zeros(16, np.float64)
-        cnt = np.zeros(16, np.uint64)
-        self._check(self._L.sdb_profile_read(self._h, _p(ms), _p(cnt)))
-        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.PROFILE_KINDS)}
+        """{kernel class: (total ms, launches)} over PROFILE_KINDS_ALL, measured with CUDA events on the launching stream."""
+        n = len(self.PROFILE_KINDS_ALL)
+        ms = np.zeros(n, np.float64)
+        cnt = np.zeros(n, np.uint64)
+        self._check(self._L.sdb_profile_read_n(self._h, n, _p(ms), _p(cnt)))
+        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.PROFILE_KINDS_ALL)}
 
     # ------------------------------------------------------------------ registry / groups
     def register(self, idx) -> None:
@@ -572,6 +591,50 @@ class Shard:
                                                 _p(pay), pay.nbytes, flags, C.cast(C.byref(restored), C.c_void_p),
                                                 C.cast(C.byref(seq_end), C.c_void_p)))
         return int(restored.value), int(seq_end.value)
+
+    # ------------------------------------------------------------------ leases (include/swarmdb_b200.h: sdb_lease_*)
+    def lease_reserve(self, max_records: int, max_payload_bytes: int) -> None:
+        """Allocate the device lease store (0 records frees it); refused while it holds live leases."""
+        self._check(self._L.sdb_lease_reserve(self._h, int(max_records), int(max_payload_bytes)))
+
+    def receive_leased(self, agents, max_messages: int, deadline: float, flags: int = 0,
+                       out_entries: Optional[np.ndarray] = None, out_sends: Optional[np.ndarray] = None,
+                       out_payload: Optional[np.ndarray] = None):
+        """receive_compact's records and result, each also kept in the lease store with `deadline` until it is acked or
+        redelivered.  Returns (counts, entries, sends, payload, lease_base): entry r holds lease lease_base + r."""
+        a, n, counts = self._agents_arg(agents)
+        ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
+        total, n_sends, pbytes, base = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_receive_leased(self._h, n, _p(a), max_messages, flags, float(deadline), _p(counts), _p(ent),
+                                               len(ent), _p(snd), len(snd), _p(pay), pay.nbytes,
+                                               C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
+                                               C.cast(C.byref(pbytes), C.c_void_p), C.cast(C.byref(base), C.c_void_p)))
+        if agents is None:
+            counts = self._served_counts(counts, flags)
+        return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value], int(base.value)
+
+    def lease_settle(self, lease_ids, op: int, deadline: float = 0.0) -> Tuple[np.ndarray, int]:
+        """Ack (LEASE_ACK) or renew (LEASE_RENEW, new deadline) leases.  Returns (settled[n] uint8: 1 where the lease was
+        live, number settled)."""
+        ids = _arr(np.atleast_1d(lease_ids), np.uint64)
+        out = np.zeros(len(ids), np.uint8)
+        n = C.c_uint64(0)
+        self._check(self._L.sdb_lease_settle(self._h, len(ids), _p(ids), op, float(deadline), _p(out),
+                                             C.cast(C.byref(n), C.c_void_p)))
+        return out, int(n.value)
+
+    def lease_sweep(self, now: float, flags: int = 0) -> Tuple[int, int, int]:
+        """Redeliver due leases (one compact receive's capacity per call).  Returns (redelivered, blocked agents,
+        due records left for the next call)."""
+        red, blk, left = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_lease_sweep(self._h, float(now), flags, C.cast(C.byref(red), C.c_void_p),
+                                            C.cast(C.byref(blk), C.c_void_p), C.cast(C.byref(left), C.c_void_p)))
+        return int(red.value), int(blk.value), int(left.value)
+
+    def lease_stats(self) -> dict:
+        s = SdbLeaseSummary()
+        self._check(self._L.sdb_lease_stats(self._h, C.byref(s)))
+        return {n: int(getattr(s, n)) for n, _ in SdbLeaseSummary._fields_}
 
     def expire(self, agents, older_than: float, flags: int = 0, archive: bool = True,
                out_entries: Optional[np.ndarray] = None, out_sends: Optional[np.ndarray] = None,

@@ -24,6 +24,7 @@ Bulk entry points for index-level traffic (`send_to_group_batch`, `send_batch`,
 from __future__ import annotations
 
 import datetime
+import heapq
 import json
 import os
 import secrets
@@ -158,6 +159,8 @@ class GpuConfig:
     fanout_variant: Optional[int] = None      # None: the library default (_native.DEFAULT_FANOUT_VARIANT)
     shard_id: int = 0                     # multi-GPU: this process's shard / total shards (see sharded.ShardedSwarmsDB)
     num_shards: int = 1
+    lease_records: int = 0                # leased receives: device lease store entries (0: no store, no memory)
+    lease_payload_bytes: int = 0          # ... and payload bytes (0: lease_records x pad32(max_payload_bytes))
 
 
 def _encode_content(content: Any) -> (bytes, int):
@@ -268,6 +271,12 @@ class SwarmsDB:
         self._next_seq = 1                      # mirror of the handle's sequence counter
         self._list_cap = 2 * g.max_agents + 1024 - 8      # the handle's default list_pool_entries, minus slack
         self._seq_to_id: Dict[int, str] = {}
+        # leased receives: message id -> [(agent index, lease id)] (a broadcast is leased by each of its receivers under
+        # one id), and a heap of the deadlines set, so a receive sweeps only once one may have passed
+        self._leases: Dict[str, List[Tuple[int, int]]] = {}
+        self._lease_deadlines: List[float] = []
+        if g.lease_records:
+            self.shard.lease_reserve(g.lease_records, g.lease_payload_bytes or g.lease_records * pad32(g.max_payload_bytes))
         self._reset_buffer()
         self._closed = False
         self.admin_client = _TransportAdmin(self)          # M:202-204: callers only list topics through it
@@ -676,6 +685,117 @@ class SwarmsDB:
                 break
         return out
 
+    # ------------------------------------------------------------------ leased receive (at-least-once delivery)
+    def receive_messages_leased(self, agent_id: str, max_messages: int = 100, visibility_timeout: float = 30.0) -> List[Message]:
+        """receive_messages with at-least-once delivery: the messages read READ, and each stays owed until it is acked
+        (ack_messages, mark_message_as_processed).  One not acked within `visibility_timeout` seconds goes back behind
+        what the agent has pending and is delivered again, with its id (an SQS visibility timeout).  Expired leases are
+        swept back first, so they are visible to this call.  Needs GpuConfig.lease_records."""
+        self._prepare_receive(agent_id)
+        now = time.time()
+        self._sweep_due(now)
+        if max_messages <= 0:
+            return []
+        flags = RECV_PRIORITY if self.gpu_config.priority_dequeue else 0
+        a = self._index(agent_id)
+        deadline = now + visibility_timeout
+        out: List[Message] = []
+        remaining = max_messages
+        while remaining > 0:
+            try:
+                _, ent, snd, pay, base = self.shard.receive_leased([a], remaining, deadline, flags)
+            except SdbError as e:
+                if out and e.code == -6:                   # SDB_ECAPACITY
+                    break                                  # the store is full: what was leased so far is returned
+                raise
+            if len(ent) == 0:
+                break
+            hdr, full = _native.expand_compact(ent, snd, pay)
+            msgs = self._decode(hdr, full, agent_id)
+            for k, m in enumerate(msgs):
+                self._leases.setdefault(m.id, []).append((a, base + k))
+            out += msgs
+            remaining -= len(ent)
+        if out:
+            heapq.heappush(self._lease_deadlines, deadline)
+        return out
+
+    def receive_batch_leased(self, agent_idx=None, max_messages: int = 100, visibility_timeout: float = 30.0,
+                             priority: Optional[bool] = None, **kw):
+        """receive_batch_compact, leased (Shard.receive_leased): (counts, entries, sends, payload, lease_base); entry r
+        holds lease lease_base + r, for settle_leases.  Index-level: no host message records."""
+        self.flush()
+        pr = self.gpu_config.priority_dequeue if priority is None else priority
+        deadline = time.time() + visibility_timeout
+        res = self.shard.receive_leased(agent_idx, max_messages, deadline, RECV_PRIORITY if pr else 0, **kw)
+        if len(res[1]):
+            heapq.heappush(self._lease_deadlines, deadline)
+        return res
+
+    def settle_leases(self, lease_ids, op: int = _native.LEASE_ACK, deadline: float = 0.0) -> np.ndarray:
+        """Bulk settle by lease id: op LEASE_ACK, or LEASE_RENEW with a new deadline (-inf: due now).  Returns one flag
+        per id, 1 where the lease was live."""
+        if op == _native.LEASE_RENEW:
+            heapq.heappush(self._lease_deadlines, float(deadline))
+        return self.shard.lease_settle(lease_ids, op, deadline)[0]
+
+    def _agent_leases(self, agent_id: str, message_ids: Iterable[str]) -> List[int]:
+        a = self._agent_idx.get(agent_id)
+        return [lid for mid in message_ids for (x, lid) in self._leases.get(mid, []) if x == a]
+
+    def _forget(self, agent_idx: Optional[int], message_ids: Iterable[str]) -> None:
+        for mid in message_ids:
+            left = [(x, lid) for (x, lid) in self._leases.get(mid, []) if agent_idx is not None and x != agent_idx]
+            if left:
+                self._leases[mid] = left
+            else:
+                self._leases.pop(mid, None)
+
+    def ack_messages(self, agent_id: str, message_ids: Iterable[str]) -> int:
+        """The agent is done with these messages: their leases are settled and never redelivered.  Returns how many were
+        still leased (a message already redelivered, or never leased, counts 0)."""
+        message_ids = list(message_ids)
+        ids = self._agent_leases(agent_id, message_ids)
+        n = int(self.shard.lease_settle(ids, _native.LEASE_ACK)[1]) if ids else 0
+        self._forget(self._agent_idx.get(agent_id), message_ids)
+        for mid in message_ids:
+            if mid in self.messages:
+                self.messages[mid].status = MessageStatus.PROCESSED
+        return n
+
+    def nack_messages(self, agent_id: str, message_ids: Iterable[str]) -> int:
+        """Give the messages back now: the next sweep (the next leased receive, or redeliver_expired) redelivers them."""
+        return self.extend_leases(agent_id, message_ids, visibility_timeout=-np.inf)
+
+    def extend_leases(self, agent_id: str, message_ids: Iterable[str], visibility_timeout: float = 30.0) -> int:
+        """Move the deadline of the agent's live leases on these messages to now + visibility_timeout."""
+        ids = self._agent_leases(agent_id, message_ids)
+        if not ids:
+            return 0
+        deadline = time.time() + visibility_timeout
+        heapq.heappush(self._lease_deadlines, deadline)
+        return int(self.shard.lease_settle(ids, _native.LEASE_RENEW, deadline)[1])
+
+    def redeliver_expired(self, now: Optional[float] = None, all: bool = False) -> int:
+        """Sweep every lease whose deadline has passed (all=True: every live lease) back to its agent's queue, behind
+        what is pending.  Returns the messages redelivered; agents whose queue is full keep theirs leased."""
+        self.flush()
+        now = time.time() if now is None else now
+        total = 0
+        while True:
+            red, blocked, left = self.shard.lease_sweep(now, _native.LEASE_ALL if all else 0)
+            total += red
+            if left == 0 or red == 0:
+                break
+        if not all and not blocked:
+            while self._lease_deadlines and self._lease_deadlines[0] <= now:
+                heapq.heappop(self._lease_deadlines)
+        return total
+
+    def _sweep_due(self, now: float) -> None:
+        if self._lease_deadlines and self._lease_deadlines[0] <= now:
+            self.redeliver_expired(now)
+
     def _pre_read(self) -> None:
         """Make buffered sends visible before a read (a sharded front-end reads only what earlier collective
         flushes delivered, so it overrides this with a no-op)."""
@@ -903,9 +1023,15 @@ class SwarmsDB:
         into a fresh instance: the agent and group tables in index order, the id nonce, the sequence counter and the
         pending records as PEEK compact receives in stream order (rows renumbered by smallest seq).  Nothing is
         consumed.  An agent with more pending records than one receive call holds raises: a snapshot is complete or it
-        is not written."""
+        is not written.  Leased messages not yet acked are in flight, not pending, and are not in the snapshot: call
+        redeliver_expired(all=True) first to include them."""
         self.flush()
         g = self.gpu_config
+        if g.lease_records:
+            live = self.shard.lease_stats()["live"]
+            if live:
+                logger.warning(f"queue snapshot leaves out {live} leased messages in flight "
+                               f"(redeliver_expired(all=True) first to include them)")
         cap = recv_capacity(g)
         agents = np.arange(len(self._agent_name), dtype=np.uint32)
         parts: List[Tuple[np.ndarray, ...]] = []
@@ -1086,6 +1212,9 @@ class SwarmsDB:
         return picked
 
     def mark_message_as_processed(self, message_id: str) -> bool:
+        leased = [lid for _, lid in self._leases.pop(message_id, [])]
+        if leased:                                     # a leased message is done: every live lease on it is acked
+            self.shard.lease_settle(leased, _native.LEASE_ACK)
         m = self.messages.get(message_id)
         if m is None:
             return False
@@ -1196,10 +1325,13 @@ class SwarmsDB:
                 recv[m.receiver_id] = recv.get(m.receiver_id, 0) + 1
         by_agent = {a: {"sent": sent.get(a, 0), "received": recv.get(a, 0), "total": sent.get(a, 0) + recv.get(a, 0)}
                     for a in self.registered_agents}
-        return {"total_messages": self.message_count, "active_agents": len(self.registered_agents),
-                "messages_by_type": by_type, "messages_by_status": by_status, "messages_by_agent": by_agent,
-                "last_save_time": self.last_save_time, "device": self.shard.stats(),
-                "queue": self.shard.queue_stats()}            # pending totals / priority histogram / deepest inbox, computed on the device
+        out = {"total_messages": self.message_count, "active_agents": len(self.registered_agents),
+               "messages_by_type": by_type, "messages_by_status": by_status, "messages_by_agent": by_agent,
+               "last_save_time": self.last_save_time, "device": self.shard.stats(),
+               "queue": self.shard.queue_stats()}             # pending totals / priority histogram / deepest inbox, computed on the device
+        if self.gpu_config.lease_records:
+            out["leases"] = self.shard.lease_stats()
+        return out
 
     def resend_failed_messages(self) -> List[str]:
         resent: List[str] = []

@@ -69,6 +69,20 @@ cudaError_t sdb_launch_restore_plan(const sdb_dev_view*, const sdb_restore_args*
 cudaError_t sdb_launch_restore_write(const sdb_dev_view*, const sdb_restore_args*, unsigned long long, uint32_t, cudaStream_t,
                                      sdb_profiler*, int*, int);
 const void* sdb_restore_kernel_anchor();
+cudaError_t sdb_launch_lease_append(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_compact_args*, const uint32_t*,
+                                    const unsigned long long*, const uint32_t*, uint32_t, uint32_t, uint32_t, unsigned long long,
+                                    unsigned long long, double, uint64_t, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_settle(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t, double, cudaStream_t,
+                                    sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_due(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, double, uint32_t, cudaStream_t, sdb_profiler*,
+                                 int*);
+cudaError_t sdb_launch_lease_select(const sdb_dev_view*, const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t,
+                                    uint32_t*, uint32_t*, uint32_t*, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_stage(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, unsigned long long,
+                                   const sdb_compact_args*, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_compact(const sdb_lease_buf*, const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t,
+                                     cudaStream_t, sdb_profiler*, int*, int);
+const void* sdb_lease_kernel_anchor();
 }
 
 #define SDB_SCAN_TILE 4096u
@@ -201,6 +215,17 @@ struct sdb_ctx {
   uint32_t* rs_agent = nullptr;                          // restore: per-agent tables [6][max_agents] + scan tops, allocated
   unsigned long long* rs_tot = nullptr;                  // on first use; totals [8]
   uint32_t* rs_sort = nullptr;                           // restore: radix-sort keys / values [4][max_recv_records] + digit tables
+  // lease store (sdb_lease_reserve): two buffers (a sweep compacts one into the other), scratch, host bookkeeping
+  struct LeaseStore {
+    sdb_lease_buf buf[2]{}; int cur = 0;
+    sdb_lease_scratch s{};
+    unsigned long long* th = nullptr;                    // pinned mirror of s.tot
+    std::vector<void*> mem;                              // every device allocation of the store
+    uint64_t cap = 0, pay_cap = 0;                       // entries (and rows), payload bytes
+    uint64_t used = 0, rows = 0, pay = 0;                // in buf[cur]
+    uint64_t next_id = 0;                                // lease ids, monotonic per handle
+    uint64_t live = 0, acked = 0, redelivered_total = 0, acked_total = 0;
+  } lease;
   // backends
   uint32_t* be_weight = nullptr; unsigned long long* be_load = nullptr; uint32_t n_backends = 0;
   uint32_t* be_req_cost = nullptr; uint32_t* be_out = nullptr; unsigned long long* be_scratch = nullptr;
@@ -296,7 +321,7 @@ cudaError_t load_all_kernels() {
     if (q != cudaDriverEntryPointSuccess || !*fp) return cudaErrorNotSupported;
   }
   for (const void* anchor : {sdb_send_kernel_anchor(), sdb_recv_kernel_anchor(), sdb_balance_kernel_anchor(), sdb_xshard_kernel_anchor(),
-                              sdb_restore_kernel_anchor()}) {
+                              sdb_restore_kernel_anchor(), sdb_lease_kernel_anchor()}) {
     cudaFunction_t f = nullptr;
     cudaError_t e = cudaGetFuncBySymbol(&f, anchor);
     if (e != cudaSuccess) return e;
@@ -950,6 +975,8 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
   return SDB_OK;
 }
 
+static void lease_free(sdb_ctx* h);
+
 int sdb_destroy(sdb_handle h) {
   if (!h) return SDB_EINVAL;
   cudaSetDevice(h->cfg.device);
@@ -981,6 +1008,7 @@ int sdb_destroy(sdb_handle h) {
                  h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out, h->where_bits, h->where_kw,
                  h->rs_agent, h->rs_tot, h->rs_sort};
   for (void* p : dev) if (p) cudaFree(p);
+  lease_free(h);
   if (h->descs_host) cudaFreeHost(h->descs_host);
   if (h->list_host) cudaFreeHost(h->list_host);
   if (h->lp_host) cudaFreeHost(h->lp_host);
@@ -1035,19 +1063,25 @@ int sdb_profile(sdb_handle h, int enable) {
   return SDB_OK;
 }
 
-int sdb_profile_read(sdb_handle h, double* ms_out, uint64_t* count_out) {
+int sdb_profile_read_n(sdb_handle h, uint32_t n, double* ms_out, uint64_t* count_out) {
   if (!h || !ms_out || !count_out) return SDB_EINVAL;
-  for (int k = 0; k < SDB_PK_N; ++k) { ms_out[k] = 0.0; count_out[k] = 0; }
+  for (uint32_t k = 0; k < n; ++k) { ms_out[k] = 0.0; count_out[k] = 0; }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  const int classes = static_cast<int>(std::min<uint32_t>(n, SDB_PK_ALL));
   sdb_profiler& p = h->prof;
   for (int i = 0; i < p.n; ++i) {
     float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, p.ev_a[i], p.ev_b[i]) == cudaSuccess && p.kind[i] < SDB_PK_N) {
+    if (cudaEventElapsedTime(&ms, p.ev_a[i], p.ev_b[i]) == cudaSuccess && p.kind[i] < classes) {
       ms_out[p.kind[i]] += ms; count_out[p.kind[i]] += 1;
     }
   }
   p.n = 0;
   return SDB_OK;
+}
+
+// ABI-1 callers pass arrays of SDB_PK_N entries: the classes past it are left out
+int sdb_profile_read(sdb_handle h, double* ms_out, uint64_t* count_out) {
+  return sdb_profile_read_n(h, SDB_PK_N, ms_out, count_out);
 }
 
 int sdb_get_stats(sdb_handle h, sdb_stats* out) {
@@ -1975,6 +2009,10 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
   return SDB_OK;
 }
 
+static int restore_ensure(sdb_ctx* h);
+static int restore_staged(sdb_ctx* h, uint32_t n_agents, uint64_t n_entries, uint64_t n_sends, uint64_t payload_bytes, bool owned,
+                          uint64_t* records_out);
+
 int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, const uint32_t* count,
                         const sdb_recv_entry* entries, uint64_t n_entries, const sdb_recv_send* sends, uint64_t n_sends,
                         const uint8_t* payload, uint64_t payload_bytes, uint32_t flags, uint64_t* restored_out,
@@ -1996,19 +2034,11 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
   if (n_entries > rec_cap || n_sends > rec_cap || payload_bytes > rec_cap * pad32(h->cfg.max_payload_bytes))
     return fail(h, SDB_ECAPACITY, "sdb_restore_compact: input larger than one compact receive's capacity");
   if (n_agents == 0) return SDB_OK;
-  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
-  const size_t A = h->cfg.max_agents, tiles = A / SDB_SCAN_TILE + 2;
-  const size_t R = h->cfg.max_recv_records, H = 256 * (R / 1024 + 1);
-  if (!h->rs_agent) {
-    const int rc = dmalloc_set(h, {{&h->rs_sort, 4 * R + 2 * H + H / SDB_SCAN_TILE + 2}, {&h->rs_tot, 8}, {&h->rs_agent, 6 * A + tiles}},
-                               "restore: device allocation failed");
-    if (rc != SDB_OK) return rc;
-  }
+  { const int rc = restore_ensure(h); if (rc != SDB_OK) return rc; }
+  const size_t A = h->cfg.max_agents;
   std::vector<uint32_t> first(n_agents);
   { uint32_t run = 0; for (uint32_t i = 0; i < n_agents; ++i) { first[i] = run; run += count[i]; } }
-  sdb_restore_args r{};
   uint32_t* t = h->rs_agent;
-  r.agent = t; r.count = t + A; r.first = t + 2 * A; r.nsh = t + 3 * A; r.pgran = t + 4 * A; r.p_local = t + 5 * A; r.p_tops = t + 6 * A;
   const size_t n = n_agents;
   CUDA_TRY(h, cudaMemcpyAsync(t, agent_idx, n * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaMemcpyAsync(t + A, count, n * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
@@ -2017,11 +2047,43 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
   if (n_entries) CUDA_TRY(h, cudaMemcpyAsync(c.entry_out, entries, n_entries * sizeof(sdb_recv_entry), cudaMemcpyHostToDevice, h->stream));
   if (n_sends) CUDA_TRY(h, cudaMemcpyAsync(c.send_out, sends, n_sends * sizeof(sdb_recv_send), cudaMemcpyHostToDevice, h->stream));
   if (payload_bytes) CUDA_TRY(h, cudaMemcpyAsync(c.payload_out, payload, payload_bytes, cudaMemcpyHostToDevice, h->stream));
+  uint64_t records = 0;
+  { const int rc = restore_staged(h, n_agents, n_entries, n_sends, payload_bytes, (flags & SDB_RECV_OWNED) && h->sharded, &records);
+    if (rc != SDB_OK) return rc; }
+  for (uint32_t i = 0; i < n_agents; ++i) h->n_agents = std::max(h->n_agents, agent_idx[i] + 1);
+  h->stream_busy = false;
+  if (restored_out) *restored_out = records;
+  if (seq_end_out) *seq_end_out = h->next_seq;
+  return SDB_OK;
+}
+
+// restore's per-agent tables and radix-sort scratch (and the compact receive buffers its input is staged in), allocated on
+// the first restore or lease sweep
+static int restore_ensure(sdb_ctx* h) {
+  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  if (h->rs_agent) return SDB_OK;
+  const size_t A = h->cfg.max_agents, tiles = A / SDB_SCAN_TILE + 2;
+  const size_t R = h->cfg.max_recv_records, H = 256 * (R / 1024 + 1);
+  return dmalloc_set(h, {{&h->rs_sort, 4 * R + 2 * H + H / SDB_SCAN_TILE + 2}, {&h->rs_tot, 8}, {&h->rs_agent, 6 * A + tiles}},
+                     "restore: device allocation failed");
+}
+
+// Plans and writes a restore whose input is staged on the device: the records in the compact receive's entry_out /
+// send_out / payload_out and the per-agent tables (agent, count, first) in rs_agent.  Validates and plans, synchronises
+// once, reserves arena space and writes; on any error nothing was written.  *records_out = records enqueued.
+static int restore_staged(sdb_ctx* h, uint32_t n_agents, uint64_t n_entries, uint64_t n_sends, uint64_t payload_bytes, bool owned,
+                          uint64_t* records_out) {
+  const size_t A = h->cfg.max_agents;
+  const size_t R = h->cfg.max_recv_records, H = 256 * (R / 1024 + 1);
+  sdb_restore_args r{};
+  uint32_t* t = h->rs_agent;
+  r.agent = t; r.count = t + A; r.first = t + 2 * A; r.nsh = t + 3 * A; r.pgran = t + 4 * A; r.p_local = t + 5 * A; r.p_tops = t + 6 * A;
+  sdb_compact_args& c = h->cx;
   r.ent = c.entry_out; r.snd = c.send_out; r.payload = c.payload_out; r.payload_bytes = payload_bytes;
   r.n = n_agents; r.n_entries = static_cast<uint32_t>(n_entries); r.n_sends = static_cast<uint32_t>(n_sends);
   r.max_payload = h->cfg.max_payload_bytes;
   r.shared = h->shared_cfg ? 1u : 0u;
-  r.owned = (flags & SDB_RECV_OWNED) && h->sharded ? 1u : 0u; r.shard_id = h->cfg.shard_id; r.shard_of = h->shard_of_dev;
+  r.owned = owned ? 1u : 0u; r.shard_id = h->cfg.shard_id; r.shard_of = h->shard_of_dev;
   // scratch of the compact receive (max_recv_records entries each; the hash table holds >= 4 x that many words) and of
   // the restore's radix sort
   uint32_t* tw = reinterpret_cast<uint32_t*>(c.table);
@@ -2062,10 +2124,213 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
     if (tot[2] + 1 > h->next_seq) h->next_seq = tot[2] + 1;
     h->dev_stale = true;
   }
-  for (uint32_t i = 0; i < n_agents; ++i) h->n_agents = std::max(h->n_agents, agent_idx[i] + 1);
+  *records_out = records;
+  return SDB_OK;
+}
+
+// ---- lease store: leased receive, settle, sweep ----------------------------------------------------------------------
+static void lease_free(sdb_ctx* h) {
+  sdb_ctx::LeaseStore& L = h->lease;
+  for (void* p : L.mem) cudaFree(p);
+  if (L.th) cudaFreeHost(L.th);
+  L.mem.clear(); L.th = nullptr;
+  L.buf[0] = L.buf[1] = sdb_lease_buf{}; L.s = sdb_lease_scratch{};
+  L.cap = L.pay_cap = L.used = L.rows = L.pay = L.acked = 0; L.cur = 0;
+}
+int sdb_lease_reserve(sdb_handle h, uint64_t max_records, uint64_t max_payload_bytes) {
+  if (!h) return SDB_EINVAL;
+  auto lease_alloc = [](sdb_ctx* c, auto** p, size_t n) {
+    void* q = nullptr;
+    if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(**p)) != cudaSuccess) return false;
+    c->lease.mem.push_back(q);
+    *p = static_cast<std::remove_reference_t<decltype(*p)>>(q);
+    return true;
+  };
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (L.live) return fail(h, SDB_EINVAL, "sdb_lease_reserve: the store holds live leases (ack them or sweep them back first)");
+  if (max_records > 0xFFFFFFF0ull) return fail(h, SDB_EINVAL, "sdb_lease_reserve: max_records above 2^32 - 16");
+  { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }        // cudaFree / cudaMalloc wait for running kernels
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   h->stream_busy = false;
-  if (restored_out) *restored_out = records;
-  if (seq_end_out) *seq_end_out = h->next_seq;
+  lease_free(h);
+  if (!max_records) return SDB_OK;
+  const uint64_t P = (max_payload_bytes + SDB_GRANULE - 1) & ~static_cast<uint64_t>(SDB_GRANULE - 1);
+  const size_t cap = max_records, R = h->cfg.max_recv_records, S = std::max(cap, R), A = h->cfg.max_agents;
+  const size_t tS = S / SDB_SCAN_TILE + 2, tR = R / SDB_SCAN_TILE + 2, tC = cap / SDB_SCAN_TILE + 2, tA = A / SDB_SCAN_TILE + 2;
+  const size_t H = 256 * (R / 1024 + 1);
+  bool ok = true;
+  for (sdb_lease_buf& b : L.buf)
+    ok = ok && lease_alloc(h, &b.ent, cap) && lease_alloc(h, &b.agent, cap) && lease_alloc(h, &b.id, cap) &&
+         lease_alloc(h, &b.deadline, cap) && lease_alloc(h, &b.state, cap) && lease_alloc(h, &b.rows, cap) &&
+         lease_alloc(h, &b.payload, P);
+  sdb_lease_scratch& s = L.s;
+  ok = ok && lease_alloc(h, &s.flag, S) && lease_alloc(h, &s.f_local, S) && lease_alloc(h, &s.f_tops, tS) &&
+       lease_alloc(h, &s.gran, S) && lease_alloc(h, &s.g_local, S) && lease_alloc(h, &s.g_tops, tS) &&
+       lease_alloc(h, &s.rfirst, cap) && lease_alloc(h, &s.rmap, cap) &&
+       lease_alloc(h, &s.rg, cap) && lease_alloc(h, &s.rg_local, cap) && lease_alloc(h, &s.rg_tops, tC) &&
+       lease_alloc(h, &s.chunk, R) && lease_alloc(h, &s.staged, R) && lease_alloc(h, &s.key_a, R) && lease_alloc(h, &s.key_b, R) &&
+       lease_alloc(h, &s.val_a, R) && lease_alloc(h, &s.val_b, R) &&
+       lease_alloc(h, &s.hist, H) && lease_alloc(h, &s.h_local, H) && lease_alloc(h, &s.h_tops, H / SDB_SCAN_TILE + 2) &&
+       lease_alloc(h, &s.run_begin, R + 1) && lease_alloc(h, &s.kcnt, R) && lease_alloc(h, &s.k_local, R) &&
+       lease_alloc(h, &s.k_tops, tR) && lease_alloc(h, &s.kflag, R) && lease_alloc(h, &s.kf_local, R) && lease_alloc(h, &s.kf_tops, tR) &&
+       lease_alloc(h, &s.a_local, A) && lease_alloc(h, &s.a_tops, tA) &&
+       lease_alloc(h, &s.req, SDB_LS_SETTLE_CHUNK) && lease_alloc(h, &s.at, SDB_LS_SETTLE_CHUNK) &&
+       lease_alloc(h, &s.settled, SDB_LS_SETTLE_CHUNK) && lease_alloc(h, &s.tot, 16);
+  ok = ok && cudaHostAlloc(reinterpret_cast<void**>(&L.th), 16 * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
+  if (!ok) {
+    lease_free(h);
+    cudaGetLastError();
+    return fail(h, SDB_ENOMEM, "sdb_lease_reserve: device allocation failed");
+  }
+  L.cap = cap; L.pay_cap = P;
+  return SDB_OK;
+}
+
+int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                       double deadline, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                       sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                       uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out, uint64_t* lease_base_out) {
+  if (!h) return SDB_EINVAL;
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (lease_base_out) *lease_base_out = L.next_id;
+  if (flags & ~(SDB_RECV_PRIORITY | SDB_RECV_OWNED))
+    return fail(h, SDB_EINVAL, "sdb_receive_leased accepts SDB_RECV_PRIORITY and SDB_RECV_OWNED only");
+  if (!L.cap) return fail(h, SDB_EINVAL, "sdb_receive_leased: no lease store (sdb_lease_reserve)");
+  const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
+  if (n_agents == 0 || max_messages == 0) return SDB_OK;
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
+  uint64_t rec_cap = 0;
+  { const int rc = out_rec_cap(h, std::min(room(entry_out, entry_cap), room(send_out, send_cap)), room(payload_out, payload_cap), &rec_cap);
+    if (rc != SDB_OK) return rc; }
+  const uint32_t P = pad32(h->cfg.max_payload_bytes);
+  rec_cap = std::min({rec_cap, L.cap - L.used, (L.pay_cap - L.pay) / P});     // the store takes every record of the call
+  if (rec_cap == 0) return fail(h, SDB_ECAPACITY, "lease store full: settle or sweep");
+  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  sdb_recv_args r{};
+  { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & SDB_RECV_PRIORITY, rec_cap, &r); if (rc != SDB_OK) return rc; }
+  int nl = 0;
+  cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx);
+  h->last_rx_valid = false; h->last_rx_compact = true;
+  if (e == cudaSuccess)
+    e = sdb_launch_lease_append(&L.buf[L.cur], &L.s, &h->cx, h->rx_count, h->rx_totals, r.agent_idx, n_agents,
+                                static_cast<uint32_t>(L.used), static_cast<uint32_t>(L.rows), L.pay, L.next_id, deadline, rec_cap,
+                                P, h->stream, &h->prof, &nl, h->sm_count);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("leased receive launch: ") + cudaGetErrorString(e));
+  uint64_t total = 0, n_sends = 0, pbytes = 0;
+  { const int rc = copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, &total, &n_sends, &pbytes);
+    if (rc != SDB_OK) return rc; }
+  L.used += total; L.rows += n_sends; L.pay += pbytes; L.live += total; L.next_id += total;
+  if (total_out) *total_out = total;
+  if (n_sends_out) *n_sends_out = n_sends;
+  if (payload_bytes_out) *payload_bytes_out = pbytes;
+  return SDB_OK;
+}
+
+int sdb_lease_settle(sdb_handle h, uint64_t n, const uint64_t* lease_id, uint32_t op, double deadline, uint8_t* settled_out,
+                     uint64_t* n_settled_out) {
+  if (!h) return SDB_EINVAL;
+  if (n_settled_out) *n_settled_out = 0;
+  if (op != SDB_LEASE_ACK && op != SDB_LEASE_RENEW) return fail(h, SDB_EINVAL, "sdb_lease_settle: op is SDB_LEASE_ACK or SDB_LEASE_RENEW");
+  if (n && !lease_id) return fail(h, SDB_EINVAL, "sdb_lease_settle: lease_id is NULL");
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (!L.cap) return fail(h, SDB_EINVAL, "sdb_lease_settle: no lease store (sdb_lease_reserve)");
+  uint64_t settled = 0, moved = 0;
+  for (uint64_t o = 0; o < n; o += SDB_LS_SETTLE_CHUNK) {
+    const uint32_t m = static_cast<uint32_t>(std::min<uint64_t>(SDB_LS_SETTLE_CHUNK, n - o));
+    CUDA_TRY(h, cudaMemcpyAsync(L.s.req, lease_id + o, m * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+    int nl = 0;
+    cudaError_t e = sdb_launch_lease_settle(&L.buf[L.cur], &L.s, static_cast<uint32_t>(L.used), m, op, deadline, h->stream, &h->prof, &nl);
+    h->launches += nl;
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease settle launch: ") + cudaGetErrorString(e));
+    CUDA_TRY(h, cudaMemcpyAsync(L.th, L.s.tot, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    if (settled_out) CUDA_TRY(h, cudaMemcpyAsync(settled_out + o, L.s.settled, m, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    settled += L.th[0]; moved += L.th[1];
+  }
+  h->stream_busy = false;
+  L.live -= moved; L.acked += moved; L.acked_total += moved;
+  if (n_settled_out) *n_settled_out = settled;
+  return SDB_OK;
+}
+
+// reads s.tot[lo, lo + k) into the store's pinned mirror, synchronising
+static int lease_totals(sdb_ctx* h, uint32_t lo, uint32_t k) {
+  CUDA_TRY(h, cudaMemcpyAsync(h->lease.th + lo, h->lease.s.tot + lo, k * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  return SDB_OK;
+}
+
+int sdb_lease_sweep(sdb_handle h, double now, uint32_t flags, uint64_t* redelivered_out, uint64_t* blocked_out,
+                    uint64_t* due_left_out) {
+  if (!h) return SDB_EINVAL;
+  if (redelivered_out) *redelivered_out = 0;
+  if (blocked_out) *blocked_out = 0;
+  if (due_left_out) *due_left_out = 0;
+  if (flags & ~SDB_LEASE_ALL) return fail(h, SDB_EINVAL, "sdb_lease_sweep accepts SDB_LEASE_ALL only");
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (!L.cap) return fail(h, SDB_EINVAL, "sdb_lease_sweep: no lease store (sdb_lease_reserve)");
+  { int rcc = cursor_to_host(h); if (rcc != SDB_OK) return rcc; }      // redelivery is a host-placed write, like a send
+  if (L.used == 0) return SDB_OK;
+  { const int rc = restore_ensure(h); if (rc != SDB_OK) return rc; }
+  const sdb_lease_buf& b = L.buf[L.cur];
+  const uint32_t used = static_cast<uint32_t>(L.used), rows = static_cast<uint32_t>(L.rows);
+  int nl = 0;
+  cudaError_t e = sdb_launch_lease_due(&b, &L.s, used, now, flags & SDB_LEASE_ALL, h->stream, &h->prof, &nl);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease sweep launch: ") + cudaGetErrorString(e));
+  { const int rc = lease_totals(h, 0, 1); if (rc != SDB_OK) return rc; }
+  const uint64_t due = L.th[0];
+  const uint32_t n = static_cast<uint32_t>(std::min<uint64_t>(due, recv_rec_cap(h)));    // one compact receive's capacity
+  uint64_t staged = 0, blocked = 0, redelivered = 0;
+  if (n) {
+    const size_t A = h->cfg.max_agents;
+    nl = 0;
+    e = sdb_launch_lease_select(&h->view, &b, &L.s, used, n, h->cfg.max_agents, h->rs_agent, h->rs_agent + A, h->rs_agent + 2 * A,
+                                h->stream, &h->prof, &nl);
+    h->launches += nl;
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease sweep launch: ") + cudaGetErrorString(e));
+    { const int rc = lease_totals(h, 1, 5); if (rc != SDB_OK) return rc; }
+    staged = L.th[2]; blocked = L.th[4];
+    const uint32_t kept_runs = static_cast<uint32_t>(L.th[3]), agent_end = static_cast<uint32_t>(L.th[5]);
+    if (staged) {
+      nl = 0;
+      e = sdb_launch_lease_stage(&b, &L.s, rows, static_cast<uint32_t>(staged), h->next_seq, &h->cx, h->stream, &h->prof, &nl, h->sm_count);
+      h->launches += nl;
+      if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease sweep launch: ") + cudaGetErrorString(e));
+      { const int rc = lease_totals(h, 6, 2); if (rc != SDB_OK) return rc; }
+      { const int rc = restore_staged(h, kept_runs, staged, L.th[6], L.th[7] * SDB_GRANULE, false, &redelivered);
+        if (rc != SDB_OK) return rc; }                                     // SDB_EARENA_FULL: nothing written, store unchanged
+      h->n_agents = std::max(h->n_agents, agent_end);
+    }
+  }
+  // compaction: redelivered and acked entries are dropped, with the rows and payloads no live entry names
+  nl = 0;
+  e = sdb_launch_lease_compact(&b, &L.buf[L.cur ^ 1], &L.s, used, rows, static_cast<uint32_t>(staged), h->stream, &h->prof, &nl,
+                               h->sm_count);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease sweep launch: ") + cudaGetErrorString(e));
+  { const int rc = lease_totals(h, 8, 3); if (rc != SDB_OK) return rc; }
+  h->stream_busy = false;
+  L.cur ^= 1;
+  L.used = L.th[8]; L.rows = L.th[9]; L.pay = L.th[10] * SDB_GRANULE;
+  L.live -= staged; L.redelivered_total += staged; L.acked = 0;
+  if (redelivered_out) *redelivered_out = staged;
+  if (blocked_out) *blocked_out = blocked;
+  if (due_left_out) *due_left_out = due - n;
+  return SDB_OK;
+}
+
+int sdb_lease_stats(sdb_handle h, sdb_lease_summary* out) {
+  if (!h || !out) return SDB_EINVAL;
+  const sdb_ctx::LeaseStore& L = h->lease;
+  out->live = L.live; out->acked_unreclaimed = L.acked;
+  out->redelivered_total = L.redelivered_total; out->acked_total = L.acked_total;
+  out->entries_used = L.used; out->entries_reserved = L.cap;
+  out->payload_used = L.pay; out->payload_reserved = L.pay_cap;
   return SDB_OK;
 }
 

@@ -229,6 +229,40 @@ struct sdb_restore_args {
 #define SDB_RS_EINVAL 1ull         // tot[3]: a bad entry or row
 #define SDB_RS_ERING 2ull          // tot[3]: some agent's ring cannot take its records
 
+// ---- lease store (sdb_receive_leased / sdb_lease_settle / sdb_lease_sweep, sdb_lease.cu): one of its two buffers.  Entries
+// are in lease-id order (append-only, then stable compaction); rows and payloads in the compact receive format.
+#define SDB_LS_LIVE 0u
+#define SDB_LS_ACKED 1u
+#define SDB_LS_REDELIVERED 2u
+struct sdb_lease_buf {
+  sdb_recv_entry* ent;             // [cap] seq, store row, receiver
+  uint32_t* agent;                 // [cap]
+  unsigned long long* id;          // [cap] lease ids, ascending
+  double* deadline;                // [cap]
+  uint32_t* state;                 // [cap] SDB_LS_*
+  sdb_recv_send* rows;             // [cap] payload_off into `payload`
+  uint8_t* payload;                // [payload cap]
+};
+// scratch of the store's kernels; S = max(cap, max_recv_records), R = max_recv_records
+struct sdb_lease_scratch {
+  uint32_t* flag; uint32_t* f_local; uint32_t* f_tops;     // [S] entry or position flags and their scan
+  uint32_t* gran; uint32_t* g_local; uint32_t* g_tops;     // [S] row flags / granules and their scan
+  uint32_t* rfirst; uint32_t* rmap;                        // [cap] per store row: first seq-sorted position, new index
+  uint32_t* rg; uint32_t* rg_local; uint32_t* rg_tops;     // [cap] compaction: granules of each kept row and their scan
+  uint32_t* chunk; uint32_t* staged;                       // [R] store entry of each chunk / staged position
+  uint32_t* key_a; uint32_t* key_b; uint32_t* val_a; uint32_t* val_b;   // [R] radix sort
+  uint32_t* hist; uint32_t* h_local; uint32_t* h_tops;     // radix sort digit tables
+  uint32_t* run_begin;                                     // [R + 1] first chunk position of each agent run
+  uint32_t* kcnt; uint32_t* k_local; uint32_t* k_tops;     // [R] entries each run keeps, and their scan
+  uint32_t* kflag; uint32_t* kf_local; uint32_t* kf_tops;  // [R] 1 for a kept run, and the scan
+  uint32_t* a_local; uint32_t* a_tops;                     // [max_agents] append: scan of the receive's counts
+  unsigned long long* req;                                 // [SDB_LS_SETTLE_CHUNK] settle: lease ids ...
+  uint32_t* at;                                            // ... their store entries ...
+  uint8_t* settled;                                        // ... and the verdicts
+  unsigned long long* tot;                                 // [16]
+};
+#define SDB_LS_SETTLE_CHUNK (1u << 20)
+
 // ---- asynchronous import (sdb_import_wire_ptrs_async): everything the host used to learn through a sync lives on
 // the device.  `sdb_cursor` is the device-resident twin of the host's arena / sequence counters (whoever advanced
 // them last marks the other side stale); `sdb_batch_base` carries one import's placement from the kernel that

@@ -1,0 +1,459 @@
+// sdb_lease.cu - the lease store of leased receives (sdb_receive_leased, sdb_lease_settle, sdb_lease_sweep), sm_90a.
+//
+// The store holds a copy of every record a leased receive handed out, in the compact receive format: per entry its
+// sdb_recv_entry (send = store row), agent, lease id, deadline and state; rows with payload_off into the store's payload.
+// Entries stay in lease-id order: appends go to the tail and compaction is stable, so a settle is a binary search.
+//
+// Append (after the compact receive's back end, same stream)
+//   k_lease_append_agents  one warp per listed agent: agent, lease id, deadline, state of its entries (offsets = scan of
+//                          the receive's counts)
+//   k_lease_append_copy    entries (send rebased), rows (payload_off rebased) and payload granules behind the tail
+// Settle
+//   k_lease_settle_find    one thread per request: binary search over the ascending ids, verdict = live before the call
+//   k_lease_settle_apply   the transition (ack: live -> acked once; renew: new deadline)
+// Sweep (the host synchronises between the phases to size the next one)
+//   due      k_lease_due + scan: live and due entries
+//   select   k_lease_chunk (first C due entries in lease-id order, keyed by agent), stable radix sort by agent
+//            (sdb_radix_sort_u32, restore's kernels), k_lease_run_heads + scan + k_lease_run_begin (agent runs),
+//            k_lease_ring_check (blocked agents keep their records), scans, k_lease_stage_list (store entries in agent
+//            order + the restore's per-agent tables)
+//   stage    stable radix sort of the staged entries by seq, k_lease_row_first / k_lease_row_heads + scans (rows numbered
+//            by their smallest staged seq), k_lease_stage_rows (rows + payloads into the compact scratch),
+//            k_lease_stage_entries
+//   (the host then runs restore's plan and write phases on the staged input)
+//   compact  k_lease_mark (staged -> redelivered), k_lease_keep + scans, k_lease_keep_rows + scans, k_lease_copy_entries,
+//            k_lease_copy_rows into the other buffer
+#include "sdb_common.cuh"
+
+#define SDB_SCAN_TILE 4096u
+
+extern "C" cudaError_t sdb_scan_u32(const uint32_t* in, uint32_t* local, uint32_t* tops, uint32_t n,
+                                    unsigned long long* total_out, uint32_t* out, cudaStream_t stream);
+extern "C" cudaError_t sdb_radix_sort_u32(uint32_t* ka, uint32_t* va, uint32_t* kb, uint32_t* vb, uint32_t n, uint32_t bits,
+                                          uint32_t* hist, uint32_t* h_local, uint32_t* h_tops, uint32_t** kres, uint32_t** vres,
+                                          cudaStream_t stream, int* n_launches);
+
+__device__ __forceinline__ uint32_t ls_scan(const uint32_t* local, const uint32_t* tops, uint32_t i) {
+  return local[i] + tops[i / SDB_SCAN_TILE];
+}
+__device__ __forceinline__ uint32_t ls_pg(uint32_t len) { return ((len + 31u) & ~31u) >> 5; }
+// row i as two 16-byte words: {timestamp, payload_off}, {sender, group, len | prio << 16 | type << 24, reserved}
+__device__ __forceinline__ void ls_row(const sdb_recv_send* rows, uint32_t i, uint4& lo, uint4& hi) {
+  const uint4* p = reinterpret_cast<const uint4*>(rows + i);
+  lo = p[0]; hi = p[1];
+}
+__device__ __forceinline__ void ls_put_row(sdb_recv_send* rows, uint32_t i, uint4 lo, const uint4& hi, unsigned long long off) {
+  uint4* p = reinterpret_cast<uint4*>(rows + i);
+  lo.z = static_cast<uint32_t>(off); lo.w = static_cast<uint32_t>(off >> 32);
+  p[0] = lo; p[1] = hi;
+}
+// the warp copies the row's padded payload, 16 bytes per lane and step
+__device__ __forceinline__ void ls_copy_payload(const uint8_t* base, const uint4& lo, const uint4& hi, uint8_t* dst, uint32_t lane) {
+  const uint4* src = reinterpret_cast<const uint4*>(base + ((static_cast<unsigned long long>(lo.w) << 32) | lo.z));
+  uint4* d = reinterpret_cast<uint4*>(dst);
+  const uint32_t n = 2u * ls_pg(hi.z & 0xFFFFu);
+  for (uint32_t c = lane; c < n; c += 32) d[c] = src[c];
+}
+
+static uint32_t ls_grid(uint64_t items, uint64_t per_block, int sm_count) {
+  uint64_t g = (items + per_block - 1) / per_block;
+  const uint64_t cap = static_cast<uint64_t>(sm_count) * 8;
+  if (g > cap) g = cap;
+  return static_cast<uint32_t>(g ? g : 1);
+}
+static uint32_t ls_bits(uint64_t max_key) {
+  uint32_t b = 1;
+  while (b < 32 && (max_key >> b)) ++b;
+  return b;
+}
+
+// ---- append -----------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_lease_append_agents(sdb_lease_buf b, const uint32_t* __restrict__ count, const uint32_t* __restrict__ local,
+                      const uint32_t* __restrict__ tops, const uint32_t* __restrict__ agents, uint32_t n, uint32_t used,
+                      unsigned long long id_base, double deadline) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t q = gw; q < n; q += nw) {
+    const uint32_t c = count[q];
+    if (!c) continue;
+    const uint32_t off = ls_scan(local, tops, q), a = agents ? agents[q] : q;
+    for (uint32_t j = lane; j < c; j += 32) {
+      const uint32_t e = used + off + j;
+      b.agent[e] = a; b.id[e] = id_base + off + j; b.deadline[e] = deadline; b.state[e] = SDB_LS_LIVE;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_lease_append_copy(sdb_lease_buf b, const sdb_recv_entry* __restrict__ ent, const sdb_recv_send* __restrict__ snd,
+                    const uint8_t* __restrict__ pay, const unsigned long long* __restrict__ rx_totals,
+                    const unsigned long long* __restrict__ cx_totals, uint32_t used, uint32_t rows_used,
+                    unsigned long long pay_used) {
+  const uint64_t n = rx_totals[0], nr = cx_totals[0], nc = cx_totals[1] * 2;     // 16-byte chunks of payload
+  const uint64_t m = n > nr ? (n > nc ? n : nc) : (nr > nc ? nr : nc);
+  for (uint64_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+    if (i < n) { sdb_recv_entry e = ent[i]; e.send += rows_used; b.ent[used + i] = e; }
+    if (i < nr) { sdb_recv_send s = snd[i]; s.payload_off += pay_used; b.rows[rows_used + i] = s; }
+    if (i < nc) reinterpret_cast<uint4*>(b.payload + pay_used)[i] = reinterpret_cast<const uint4*>(pay)[i];
+  }
+}
+
+// ---- settle -----------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_lease_settle_find(sdb_lease_buf b, uint32_t used, sdb_lease_scratch s, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool live = false;
+  if (i < n) {
+    const unsigned long long x = s.req[i];
+    uint32_t lo = 0, hi = used;
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (b.id[mid] < x) lo = mid + 1; else hi = mid;
+    }
+    live = lo < used && b.id[lo] == x && b.state[lo] == SDB_LS_LIVE;
+    s.at[i] = live ? lo : 0xFFFFFFFFu;
+    s.settled[i] = live ? 1 : 0;
+  }
+  const uint32_t c = __popc(__ballot_sync(0xFFFFFFFFu, live));
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(s.tot + 0, static_cast<unsigned long long>(c));
+}
+
+__global__ void __launch_bounds__(256)
+k_lease_settle_apply(sdb_lease_buf b, sdb_lease_scratch s, uint32_t n, uint32_t op, double deadline) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool moved = false;
+  if (i < n) {
+    const uint32_t e = s.at[i];
+    if (e != 0xFFFFFFFFu) {
+      if (op == 0u) moved = atomicCAS(b.state + e, SDB_LS_LIVE, SDB_LS_ACKED) == SDB_LS_LIVE;
+      else b.deadline[e] = deadline;
+    }
+  }
+  const uint32_t c = __popc(__ballot_sync(0xFFFFFFFFu, moved));
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(s.tot + 1, static_cast<unsigned long long>(c));
+}
+
+// ---- sweep: due ---------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_lease_due(sdb_lease_buf b, uint32_t used, double now, uint32_t all, uint32_t* __restrict__ flag) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= used) return;
+  flag[e] = b.state[e] == SDB_LS_LIVE && (all || b.deadline[e] <= now) ? 1u : 0u;   // NaN on either side: not due
+}
+
+// ---- sweep: select ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_lease_chunk(sdb_lease_buf b, uint32_t used, sdb_lease_scratch s, uint32_t C) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= used || !s.flag[e]) return;
+  const uint32_t p = ls_scan(s.f_local, s.f_tops, e);
+  if (p >= C) return;
+  s.chunk[p] = e; s.key_a[p] = b.agent[e]; s.val_a[p] = p;
+}
+
+__global__ void __launch_bounds__(256)
+k_lease_run_heads(const uint32_t* __restrict__ key, uint32_t n, uint32_t* __restrict__ head) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) head[i] = (i == 0 || key[i] != key[i - 1]) ? 1u : 0u;
+}
+
+__global__ void __launch_bounds__(256)
+k_lease_run_begin(sdb_lease_scratch s, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (s.gran[i]) s.run_begin[ls_scan(s.g_local, s.g_tops, i)] = i;
+  if (i == 0) s.run_begin[s.tot[1]] = n;
+}
+
+// one thread per run: an agent whose ring cannot take all of its records keeps them in the store
+__global__ void __launch_bounds__(256)
+k_lease_ring_check(sdb_dev_view v, sdb_lease_scratch s, const uint32_t* __restrict__ key, uint32_t n) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t runs = static_cast<uint32_t>(s.tot[1]);
+  bool blocked = false;
+  if (r < runs) {
+    const uint32_t i0 = s.run_begin[r], c = s.run_begin[r + 1] - i0;
+    const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + key[i0]);   // {head, tail, ..}
+    blocked = static_cast<uint64_t>(h.y - h.x) + c > v.ring_slots;
+    s.kcnt[r] = blocked ? 0u : c;
+    s.kflag[r] = blocked ? 0u : 1u;
+  } else if (r < n) {
+    s.kcnt[r] = 0u; s.kflag[r] = 0u;                      // the scans run over n slots
+  }
+  const uint32_t k = __popc(__ballot_sync(0xFFFFFFFFu, blocked));
+  if ((threadIdx.x & 31) == 0 && k) atomicAdd(s.tot + 4, static_cast<unsigned long long>(k));
+}
+
+// chunk position i (agent order): its store entry goes to the staged list; a kept run's head fills the restore's tables
+__global__ void __launch_bounds__(256)
+k_lease_stage_list(sdb_lease_scratch s, const uint32_t* __restrict__ key, const uint32_t* __restrict__ val, uint32_t n,
+                   uint32_t* __restrict__ rs_agent, uint32_t* __restrict__ rs_count, uint32_t* __restrict__ rs_first) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t head = s.gran[i];
+  const uint32_t r = ls_scan(s.g_local, s.g_tops, i) + head - 1u;
+  const uint32_t c = s.kcnt[r];
+  if (!c) return;
+  const uint32_t base = ls_scan(s.k_local, s.k_tops, r);
+  s.staged[base + i - s.run_begin[r]] = s.chunk[val[i]];
+  if (head) {
+    const uint32_t q = ls_scan(s.kf_local, s.kf_tops, r);
+    rs_agent[q] = key[i]; rs_count[q] = c; rs_first[q] = base;
+    atomicMax(s.tot + 5, static_cast<unsigned long long>(key[i]) + 1ull);
+  }
+}
+
+// ---- sweep: stage -------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_lease_seq_keys(sdb_lease_buf b, sdb_lease_scratch s, uint32_t n) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  s.key_a[k] = static_cast<uint32_t>(b.ent[s.staged[k]].seq);
+  s.val_a[k] = k;
+}
+// the high words of the seqs in the order of the first pass (sequence numbers of 2^32 and above)
+__global__ void __launch_bounds__(256)
+k_lease_seq_hi(sdb_lease_buf b, sdb_lease_scratch s, const uint32_t* __restrict__ val, uint32_t* __restrict__ key, uint32_t n) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < n) key[p] = static_cast<uint32_t>(b.ent[s.staged[val[p]]].seq >> 32);
+}
+
+__global__ void __launch_bounds__(256)
+k_lease_row_first(sdb_lease_buf b, sdb_lease_scratch s, const uint32_t* __restrict__ sv, uint32_t n) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < n) atomicMin(s.rfirst + b.ent[s.staged[sv[p]]].send, p);
+}
+
+// seq-sorted position p heads its row when it is the row's first: rows are numbered in order of their smallest seq
+__global__ void __launch_bounds__(256)
+k_lease_row_heads(sdb_lease_buf b, sdb_lease_scratch s, const uint32_t* __restrict__ sv, uint32_t n) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const uint32_t row = b.ent[s.staged[sv[p]]].send;
+  const bool h = s.rfirst[row] == p;
+  s.flag[p] = h ? 1u : 0u;
+  s.gran[p] = h ? ls_pg(b.rows[row].len) : 0u;
+}
+
+// one warp per seq-sorted position: a head writes its row and payload into the compact scratch
+__global__ void __launch_bounds__(256)
+k_lease_stage_rows(sdb_lease_buf b, sdb_lease_scratch s, const uint32_t* __restrict__ sv, uint32_t n,
+                   sdb_recv_send* __restrict__ send_out, uint8_t* __restrict__ payload_out) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t p = gw; p < n; p += nw) {
+    if (!s.flag[p]) continue;
+    const uint32_t row = b.ent[s.staged[sv[p]]].send;
+    const uint32_t nr = ls_scan(s.f_local, s.f_tops, p);
+    const unsigned long long off = static_cast<unsigned long long>(ls_scan(s.g_local, s.g_tops, p)) << 5;
+    uint4 lo, hi;
+    ls_row(b.rows, row, lo, hi);
+    ls_copy_payload(b.payload, lo, hi, payload_out + off, lane);
+    if (lane == 0) {
+      s.rmap[row] = nr;
+      ls_put_row(send_out, nr, lo, hi, off);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_lease_stage_entries(sdb_lease_buf b, sdb_lease_scratch s, uint32_t n, sdb_recv_entry* __restrict__ entry_out) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  sdb_recv_entry e = b.ent[s.staged[k]];
+  e.send = s.rmap[e.send];
+  entry_out[k] = e;
+}
+
+// ---- sweep: compact -----------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_lease_mark(sdb_lease_buf b, sdb_lease_scratch s, uint32_t n) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) b.state[s.staged[k]] = SDB_LS_REDELIVERED;
+}
+
+// kept entries (live) and the rows they name
+__global__ void __launch_bounds__(256)
+k_lease_keep(sdb_lease_buf b, sdb_lease_scratch s, uint32_t used) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= used) return;
+  const bool keep = b.state[e] == SDB_LS_LIVE;
+  s.flag[e] = keep ? 1u : 0u;
+  if (keep) s.gran[b.ent[e].send] = 1u;
+}
+
+__global__ void __launch_bounds__(256)
+k_lease_keep_rows(sdb_lease_buf b, sdb_lease_scratch s, uint32_t rows) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < rows) s.rg[r] = s.gran[r] ? ls_pg(b.rows[r].len) : 0u;
+}
+
+__global__ void __launch_bounds__(256)
+k_lease_copy_entries(sdb_lease_buf in, sdb_lease_buf out, sdb_lease_scratch s, uint32_t used) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= used || !s.flag[e]) return;
+  const uint32_t k = ls_scan(s.f_local, s.f_tops, e);
+  sdb_recv_entry en = in.ent[e];
+  en.send = ls_scan(s.g_local, s.g_tops, en.send);
+  out.ent[k] = en; out.agent[k] = in.agent[e]; out.id[k] = in.id[e]; out.deadline[k] = in.deadline[e];
+  out.state[k] = SDB_LS_LIVE;
+}
+
+// one warp per row: a kept row and its payload
+__global__ void __launch_bounds__(256)
+k_lease_copy_rows(sdb_lease_buf in, sdb_lease_buf out, sdb_lease_scratch s, uint32_t rows) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t r = gw; r < rows; r += nw) {
+    if (!s.gran[r]) continue;
+    const uint32_t k = ls_scan(s.g_local, s.g_tops, r);
+    const unsigned long long off = static_cast<unsigned long long>(ls_scan(s.rg_local, s.rg_tops, r)) << 5;
+    uint4 lo, hi;
+    ls_row(in.rows, r, lo, hi);
+    ls_copy_payload(in.payload, lo, hi, out.payload + off, lane);
+    if (lane == 0) ls_put_row(out.rows, k, lo, hi, off);
+  }
+}
+
+// ---- launchers ----------------------------------------------------------------------------------------------------
+#define LS_LAUNCH(n_items, kern, ...)                                                        \
+  do {                                                                                       \
+    if ((n_items) > 0) { kern<<<((n_items) + 255) / 256, 256, 0, stream>>>(__VA_ARGS__); ++nl; } \
+  } while (0)
+
+// after a compact receive: its entries, rows and payloads (device totals) go to the store's tail
+extern "C" cudaError_t sdb_launch_lease_append(const sdb_lease_buf* b, const sdb_lease_scratch* s, const sdb_compact_args* cx,
+                                               const uint32_t* count, const unsigned long long* rx_totals, const uint32_t* agents,
+                                               uint32_t n_agents, uint32_t used, uint32_t rows_used, unsigned long long pay_used,
+                                               unsigned long long id_base, double deadline, uint64_t rec_cap, uint32_t max_pad,
+                                               cudaStream_t stream, sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  cudaError_t e = sdb_scan_u32(count, s->a_local, s->a_tops, n_agents, nullptr, nullptr, stream);
+  nl += 2;
+  k_lease_append_agents<<<ls_grid(n_agents, 8, sm_count * 4), 256, 0, stream>>>(*b, count, s->a_local, s->a_tops, agents, n_agents,
+                                                                                used, id_base, deadline);
+  const uint64_t items = rec_cap * (max_pad / 16u > 1u ? max_pad / 16u : 1u);
+  k_lease_append_copy<<<ls_grid(items, 256, sm_count * 4), 256, 0, stream>>>(*b, cx->entry_out, cx->send_out, cx->payload_out,
+                                                                             rx_totals, cx->totals, used, rows_used, pay_used);
+  nl += 2;
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// s->req[0, n) holds the ids; verdicts to s->settled, s->tot[0] = live requests, s->tot[1] = transitions
+extern "C" cudaError_t sdb_launch_lease_settle(const sdb_lease_buf* b, const sdb_lease_scratch* s, uint32_t used, uint32_t n,
+                                               uint32_t op, double deadline, cudaStream_t stream, sdb_profiler* prof,
+                                               int* n_launches) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  cudaMemsetAsync(s->tot, 0, 2 * sizeof(unsigned long long), stream);
+  LS_LAUNCH(n, k_lease_settle_find, *b, used, *s, n);
+  LS_LAUNCH(n, k_lease_settle_apply, *b, *s, n, op, deadline);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return cudaGetLastError();
+}
+
+// tot[0] = due entries
+extern "C" cudaError_t sdb_launch_lease_due(const sdb_lease_buf* b, const sdb_lease_scratch* s, uint32_t used, double now,
+                                            uint32_t all, cudaStream_t stream, sdb_profiler* prof, int* n_launches) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  cudaMemsetAsync(s->tot, 0, 16 * sizeof(unsigned long long), stream);
+  LS_LAUNCH(used, k_lease_due, *b, used, now, all, s->flag);
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream);
+  nl += used ? 2 : 0;
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// the first n due entries, sorted by agent, blocked agents dropped; writes s->staged and the restore's per-agent tables.
+// tot[1] = agent runs, tot[2] = staged entries, tot[3] = kept runs, tot[4] = blocked agents, tot[5] = largest agent + 1
+extern "C" cudaError_t sdb_launch_lease_select(const sdb_dev_view* v, const sdb_lease_buf* b, const sdb_lease_scratch* s,
+                                               uint32_t used, uint32_t n, uint32_t max_agents, uint32_t* rs_agent,
+                                               uint32_t* rs_count, uint32_t* rs_first, cudaStream_t stream, sdb_profiler* prof,
+                                               int* n_launches) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  LS_LAUNCH(used, k_lease_chunk, *b, used, *s, n);
+  uint32_t *ks = nullptr, *vs = nullptr;
+  cudaError_t e = sdb_radix_sort_u32(s->key_a, s->val_a, s->key_b, s->val_b, n, ls_bits(max_agents - 1u), s->hist, s->h_local,
+                                     s->h_tops, &ks, &vs, stream, &nl);
+  LS_LAUNCH(n, k_lease_run_heads, ks, n, s->gran);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, n, s->tot + 1, nullptr, stream);
+  LS_LAUNCH(n, k_lease_run_begin, *s, n);
+  LS_LAUNCH(n, k_lease_ring_check, *v, *s, ks, n);          // runs <= n: the slots past the run count read 0
+  if (e == cudaSuccess) e = sdb_scan_u32(s->kcnt, s->k_local, s->k_tops, n, s->tot + 2, nullptr, stream);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->kflag, s->kf_local, s->kf_tops, n, s->tot + 3, nullptr, stream);
+  LS_LAUNCH(n, k_lease_stage_list, *s, ks, vs, n, rs_agent, rs_count, rs_first);
+  nl += 6;
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// the n staged entries into the compact scratch: rows numbered by smallest seq.  tot[6] = rows, tot[7] = payload granules
+extern "C" cudaError_t sdb_launch_lease_stage(const sdb_lease_buf* b, const sdb_lease_scratch* s, uint32_t rows_used, uint32_t n,
+                                              unsigned long long seq_end, const sdb_compact_args* cx, cudaStream_t stream,
+                                              sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  LS_LAUNCH(n, k_lease_seq_keys, *b, *s, n);
+  const unsigned long long top = seq_end ? seq_end - 1ull : 0ull;
+  uint32_t *ks = nullptr, *vs = nullptr;
+  cudaError_t e = sdb_radix_sort_u32(s->key_a, s->val_a, s->key_b, s->val_b, n, top >> 32 ? 32u : ls_bits(top), s->hist,
+                                     s->h_local, s->h_tops, &ks, &vs, stream, &nl);
+  if (e == cudaSuccess && (top >> 32)) {
+    uint32_t* kh = ks == s->key_a ? s->key_b : s->key_a;
+    uint32_t* vh = vs == s->val_a ? s->val_b : s->val_a;
+    LS_LAUNCH(n, k_lease_seq_hi, *b, *s, vs, ks, n);          // the used keys are rewritten in place
+    e = sdb_radix_sort_u32(ks, vs, kh, vh, n, ls_bits(top >> 32), s->hist, s->h_local, s->h_tops, &ks, &vs, stream, &nl);
+  }
+  if (rows_used) cudaMemsetAsync(s->rfirst, 0xFF, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
+  LS_LAUNCH(n, k_lease_row_first, *b, *s, vs, n);
+  LS_LAUNCH(n, k_lease_row_heads, *b, *s, vs, n);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, n, s->tot + 6, nullptr, stream);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, n, s->tot + 7, nullptr, stream);
+  nl += 4;
+  if (n) {
+    k_lease_stage_rows<<<ls_grid(n, 8, sm_count * 4), 256, 0, stream>>>(*b, *s, vs, n, cx->send_out, cx->payload_out);
+    ++nl;
+  }
+  LS_LAUNCH(n, k_lease_stage_entries, *b, *s, n, cx->entry_out);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// marks the n staged entries redelivered, then copies the live entries and the rows they name into `out`.
+// tot[8] = kept entries, tot[9] = kept rows, tot[10] = their payload granules
+extern "C" cudaError_t sdb_launch_lease_compact(const sdb_lease_buf* in, const sdb_lease_buf* out, const sdb_lease_scratch* s,
+                                                uint32_t used, uint32_t rows_used, uint32_t n_staged, cudaStream_t stream,
+                                                sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  cudaMemsetAsync(s->tot + 8, 0, 3 * sizeof(unsigned long long), stream);
+  LS_LAUNCH(n_staged, k_lease_mark, *in, *s, n_staged);
+  if (rows_used) cudaMemsetAsync(s->gran, 0, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
+  LS_LAUNCH(used, k_lease_keep, *in, *s, used);
+  LS_LAUNCH(rows_used, k_lease_keep_rows, *in, *s, rows_used);
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 8, nullptr, stream);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, rows_used, s->tot + 9, nullptr, stream);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->rg, s->rg_local, s->rg_tops, rows_used, s->tot + 10, nullptr, stream);
+  nl += (used ? 2 : 0) + (rows_used ? 4 : 0);
+  LS_LAUNCH(used, k_lease_copy_entries, *in, *out, *s, used);
+  if (rows_used) {
+    k_lease_copy_rows<<<ls_grid(rows_used, 8, sm_count * 4), 256, 0, stream>>>(*in, *out, *s, rows_used);
+    ++nl;
+  }
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// any kernel of this file: its module is loaded as a whole before the latency server starts (sdb_api.cu)
+extern "C" const void* sdb_lease_kernel_anchor() { return reinterpret_cast<const void*>(&k_lease_due); }

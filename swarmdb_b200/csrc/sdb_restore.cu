@@ -371,5 +371,28 @@ extern "C" cudaError_t sdb_launch_restore_write(const sdb_dev_view* v, const sdb
   return e == cudaSuccess ? cudaGetLastError() : e;
 }
 
+// The radix sort above for other callers (the lease sweep): stable sort of n (key, value) pairs by the low `bits` bits of
+// the keys.  hist / h_local take 256 x ceil(n / 1024) words, h_tops that / 4096 + 1.  *kres / *vres name the buffers
+// holding the result: the a pair or the b pair.
+extern "C" cudaError_t sdb_radix_sort_u32(uint32_t* ka, uint32_t* va, uint32_t* kb, uint32_t* vb, uint32_t n, uint32_t bits,
+                                          uint32_t* hist, uint32_t* h_local, uint32_t* h_tops, uint32_t** kres, uint32_t** vres,
+                                          cudaStream_t stream, int* n_launches) {
+  uint32_t *kin = ka, *vin = va, *kout = kb, *vout = vb;
+  cudaError_t e = cudaSuccess;
+  const uint32_t tiles = (n + SDB_RS_TILE - 1) / SDB_RS_TILE;
+  int nl = 0;
+  for (uint32_t shift = 0; n && shift < bits && e == cudaSuccess; shift += 8) {
+    k_rs_hist<<<tiles, 32, 0, stream>>>(kin, n, shift, hist, tiles);
+    e = sdb_scan_u32(hist, h_local, h_tops, 256u * tiles, nullptr, nullptr, stream);
+    k_rs_scatter<<<tiles, 32, 0, stream>>>(kin, vin, kout, vout, n, shift, h_local, h_tops, tiles);
+    nl += 4;
+    uint32_t* t = kin; kin = kout; kout = t;
+    t = vin; vin = vout; vout = t;
+  }
+  *kres = kin; *vres = vin;
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
 // any kernel of this file: its module is loaded as a whole before the latency server starts (sdb_api.cu)
 extern "C" const void* sdb_restore_kernel_anchor() { return reinterpret_cast<const void*>(&k_restore_plan); }

@@ -511,6 +511,8 @@ class ShardedSwarmsDB(SwarmsDB):
         if g.id_nonce is None and not g.deterministic_ids:
             g = dataclasses.replace(g, deterministic_ids=True)       # ids must agree across ranks
         g = dataclasses.replace(g, shard_id=rank, num_shards=world)
+        if g.lease_records:
+            self._no_leases()
         k["gpu_config"] = g
         super().__init__(*a, _shard=shard, **k)
         self.rank, self.world = rank, world
@@ -730,6 +732,14 @@ class ShardedSwarmsDB(SwarmsDB):
     def requeue_batch_compact(self, counts, entries, sends, payload, agent_idx):
         raise NotImplementedError("ShardedSwarmsDB does not requeue yet: restored ids must stay below the composite "
                                   "sequence numbers of later rounds")
+
+    # ---- leased receives redeliver with the original ids, which meets the composite-round numbering as requeue does
+    def _no_leases(self, *args, **kwargs):
+        raise NotImplementedError("ShardedSwarmsDB does not lease yet: redelivered ids must stay below the composite "
+                                  "sequence numbers of later rounds (see requeue_batch_compact)")
+
+    receive_messages_leased = receive_batch_leased = settle_leases = _no_leases
+    ack_messages = nack_messages = extend_leases = redeliver_expired = _no_leases
 
     def close(self) -> None:
         """Collective like flush(): every rank closes.  Buffered sends are NOT flushed here (a flush is a collective
