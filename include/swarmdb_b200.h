@@ -497,6 +497,10 @@ int sdb_import_wire_ptrs_async(sdb_handle h, uint32_t n_src, const void* const* 
 int sdb_import_prefetch(sdb_handle h, uint32_t n_src, const void* const* wire_ptrs, uint64_t wire_bytes, uint32_t step);
 
 /* ---- which records were lost to full rings (delivery report, M:374-391 / M:501-519)
+ * A ring is full when tail - head = ring_slots.  The window [head, tail) holds tombstones too (records consumed out of
+ * stream order by priority receives, sdb_receive_where and sdb_expire), and after every retiring call head is the
+ * oldest pending record (tail when none is left): so a ring takes ring_slots - (tail - head) more records, whichever
+ * receive, filtered take, expiry or leased receive consumed the earlier ones.
  * `ring_overflow` in sdb_stats says how many records found their receiver's ring full; this call says WHICH: up to
  * `cap` (receiver agent, sequence number) pairs of records dropped since the previous call, in no particular order
  * (the device logs the first 4096 per interval; *dropped_out = how many were dropped in the interval).  Reading

@@ -162,6 +162,19 @@ __device__ __forceinline__ uint32_t lane_prefix(uint32_t ballot, uint32_t lane) 
   return __popc(ballot & ((1u << lane) - 1u));
 }
 
+// whole warp: the first live entry of [P, T), or T.  After a retiring selection head goes there, so that head is always
+// the oldest pending record and the ring's free slots (R - (tail - head)) never include a tombstone at the window's start.
+// Past the selected range only tombstones are walked (at most ntomb of them) before the first live entry.
+__device__ __forceinline__ uint32_t first_live_from(const uint2* rs, uint32_t mask, uint32_t P, uint32_t T, uint32_t lane) {
+  for (uint32_t q0 = P; static_cast<int32_t>(T - q0) > 0; q0 += 32) {
+    const uint32_t p = q0 + lane;
+    const bool live = static_cast<int32_t>(T - p) > 0 && (rs[p & mask].y & 0xFFFFu) != SDB_META_TOMB;
+    const uint32_t b = __ballot_sync(0xFFFFFFFFu, live);
+    if (b) return q0 + (__ffs(b) - 1);
+  }
+  return T;
+}
+
 // one agent, whole warp: choose the C entries to deliver from the window [H, T), write their plan at
 // output index RO.., retire them (advance head / tombstone).  Stream order when !prio_mode.  The plan's payload
 // offsets (.y) are filled later (record-level scan / fill_offsets_warp).
@@ -260,7 +273,7 @@ __device__ __forceinline__ void select_agent_warp(const sdb_dev_view& v, uint4* 
   }
   const uint32_t scan_end = static_cast<int32_t>(T - p0) > 0 ? p0 : T;
   uint32_t nh = first_unsel;
-  if (static_cast<int32_t>(nh - scan_end) > 0) nh = scan_end;
+  if (static_cast<int32_t>(nh - scan_end) >= 0 && retire) nh = first_live_from(rs, mask, scan_end, T, lane);
   if (lane == 0 && retire) {
     v.ring_hdr[A].head = nh;
     v.ring_hdr[A].ntomb = NT + got - (nh - H);
@@ -383,14 +396,8 @@ __device__ __forceinline__ void select_agent_warp_bounded(const sdb_dev_view& v,
   }
   if (!retire) return;
   __syncwarp();
-  // new head: first live entry left behind inside the scanned range (the tombstones just written count as consumed)
-  uint32_t nh = scan_end;
-  for (uint32_t q0 = H; static_cast<int32_t>(scan_end - q0) > 0; q0 += 32) {
-    const uint32_t p = q0 + lane;
-    const bool live = static_cast<int32_t>(scan_end - p) > 0 && (rs[p & mask].y & 0xFFFFu) != SDB_META_TOMB;
-    const uint32_t b = __ballot_sync(0xFFFFFFFFu, live);
-    if (b) { nh = q0 + (__ffs(b) - 1); break; }
-  }
+  // new head: the first live entry left (the tombstones just written count as consumed)
+  const uint32_t nh = first_live_from(rs, mask, H, T, lane);
   if (lane == 0) {
     v.ring_hdr[A].head = nh;
     v.ring_hdr[A].ntomb = NT + got - (nh - H);

@@ -24,8 +24,10 @@ def _pad32(n):
 
 
 class LeaseModel:
-    def __init__(self, oracle, groups, rec_cap, ring_slots, cap, shared=True):
-        self.o, self.groups, self.rec_cap, self.R, self.cap, self.shared = oracle, groups, rec_cap, ring_slots, cap, shared
+    """`oracle` is a tests/ring_ref.py::BoundedOracle: its ring model decides which agents a sweep blocks."""
+
+    def __init__(self, oracle, groups, rec_cap, cap, shared=True):
+        self.o, self.groups, self.rec_cap, self.cap, self.shared = oracle, groups, rec_cap, cap, shared
         self.recs = []            # dicts in lease-id order
         self.next_id = 0
         self.n_leases = 0         # leased calls so far (row keys are (call, row))
@@ -104,7 +106,7 @@ class LeaseModel:
         staged, blocked = [], 0
         for a in sorted(by_agent):
             rs = by_agent[a]
-            if int(self.o.pending(a)) + len(rs) > self.R:
+            if len(rs) > self.o.capacity(a):         # tail - head counts tombstones: pending records alone do not
                 blocked += 1
             else:
                 staged.append((a, rs))
@@ -132,7 +134,8 @@ class LeaseModel:
             payload = np.concatenate(pays) if pays else np.zeros(0, np.uint8)
             agents = np.array([a for a, _ in staged], np.uint32)
             counts = np.array([len(rs) for _, rs in staged], np.uint32)
-            restore_append(self.o, self.groups, agents, counts, ent, snd, payload)
+            with self.o.appending():
+                restore_append(self.o, self.groups, agents, counts, ent, snd, payload)
             self.last_granules = restore_granules(counts, ent, snd, self.shared, agents)
             for r in flat:
                 r["state"] = REDELIVERED

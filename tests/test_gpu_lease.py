@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 from tests.lease_ref import LeaseModel
+from tests.ring_ref import BoundedOracle
 from tests.test_gpu_compact_receive import Rig, _same
 from tests.test_gpu_restore import _every_path, _expand, _groups, _loads_equal
 
@@ -21,8 +22,12 @@ BIG = 1 << 20
 
 
 def _model(rig, cap, shared, rec_cap=None):
+    """The lease model over the rig's oracle, bounded by the handle's rings from here on (the rig has only sent so
+    far: its windows are contiguous)."""
     from swarmdb_b200._native import recv_capacity
-    return LeaseModel(rig.c, _groups(rig), rec_cap or recv_capacity(rig.g.cfg), int(rig.g.cfg.ring_slots), cap, shared)
+    if not isinstance(rig.c, BoundedOracle):
+        rig.c = BoundedOracle(rig.c, rig.G, int(rig.g.cfg.ring_slots), _groups(rig), rig.A)
+    return LeaseModel(rig.c, _groups(rig), rec_cap or recv_capacity(rig.g.cfg), cap, shared)
 
 
 def _lease(rig, m, agents, k, deadline, flags=0):

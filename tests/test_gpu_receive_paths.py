@@ -11,8 +11,9 @@ change of a threshold cannot quietly move a case elsewhere:
   bulk, priority      k_recv_count, scans, k_recv_select(_big), gather                   recv_count
 
 After every call the counts, every header field and the padded payload bytes, stats()["delivered"] and agent_loads()
-(pending, pending_by_prio) must equal the oracle's: a wrong head or ntomb shows in the loads even when the returned
-records happen to be right.
+(pending, pending_by_prio) must equal the oracle's: an ntomb that disagrees with head shows in the loads even when the
+returned records happen to be right.  Where head lands does not (pending = tail - head - ntomb is the same either way);
+it decides the ring's free slots, which tests/test_gpu_ring_capacity.py checks against a bounded-ring model.
 
 Capacity (include/swarmdb_b200.h): records are laid out agent by agent in list order; an agent whose records do not
 all fit is truncated together with every later agent (they stay queued), except an agent first in the output, which
@@ -220,8 +221,8 @@ def _state(rig, name, targets):
         _bulk(rig, targets, 301, 0, "prep")
         fill(rand(400))
     elif name == "tombstones_then_last":
-        # 300 entries: 0, 3 x 298, 0.  The priority receive takes the 298, the stream receive the first entry: the
-        # window is then 167 tombstones and one live entry at its end
+        # 300 entries: 0, 3 x 298, 0.  The priority receive takes the 298, the stream receive the first entry: head
+        # then jumps over the 298 tombstones to the one live entry left
         fill([0] + [3] * 298 + [0])
         _bulk(rig, targets, 298, RECV_PRIORITY, "prep")
         _bulk(rig, targets, 1, 0, "prep")

@@ -7,6 +7,7 @@ import pytest
 
 from tests.fake_shard import OracleShard
 from tests.lease_ref import LeaseModel
+from tests.ring_ref import BoundedOracle
 
 A, G, R = 16, 2, 8
 ROOT = __import__("pathlib").Path(__file__).resolve().parent.parent
@@ -30,10 +31,11 @@ def test_header_declares_lease_calls_and_profiler_slot():
     assert C.sizeof(SdbLeaseSummary) == 64
 
 
-def _oracle_with_traffic(seed=0, n=40):
+def _oracle_with_traffic(seed=0, n=40, ring_slots=64):
+    """An oracle bounded by rings of `ring_slots` (tests/ring_ref.py) and some p2p and group traffic."""
     from oracle.cpu_ref import CpuOracle
     rng = np.random.default_rng(seed)
-    c = CpuOracle(A, G)
+    c = BoundedOracle(CpuOracle(A, G), G, ring_slots)
     groups = {0: np.arange(0, 4, dtype=np.uint32), 1: np.arange(4, 8, dtype=np.uint32)}
     for g, m in groups.items():
         c.create_group(g, m)
@@ -53,7 +55,7 @@ def _pending(c):
 def test_lease_ids_acks_renew_and_sweep_order():
     c, groups, _ = _oracle_with_traffic()
     before = _pending(c)
-    m = LeaseModel(c, groups, rec_cap=1 << 10, ring_slots=64, cap=1 << 10)
+    m = LeaseModel(c, groups, rec_cap=1 << 10, cap=1 << 10)
     cnt, hdr, pay, base = m.lease(None, 2, 10.0)
     assert base == 0 and len(hdr) == int(cnt.sum()) > 0
     ids = np.arange(len(hdr), dtype=np.uint64)
@@ -79,7 +81,7 @@ def _acked(cnt, k, n_agents):
 
 def test_redelivery_goes_behind_newer_records_in_lease_order():
     c, groups, rng = _oracle_with_traffic(1)
-    m = LeaseModel(c, groups, rec_cap=1 << 10, ring_slots=64, cap=1 << 10)
+    m = LeaseModel(c, groups, rec_cap=1 << 10, cap=1 << 10)
     _, hdr, _, _ = m.lease([9], 100, 1.0)
     assert len(hdr) > 1
     c.send_batch([3], [9], [1], None, [5], [0], np.full(64, 65, np.uint8))
@@ -90,8 +92,8 @@ def test_redelivery_goes_behind_newer_records_in_lease_order():
 
 
 def test_all_flag_chunks_and_blocked_agents():
-    c, groups, rng = _oracle_with_traffic(2, n=120)
-    m = LeaseModel(c, groups, rec_cap=5, ring_slots=R, cap=1 << 10)
+    c, groups, rng = _oracle_with_traffic(2, n=120, ring_slots=R)
+    m = LeaseModel(c, groups, rec_cap=5, cap=1 << 10)
     total = 0
     while True:
         got = m.lease(None, 1 << 10, math.inf)[1]
@@ -102,7 +104,7 @@ def test_all_flag_chunks_and_blocked_agents():
     # fill agent 9's ring with newer records: its leases stay in the store while every other agent is served
     n9 = sum(1 for r in m.recs if r["agent"] == 9)
     assert n9 > 0
-    k = R - int(c.pending(9))
+    k = c.capacity(9)
     c.send_batch([3] * k, [9] * k, [1] * k, None, [1] * k, np.zeros(k, np.uint64), np.full(64, 65, np.uint8))
     red_total, blocked_seen, calls = 0, 0, 0
     while True:
@@ -126,12 +128,15 @@ def test_all_flag_chunks_and_blocked_agents():
 class LeaseShard(OracleShard):
     """OracleShard plus the lease calls, answered by tests/lease_ref.py in the compact format (one row per record)."""
 
-    def __init__(self, *a, **k):
-        super().__init__(*a, **k)
+    def __init__(self, max_agents, max_groups, rank, world):
+        super().__init__(max_agents, max_groups, rank, world)
+        self.max_groups = max_groups
         self.model = None
 
     def lease_reserve(self, max_records, max_payload_bytes):
-        self.model = LeaseModel(self.o, self.groups, 1 << 16, 64, max_records) if max_records else None
+        if max_records and not isinstance(self.o, BoundedOracle):
+            self.o = BoundedOracle(self.o, self.max_groups, 64, self.groups)
+        self.model = LeaseModel(self.o, self.groups, 1 << 16, max_records) if max_records else None
 
     def receive_leased(self, agents, max_messages, deadline, flags=0):
         from swarmdb_b200._native import ENTRY_DTYPE, SEND_DTYPE
