@@ -371,8 +371,8 @@ class SwarmsDB:
         """Delivery report for a batch that overflowed rings (M:374-391): the device logs (receiver, sequence number)
         of every dropped record (sdb_overflow_log).  Point-to-point and group messages have one record each (id <->
         sequence number): exactly those are marked FAILED, the rest of the batch stays DELIVERED.  A broadcast is one
-        message with many copies: it stays DELIVERED and names the receivers that missed it in
-        metadata["undelivered_to"].  Returns False when the log could not name every dropped record (more than its
+        message with many copies: it stays DELIVERED, names the receivers that missed it in
+        metadata["undelivered_to"] and leaves their inboxes (it is not unread for an agent that never got it).  Returns False when the log could not name every dropped record (more than its
         capacity in one batch): the caller then fails the whole batch, as before."""
         agents, seqs, dropped = self.shard.overflow_log()
         if dropped != len(seqs):
@@ -383,7 +383,11 @@ class SwarmsDB:
             if m is None or id(m) not in in_batch:
                 return False
             if m.receiver_id is None:
-                m.metadata.setdefault("undelivered_to", []).append(self._agent_name[a] if a < len(self._agent_name) else a)
+                name = self._agent_name[a] if a < len(self._agent_name) else a
+                m.metadata.setdefault("undelivered_to", []).append(name)
+                inbox = self.agent_inbox.get(name)
+                if inbox and m.id in inbox:          # never queued for this receiver: not unread there
+                    inbox.remove(m.id)
             else:
                 m.status = MessageStatus.FAILED
                 m.metadata["error"] = error
@@ -1108,6 +1112,23 @@ class SwarmsDB:
         self.shard.advance_seq(nxt)
         self._next_seq = max(self._next_seq, nxt); self._b_first_seq = self._next_seq
 
+    def _check_snapshot_fits(self, snap: Dict[str, np.ndarray]) -> None:
+        """Refuse a snapshot this instance cannot hold before anything of it is adopted: the instance is fresh, so every
+        ring is empty and an agent's records fit exactly when they number at most ring_slots (and one restore call).
+        A refusal found chunk by chunk would leave the earlier chunks restored and the instance no longer fresh."""
+        agents, counts = snap["agents"].astype(np.int64), snap["counts"].astype(np.int64)
+        if not len(agents):
+            return
+        per_agent = np.bincount(agents, weights=counts).astype(np.int64)
+        worst = int(np.argmax(per_agent))
+        cap = recv_capacity(self.gpu_config)
+        if counts.max() > cap:
+            raise RuntimeError(f"snapshot agent with {int(counts.max())} records does not fit one restore call ({cap})")
+        if per_agent[worst] > self.gpu_config.ring_slots:
+            raise SdbError(-4, f"snapshot agent {snap['agent_names'][worst]} has {int(per_agent[worst])} records, more than "
+                               f"its ring holds "
+                               f"(GpuConfig.ring_slots={self.gpu_config.ring_slots}): nothing restored")
+
     def _restore_chunks(self, snap: Dict[str, np.ndarray]) -> int:
         """Restore every chunk of a snapshot, split by whole agents where this instance's receive capacity is smaller;
         returns the largest sequence number + 1 seen."""
@@ -1118,8 +1139,6 @@ class SwarmsDB:
         for k in range(len(off) - 1):
             a0, a1, e0 = off[k, 0], off[k + 1, 0], off[k, 1]
             ca = counts[a0:a1].astype(np.int64)
-            if len(ca) and ca.max() > cap:
-                raise RuntimeError(f"snapshot agent with {int(ca.max())} records does not fit one restore call ({cap})")
             first = e0 + np.concatenate([[0], np.cumsum(ca)])
             i = 0
             while i < len(ca):
@@ -1135,9 +1154,13 @@ class SwarmsDB:
     def load_queue_snapshot(self, path: Union[str, Path]) -> None:
         """Put a snapshot written by save_queue_snapshot back into this instance, which must be fresh: the agents and
         groups are re-created in the snapshot's index order, its id nonce is adopted (GpuConfig.id_nonce, when set, must
-        equal it) and every pending record is restored with its id, to be delivered as if it had never left."""
+        equal it) and every pending record is restored with its id, to be delivered as if it had never left.  A snapshot
+        this instance cannot hold is refused before anything of it is adopted, and the instance stays fresh: an agent
+        with more records than one receive call holds raises RuntimeError (checked first), one with more records than
+        its ring holds raises SdbError (code -4)."""
         self._check_fresh()
         snap = self._read_snapshot(path)
+        self._check_snapshot_fits(snap)
         self._adopt_tables(snap)
         seq_end = self._restore_chunks(snap)
         self._next_seq = max(self._next_seq, seq_end); self._b_first_seq = self._next_seq

@@ -161,7 +161,8 @@ class BoundedOracle(WhereOracle):
                         kept_pos.append(i)
                         k += 1
                 assert k == len(want), (a, "survivors that were not sent", want[k:])
-                assert len(want) == min(len(new), self.ring.capacity(a)), (a, len(want), len(new), self.ring.capacity(a))
+                assert len(want) == min(len(new), self.ring.capacity(a)), \
+                    (a, "survivors must fill the free slots", len(want), len(new), self.ring.capacity(a))
                 kept = set(kept_pos)
             else:
                 kept = set(range(min(len(new), self.ring.capacity(a))))

@@ -59,12 +59,12 @@ def _same(res_gpu, res_cpu, what=""):
 class Rig:
     """A Shard and the oracle in lockstep; agents 0 .. EMPTY - 1 stay empty."""
 
-    def __init__(self, rng, A, max_len=64, **kw):
+    def __init__(self, rng, A, max_len=64, G=1, **kw):
         from oracle.cpu_ref import CpuOracle
         from swarmdb_b200._native import Shard
         self.rng, self.A, self.max_len = rng, A, max_len
-        self.g = Shard(max_agents=A, **kw)
-        self.c = CpuOracle(A, 1)
+        self.g = Shard(max_agents=A, max_groups=G, **kw)
+        self.c = CpuOracle(A, G)
         idx = np.arange(A, dtype=np.uint32)
         self.g.register(idx); self.c.register(idx)
         self.empties = idx[:EMPTY]

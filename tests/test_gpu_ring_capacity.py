@@ -298,11 +298,14 @@ def test_restore_and_lease_sweep_at_the_boundary(shared):
         rig.close()
 
 
-def _bounded_send(rig, members, dev_send, orc_send, ordered, index, what):
+def _bounded_send(rig, members, dev_send, orc_send, ordered, index, what, launches=None, commit=None, lossy=True):
     """One send on the device and in the model, into holey, nearly full rings.  ordered: an index build, which keeps the
     first records of the call in send order, so survivors and log are exact.  Otherwise an atomic-claim path: the
     survivors are read from the device (they must come out in seq order), and the model checks that each ring took
-    exactly as many as it had free slots and that survivors and logged records split the call's records."""
+    exactly as many as it had free slots and that survivors and logged records split the call's records.
+    launches / commit, when given: the kernel_launches delta of the call and whether the commit class ran (the profiler's
+    index class times both pull kernels as one, so the launch count tells which of them ran).  lossy: whether some record
+    is dropped (None: either)."""
     from swarmdb_b200._native import RECV_PEEK
     R_ = rig.c.ring.R
     assert rig.g.overflow_log()[2] == 0
@@ -311,7 +314,13 @@ def _bounded_send(rig, members, dev_send, orc_send, ordered, index, what):
     base = st0["next_seq"]
     rig.g.profile_read()
     dev_send()
-    assert (rig.g.profile_read()["index"][1] > 0) == index, what
+    prof = rig.g.profile_read()
+    assert (prof["index"][1] > 0) == index, what
+    if commit is not None:
+        assert (prof["commit"][1] > 0) == commit, what
+    if launches is not None:
+        assert rig.g.stats()["kernel_launches"] - st0["kernel_launches"] == launches, \
+            (what, rig.g.stats()["kernel_launches"] - st0["kernel_launches"], launches)
     if ordered:
         rig.c.enqueue(orc_send, ordered=True)
     else:
@@ -326,7 +335,8 @@ def _bounded_send(rig, members, dev_send, orc_send, ordered, index, what):
         rig.c.enqueue(orc_send, keep=keep)
     want = rig.c.take_dropped()
     st1 = rig.g.stats()
-    assert st1["ring_overflow"] - st0["ring_overflow"] == len(want) > 0, (what, st1["ring_overflow"] - st0["ring_overflow"], len(want))
+    assert st1["ring_overflow"] - st0["ring_overflow"] == len(want), (what, st1["ring_overflow"] - st0["ring_overflow"], len(want))
+    assert lossy is None or (len(want) > 0) == lossy, (what, len(want))
     ag, sq, dropped = rig.g.overflow_log(1 << 16)
     assert dropped == len(want), what
     got = sorted(zip(ag.tolist(), sq.tolist()))

@@ -113,6 +113,61 @@ def test_renumber_and_compact_rows():
     assert h3.tobytes() == h4.tobytes() and q3.tobytes() == q4.tobytes()
 
 
+def test_snapshot_that_overfills_a_ring_is_refused_before_any_restore(tmp_path):
+    """load_queue_snapshot restores chunk by chunk; an agent with more records than ring_slots in a later chunk used to
+    be found only after the earlier chunks were restored, leaving the instance half-loaded and no longer fresh.  The
+    whole snapshot is checked first: nothing reaches the device and the instance can still load another snapshot."""
+    import pytest
+
+    import swarmdb_b200 as sdb
+    from swarmdb_b200._native import ENTRY_DTYPE, SEND_DTYPE, SdbError
+    from tests.fake_shard import OracleShard
+
+    class Recording(OracleShard):
+        def __init__(self, *a):
+            super().__init__(*a)
+            self.calls = []
+
+        def stats(self):
+            return {**super().stats(), "enqueued": sum(int(np.sum(c)) for _, c in self.calls)}
+
+        def restore_compact(self, agents, counts, entries, sends, payload, flags=0):
+            self.calls.append((np.asarray(agents).tolist(), np.asarray(counts).tolist()))
+            return int(np.sum(counts)), int(entries["seq"].max()) + 1
+
+    def snapshot(path, counts):
+        chunks = [[0, 1], [2]]                              # two chunks; agent 2 alone in the last one
+        n = sum(counts)
+        ent = np.zeros(n, ENTRY_DTYPE)
+        ent["seq"] = np.arange(1, n + 1); ent["send"] = np.arange(n); ent["receiver"] = np.repeat([0, 1, 2], counts)
+        snd = np.zeros(n, SEND_DTYPE)
+        off = np.zeros((3, 4), np.uint64)
+        for k, c in enumerate(chunks):
+            m = sum(counts[a] for a in c)
+            off[k + 1] = off[k] + [len(c), m, m, 0]
+        np.savez(path, version=np.uint32(sdb.SwarmsDB.SNAPSHOT_VERSION), shard=np.array([0, 1], np.uint32),
+                 id_nonce=np.uint64(0), next_seq=np.uint64(n + 1), agent_names=np.array(["a", "b", "c"], np.str_),
+                 registered=np.ones(3, bool), group_names=np.zeros(0, np.str_), group_off=np.zeros(1, np.uint64),
+                 group_members=np.zeros(0, np.uint32), chunk_off=off, agents=np.array([0, 1, 2], np.uint32),
+                 counts=np.array(counts, np.uint32), entries=ent, sends=snd, payload=np.zeros(0, np.uint8))
+        return path
+
+    def fresh():
+        shard = Recording(64, 4, 0, 1)
+        cfg = sdb.GpuConfig(max_agents=64, max_groups=4, ring_slots=16, max_recv_records=64, deterministic_ids=True)
+        return shard, sdb.SwarmsDB(save_dir=str(tmp_path), auto_save=False, gpu_config=cfg, _shard=shard)
+
+    shard, db = fresh()
+    with pytest.raises(SdbError) as ei:
+        db.load_queue_snapshot(snapshot(tmp_path / "over.npz", [2, 3, 17]))
+    assert ei.value.code == -4 and "ring_slots=16" in str(ei.value)
+    assert shard.calls == []
+    db._check_fresh()                                       # still fresh: a snapshot that fits loads into it
+    db.load_queue_snapshot(snapshot(tmp_path / "fits.npz", [2, 3, 16]))
+    assert shard.calls == [([0, 1], [2, 3]), ([2], [16])]
+    db.close()
+
+
 def test_sharded_front_end_refuses_snapshots_and_requeue(tmp_path):
     """A sharded deployment does not snapshot or requeue yet: the inherited single-shard versions would restore every
     agent's records on every rank, so the sharded class refuses them."""

@@ -180,6 +180,74 @@ def test_group_and_list_drops_need_the_path_declared():
     o.close()
 
 
+def test_offer_order_for_an_agent_in_several_groups_and_listed_twice():
+    """The index build merges an agent's records by (send, member position): group 0 lists agent 2 twice, group 1 holds
+    it once, so a batch g0, g1, g0 delivers it positions 0 and 2 of send 0, position 1 of send 1, then send 2; a sender
+    inside a group skips its own records.  A 4-slot ring keeps the first four."""
+    z = np.zeros(64, np.uint8)
+    o = _bounded(4, {0: np.array([2, 3, 2], np.uint32), 1: np.array([4, 2], np.uint32)})
+    b = o.next_seq
+    o.enqueue(lambda: o.send_group_batch([0, 0, 0, 2], [0, 1, 0, 1], None, None, [8] * 4, np.zeros(4, np.uint64), z),
+              ordered=True)
+    # records: send 0 -> b .. b+2 (2, 3, 2), send 1 -> b+3, b+4 (4, 2), send 2 -> b+5 .. b+7, send 3 (sender 2) -> b+8, b+9
+    assert o.ring.live_seqs(2) == [b, b + 2, b + 4, b + 5]
+    assert o.take_dropped() == [(2, b + 7)]
+    assert o.ring.live_seqs(3) == [b + 1, b + 6] and o.ring.live_seqs(4) == [b + 3, b + 8]
+    assert o.receive_batch([2], 10)[1]["seq"].tolist() == [b, b + 2, b + 4, b + 5]
+    o.close()
+
+
+def test_import_replayed_through_the_oracle_shard_with_composite_seqs():
+    """A cross-shard import bounded as one call: OracleShard replays the wire into a BoundedOracle, keeps the members
+    this rank owns, and numbers records from the wire's explicit (composite) sequence base, which the drops carry."""
+    from tests.fake_shard import OracleShard
+    z = np.zeros(64, np.uint8)
+    members = np.array([2, 3, 4, 5], np.uint32)
+    src, dst = OracleShard(A, G, 1, 2), OracleShard(A, G, 0, 2)
+    dst.o = BoundedOracle(dst.o, G, 2)
+    dst.o.register(np.arange(A, dtype=np.uint32))
+    owner = np.arange(A) % 2                                          # even agents live on rank 0
+    for sh in (src, dst):
+        sh.set_agent_shards(owner)
+        sh.create_group(0, members)
+    sb = (5 << 40) + 1000
+    cap = 1 << 14
+    wire = np.zeros(cap, np.uint8)
+    src.export_group_batch(np.zeros(3, np.uint32), np.zeros(3, np.uint32), np.zeros(3, np.uint8), np.zeros(3, np.uint8),
+                           np.full(3, 8, np.uint16), np.zeros(3, np.uint64), z, wire, cap)
+    hdr = wire[:56].view(np.int64).copy()
+    hdr[4] = sb                                                       # the wire's explicit sequence base
+    wire[:56] = hdr.view(np.uint8)
+    with dst.o.appending(ordered=True):
+        dst.import_wire_batches(1, wire, cap)
+    # member position j of send i is record sb + 4 i + j; rank 0 owns agents 2 (position 0) and 4 (position 2)
+    assert dst.o.ring.live_seqs(2) == [sb, sb + 4] and dst.o.ring.live_seqs(4) == [sb + 2, sb + 6]
+    assert dst.o.take_dropped() == [(2, sb + 8), (4, sb + 10)]
+    assert dst.o.ring.live_seqs(3) == [] and dst.o.overflow == 2
+    src.close(); dst.close()
+
+
+def test_keep_for_pull_and_atomic_entries_to_one_agent():
+    """A mixed batch with group traffic above the pull threshold: the fan-out's atomic claims land before the index
+    build appends, so the survivors need not be the first records of the call.  keep= takes any subsequence of the
+    new records in seq order, of exactly as many records as the ring has free slots."""
+    z = np.zeros(64, np.uint8)
+    o = _bounded(4, {0: np.array([2, 3], np.uint32)})
+    _p2p(o, [2])
+    b = o.next_seq
+
+    def mixed():
+        o.send_group_batch([0, 0], [0, 0], None, None, [8, 8], np.zeros(2, np.uint64), z)     # b .. b+3
+        _p2p(o, [2, 2, 3])                                                                      # b+4 .. b+6
+    o.enqueue(mixed, keep={2: [b, b + 4, b + 5], 3: [b + 1, b + 3, b + 6]})
+    assert sorted(o.take_dropped()) == [(2, b + 2)]
+    assert o.ring.live_seqs(2)[1:] == [b, b + 4, b + 5] and o.ring.capacity(2) == 0
+    assert o.ring.capacity(3) == 1
+    with pytest.raises(AssertionError, match="survivors must fill the free slots"):     # agent 3 keeps none of three
+        o.enqueue(mixed, keep={2: [], 3: []})
+    o.close()
+
+
 def test_lease_sweep_blocks_on_tombstones_not_on_pending():
     """Priority leases that leave record 0 behind fill the window: with R = 8 and the window 8 slots long, two records
     pending and six leased, a sweep of those six is blocked (pending + six would have fit)."""
