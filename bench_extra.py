@@ -819,6 +819,109 @@ def lease(rounds=3):
     return out
 
 
+def deadletter(rounds=3):
+    """Dead letters on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 records), every leased record
+    nacked before each sweep:
+      - a leased receive of the whole backlog with the policy on and an empty ledger, alternated with the policy off;
+      - with M = 1, the sweep that dead-letters every record, the take of all of them into pinned buffers, and the
+        redrive of what was taken (sdb_restore_compact of it as it stands);
+      - with M = 2, the sweep that fills the ledger and the leased receive that looks every record up, against the same
+        sweep and receive with the policy off.
+    Per call: wall clock around the synchronising call and the `lease` (and `restore`) kernel time from the profiler."""
+    import torch
+    from bench import ClockSampler, Workload
+    from swarmdb_b200._native import ENTRY_DTYPE, LEASE_ACK, LEASE_RENEW, SEND_DTYPE, Shard, pad32
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py deadletter: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    s = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+              member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+              max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+    s.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        s.create_group(g, wl.members(g))
+    s.lease_reserve(rec_cap, rec_cap * pad32(wl.L))
+    pin = lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True).numpy()          # noqa: E731
+    pin_ent, pin_snd, pin_pay = pin(rec_cap * 16).view(ENTRY_DTYPE), pin(rec_cap * 32).view(SEND_DTYPE), pin(rec_cap * wl.L)
+    batch = wl.batch()
+
+    def drain():
+        while s.receive_batch(None, 1 << 10, copy_out=False)[1]:
+            pass
+
+    def clear():                              # every lease was acked or taken: compact the store, drain, fresh backlog
+        s.lease_sweep(0.0)
+        assert s.lease_stats()["entries_used"] == 0
+        drain()
+        s.send_group_batch(*batch)
+
+    def call(fn):
+        s.sync(); s.profile(True)
+        t = time.perf_counter()
+        r = fn()
+        wall = (time.perf_counter() - t) * 1e3
+        prof = s.profile_read(); s.profile(False)
+        return r, {"wall_ms": wall, "lease_kernel_ms": prof["lease"][0], "restore_kernel_ms": prof["restore"][0]}
+
+    def med(rows):
+        return {k: float(np.median([r[k] for r in rows])) for k in rows[0]} | {"per_round": rows}
+
+    def lease():
+        return s.receive_leased(None, 1 << 10, 1.0, 0, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_pay)
+
+    def nack(base):
+        s.lease_settle(np.arange(base, base + per_step, dtype=np.uint64), LEASE_RENEW, -np.inf)
+
+    clocks = ClockSampler(0); clocks.start()
+    rows = {k: [] for k in ("lease_policy_off", "lease_policy_on_empty_ledger", "sweep_m1_dead_letters_all", "take_all",
+                            "redrive_all", "sweep_m2_fills_ledger", "lease_m2_looks_up_all", "sweep_policy_off",
+                            "lease_after_sweep_policy_off")}
+    for _ in range(rounds):
+        for on in (False, True):
+            clear()
+            s.lease_set_policy(0xFFFFFFFF if on else 0, rec_cap if on else 0)
+            r, t = call(lease)
+            assert len(r[1]) == per_step
+            rows["lease_policy_on_empty_ledger" if on else "lease_policy_off"].append(t)
+            s.lease_settle(np.arange(r[4], r[4] + per_step, dtype=np.uint64), LEASE_ACK)
+        # M = 1: every record dies; take them all; redrive them
+        clear(); s.lease_set_policy(0, 0); s.lease_set_policy(1, rec_cap)
+        r = lease(); nack(r[4])
+        (red, blocked, left), t = call(lambda: s.lease_sweep(0.0))
+        assert red == 0 and s.lease_policy_stats()["dead"] == per_step
+        rows["sweep_m1_dead_letters_all"].append(t)
+        (c, e, sn, p, d), t = call(lambda: s.lease_dead_letters(None, 0, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_pay))
+        assert len(e) == per_step
+        rows["take_all"].append(t)
+        (n, _), t = call(lambda: s.restore_compact(np.arange(len(c), dtype=np.uint32), c, e, sn, p))
+        assert n == per_step
+        rows["redrive_all"].append(t)
+        # M = 2 against no policy: the sweep after a nack of everything, then the leased receive of the redelivered records
+        for on in (True, False):
+            clear(); s.lease_set_policy(0, 0)
+            if on:
+                s.lease_set_policy(2, rec_cap)
+            r = lease(); nack(r[4])
+            (red, _, _), t = call(lambda: s.lease_sweep(0.0))
+            assert red == per_step
+            rows["sweep_m2_fills_ledger" if on else "sweep_policy_off"].append(t)
+            r, t = call(lease)
+            assert len(r[1]) == per_step
+            rows["lease_m2_looks_up_all" if on else "lease_after_sweep_policy_off"].append(t)
+            if on:
+                assert int(s.lease_deliveries(np.array([r[4]], np.uint64))[0]) == 2
+            s.lease_settle(np.arange(r[4], r[4] + per_step, dtype=np.uint64), LEASE_ACK)
+    clk = clocks.stop()
+    s.close()
+    out = {k: med(v) for k, v in rows.items()}
+    out.update({"config": f"c2 backlog: {wl.A} agents, {wl.S} group sends x {wl.F} members = {per_step} records, {wl.L}-B "
+                          f"payloads; pinned host buffers; {rounds} rounds", "records": per_step, "clocks": clk})
+    out.update(_gpu_card(0))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", nargs="*", default=["c1", "c4", "c5", "k1", "bcast"])

@@ -378,6 +378,49 @@ int sdb_lease_settle(sdb_handle h, uint64_t n, const uint64_t* lease_id, uint32_
 int sdb_lease_sweep(sdb_handle h, double now, uint32_t flags, uint64_t* redelivered_out, uint64_t* blocked_out,
                     uint64_t* due_left_out);
 int sdb_lease_stats(sdb_handle h, sdb_lease_summary* out);
+/* ---- dead letters: delivery counts and a redelivery limit for leased receives (a poison message is redelivered at most
+ * max_deliveries times, then parked).  Off by default; nothing below allocates or launches anything until it is set.
+ *   Delivery count  a record returned by a leased receive has deliveries = 1, except when a sweep redelivered it from a
+ *                   lease with count k and it stayed pending since (no plain, priority, filtered or compact receive took
+ *                   it, no expiry or purge retired it): then the next leased receive that returns it gives it k + 1.
+ *                   Records put back by sdb_restore_compact (requeue, redrive) start again at 1.  Records are identified by
+ *                   (agent, seq); when two pending copies share both, which one inherits the count is unspecified.
+ *   Ledger          the counts of redelivered records wait in a device table keyed by (agent, seq) holding the ring
+ *                   position and arena handle restore gave the record (56 bytes per entry).  Each leased receive and
+ *                   sweep first drops the entries whose record is no longer that one (left the window, consumed, or the
+ *                   slot names another handle), so a count is never inherited by a different record.  A sweep redelivers
+ *                   at most the ledger's free room: the rest stays leased and is counted in *due_left_out.
+ *   sdb_lease_set_policy  max_deliveries = 0 turns the policy off and frees its memory; max_deliveries >= 1 needs
+ *                   ledger_entries >= 1 (0xFFFFFFFF: counts without a limit).  Clears the ledger.  SDB_EINVAL without a
+ *                   reserved store, while the store holds live leases or dead letters, or for M > 0 with no ledger.
+ *                   sdb_lease_reserve turns the policy off.
+ *   Sweep           with M > 0, every live due lease (every live lease under SDB_LEASE_ALL) whose deliveries >= M becomes a
+ *                   dead letter instead of being redelivered; dead letters are not counted in *redelivered_out,
+ *                   *blocked_out or *due_left_out.  They stay in the store (entries_used, payload_used) and shrink a
+ *                   leased receive's capacity until they are taken.  Settle reads them as not live.  A sweep that fails
+ *                   with SDB_EARENA_FULL leaves store, ledger, rings and stats as they were.
+ *   sdb_lease_deliveries  the count of each live or dead lease; 0 for an unknown, acked or redelivered id.
+ *   sdb_lease_dead_letters  the dead letters of the listed agents (agent_idx NULL: every index below the watermark; an
+ *                   agent listed twice: SDB_EINVAL), agents in list order and lease-id order within an agent, in the
+ *                   compact format (sdb_receive_compact's points 1-3: rows shared by records of one store row, numbered by
+ *                   first appearance) with its capacity rule (point 4, lead-agent exception included): loop until
+ *                   *total_out == 0.  deliveries_out[total] (nullable) = each record's count.  SDB_RECV_PEEK leaves them
+ *                   in the store; without it they leave the store and their space is freed.  Other flag bits: SDB_EINVAL.
+ *                   The output is valid sdb_restore_compact input as it stands: a redrive is a take and a restore (ids
+ *                   kept, counts restart at 1).
+ *   sdb_lease_policy_stats  host bookkeeping (no synchronisation): ledger_used as of the last collection or lookup,
+ *                   held_by_ledger_total = due leases sweeps left in the store because the ledger was full.
+ * All but sdb_lease_policy_stats are stream-ordered and synchronise; refused calls zero their outputs and change nothing. */
+typedef struct sdb_lease_policy_summary {
+  uint64_t max_deliveries, dead, dead_total, ledger_used, ledger_cap, held_by_ledger_total;
+} sdb_lease_policy_summary;
+int sdb_lease_set_policy(sdb_handle h, uint32_t max_deliveries, uint64_t ledger_entries);
+int sdb_lease_deliveries(sdb_handle h, uint64_t n, const uint64_t* lease_id, uint32_t* deliveries_out);
+int sdb_lease_dead_letters(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t flags,
+                           uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                           sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                           uint32_t* deliveries_out, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
+int sdb_lease_policy_stats(sdb_handle h, sdb_lease_policy_summary* out);
 /* Low-latency dequeue server (opt-in): receive_messages (M:521-601) for ONE agent in a few microseconds.
  * enable = 1 starts a persistent single-CTA kernel on its own stream that polls a mailbox in mapped pinned host memory;
  * sdb_receive_batch calls naming exactly one agent with host outputs (what the Python surface's receive_messages makes)

@@ -129,6 +129,11 @@ class SdbLeaseSummary(C.Structure):
                                           "entries_reserved", "payload_used", "payload_reserved")]
 
 
+class SdbLeasePolicySummary(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("max_deliveries", "dead", "dead_total", "ledger_used", "ledger_cap",
+                                          "held_by_ledger_total")]
+
+
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_profile_read_n", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
@@ -138,7 +143,8 @@ EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sd
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
            "sdb_release_backends", "sdb_select_backend_batch", "sdb_agent_loads", "sdb_queue_stats",
            "sdb_assign_agent_backends", "sdb_backend_loads_from_queues", "sdb_lease_reserve", "sdb_receive_leased",
-           "sdb_lease_settle", "sdb_lease_sweep", "sdb_lease_stats"]
+           "sdb_lease_settle", "sdb_lease_sweep", "sdb_lease_stats", "sdb_lease_set_policy", "sdb_lease_deliveries",
+           "sdb_lease_dead_letters", "sdb_lease_policy_stats"]
 
 _lib = None
 
@@ -189,6 +195,11 @@ def load_library() -> C.CDLL:
     L.sdb_lease_settle.restype = i32; L.sdb_lease_settle.argtypes = [vp, u64, vp, u32, C.c_double, vp, vp]
     L.sdb_lease_sweep.restype = i32; L.sdb_lease_sweep.argtypes = [vp, C.c_double, u32, vp, vp, vp]
     L.sdb_lease_stats.restype = i32; L.sdb_lease_stats.argtypes = [vp, C.POINTER(SdbLeaseSummary)]
+    L.sdb_lease_set_policy.restype = i32; L.sdb_lease_set_policy.argtypes = [vp, u32, u64]
+    L.sdb_lease_deliveries.restype = i32; L.sdb_lease_deliveries.argtypes = [vp, u64, vp, vp]
+    L.sdb_lease_dead_letters.restype = i32
+    L.sdb_lease_dead_letters.argtypes = [vp, u32, vp, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp, vp]
+    L.sdb_lease_policy_stats.restype = i32; L.sdb_lease_policy_stats.argtypes = [vp, C.POINTER(SdbLeasePolicySummary)]
     L.sdb_expire.restype = i32
     L.sdb_expire.argtypes = [vp, u32, vp, C.c_double, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_receive_where.restype = i32
@@ -635,6 +646,38 @@ class Shard:
         s = SdbLeaseSummary()
         self._check(self._L.sdb_lease_stats(self._h, C.byref(s)))
         return {n: int(getattr(s, n)) for n, _ in SdbLeaseSummary._fields_}
+
+    def lease_set_policy(self, max_deliveries: int, ledger_entries: int) -> None:
+        """Redelivery limit and ledger size (include/swarmdb_b200.h: sdb_lease_set_policy); (0, 0) turns it off."""
+        self._check(self._L.sdb_lease_set_policy(self._h, int(max_deliveries), int(ledger_entries)))
+
+    def lease_deliveries(self, lease_ids) -> np.ndarray:
+        """Delivery count of each live or dead lease (uint32), 0 for unknown, acked or redelivered ids."""
+        ids = _arr(np.atleast_1d(lease_ids), np.uint64)
+        out = np.zeros(len(ids), np.uint32)
+        self._check(self._L.sdb_lease_deliveries(self._h, len(ids), _p(ids), _p(out)))
+        return out
+
+    def lease_dead_letters(self, agents, flags: int = 0, out_entries: Optional[np.ndarray] = None,
+                           out_sends: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+        """The listed agents' dead letters in receive_compact's shape (PEEK leaves them in the store).  Returns
+        (counts, entries, sends, payload, deliveries); the first four are valid restore_compact input as they stand."""
+        a, n, counts = self._agents_arg(agents)
+        ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
+        deliv = np.zeros(len(ent), np.uint32)
+        total, n_sends, pbytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_lease_dead_letters(self._h, n, _p(a), flags, _p(counts), _p(ent), len(ent), _p(snd),
+                                                   len(snd), _p(pay), pay.nbytes, _p(deliv),
+                                                   C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
+                                                   C.cast(C.byref(pbytes), C.c_void_p)))
+        if agents is None:
+            counts = counts[: self.stats_n_agents()]
+        return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value], deliv[: total.value]
+
+    def lease_policy_stats(self) -> dict:
+        s = SdbLeasePolicySummary()
+        self._check(self._L.sdb_lease_policy_stats(self._h, C.byref(s)))
+        return {n: int(getattr(s, n)) for n, _ in SdbLeasePolicySummary._fields_}
 
     def expire(self, agents, older_than: float, flags: int = 0, archive: bool = True,
                out_entries: Optional[np.ndarray] = None, out_sends: Optional[np.ndarray] = None,

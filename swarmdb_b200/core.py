@@ -161,6 +161,21 @@ class GpuConfig:
     num_shards: int = 1
     lease_records: int = 0                # leased receives: device lease store entries (0: no store, no memory)
     lease_payload_bytes: int = 0          # ... and payload bytes (0: lease_records x pad32(max_payload_bytes))
+    lease_max_deliveries: int = 0         # dead letters: deliveries after which a leased message is parked (0: no limit,
+                                          # no counts); needs lease_records
+    lease_ledger_entries: int = 0         # ... and the device ledger of redelivered records' counts (0: lease_records)
+
+
+def _check_lease_policy(g: GpuConfig) -> None:
+    """The dead-letter settings of a GpuConfig, checked before any device work."""
+    if not 0 <= g.lease_max_deliveries <= 0xFFFFFFFF:
+        raise ValueError(f"GpuConfig.lease_max_deliveries={g.lease_max_deliveries} is outside [0, 2^32 - 1]")
+    if not 0 <= g.lease_ledger_entries < (1 << 31):
+        raise ValueError(f"GpuConfig.lease_ledger_entries={g.lease_ledger_entries} is outside [0, 2^31)")
+    if g.lease_max_deliveries and not g.lease_records:
+        raise ValueError("GpuConfig.lease_max_deliveries needs a lease store (GpuConfig.lease_records)")
+    if g.lease_ledger_entries and not g.lease_max_deliveries:
+        raise ValueError("GpuConfig.lease_ledger_entries is used only with GpuConfig.lease_max_deliveries")
 
 
 def _encode_content(content: Any) -> (bytes, int):
@@ -234,6 +249,7 @@ class SwarmsDB:
         self.config = config or KafkaConfig()
         self.gpu_config = gpu_config or GpuConfig()
         g = self.gpu_config
+        _check_lease_policy(g)
         # the transport: constructing it fails loudly when the CUDA library or a device is missing
         self.shard = _shard if _shard is not None else Shard(
             max_agents=g.max_agents, ring_slots=g.ring_slots, arena_bytes=g.arena_bytes,
@@ -277,6 +293,8 @@ class SwarmsDB:
         self._lease_deadlines: List[float] = []
         if g.lease_records:
             self.shard.lease_reserve(g.lease_records, g.lease_payload_bytes or g.lease_records * pad32(g.max_payload_bytes))
+        if g.lease_max_deliveries:
+            self.shard.lease_set_policy(g.lease_max_deliveries, g.lease_ledger_entries or g.lease_records)
         self._reset_buffer()
         self._closed = False
         self.admin_client = _TransportAdmin(self)          # M:202-204: callers only list topics through it
@@ -716,6 +734,10 @@ class SwarmsDB:
                 break
             hdr, full = _native.expand_compact(ent, snd, pay)
             msgs = self._decode(hdr, full, agent_id)
+            if self.gpu_config.lease_max_deliveries:       # one lookup per chunk: how often each message was delivered
+                counts = self.shard.lease_deliveries(np.arange(base, base + len(ent), dtype=np.uint64)).tolist()
+                for m, c in zip(msgs, counts):
+                    m.metadata["delivery_count"] = int(c)
             for k, m in enumerate(msgs):
                 self._leases.setdefault(m.id, []).append((a, base + k))
             out += msgs
@@ -795,6 +817,64 @@ class SwarmsDB:
             while self._lease_deadlines and self._lease_deadlines[0] <= now:
                 heapq.heappop(self._lease_deadlines)
         return total
+
+    # ------------------------------------------------------------------ dead letters (GpuConfig.lease_max_deliveries)
+    def _dead_letter_agents(self, agent_ids) -> Optional[np.ndarray]:
+        if not self.gpu_config.lease_max_deliveries:
+            raise SdbError(-1, "dead letters need GpuConfig.lease_max_deliveries")
+        self.flush()
+        return None if agent_ids is None else np.array([self._index(a) for a in agent_ids], np.uint32)
+
+    def dead_letters(self, agent_id: Optional[str] = None, max_messages: int = 100, peek: bool = False) -> List[Message]:
+        """Messages parked after GpuConfig.lease_max_deliveries deliveries without an ack, oldest lease first (agent by
+        agent when agent_id is None): status FAILED and metadata["delivery_count"].  peek=False takes them out of the
+        device store and marks the host's records FAILED, so resend_failed_messages sends them again as new messages;
+        redrive_dead_letters puts them back with their ids instead."""
+        agents = self._dead_letter_agents(None if agent_id is None else [agent_id])
+        out: List[Message] = []
+        while len(out) < max_messages:
+            k = min(max_messages - len(out), self.shard.max_recv_records)
+            cnt, ent, snd, pay, deliv = self.shard.lease_dead_letters(
+                agents, _native.RECV_PEEK if peek else 0, out_entries=np.zeros(k, _native.ENTRY_DTYPE),
+                out_sends=np.zeros(k, _native.SEND_DTYPE))
+            if len(ent) == 0:
+                break
+            hdr, full = _native.expand_compact(ent, snd, pay)
+            who = np.repeat(agents if agents is not None else np.arange(len(cnt), dtype=np.uint32), cnt.astype(np.int64))
+            msgs = self._decode(hdr, full, agent_id or "", record=False, status=MessageStatus.FAILED)
+            for m, c, a in zip(msgs, deliv.tolist(), who.tolist()):
+                m.metadata["delivery_count"] = int(c)
+                if not peek:
+                    if m.id in self.messages:
+                        self.messages[m.id].status = MessageStatus.FAILED
+                    else:
+                        self.messages[m.id] = m
+                    self._forget(a, [m.id])
+            out += msgs
+            if peek:
+                break
+        return out
+
+    def redrive_dead_letters(self, agent_ids: Optional[Iterable[str]] = None) -> int:
+        """Put dead letters back behind what their agents have pending, with their ids (a redrive); their delivery counts
+        start again at 1.  Each chunk is restored before it leaves the dead-letter store, so a refused restore (a full
+        ring) loses nothing.  Returns the messages redriven."""
+        agents = self._dead_letter_agents(None if agent_ids is None else list(agent_ids))
+        total = 0
+        while True:
+            cnt, ent, snd, pay, _ = self.shard.lease_dead_letters(agents, _native.RECV_PEEK)
+            if len(ent) == 0:
+                return total
+            idx = agents if agents is not None else np.arange(len(cnt), dtype=np.uint32)
+            ids = [self._make_id(int(x)) for x in ent["seq"].tolist()]
+            who = np.repeat(idx, cnt.astype(np.int64)).tolist()
+            n, seq_end = self.shard.restore_compact(idx, cnt, ent, snd, pay)
+            self._next_seq = max(self._next_seq, seq_end); self._b_first_seq = self._next_seq
+            taken = self.shard.lease_dead_letters(agents, 0)[1]
+            assert len(taken) == n, (len(taken), n)                 # the same chunk: nothing changed the store between
+            for a, mid in zip(who, ids):
+                self._forget(a, [mid])
+            total += n
 
     def _sweep_due(self, now: float) -> None:
         if self._lease_deadlines and self._lease_deadlines[0] <= now:
@@ -1036,6 +1116,9 @@ class SwarmsDB:
             if live:
                 logger.warning(f"queue snapshot leaves out {live} leased messages in flight "
                                f"(redeliver_expired(all=True) first to include them)")
+            dead = self.shard.lease_policy_stats()["dead"] if g.lease_max_deliveries else 0
+            if dead:
+                logger.warning(f"queue snapshot leaves out {dead} dead letters (redrive_dead_letters() first to include them)")
         cap = recv_capacity(g)
         agents = np.arange(len(self._agent_name), dtype=np.uint32)
         parts: List[Tuple[np.ndarray, ...]] = []
@@ -1354,6 +1437,8 @@ class SwarmsDB:
                "queue": self.shard.queue_stats()}             # pending totals / priority histogram / deepest inbox, computed on the device
         if self.gpu_config.lease_records:
             out["leases"] = self.shard.lease_stats()
+        if self.gpu_config.lease_max_deliveries:
+            out["dead_letters"] = self.shard.lease_policy_stats()["dead"]
         return out
 
     def resend_failed_messages(self) -> List[str]:

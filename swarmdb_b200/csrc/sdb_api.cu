@@ -74,14 +74,26 @@ cudaError_t sdb_launch_lease_append(const sdb_lease_buf*, const sdb_lease_scratc
                                     unsigned long long, double, uint64_t, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
 cudaError_t sdb_launch_lease_settle(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t, double, cudaStream_t,
                                     sdb_profiler*, int*);
-cudaError_t sdb_launch_lease_due(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, double, uint32_t, cudaStream_t, sdb_profiler*,
-                                 int*);
+cudaError_t sdb_launch_lease_due(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, double, uint32_t, uint32_t, cudaStream_t,
+                                 sdb_profiler*, int*);
 cudaError_t sdb_launch_lease_select(const sdb_dev_view*, const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t,
                                     uint32_t*, uint32_t*, uint32_t*, cudaStream_t, sdb_profiler*, int*);
 cudaError_t sdb_launch_lease_stage(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, unsigned long long,
                                    const sdb_compact_args*, cudaStream_t, sdb_profiler*, int*, int);
 cudaError_t sdb_launch_lease_compact(const sdb_lease_buf*, const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t,
-                                     cudaStream_t, sdb_profiler*, int*, int);
+                                     uint32_t, double, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_ledger_collect(const sdb_dev_view*, const sdb_ledger*, uint32_t, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_ledger_insert(const sdb_dev_view*, const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_ledger*,
+                                     const uint32_t*, const uint32_t*, const uint32_t*, uint32_t, uint32_t, cudaStream_t, sdb_profiler*,
+                                     int*, int);
+cudaError_t sdb_launch_ledger_take(const sdb_lease_buf*, const sdb_ledger*, const sdb_compact_args*, const unsigned long long*, uint32_t,
+                                   uint64_t, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_deliveries(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, cudaStream_t, sdb_profiler*,
+                                        int*);
+cudaError_t sdb_launch_lease_dl_select(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_dl_scratch*, uint32_t, const uint32_t*,
+                                       uint32_t, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_dl_scratch*, uint32_t, uint32_t, uint32_t,
+                                     uint32_t, uint32_t, const sdb_compact_args*, uint32_t**, cudaStream_t, sdb_profiler*, int*, int);
 const void* sdb_lease_kernel_anchor();
 }
 
@@ -225,6 +237,15 @@ struct sdb_ctx {
     uint64_t used = 0, rows = 0, pay = 0;                // in buf[cur]
     uint64_t next_id = 0;                                // lease ids, monotonic per handle
     uint64_t live = 0, acked = 0, redelivered_total = 0, acked_total = 0;
+    // redelivery policy (sdb_lease_set_policy): delivery counts, the ledger and the dead-letter scratch, or nothing
+    std::vector<void*> pmem;                             // every device allocation of the policy
+    uint32_t max_deliveries = 0;                         // 0: no policy
+    bool policy = false;
+    sdb_ledger led{}; uint64_t led_cap = 0;
+    uint64_t led_n = 0, led_live = 0;                    // dense entries (taken ones included until a collection), held
+    unsigned long long* lth = nullptr;                   // pinned mirror of led.tot
+    sdb_dl_scratch dl{};
+    uint64_t dead = 0, dead_total = 0, held_total = 0;
   } lease;
   // backends
   uint32_t* be_weight = nullptr; unsigned long long* be_load = nullptr; uint32_t n_backends = 0;
@@ -2129,8 +2150,19 @@ static int restore_staged(sdb_ctx* h, uint32_t n_agents, uint64_t n_entries, uin
 }
 
 // ---- lease store: leased receive, settle, sweep ----------------------------------------------------------------------
+static void lease_policy_free(sdb_ctx* h) {
+  sdb_ctx::LeaseStore& L = h->lease;
+  for (void* p : L.pmem) cudaFree(p);
+  if (L.lth) cudaFreeHost(L.lth);
+  L.pmem.clear(); L.lth = nullptr;
+  L.buf[0].deliveries = L.buf[1].deliveries = nullptr;
+  L.led = sdb_ledger{}; L.dl = sdb_dl_scratch{};
+  L.policy = false; L.max_deliveries = 0; L.led_cap = L.led_n = L.led_live = 0;
+  L.dead = 0;
+}
 static void lease_free(sdb_ctx* h) {
   sdb_ctx::LeaseStore& L = h->lease;
+  lease_policy_free(h);
   for (void* p : L.mem) cudaFree(p);
   if (L.th) cudaFreeHost(L.th);
   L.mem.clear(); L.th = nullptr;
@@ -2148,6 +2180,7 @@ int sdb_lease_reserve(sdb_handle h, uint64_t max_records, uint64_t max_payload_b
   };
   sdb_ctx::LeaseStore& L = h->lease;
   if (L.live) return fail(h, SDB_EINVAL, "sdb_lease_reserve: the store holds live leases (ack them or sweep them back first)");
+  if (L.dead) return fail(h, SDB_EINVAL, "sdb_lease_reserve: the store holds dead letters (sdb_lease_dead_letters first)");
   if (max_records > 0xFFFFFFF0ull) return fail(h, SDB_EINVAL, "sdb_lease_reserve: max_records above 2^32 - 16");
   { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }        // cudaFree / cudaMalloc wait for running kernels
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
@@ -2186,6 +2219,17 @@ int sdb_lease_reserve(sdb_handle h, uint64_t max_records, uint64_t max_payload_b
   return SDB_OK;
 }
 
+// Collection pass of the redelivery ledger (stream-ordered, no synchronisation): the entries whose record is still the
+// one a sweep put back are rebuilt into the other buffer and re-indexed; led.tot[0] counts them.
+static cudaError_t ledger_collect(sdb_ctx* h) {
+  sdb_ctx::LeaseStore& L = h->lease;
+  int nl = 0;
+  cudaError_t e = sdb_launch_ledger_collect(&h->view, &L.led, static_cast<uint32_t>(L.led_n), h->stream, &h->prof, &nl);
+  h->launches += nl;
+  std::swap(L.led.ent, L.led.alt);
+  return e;
+}
+
 int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
                        double deadline, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
                        sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
@@ -2212,17 +2256,25 @@ int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_id
   sdb_recv_args r{};
   { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & SDB_RECV_PRIORITY, rec_cap, &r); if (rc != SDB_OK) return rc; }
   int nl = 0;
-  cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx);
+  const bool ledger = L.policy && L.led_n;      // the ledger holds entries: collect before anything is retired, look up after
+  cudaError_t e = ledger ? ledger_collect(h) : cudaSuccess;
+  if (e == cudaSuccess) e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx);
   h->last_rx_valid = false; h->last_rx_compact = true;
   if (e == cudaSuccess)
     e = sdb_launch_lease_append(&L.buf[L.cur], &L.s, &h->cx, h->rx_count, h->rx_totals, r.agent_idx, n_agents,
                                 static_cast<uint32_t>(L.used), static_cast<uint32_t>(L.rows), L.pay, L.next_id, deadline, rec_cap,
                                 P, h->stream, &h->prof, &nl, h->sm_count);
+  if (e == cudaSuccess && ledger)
+    e = sdb_launch_ledger_take(&L.buf[L.cur], &L.led, &h->cx, h->rx_totals, static_cast<uint32_t>(L.used), rec_cap, h->stream,
+                               &h->prof, &nl, h->sm_count);
+  if (e == cudaSuccess && ledger)
+    e = cudaMemcpyAsync(L.lth, L.led.tot, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream);
   h->launches += nl;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("leased receive launch: ") + cudaGetErrorString(e));
   uint64_t total = 0, n_sends = 0, pbytes = 0;
   { const int rc = copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, &total, &n_sends, &pbytes);
     if (rc != SDB_OK) return rc; }
+  if (ledger) { L.led_n = L.lth[0]; L.led_live = L.lth[0] - L.lth[1]; }
   L.used += total; L.rows += n_sends; L.pay += pbytes; L.live += total; L.next_id += total;
   if (total_out) *total_out = total;
   if (n_sends_out) *n_sends_out = n_sends;
@@ -2278,13 +2330,24 @@ int sdb_lease_sweep(sdb_handle h, double now, uint32_t flags, uint64_t* redelive
   { const int rc = restore_ensure(h); if (rc != SDB_OK) return rc; }
   const sdb_lease_buf& b = L.buf[L.cur];
   const uint32_t used = static_cast<uint32_t>(L.used), rows = static_cast<uint32_t>(L.rows);
+  const uint32_t M = L.max_deliveries;
+  if (L.policy && L.led_n) {                    // the ledger's free room is known exactly after a collection
+    cudaError_t ec = ledger_collect(h);
+    if (ec == cudaSuccess) ec = cudaMemcpyAsync(L.lth, L.led.tot, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream);
+    if (ec != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease sweep launch: ") + cudaGetErrorString(ec));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    L.led_n = L.led_live = L.lth[0];
+  }
   int nl = 0;
-  cudaError_t e = sdb_launch_lease_due(&b, &L.s, used, now, flags & SDB_LEASE_ALL, h->stream, &h->prof, &nl);
+  cudaError_t e = sdb_launch_lease_due(&b, &L.s, used, now, flags & SDB_LEASE_ALL, M, h->stream, &h->prof, &nl);
   h->launches += nl;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease sweep launch: ") + cudaGetErrorString(e));
   { const int rc = lease_totals(h, 0, 1); if (rc != SDB_OK) return rc; }
   const uint64_t due = L.th[0];
-  const uint32_t n = static_cast<uint32_t>(std::min<uint64_t>(due, recv_rec_cap(h)));    // one compact receive's capacity
+  uint64_t n64 = std::min<uint64_t>(due, recv_rec_cap(h));                             // one compact receive's capacity
+  const uint64_t held = L.policy ? n64 - std::min<uint64_t>(n64, L.led_cap - L.led_n) : 0;   // the ledger's free room
+  n64 -= held;
+  const uint32_t n = static_cast<uint32_t>(n64);
   uint64_t staged = 0, blocked = 0, redelivered = 0;
   if (n) {
     const size_t A = h->cfg.max_agents;
@@ -2305,19 +2368,29 @@ int sdb_lease_sweep(sdb_handle h, double now, uint32_t flags, uint64_t* redelive
       { const int rc = restore_staged(h, kept_runs, staged, L.th[6], L.th[7] * SDB_GRANULE, false, &redelivered);
         if (rc != SDB_OK) return rc; }                                     // SDB_EARENA_FULL: nothing written, store unchanged
       h->n_agents = std::max(h->n_agents, agent_end);
+      if (L.policy) {                                                      // the counts follow the records into the ledger
+        nl = 0;
+        e = sdb_launch_ledger_insert(&h->view, &b, &L.s, &L.led, h->rs_agent, h->rs_agent + A, h->rs_agent + 2 * A, kept_runs,
+                                     static_cast<uint32_t>(L.led_n), h->stream, &h->prof, &nl, h->sm_count);
+        h->launches += nl;
+        if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease sweep launch: ") + cudaGetErrorString(e));
+        L.led_n += staged; L.led_live += staged;
+      }
     }
   }
   // compaction: redelivered and acked entries are dropped, with the rows and payloads no live entry names
   nl = 0;
-  e = sdb_launch_lease_compact(&b, &L.buf[L.cur ^ 1], &L.s, used, rows, static_cast<uint32_t>(staged), h->stream, &h->prof, &nl,
-                               h->sm_count);
+  e = sdb_launch_lease_compact(&b, &L.buf[L.cur ^ 1], &L.s, used, rows, static_cast<uint32_t>(staged), M, now, flags & SDB_LEASE_ALL,
+                               h->stream, &h->prof, &nl, h->sm_count);
   h->launches += nl;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease sweep launch: ") + cudaGetErrorString(e));
-  { const int rc = lease_totals(h, 8, 3); if (rc != SDB_OK) return rc; }
+  { const int rc = lease_totals(h, 8, M ? 4 : 3); if (rc != SDB_OK) return rc; }
   h->stream_busy = false;
   L.cur ^= 1;
   L.used = L.th[8]; L.rows = L.th[9]; L.pay = L.th[10] * SDB_GRANULE;
-  L.live -= staged; L.redelivered_total += staged; L.acked = 0;
+  const uint64_t killed = M ? L.th[11] : 0;
+  L.live -= staged + killed; L.redelivered_total += staged; L.acked = 0;
+  L.dead += killed; L.dead_total += killed; L.held_total += held;
   if (redelivered_out) *redelivered_out = staged;
   if (blocked_out) *blocked_out = blocked;
   if (due_left_out) *due_left_out = due - n;
@@ -2331,6 +2404,145 @@ int sdb_lease_stats(sdb_handle h, sdb_lease_summary* out) {
   out->redelivered_total = L.redelivered_total; out->acked_total = L.acked_total;
   out->entries_used = L.used; out->entries_reserved = L.cap;
   out->payload_used = L.pay; out->payload_reserved = L.pay_cap;
+  return SDB_OK;
+}
+
+int sdb_lease_set_policy(sdb_handle h, uint32_t max_deliveries, uint64_t ledger_entries) {
+  if (!h) return SDB_EINVAL;
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (!L.cap) return fail(h, SDB_EINVAL, "sdb_lease_set_policy: no lease store (sdb_lease_reserve)");
+  if (L.live || L.dead) return fail(h, SDB_EINVAL, "sdb_lease_set_policy: the store holds live leases or dead letters");
+  if (max_deliveries && !ledger_entries) return fail(h, SDB_EINVAL, "sdb_lease_set_policy: a redelivery limit needs ledger entries");
+  if (ledger_entries > 0x7FFFFFF0ull) return fail(h, SDB_EINVAL, "sdb_lease_set_policy: ledger_entries above 2^31 - 16");
+  { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }        // cudaFree / cudaMalloc wait for running kernels
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  lease_policy_free(h);
+  if (!max_deliveries) return SDB_OK;
+  auto alloc = [h](auto** p, size_t n) {
+    void* q = nullptr;
+    if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(**p)) != cudaSuccess) return false;
+    h->lease.pmem.push_back(q);
+    *p = static_cast<std::remove_reference_t<decltype(*p)>>(q);
+    return true;
+  };
+  const size_t cap = L.cap, N = ledger_entries, A = h->cfg.max_agents, H = 256 * (cap / 1024 + 1);
+  sdb_dl_scratch& d = L.dl;
+  bool ok = alloc(&L.buf[0].deliveries, cap) && alloc(&L.buf[1].deliveries, cap) && alloc(&L.led.ent, N) && alloc(&L.led.alt, N) &&
+            alloc(&L.led.index, 2 * N) && alloc(&L.led.tot, 2) &&
+            alloc(&d.key_a, cap) && alloc(&d.key_b, cap) && alloc(&d.val_a, cap) && alloc(&d.val_b, cap) && alloc(&d.staged, cap) &&
+            alloc(&d.hist, H) && alloc(&d.h_local, H) && alloc(&d.h_tops, H / SDB_SCAN_TILE + 2) && alloc(&d.pos, A) && alloc(&d.cnt, A);
+  ok = ok && cudaHostAlloc(reinterpret_cast<void**>(&L.lth), 2 * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(d.pos, 0xFF, A * sizeof(uint32_t), h->stream) == cudaSuccess &&
+       cudaMemsetAsync(L.led.index, 0xFF, 2 * N * sizeof(uint32_t), h->stream) == cudaSuccess &&
+       cudaStreamSynchronize(h->stream) == cudaSuccess;
+  if (!ok) {
+    lease_policy_free(h);
+    cudaGetLastError();
+    return fail(h, SDB_ENOMEM, "sdb_lease_set_policy: device allocation failed");
+  }
+  L.led.slots = static_cast<uint32_t>(2 * N);
+  L.policy = true; L.max_deliveries = max_deliveries; L.led_cap = N;
+  return SDB_OK;
+}
+
+int sdb_lease_deliveries(sdb_handle h, uint64_t n, const uint64_t* lease_id, uint32_t* deliveries_out) {
+  if (!h) return SDB_EINVAL;
+  if (deliveries_out) std::memset(deliveries_out, 0, n * sizeof(uint32_t));
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (!L.policy) return fail(h, SDB_EINVAL, "sdb_lease_deliveries: no redelivery policy (sdb_lease_set_policy)");
+  if (n && (!lease_id || !deliveries_out)) return fail(h, SDB_EINVAL, "sdb_lease_deliveries: lease_id or deliveries_out is NULL");
+  for (uint64_t o = 0; o < n; o += SDB_LS_SETTLE_CHUNK) {
+    const uint32_t m = static_cast<uint32_t>(std::min<uint64_t>(SDB_LS_SETTLE_CHUNK, n - o));
+    CUDA_TRY(h, cudaMemcpyAsync(L.s.req, lease_id + o, m * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+    int nl = 0;
+    cudaError_t e = sdb_launch_lease_deliveries(&L.buf[L.cur], &L.s, static_cast<uint32_t>(L.used), m, h->stream, &h->prof, &nl);
+    h->launches += nl;
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease deliveries launch: ") + cudaGetErrorString(e));
+    CUDA_TRY(h, cudaMemcpyAsync(deliveries_out + o, L.s.at, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  h->stream_busy = false;
+  return SDB_OK;
+}
+
+int sdb_lease_dead_letters(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t flags,
+                           uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                           sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                           uint32_t* deliveries_out, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  sdb_ctx::LeaseStore& L = h->lease;
+  recv_agents(h, 0, agent_idx, &n_agents);
+  if (count_out && n_agents <= h->cfg.max_agents) std::memset(count_out, 0, static_cast<size_t>(n_agents) * sizeof(uint32_t));
+  if (flags & ~SDB_RECV_PEEK) return fail(h, SDB_EINVAL, "sdb_lease_dead_letters accepts SDB_RECV_PEEK only");
+  if (!L.policy) return fail(h, SDB_EINVAL, "sdb_lease_dead_letters: no redelivery policy (sdb_lease_set_policy)");
+  uint64_t rec_cap = 0;
+  { const int rc = out_rec_cap(h, std::min(room(entry_out, entry_cap), room(send_out, send_cap)), room(payload_out, payload_cap), &rec_cap);
+    if (rc != SDB_OK) return rc; }
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
+  if (n_agents == 0 || L.dead == 0) return SDB_OK;
+  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  const sdb_lease_buf& b = L.buf[L.cur];
+  const uint32_t used = static_cast<uint32_t>(L.used), rows = static_cast<uint32_t>(L.rows);
+  if (agent_idx)
+    CUDA_TRY(h, cudaMemcpyAsync(h->rx_agent, agent_idx, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  int nl = 0;
+  cudaError_t e = sdb_launch_lease_dl_select(&b, &L.s, &L.dl, used, agent_idx ? h->rx_agent : nullptr, n_agents, h->stream, &h->prof, &nl);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dead-letter launch: ") + cudaGetErrorString(e));
+  std::vector<uint32_t> cnt(n_agents);
+  CUDA_TRY(h, cudaMemcpyAsync(cnt.data(), L.dl.cnt, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  { const int rc = lease_totals(h, 0, 1); if (rc != SDB_OK) return rc; }
+  const uint64_t n_dead = L.th[0];
+  // the receive capacity rule: agents in list order while they fit, or the lead agent alone with its first rec_cap
+  uint64_t m = 0;
+  uint32_t q = 0;
+  for (; q < n_agents && m + cnt[q] <= rec_cap; ++q) m += cnt[q];
+  if (q < n_agents && m == 0) { cnt[q] = static_cast<uint32_t>(rec_cap); m = rec_cap; ++q; }
+  for (; q < n_agents; ++q) cnt[q] = 0;
+  if (count_out) std::memcpy(count_out, cnt.data(), static_cast<size_t>(n_agents) * sizeof(uint32_t));
+  if (m == 0) { h->stream_busy = false; return SDB_OK; }
+  const bool take = !(flags & SDB_RECV_PEEK);
+  uint32_t* dv = nullptr;
+  nl = 0;
+  e = sdb_launch_lease_dl_emit(&b, &L.s, &L.dl, rows, static_cast<uint32_t>(n_dead), static_cast<uint32_t>(m), n_agents, take ? 1u : 0u,
+                               &h->cx, &dv, h->stream, &h->prof, &nl, h->sm_count);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dead-letter launch: ") + cudaGetErrorString(e));
+  { const int rc = lease_totals(h, 6, 2); if (rc != SDB_OK) return rc; }
+  const uint64_t n_sends = L.th[6], pbytes = L.th[7] * SDB_GRANULE;
+  if (entry_out) CUDA_TRY(h, cudaMemcpyAsync(entry_out, h->cx.entry_out, m * sizeof(sdb_recv_entry), cudaMemcpyDeviceToHost, h->stream));
+  if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
+  if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
+  if (deliveries_out) CUDA_TRY(h, cudaMemcpyAsync(deliveries_out, dv, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  if (take) {                                   // the taken entries leave the store: compaction, as after a sweep
+    nl = 0;
+    e = sdb_launch_lease_compact(&b, &L.buf[L.cur ^ 1], &L.s, used, rows, 0u, 0u, 0.0, 0u, h->stream, &h->prof, &nl, h->sm_count);
+    h->launches += nl;
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dead-letter launch: ") + cudaGetErrorString(e));
+    { const int rc = lease_totals(h, 8, 3); if (rc != SDB_OK) return rc; }
+    L.cur ^= 1;
+    L.used = L.th[8]; L.rows = L.th[9]; L.pay = L.th[10] * SDB_GRANULE;
+    L.dead -= m; L.acked = 0;
+  } else {
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  h->stream_busy = false;
+  h->last_rx_valid = false; h->last_rx_compact = true;            // the compact receive's buffers were reused
+  if (total_out) *total_out = m;
+  if (n_sends_out) *n_sends_out = n_sends;
+  if (payload_bytes_out) *payload_bytes_out = pbytes;
+  return SDB_OK;
+}
+
+int sdb_lease_policy_stats(sdb_handle h, sdb_lease_policy_summary* out) {
+  if (!h || !out) return SDB_EINVAL;
+  const sdb_ctx::LeaseStore& L = h->lease;
+  out->max_deliveries = L.max_deliveries; out->dead = L.dead; out->dead_total = L.dead_total;
+  out->ledger_used = L.led_live; out->ledger_cap = L.led_cap; out->held_by_ledger_total = L.held_total;
   return SDB_OK;
 }
 

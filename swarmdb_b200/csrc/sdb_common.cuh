@@ -234,6 +234,7 @@ struct sdb_restore_args {
 #define SDB_LS_LIVE 0u
 #define SDB_LS_ACKED 1u
 #define SDB_LS_REDELIVERED 2u
+#define SDB_LS_DEAD 3u                 // past the redelivery limit (sdb_lease_set_policy): kept until sdb_lease_dead_letters
 struct sdb_lease_buf {
   sdb_recv_entry* ent;             // [cap] seq, store row, receiver
   uint32_t* agent;                 // [cap]
@@ -242,6 +243,32 @@ struct sdb_lease_buf {
   uint32_t* state;                 // [cap] SDB_LS_*
   sdb_recv_send* rows;             // [cap] payload_off into `payload`
   uint8_t* payload;                // [payload cap]
+  uint32_t* deliveries;            // [cap] delivery count of each lease; nullptr while no policy is set
+};
+// ---- redelivery ledger (sdb_lease_set_policy): the delivery count of every record a sweep put back, keyed by
+// (agent, seq), with the ring position p and arena handle restore gave it.  Dense entries in any order (a collection
+// rebuilds them into `alt` and swaps), plus an open-addressing index over them (load factor <= 1/2).
+struct sdb_ledger_ent {
+  unsigned long long seq;
+  uint32_t agent;
+  uint32_t count;                  // delivery count at redelivery; 0: taken by a leased receive
+  uint32_t p;                      // absolute ring position
+  uint32_t handle;                 // arena handle of the ring entry at p
+};
+static_assert(sizeof(sdb_ledger_ent) == 24, "ledger entries are 24 bytes");
+struct sdb_ledger {
+  sdb_ledger_ent* ent;             // [cap]
+  sdb_ledger_ent* alt;             // [cap]
+  uint32_t* index;                 // [slots] entry numbers, ~0 = empty
+  uint32_t slots;                  // 2 x cap
+  unsigned long long* tot;         // [2] entries kept by the last collection, entries taken by lookups since
+};
+// scratch of a dead-letter readout (sdb_lease_dead_letters), allocated with the policy: [cap] sort keys / values and
+// staged entries, radix digit tables for cap keys, [max_agents] list positions (~0 between calls) and per-position counts
+struct sdb_dl_scratch {
+  uint32_t *key_a, *key_b, *val_a, *val_b, *staged;
+  uint32_t *hist, *h_local, *h_tops;
+  uint32_t *pos, *cnt;
 };
 // scratch of the store's kernels; S = max(cap, max_recv_records), R = max_recv_records
 struct sdb_lease_scratch {

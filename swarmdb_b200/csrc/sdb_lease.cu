@@ -81,6 +81,7 @@ k_lease_append_agents(sdb_lease_buf b, const uint32_t* __restrict__ count, const
     for (uint32_t j = lane; j < c; j += 32) {
       const uint32_t e = used + off + j;
       b.agent[e] = a; b.id[e] = id_base + off + j; b.deadline[e] = deadline; b.state[e] = SDB_LS_LIVE;
+      if (b.deliveries) b.deliveries[e] = 1u;
     }
   }
 }
@@ -136,10 +137,12 @@ k_lease_settle_apply(sdb_lease_buf b, sdb_lease_scratch s, uint32_t n, uint32_t 
 
 // ---- sweep: due ---------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-k_lease_due(sdb_lease_buf b, uint32_t used, double now, uint32_t all, uint32_t* __restrict__ flag) {
+k_lease_due(sdb_lease_buf b, uint32_t used, double now, uint32_t all, uint32_t max_deliveries, uint32_t* __restrict__ flag) {
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= used) return;
-  flag[e] = b.state[e] == SDB_LS_LIVE && (all || b.deadline[e] <= now) ? 1u : 0u;   // NaN on either side: not due
+  bool due = b.state[e] == SDB_LS_LIVE && (all || b.deadline[e] <= now);         // NaN on either side: not due
+  if (max_deliveries && due) due = b.deliveries[e] < max_deliveries;              // at the limit: dead-lettered instead
+  flag[e] = due ? 1u : 0u;
 }
 
 // ---- sweep: select ------------------------------------------------------------------------------------------------
@@ -267,18 +270,33 @@ k_lease_stage_entries(sdb_lease_buf b, sdb_lease_scratch s, uint32_t n, sdb_recv
 }
 
 // ---- sweep: compact -----------------------------------------------------------------------------------------------
+// the redelivery limit: live due entries (the sweep's rule) with deliveries >= max_deliveries become dead letters.  Runs
+// after the redelivery succeeded, so a failed sweep leaves every state as it was.
+__global__ void __launch_bounds__(256)
+k_lease_kill(sdb_lease_buf b, uint32_t used, double now, uint32_t all, uint32_t max_deliveries, unsigned long long* __restrict__ tot) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  bool dead = false;
+  if (e < used && b.state[e] == SDB_LS_LIVE && (all || b.deadline[e] <= now) && b.deliveries[e] >= max_deliveries) {
+    b.state[e] = SDB_LS_DEAD;
+    dead = true;
+  }
+  const uint32_t c = __popc(__ballot_sync(0xFFFFFFFFu, dead));
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(tot, static_cast<unsigned long long>(c));
+}
+
 __global__ void __launch_bounds__(256)
 k_lease_mark(sdb_lease_buf b, sdb_lease_scratch s, uint32_t n) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k < n) b.state[s.staged[k]] = SDB_LS_REDELIVERED;
 }
 
-// kept entries (live) and the rows they name
+// kept entries (live and dead) and the rows they name
 __global__ void __launch_bounds__(256)
 k_lease_keep(sdb_lease_buf b, sdb_lease_scratch s, uint32_t used) {
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= used) return;
-  const bool keep = b.state[e] == SDB_LS_LIVE;
+  const uint32_t st = b.state[e];
+  const bool keep = st == SDB_LS_LIVE || st == SDB_LS_DEAD;
   s.flag[e] = keep ? 1u : 0u;
   if (keep) s.gran[b.ent[e].send] = 1u;
 }
@@ -297,7 +315,8 @@ k_lease_copy_entries(sdb_lease_buf in, sdb_lease_buf out, sdb_lease_scratch s, u
   sdb_recv_entry en = in.ent[e];
   en.send = ls_scan(s.g_local, s.g_tops, en.send);
   out.ent[k] = en; out.agent[k] = in.agent[e]; out.id[k] = in.id[e]; out.deadline[k] = in.deadline[e];
-  out.state[k] = SDB_LS_LIVE;
+  out.state[k] = in.state[e];
+  if (in.deliveries) out.deliveries[k] = in.deliveries[e];
 }
 
 // one warp per row: a kept row and its payload
@@ -357,13 +376,14 @@ extern "C" cudaError_t sdb_launch_lease_settle(const sdb_lease_buf* b, const sdb
   return cudaGetLastError();
 }
 
-// tot[0] = due entries
+// tot[0] = due entries (with a redelivery limit: those below it)
 extern "C" cudaError_t sdb_launch_lease_due(const sdb_lease_buf* b, const sdb_lease_scratch* s, uint32_t used, double now,
-                                            uint32_t all, cudaStream_t stream, sdb_profiler* prof, int* n_launches) {
+                                            uint32_t all, uint32_t max_deliveries, cudaStream_t stream, sdb_profiler* prof,
+                                            int* n_launches) {
   const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
   int nl = 0;
   cudaMemsetAsync(s->tot, 0, 16 * sizeof(unsigned long long), stream);
-  LS_LAUNCH(used, k_lease_due, *b, used, now, all, s->flag);
+  LS_LAUNCH(used, k_lease_due, *b, used, now, all, max_deliveries, s->flag);
   cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream);
   nl += used ? 2 : 0;
   sdb_prof_end(prof, pi, stream);
@@ -429,15 +449,18 @@ extern "C" cudaError_t sdb_launch_lease_stage(const sdb_lease_buf* b, const sdb_
   return e == cudaSuccess ? cudaGetLastError() : e;
 }
 
-// marks the n staged entries redelivered, then copies the live entries and the rows they name into `out`.
-// tot[8] = kept entries, tot[9] = kept rows, tot[10] = their payload granules
+// marks the n staged entries redelivered and, with a redelivery limit, the due live entries at it dead; then copies the
+// live and dead entries and the rows they name into `out`.
+// tot[8] = kept entries, tot[9] = kept rows, tot[10] = their payload granules, tot[11] = entries marked dead
 extern "C" cudaError_t sdb_launch_lease_compact(const sdb_lease_buf* in, const sdb_lease_buf* out, const sdb_lease_scratch* s,
-                                                uint32_t used, uint32_t rows_used, uint32_t n_staged, cudaStream_t stream,
-                                                sdb_profiler* prof, int* n_launches, int sm_count) {
+                                                uint32_t used, uint32_t rows_used, uint32_t n_staged, uint32_t max_deliveries,
+                                                double now, uint32_t all, cudaStream_t stream, sdb_profiler* prof,
+                                                int* n_launches, int sm_count) {
   const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
   int nl = 0;
-  cudaMemsetAsync(s->tot + 8, 0, 3 * sizeof(unsigned long long), stream);
+  cudaMemsetAsync(s->tot + 8, 0, (max_deliveries ? 4 : 3) * sizeof(unsigned long long), stream);
   LS_LAUNCH(n_staged, k_lease_mark, *in, *s, n_staged);
+  if (max_deliveries) LS_LAUNCH(used, k_lease_kill, *in, used, now, all, max_deliveries, s->tot + 11);
   if (rows_used) cudaMemsetAsync(s->gran, 0, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
   LS_LAUNCH(used, k_lease_keep, *in, *s, used);
   LS_LAUNCH(rows_used, k_lease_keep_rows, *in, *s, rows_used);
@@ -450,6 +473,260 @@ extern "C" cudaError_t sdb_launch_lease_compact(const sdb_lease_buf* in, const s
     k_lease_copy_rows<<<ls_grid(rows_used, 8, sm_count * 4), 256, 0, stream>>>(*in, *out, *s, rows_used);
     ++nl;
   }
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// ---- redelivery ledger (sdb_lease_set_policy) -------------------------------------------------------------------
+__device__ __forceinline__ uint32_t lg_slot(uint32_t a, unsigned long long seq, uint32_t slots) {
+  unsigned long long x = seq ^ (static_cast<unsigned long long>(a) * 0x9E3779B97F4A7C15ull);
+  x ^= x >> 33; x *= 0xFF51AFD7ED558CCDull; x ^= x >> 33; x *= 0xC4CEB9FE1A85EC53ull; x ^= x >> 33;
+  return static_cast<uint32_t>(__umul64hi(x, slots));
+}
+__device__ __forceinline__ void lg_index(const sdb_ledger& L, uint32_t k, uint32_t a, unsigned long long seq) {
+  for (uint32_t i = lg_slot(a, seq, L.slots);; i = i + 1 == L.slots ? 0u : i + 1)
+    if (atomicCAS(L.index + i, 0xFFFFFFFFu, k) == 0xFFFFFFFFu) return;
+}
+
+// Collection: an entry stays while its record is still the one the sweep put back: p inside the window [head, tail),
+// the ring entry at p not consumed and still naming the same arena handle (handles are unique while a record is
+// pending).  Kept entries go to L.alt in any order; tot[0] counts them.
+__global__ void __launch_bounds__(256)
+k_ledger_collect(sdb_dev_view v, sdb_ledger L, uint32_t n) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  bool keep = false;
+  sdb_ledger_ent en{};
+  if (e < n) {
+    en = L.ent[e];
+    if (en.count) {
+      const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + en.agent);
+      if (en.p - h.x < h.y - h.x) {
+        const uint2 r = sdb_ring_of(v, en.agent)[en.p & (v.ring_slots - 1)];
+        keep = sdb_meta(r) != SDB_META_TOMB && r.x == en.handle;
+      }
+    }
+  }
+  const uint32_t m = __ballot_sync(0xFFFFFFFFu, keep);
+  uint32_t base = 0;
+  if ((threadIdx.x & 31) == 0 && m) base = static_cast<uint32_t>(atomicAdd(L.tot, static_cast<unsigned long long>(__popc(m))));
+  base = __shfl_sync(0xFFFFFFFFu, base, 0);
+  if (keep) L.alt[base + __popc(m & ((1u << (threadIdx.x & 31)) - 1u))] = en;
+}
+
+// the index over the kept entries (L.ent is the collected buffer by now)
+__global__ void __launch_bounds__(256)
+k_ledger_reindex(sdb_ledger L, uint32_t n_bound) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_bound || k >= L.tot[0]) return;
+  const sdb_ledger_ent en = L.ent[k];
+  lg_index(L, k, en.agent, en.seq);
+}
+
+// after a sweep's restore: one warp per redelivered agent run.  Record j of a run of c sits at tail - c + j (restore
+// appends in entry order); its entry takes number n0 + (staged position).
+__global__ void __launch_bounds__(256)
+k_ledger_insert(sdb_dev_view v, sdb_lease_buf b, sdb_lease_scratch s, sdb_ledger L, const uint32_t* __restrict__ rs_agent,
+                const uint32_t* __restrict__ rs_count, const uint32_t* __restrict__ rs_first, uint32_t runs, uint32_t n0) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t q = gw; q < runs; q += nw) {
+    const uint32_t a = rs_agent[q], c = rs_count[q], f = rs_first[q];
+    const uint32_t tail = v.ring_hdr[a].tail;
+    const uint2* ring = sdb_ring_of(v, a);
+    for (uint32_t j = lane; j < c; j += 32) {
+      const uint32_t e = s.staged[f + j], p = tail - c + j;
+      sdb_ledger_ent en;
+      en.seq = b.ent[e].seq; en.agent = a; en.count = b.deliveries[e]; en.p = p; en.handle = ring[p & (v.ring_slots - 1)].x;
+      L.ent[n0 + f + j] = en;
+      lg_index(L, n0 + f + j, a, en.seq);
+    }
+  }
+}
+
+// after a leased receive's append: record i of the call (store entry used + i) inherits count + 1 from its ledger entry,
+// which it takes; tot[1] counts the entries taken
+__global__ void __launch_bounds__(256)
+k_ledger_take(sdb_lease_buf b, sdb_ledger L, const sdb_recv_entry* __restrict__ ent, const unsigned long long* __restrict__ rx_totals,
+              uint32_t used) {
+  const uint64_t n = rx_totals[0];
+  for (uint64_t i0 = static_cast<uint64_t>(blockIdx.x) * blockDim.x; i0 < n; i0 += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+    const uint64_t i = i0 + threadIdx.x;
+    uint32_t c = 0;
+    if (i < n) {
+      const uint32_t a = b.agent[used + i];
+      const unsigned long long seq = ent[i].seq;
+      for (uint32_t t = lg_slot(a, seq, L.slots);; t = t + 1 == L.slots ? 0u : t + 1) {
+        const uint32_t k = L.index[t];
+        if (k == 0xFFFFFFFFu) break;
+        if (L.ent[k].agent == a && L.ent[k].seq == seq && (c = atomicExch(&L.ent[k].count, 0u)) != 0u) break;
+      }
+      b.deliveries[used + i] = c + 1u;
+    }
+    const uint32_t m = __popc(__ballot_sync(0xFFFFFFFFu, c != 0u));
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(L.tot + 1, static_cast<unsigned long long>(m));
+  }
+}
+
+// ---- sdb_lease_deliveries: binary search over the ascending ids; 0 unless the lease is live or dead ---------------
+__global__ void __launch_bounds__(256)
+k_lease_deliveries(sdb_lease_buf b, uint32_t used, const unsigned long long* __restrict__ req, uint32_t* __restrict__ out, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long x = req[i];
+  uint32_t lo = 0, hi = used;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (b.id[mid] < x) lo = mid + 1; else hi = mid;
+  }
+  const bool held = lo < used && b.id[lo] == x && (b.state[lo] == SDB_LS_LIVE || b.state[lo] == SDB_LS_DEAD);
+  out[i] = held ? b.deliveries[lo] : 0u;
+}
+
+// ---- sdb_lease_dead_letters --------------------------------------------------------------------------------------
+// agent -> position in the caller's list (~0: not listed)
+__global__ void __launch_bounds__(256)
+k_lease_dl_pos(const uint32_t* __restrict__ agents, uint32_t n, uint32_t* __restrict__ pos, uint32_t clear) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) pos[agents[i]] = clear ? 0xFFFFFFFFu : i;
+}
+__device__ __forceinline__ uint32_t dl_pos(const uint32_t* pos, uint32_t n_list, uint32_t a) {
+  return pos ? pos[a] : (a < n_list ? a : 0xFFFFFFFFu);
+}
+// dead entries of listed agents, counted per list position
+__global__ void __launch_bounds__(256)
+k_lease_dl_flag(sdb_lease_buf b, uint32_t used, const uint32_t* __restrict__ pos, uint32_t n_list, uint32_t* __restrict__ flag,
+                uint32_t* __restrict__ cnt) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= used) return;
+  const uint32_t q = b.state[e] == SDB_LS_DEAD ? dl_pos(pos, n_list, b.agent[e]) : 0xFFFFFFFFu;
+  flag[e] = q != 0xFFFFFFFFu ? 1u : 0u;
+  if (q != 0xFFFFFFFFu) atomicAdd(cnt + q, 1u);
+}
+// flagged entry number k (store order = lease-id order): key = list position, value k, staged[k] = store entry
+__global__ void __launch_bounds__(256)
+k_lease_dl_keys(sdb_lease_buf b, uint32_t used, sdb_lease_scratch s, const uint32_t* __restrict__ pos, uint32_t n_list,
+                uint32_t* __restrict__ staged, uint32_t* __restrict__ key, uint32_t* __restrict__ val) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= used || !s.flag[e]) return;
+  const uint32_t k = ls_scan(s.f_local, s.f_tops, e);
+  key[k] = dl_pos(pos, n_list, b.agent[e]); val[k] = k; staged[k] = e;
+}
+// sorted position p: its entry (send = output row), its count; a take marks the entry for the compaction to drop
+__global__ void __launch_bounds__(256)
+k_lease_dl_emit(sdb_lease_buf b, sdb_lease_scratch s, const uint32_t* __restrict__ sv, uint32_t n, uint32_t take,
+                sdb_recv_entry* __restrict__ entry_out, uint32_t* __restrict__ deliveries_out) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const uint32_t e = s.staged[sv[p]];
+  sdb_recv_entry en = b.ent[e];
+  en.send = s.rmap[en.send];
+  entry_out[p] = en;
+  deliveries_out[p] = b.deliveries[e];
+  if (take) b.state[e] = SDB_LS_REDELIVERED;
+}
+
+// L->tot[0] = entries kept, L->tot[1] = entries taken since (both reset here); the caller swaps L->ent and L->alt
+extern "C" cudaError_t sdb_launch_ledger_collect(const sdb_dev_view* v, const sdb_ledger* L, uint32_t n, cudaStream_t stream,
+                                                 sdb_profiler* prof, int* n_launches) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  cudaMemsetAsync(L->tot, 0, 2 * sizeof(unsigned long long), stream);
+  cudaMemsetAsync(L->index, 0xFF, static_cast<size_t>(L->slots) * sizeof(uint32_t), stream);
+  LS_LAUNCH(n, k_ledger_collect, *v, *L, n);
+  sdb_ledger sw = *L;
+  sw.ent = L->alt; sw.alt = L->ent;
+  LS_LAUNCH(n, k_ledger_reindex, sw, n);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return cudaGetLastError();
+}
+
+extern "C" cudaError_t sdb_launch_ledger_insert(const sdb_dev_view* v, const sdb_lease_buf* b, const sdb_lease_scratch* s,
+                                                const sdb_ledger* L, const uint32_t* rs_agent, const uint32_t* rs_count,
+                                                const uint32_t* rs_first, uint32_t runs, uint32_t n0, cudaStream_t stream,
+                                                sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  if (runs) {
+    k_ledger_insert<<<ls_grid(runs, 8, sm_count * 4), 256, 0, stream>>>(*v, *b, *s, *L, rs_agent, rs_count, rs_first, runs, n0);
+    ++nl;
+  }
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return cudaGetLastError();
+}
+
+extern "C" cudaError_t sdb_launch_ledger_take(const sdb_lease_buf* b, const sdb_ledger* L, const sdb_compact_args* cx,
+                                              const unsigned long long* rx_totals, uint32_t used, uint64_t rec_cap,
+                                              cudaStream_t stream, sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  k_ledger_take<<<ls_grid(rec_cap, 256, sm_count * 4), 256, 0, stream>>>(*b, *L, cx->entry_out, rx_totals, used);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += 1;
+  return cudaGetLastError();
+}
+
+// the ids in s->req[0, n): counts to s->at
+extern "C" cudaError_t sdb_launch_lease_deliveries(const sdb_lease_buf* b, const sdb_lease_scratch* s, uint32_t used, uint32_t n,
+                                                   cudaStream_t stream, sdb_profiler* prof, int* n_launches) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  LS_LAUNCH(n, k_lease_deliveries, *b, used, s->req, s->at, n);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return cudaGetLastError();
+}
+
+// phase 1: the dead entries of the listed agents (agents == nullptr: every index below n_list), counted per position
+// into d->cnt[n_list]; s->tot[0] = their number.  Leaves keys, values and staged entries in store order.
+extern "C" cudaError_t sdb_launch_lease_dl_select(const sdb_lease_buf* b, const sdb_lease_scratch* s, const sdb_dl_scratch* d,
+                                                  uint32_t used, const uint32_t* agents, uint32_t n_list, cudaStream_t stream,
+                                                  sdb_profiler* prof, int* n_launches) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  cudaMemsetAsync(s->tot, 0, 16 * sizeof(unsigned long long), stream);
+  cudaMemsetAsync(d->cnt, 0, static_cast<size_t>(n_list) * sizeof(uint32_t), stream);
+  const uint32_t* pos = agents ? d->pos : nullptr;
+  if (agents) LS_LAUNCH(n_list, k_lease_dl_pos, agents, n_list, d->pos, 0u);
+  LS_LAUNCH(used, k_lease_dl_flag, *b, used, pos, n_list, s->flag, d->cnt);
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream);
+  nl += 2;
+  LS_LAUNCH(used, k_lease_dl_keys, *b, used, *s, pos, n_list, d->staged, d->key_a, d->val_a);
+  if (agents) LS_LAUNCH(n_list, k_lease_dl_pos, agents, n_list, d->pos, 1u);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// phase 2: stable sort of the n selected entries by list position (lease-id order within an agent), then the first m of
+// them in the compact format: rows numbered by first appearance (the sweep's row kernels over the sorted order), rows
+// and payloads to cx, entries to cx->entry_out, counts to *deliveries_dev (a sort buffer the result does not use).  take: the m entries are marked for the
+// compaction to drop.  tot[6] = rows, tot[7] = payload granules
+extern "C" cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf* b, const sdb_lease_scratch* s, const sdb_dl_scratch* d,
+                                                uint32_t rows_used, uint32_t n, uint32_t m, uint32_t n_list, uint32_t take,
+                                                const sdb_compact_args* cx, uint32_t** deliveries_dev, cudaStream_t stream,
+                                                sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  uint32_t *ks = nullptr, *vs = nullptr;
+  cudaError_t e = sdb_radix_sort_u32(d->key_a, d->val_a, d->key_b, d->val_b, n, ls_bits(n_list ? n_list - 1u : 0u), d->hist,
+                                     d->h_local, d->h_tops, &ks, &vs, stream, &nl);
+  uint32_t* dv = ks == d->key_a ? d->key_b : d->key_a;
+  *deliveries_dev = dv;
+  sdb_lease_scratch t = *s;
+  t.staged = d->staged;
+  if (rows_used) cudaMemsetAsync(t.rfirst, 0xFF, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
+  LS_LAUNCH(m, k_lease_row_first, *b, t, vs, m);
+  LS_LAUNCH(m, k_lease_row_heads, *b, t, vs, m);
+  if (e == cudaSuccess) e = sdb_scan_u32(t.flag, t.f_local, t.f_tops, m, t.tot + 6, nullptr, stream);
+  if (e == cudaSuccess) e = sdb_scan_u32(t.gran, t.g_local, t.g_tops, m, t.tot + 7, nullptr, stream);
+  nl += 4;
+  if (m) {
+    k_lease_stage_rows<<<ls_grid(m, 8, sm_count * 4), 256, 0, stream>>>(*b, t, vs, m, cx->send_out, cx->payload_out);
+    ++nl;
+  }
+  LS_LAUNCH(m, k_lease_dl_emit, *b, t, vs, m, take, cx->entry_out, dv);
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
   return e == cudaSuccess ? cudaGetLastError() : e;

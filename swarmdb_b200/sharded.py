@@ -511,7 +511,7 @@ class ShardedSwarmsDB(SwarmsDB):
         if g.id_nonce is None and not g.deterministic_ids:
             g = dataclasses.replace(g, deterministic_ids=True)       # ids must agree across ranks
         g = dataclasses.replace(g, shard_id=rank, num_shards=world)
-        if g.lease_records:
+        if g.lease_records or g.lease_max_deliveries:
             self._no_leases()
         k["gpu_config"] = g
         super().__init__(*a, _shard=shard, **k)
@@ -740,6 +740,7 @@ class ShardedSwarmsDB(SwarmsDB):
 
     receive_messages_leased = receive_batch_leased = settle_leases = _no_leases
     ack_messages = nack_messages = extend_leases = redeliver_expired = _no_leases
+    dead_letters = redrive_dead_letters = _no_leases
 
     def close(self) -> None:
         """Collective like flush(): every rank closes.  Buffered sends are NOT flushed here (a flush is a collective
