@@ -479,6 +479,7 @@ extern "C" cudaError_t sdb_launch_lease_compact(const sdb_lease_buf* in, const s
 }
 
 // ---- redelivery ledger (sdb_lease_set_policy) -------------------------------------------------------------------
+// restated in tests/deadletter_ref.py::lg_slot, which tests/test_gpu_lease_edges.py uses to make probe chains wrap
 __device__ __forceinline__ uint32_t lg_slot(uint32_t a, unsigned long long seq, uint32_t slots) {
   unsigned long long x = seq ^ (static_cast<unsigned long long>(a) * 0x9E3779B97F4A7C15ull);
   x ^= x >> 33; x *= 0xFF51AFD7ED558CCDull; x ^= x >> 33; x *= 0xC4CEB9FE1A85EC53ull; x ^= x >> 33;

@@ -28,27 +28,37 @@ class DeadLetterModel(LeaseModel):
     def set_policy(self, max_deliveries, ledger_entries):
         assert not any(r["state"] in (LIVE, DEAD) for r in self.recs)
         self.M, self.lcap = int(max_deliveries), int(ledger_entries) if max_deliveries else 0
-        self.ledger = []              # {"agent", "seq", "count", "p", "slot"}
+        self.ledger = []              # {"agent", "seq", "count", "p", "slot", "taken"}; taken ones leave at a collection
+        self._by_key = {}             # (agent, seq) -> its entries in ledger order
+        self.taken = 0
 
     @property
     def policy(self):
         return self.M > 0
 
     # ---- the ledger
+    def _add(self, en):
+        en["taken"] = False
+        self.ledger.append(en)
+        self._by_key.setdefault((en["agent"], en["seq"]), []).append(en)
+
     def collect(self):
         ring = self.o.ring
-        keep = []
-        for en in self.ledger:
+        old, self.ledger, self._by_key, self.taken = self.ledger, [], {}, 0
+        for en in old:
+            if en["taken"]:
+                continue
             w, h = ring.window(en["agent"]), ring.head[en["agent"]]
             i = en["p"] - h
             if 0 <= i < len(w) and w[i] is en["slot"] and w[i][1]:
-                keep.append(en)
-        self.ledger = keep
+                self._add(en)
 
     def _take(self, a, seq):
-        for k, en in enumerate(self.ledger):
-            if en["agent"] == a and en["seq"] == seq:
-                del self.ledger[k]
+        """The first untaken entry of (agent, seq) in ledger order: its count, and the entry is taken."""
+        for en in self._by_key.get((a, seq), []):
+            if not en["taken"]:
+                en["taken"] = True
+                self.taken += 1
                 return en["count"]
         return 0
 
@@ -95,7 +105,7 @@ class DeadLetterModel(LeaseModel):
             w, h = ring.window(a), ring.head[a]
             for j, r in enumerate(rs):
                 i = len(w) - len(rs) + j
-                self.ledger.append({"agent": a, "seq": int(r["hdr"]["seq"]), "count": r["deliveries"], "p": h + i, "slot": w[i]})
+                self._add({"agent": a, "seq": int(r["hdr"]["seq"]), "count": r["deliveries"], "p": h + i, "slot": w[i]})
         for r in at_limit:
             r["state"] = DEAD
         self.live -= len(at_limit)
@@ -167,4 +177,31 @@ class DeadLetterModel(LeaseModel):
 
     def policy_stats(self):
         return {"max_deliveries": self.M, "dead": sum(1 for r in self.recs if r["state"] == DEAD),
-                "dead_total": self.dead_total, "ledger_cap": self.lcap, "held_by_ledger_total": self.held_total}
+                "dead_total": self.dead_total, "ledger_used": len(self.ledger) - self.taken, "ledger_cap": self.lcap,
+                "held_by_ledger_total": self.held_total}
+
+
+# ---- the ledger's index (sdb_lease.cu: lg_slot): open addressing over slots = 2 x ledger_entries, probes run forward
+# and wrap from the last slot to slot 0
+_M64 = (1 << 64) - 1
+
+
+def lg_slot(agent, seq, slots):
+    """The first probe slot of (agent, seq), restated from sdb_lease.cu."""
+    x = (int(seq) ^ (int(agent) * 0x9E3779B97F4A7C15)) & _M64
+    x ^= x >> 33
+    x = (x * 0xFF51AFD7ED558CCD) & _M64
+    x ^= x >> 33
+    x = (x * 0xC4CEB9FE1A85EC53) & _M64
+    x ^= x >> 33
+    return (x * int(slots)) >> 64
+
+
+def seqs_at_slot(agent, slots, slot, start, n):
+    """The first n seqs >= start whose probe for `agent` starts at `slot`."""
+    out, s = [], int(start)
+    while len(out) < n:
+        if lg_slot(agent, s, slots) == slot:
+            out.append(s)
+        s += 1
+    return out

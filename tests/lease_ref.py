@@ -33,6 +33,7 @@ class LeaseModel:
         self.n_leases = 0         # leased calls so far (row keys are (call, row))
         self.live = self.acked = self.redelivered_total = self.acked_total = 0
         self.last_granules = 0
+        self.last_staged = []     # [(agent, [records])] the last sweep redelivered
 
     # ---- sdb_receive_leased
     def lease(self, agents, max_messages, deadline, flags=0, rows=None):
@@ -97,7 +98,6 @@ class LeaseModel:
 
     # ---- sdb_lease_sweep
     def sweep(self, now, all_=False):
-        from swarmdb_b200._native import ENTRY_DTYPE, SEND_DTYPE
         due = [r for r in self.recs if r["state"] == LIVE and (all_ or r["deadline"] <= now)]
         chunk = due[: self.rec_cap]
         by_agent = {}
@@ -112,28 +112,9 @@ class LeaseModel:
                 staged.append((a, rs))
         flat = [r for _, rs in staged for r in rs]
         self.last_granules = 0
+        self.last_staged = staged
         if flat:
-            # rows numbered by smallest seq (ties: first in agent order), one payload each
-            first = {}
-            for p, r in sorted(enumerate(flat), key=lambda t: (int(t[1]["hdr"]["seq"]), t[0])):
-                first.setdefault(r["row"], len(first))
-            ent = np.zeros(len(flat), ENTRY_DTYPE)
-            snd = np.zeros(len(first), SEND_DTYPE)
-            pays = [None] * len(first)
-            for k, r in enumerate(flat):
-                j = first[r["row"]]
-                ent[k] = (r["hdr"]["seq"], j, r["hdr"]["receiver"])
-                h = r["hdr"]
-                snd[j] = (h["timestamp"], 0, h["sender"], h["group"], h["len"], h["prio"], h["type"], 0)
-                pays[j] = r["pay"]
-            off = np.zeros(len(first), np.int64)
-            lens = np.array([len(p) for p in pays], np.int64)
-            if len(first) > 1:
-                off[1:] = np.cumsum(lens)[:-1]
-            snd["payload_off"] = off.astype(np.uint64)
-            payload = np.concatenate(pays) if pays else np.zeros(0, np.uint8)
-            agents = np.array([a for a, _ in staged], np.uint32)
-            counts = np.array([len(rs) for _, rs in staged], np.uint32)
+            agents, counts, ent, snd, payload = self.staged_input(staged)
             with self.o.appending():
                 restore_append(self.o, self.groups, agents, counts, ent, snd, payload)
             self.last_granules = restore_granules(counts, ent, snd, self.shared, agents)
@@ -143,6 +124,35 @@ class LeaseModel:
         self.recs = [r for r in self.recs if r["state"] == LIVE]
         self.acked = 0
         return len(flat), blocked, len(due) - len(chunk)
+
+    @staticmethod
+    def staged_input(staged, seq_key=int):
+        """The restore input of a sweep's staged records [(agent, [records])]: (agents, counts, entries, sends,
+        payload), rows numbered by smallest seq_key(seq) (ties: first in agent order), one payload each.  A seq_key
+        other than the identity shows what a sort on part of the seq would have numbered."""
+        from swarmdb_b200._native import ENTRY_DTYPE, SEND_DTYPE
+        flat = [r for _, rs in staged for r in rs]
+        first = {}
+        for p, r in sorted(enumerate(flat), key=lambda t: (seq_key(int(t[1]["hdr"]["seq"])), t[0])):
+            first.setdefault(r["row"], len(first))
+        ent = np.zeros(len(flat), ENTRY_DTYPE)
+        snd = np.zeros(len(first), SEND_DTYPE)
+        pays = [None] * len(first)
+        for k, r in enumerate(flat):
+            j = first[r["row"]]
+            ent[k] = (r["hdr"]["seq"], j, r["hdr"]["receiver"])
+            h = r["hdr"]
+            snd[j] = (h["timestamp"], 0, h["sender"], h["group"], h["len"], h["prio"], h["type"], 0)
+            pays[j] = r["pay"]
+        off = np.zeros(len(first), np.int64)
+        lens = np.array([len(p) for p in pays], np.int64)
+        if len(first) > 1:
+            off[1:] = np.cumsum(lens)[:-1]
+        snd["payload_off"] = off.astype(np.uint64)
+        payload = np.concatenate(pays) if pays else np.zeros(0, np.uint8)
+        agents = np.array([a for a, _ in staged], np.uint32)
+        counts = np.array([len(rs) for _, rs in staged], np.uint32)
+        return agents, counts, ent, snd, payload
 
     def stats(self):
         return {"live": self.live, "acked_unreclaimed": self.acked, "redelivered_total": self.redelivered_total,

@@ -150,3 +150,37 @@ def test_sharded_front_end_refuses_a_redelivery_limit():
     with pytest.raises(NotImplementedError):
         ShardedSwarmsDB(0, 1, gpu_config=GpuConfig(lease_max_deliveries=2, lease_records=8), shard=object())
     assert ShardedSwarmsDB.dead_letters is ShardedSwarmsDB.redrive_dead_letters
+
+
+def _lg_slot_np(agent, seq, slots):
+    """lg_slot in numpy's wrapping uint64 arithmetic: an independent restatement of the Python integer one."""
+    u = np.uint64
+    with np.errstate(over="ignore"):
+        x = u(seq) ^ (u(agent) * u(0x9E3779B97F4A7C15))
+        x ^= x >> u(33); x *= u(0xFF51AFD7ED558CCD); x ^= x >> u(33); x *= u(0xC4CEB9FE1A85EC53); x ^= x >> u(33)
+    return (int(x) * slots) >> 64
+
+
+def test_crafted_ledger_keys_collide_under_the_restated_hash():
+    """The keys tests/test_gpu_lease_edges.py sends: every seq of a wrap case probes from the index's last slot, and
+    the pair of the bit-32 case shares its first probe."""
+    from tests.deadletter_ref import lg_slot, seqs_at_slot
+    a = 8 * 64
+    for N in (2, 4):
+        slots = 2 * N
+        seqs = seqs_at_slot(a + 7, slots, slots - 1, 1000, N + 1)
+        assert seqs == sorted(set(seqs)) and len(seqs) == N + 1
+        assert all(lg_slot(a + 7, q, slots) == _lg_slot_np(a + 7, q, slots) == slots - 1 for q in seqs)
+    s = (1 << 33) + 1
+    while lg_slot(a + 5, s, 4) != lg_slot(a + 5, s + (1 << 32), 4):
+        s += 1
+    assert s < (1 << 33) + 64 and _lg_slot_np(a + 5, s, 4) == _lg_slot_np(a + 5, s + (1 << 32), 4)
+    # the hash spreads keys over the slots and reads the seq's high word and the agent
+    rng = np.random.default_rng(1)
+    for _ in range(200):
+        ag, q, n = int(rng.integers(0, 1 << 32)), int(rng.integers(0, 1 << 63)), int(rng.integers(1, 1 << 31))
+        assert lg_slot(ag, q, n) == _lg_slot_np(ag, q, n) < n
+    hits = np.bincount([lg_slot(3, q, 16) for q in range(4096)], minlength=16)
+    assert hits.min() > 160
+    assert len({lg_slot(5, q << 32, 1 << 20) for q in range(64)}) > 60
+    assert len({lg_slot(ag, 77, 1 << 20) for ag in range(64)}) > 60

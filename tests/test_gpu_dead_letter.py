@@ -55,9 +55,14 @@ def _lease(rig, m, agents, k, deadline, flags=0):
 
 def _sweep(rig, m, now, all_=False):
     from swarmdb_b200._native import LEASE_ALL
+    st0 = rig.g.stats()
     got = rig.g.lease_sweep(now, LEASE_ALL if all_ else 0)
     want = m.sweep(now, all_)
     assert got == want, (got, want)
+    st1 = rig.g.stats()
+    assert st1["enqueued"] - st0["enqueued"] == got[0] and st1["next_seq"] == st0["next_seq"]
+    assert st1["arena_tail_bytes"] - st0["arena_tail_bytes"] == 32 * m.last_granules, \
+        (st1["arena_tail_bytes"] - st0["arena_tail_bytes"], 32 * m.last_granules)
     _loads_equal(rig.g, rig.c, rig.idx, "after sweep")
     ls, ps = rig.g.lease_stats(), rig.g.lease_policy_stats()
     for k, v in m.stats().items():
@@ -86,6 +91,20 @@ def _nack_all(rig, m, ids):
     got = rig.g.lease_settle(ids, LEASE_RENEW, -math.inf)
     want = m.settle(ids, LEASE_RENEW, -math.inf)
     assert np.array_equal(got[0], want[0])
+
+
+def _to_the_limit(rig, m, agents, k=1000, rounds=16):
+    """Lease, nack and sweep until the agents have nothing pending and no lease is live: every record of theirs ends
+    as a dead letter."""
+    for _ in range(rounds):
+        ids = _lease(rig, m, agents, k, 10.0)
+        if len(ids):
+            _nack_all(rig, m, ids)
+        elif m.live == 0:
+            break
+        _sweep(rig, m, 0.0)
+    assert m.live == 0 and rig.g.lease_stats()["live"] == 0
+    assert not rig.g.agent_loads(agents)["pending"].any()
 
 
 def test_counts_rise_to_the_limit_then_the_sweep_dead_letters(shared):
@@ -204,6 +223,51 @@ def test_a_full_ledger_holds_records_until_the_redelivered_ones_are_received(sha
     _lease(rig, m, None, 1000, 10.0)                                    # takes the redelivered records' ledger entries
     red, _, left = _sweep(rig, m, 0.0)
     assert red == 5 and left == len(ids) - 10
+    _every_path(rig, rig.g, rig.c, shared, rig.rng)
+    rig.close()
+
+
+def test_a_blocked_ring_under_a_policy(shared):
+    """Agents x < y < z < w with 4 leases each, a ring of 16 slots, a limit of 3 and a ledger of 12 entries: the first
+    sweep takes 12 due records (w's 4 are held by the ledger), y's refilled ring blocks it, z's ring has exactly the
+    room for its 4.  The ledger numbers x's and z's entries densely across y's dropped run."""
+    from tests.test_gpu_shared_layout import _payloads
+    R = 16
+    rig = Rig(np.random.default_rng(9), G=8, F=64, extra=64, ring_slots=R)
+    rig.check_advance = False
+    x, y, z, w = (rig.G * rig.F + k for k in (1, 2, 3, 4))
+
+    def send_to(receivers):
+        r = np.asarray(receivers, np.uint32)
+        lens, off, buf = _payloads(rig.rng, len(r), 100)
+        s = rig.rng.integers(0, rig.A, len(r))
+        assert rig.c.send_batch(s, r, None, None, lens, off, buf) == rig.g.send_batch(s, r, None, None, lens, off, buf)
+
+    send_to([x] * 4 + [y] * 4 + [z] * 4 + [w] * 4)
+    send_to(rig.rng.integers(0, x, 100))
+    m = _model(rig, shared, 3, 12)
+    agents = [x, y, z, w]
+    ids = _lease(rig, m, agents, 100, 10.0)
+    assert len(ids) == 16
+    y_ids = ids[4:8]
+    _nack_all(rig, m, ids)
+    send_to([y] * (R - 3) + [z] * (R - 4))                             # y: 3 free slots for 4 records, z: 4 for 4
+    assert rig.c.capacity(y) == 3 and rig.c.capacity(z) == 4
+    assert _sweep(rig, m, 0.0) == (8, 1, 4)
+    ps = rig.g.lease_policy_stats()
+    assert ps["held_by_ledger_total"] == 4 and ps["ledger_used"] == 8
+    assert rig.g.lease_stats()["live"] == 8
+    assert rig.g.lease_deliveries(y_ids).tolist() == [1] * 4          # y's leases stay live with their counts
+    _same(rig.g.receive_batch([y], 100), rig.c.receive_batch([y], 100), "y's newer records")
+    assert _sweep(rig, m, 0.0) == (4, 0, 4)                            # y's records come back; w's wait for room
+    _to_the_limit(rig, m, agents)                                      # counts continue to the limit
+    assert rig.g.lease_policy_stats()["dead"] == 16 + R - 4            # z's newer records too
+    cnt, ent, snd, pay, dl = _dead(rig, m, agents, peek=True)
+    assert set(dl.tolist()) == {3}
+    cnt, ent, snd, pay, _ = _dead(rig, m, agents[::-1])
+    assert rig.g.restore_compact(agents[::-1], cnt, ent, snd, pay)[0] == len(ent)
+    m.redrive(agents[::-1], cnt, ent, snd, pay)
+    assert rig.g.lease_policy_stats()["dead"] == 0
     _every_path(rig, rig.g, rig.c, shared, rig.rng)
     rig.close()
 
