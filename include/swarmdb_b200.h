@@ -610,6 +610,56 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
                sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
 
+/* ---- relocation of pinned queues: the other remedy for an agent that pins the log.  Where sdb_expire drops its records,
+ * sdb_arena_relocate keeps them: it copies the live records of the agents pinning the log to the tail of the arena and
+ * rewrites those agents' ring entries in place, so the floor can pass the old region.  Nothing is delivered, dropped,
+ * re-sequenced or reordered; every agent's stream stays byte for byte what it was.
+ *   1. Selection  an agent below the registration watermark is selected when its oldest live (non-tombstoned) ring entry
+ *                 has its header below floor_bytes (compared as the floor reclaim does: distance below the tail, mod 2^32
+ *                 granules).  Arena positions strictly increase along every ring, so that is "has a pending record below
+ *                 floor_bytes".  Every live entry of a selected agent moves, those above the cut included.  floor_bytes at
+ *                 or below the floor selects nothing and moves nothing; floor_bytes >= the tail selects every agent with
+ *                 pending records (a full compaction).
+ *   2. Layout     the marked granules are the header of every moved record and the payload granules of every distinct
+ *                 payload image a moved record names.  They are copied in arena order to a region placed at the tail as a
+ *                 send's is (it never straddles the arena's wrap; the padding is skipped_bytes); the k-th goes to base + k.
+ *                 A moved ring entry keeps its ring position, prio and record-granule bits; its handle and payload distance
+ *                 are rewritten to the copies.  head / tail / ctail / ntomb do not change and tombstones stay as they are.
+ *                 So a shared payload is copied once for all the moved members of its send, and
+ *                 moved_bytes = 32 x (records + sum over distinct images of pad32(len) / 32) - the images are exactly the
+ *                 rows a PEEK sdb_receive_compact of the selected agents returns (its contract point 2).
+ *   3. Effect     every receive path (stream, priority, few-agent, latency server, compact, filtered, leased), expiry,
+ *                 restore, lease sweeps, dead letters and digests give the records they would have given without the
+ *                 call, byte for byte.  One thing differs in the compact format: when only some members of a shared-
+ *                 payload group send moved, the moved members name the copy and the others the original, so a compact
+ *                 result holding both returns that payload as two rows (its point 2); expanded, it is unchanged.  In
+ *                 sdb_stats only arena_tail_bytes and arena_floor_bytes move; sdb_agent_loads and sdb_queue_stats do not
+ *                 change.  Afterwards every pending record sits at or above min(floor_bytes, old tail) and
+ *                 arena_floor_bytes = floor_after.  Entries of the dead-letter ledger that count a moved record follow it,
+ *                 so delivery counts survive; the lease store keeps its own copies.
+ *   4. All or nothing: the call plans on the device, synchronises once, then copies and rewrites.  A region that does not
+ *                 fit behind the tail (tail + skip + moved - floor > arena, the floor recomputed) is SDB_EARENA_FULL and
+ *                 changes nothing.  Copies never overlap a live granule, so a full arena cannot be compacted in place:
+ *                 sdb_expire is the tool then.
+ *   5. Flags      SDB_RECV_PEEK: a dry run that fills the whole summary, floor_after and tail_after as the call would leave
+ *                 them, and writes nothing.  Any other bit: SDB_EINVAL.
+ *   6. Ordering   stream-ordered on the handle's stream; synchronises.  The device cursor of the asynchronous import is
+ *                 handed over as sdb_restore_compact does, so a later sdb_import_wire_ptrs_async places behind the moved
+ *                 region; the call may sit between sdb_import_prefetch(step) and sdb_import_wire_ptrs_async(step).  Works
+ *                 while the latency server runs.  Like a send it may overwrite the images sdb_overflow_log resolves: read
+ *                 the log first.
+ *   7. Memory     a granule bitmap, one u32 popcount and one u32 rank per bitmap word (3 x arena_bytes / 256 bytes: 12 MiB
+ *                 for a 1 GiB arena) and one bit per agent, allocated on the first call.
+ * The kernels are timed under SDB_PK_ARENA_FLOOR.  *out (nullable) receives the summary; it is zeroed on a refusal. */
+typedef struct sdb_relocate_summary {
+  uint64_t agents;          /* agents whose pending records moved */
+  uint64_t records;         /* ring entries rewritten */
+  uint64_t moved_bytes;     /* granules copied x SDB_GRANULE */
+  uint64_t skipped_bytes;   /* tail padding of the wrap rule (a region never straddles the arena's wrap) */
+  uint64_t floor_before, floor_after, tail_after;   /* bytes, the scale of sdb_stats.arena_*_bytes */
+} sdb_relocate_summary;
+int sdb_arena_relocate(sdb_handle h, uint64_t floor_bytes, uint32_t flags, sdb_relocate_summary* out);
+
 /* ---- filtered receive: query_messages / search_messages / get_conversation / delete_message (M:671-808, M:1132-1157)
  * on the device queue itself, and selective receives ("my COMMAND messages", "what the coordinator sent me").
  * sdb_receive_where takes, for each listed agent (agent_idx == NULL: as in sdb_receive_batch), the first max_messages

@@ -134,6 +134,11 @@ class SdbLeasePolicySummary(C.Structure):
                                           "held_by_ledger_total")]
 
 
+class SdbRelocateSummary(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("agents", "records", "moved_bytes", "skipped_bytes", "floor_before", "floor_after",
+                                          "tail_after")]
+
+
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_profile_read_n", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
@@ -144,7 +149,7 @@ EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sd
            "sdb_release_backends", "sdb_select_backend_batch", "sdb_agent_loads", "sdb_queue_stats",
            "sdb_assign_agent_backends", "sdb_backend_loads_from_queues", "sdb_lease_reserve", "sdb_receive_leased",
            "sdb_lease_settle", "sdb_lease_sweep", "sdb_lease_stats", "sdb_lease_set_policy", "sdb_lease_deliveries",
-           "sdb_lease_dead_letters", "sdb_lease_policy_stats"]
+           "sdb_lease_dead_letters", "sdb_lease_policy_stats", "sdb_arena_relocate"]
 
 _lib = None
 
@@ -200,6 +205,7 @@ def load_library() -> C.CDLL:
     L.sdb_lease_dead_letters.restype = i32
     L.sdb_lease_dead_letters.argtypes = [vp, u32, vp, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp, vp]
     L.sdb_lease_policy_stats.restype = i32; L.sdb_lease_policy_stats.argtypes = [vp, C.POINTER(SdbLeasePolicySummary)]
+    L.sdb_arena_relocate.restype = i32; L.sdb_arena_relocate.argtypes = [vp, u64, u32, C.POINTER(SdbRelocateSummary)]
     L.sdb_expire.restype = i32
     L.sdb_expire.argtypes = [vp, u32, vp, C.c_double, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_receive_where.restype = i32
@@ -678,6 +684,13 @@ class Shard:
         s = SdbLeasePolicySummary()
         self._check(self._L.sdb_lease_policy_stats(self._h, C.byref(s)))
         return {n: int(getattr(s, n)) for n, _ in SdbLeasePolicySummary._fields_}
+
+    def relocate(self, floor_bytes: int, peek: bool = False) -> dict:
+        """Move the pending records of every agent with one below `floor_bytes` to the arena tail, in place in their
+        rings (include/swarmdb_b200.h: sdb_arena_relocate); peek=True is a dry run.  Returns the summary."""
+        s = SdbRelocateSummary()
+        self._check(self._L.sdb_arena_relocate(self._h, int(floor_bytes), RECV_PEEK if peek else 0, C.byref(s)))
+        return {n: int(getattr(s, n)) for n, _ in SdbRelocateSummary._fields_}
 
     def expire(self, agents, older_than: float, flags: int = 0, archive: bool = True,
                out_entries: Optional[np.ndarray] = None, out_sends: Optional[np.ndarray] = None,

@@ -164,6 +164,7 @@ class GpuConfig:
     lease_max_deliveries: int = 0         # dead letters: deliveries after which a leased message is parked (0: no limit,
                                           # no counts); needs lease_records
     lease_ledger_entries: int = 0         # ... and the device ledger of redelivered records' counts (0: lease_records)
+    arena_relocate: bool = False          # a flush the arena refuses relocates the agents that pin the log and retries once
 
 
 def _check_lease_policy(g: GpuConfig) -> None:
@@ -358,12 +359,19 @@ class SwarmsDB:
         msgs = self._b_msgs
         try:
             payload = np.frombuffer(bytes(self._b_payload) + b"\0" * 32, dtype=np.uint8)
-            base = self.shard.send_mixed_batch(
-                np.asarray(self._b_sender, np.uint32), np.asarray(self._b_kind, np.uint8),
-                np.asarray(self._b_target, np.uint32), np.asarray(self._b_list_off, np.uint64),
-                np.asarray(self._b_list_idx, np.uint32), np.asarray(self._b_prio, np.uint8),
-                np.asarray(self._b_type, np.uint8), np.asarray(self._b_len, np.uint16),
-                np.asarray(self._b_off, np.uint64), payload, np.asarray(self._b_ts, np.float64))
+            batch = (np.asarray(self._b_sender, np.uint32), np.asarray(self._b_kind, np.uint8),
+                     np.asarray(self._b_target, np.uint32), np.asarray(self._b_list_off, np.uint64),
+                     np.asarray(self._b_list_idx, np.uint32), np.asarray(self._b_prio, np.uint8),
+                     np.asarray(self._b_type, np.uint8), np.asarray(self._b_len, np.uint16),
+                     np.asarray(self._b_off, np.uint64), payload, np.asarray(self._b_ts, np.float64))
+            try:
+                base = self.shard.send_mixed_batch(*batch)
+            except SdbError as e:
+                # a refused batch takes no sequence numbers and writes nothing, so it can be sent again as it is
+                if e.code != -5 or not self.gpu_config.arena_relocate:
+                    raise
+                self.relocate_pinned(self._batch_bound())
+                base = self.shard.send_mixed_batch(*batch)
             if base != self._b_first_seq:
                 raise RuntimeError(f"sequence mirror out of step: device {base}, host {self._b_first_seq}")
             st = self.shard.stats()
@@ -384,6 +392,47 @@ class SwarmsDB:
             self._reset_buffer()
             raise
         self._reset_buffer()
+
+    def _batch_bound(self) -> int:
+        """Arena bytes the buffered batch can take at most: one header and one padded payload per copy."""
+        total = 0
+        for kind, target, n in zip(self._b_kind, self._b_target, self._b_len):
+            if kind == 0:
+                copies = 1
+            elif kind == 1:
+                copies = len(self._group_snapshot[target] or ())
+            else:
+                copies = self._b_list_off[target + 1] - self._b_list_off[target]
+            total += copies * (32 + pad32(n))
+        return total
+
+    def relocate_pinned(self, free_bytes: int) -> dict:
+        """Make room for at least `free_bytes` more at the arena tail by moving the queued messages of the agents that pin
+        the log (idle, slow, crashed or deregistered receivers) to the tail, without delivering or dropping any
+        (include/swarmdb_b200.h: sdb_arena_relocate).  Finds the lowest cut that leaves the room with dry runs, then
+        relocates once and returns the device's summary.  Raises SdbError -5 (SDB_EARENA_FULL) and changes nothing when no
+        cut does: the arena then holds too many live messages, and only receiving or expiring them frees it."""
+        arena = int(self.gpu_config.arena_bytes)
+        need = int(free_bytes)
+
+        def short(tail: int, floor: int) -> int:           # bytes missing for `need` behind `tail` (the wrap rule included)
+            skip = arena - tail % arena if tail % arena + need > arena else 0
+            return tail + skip + need - floor - arena
+
+        tail = self.shard.stats()["arena_tail_bytes"]
+        cut = max(0, short(tail, 0))
+        for step in range(8):
+            # each step moves the cut to the floor the last dry run would have needed; the last one is at the tail
+            cut = tail if step == 7 else min(cut, tail)
+            s = self.shard.relocate(cut, peek=True)
+            missing = short(s["tail_after"], s["floor_after"])
+            if missing <= 0:
+                return self.shard.relocate(cut)
+            if cut >= tail:
+                break
+            cut = s["floor_after"] + missing
+        raise SdbError(-5, f"relocation cannot free {need} bytes of the message arena: it is full of live messages "
+                           f"(receive or expire them, or enlarge GpuConfig.arena_bytes)")
 
     def _mark_overflowed(self, msgs: List[Message], error: str) -> bool:
         """Delivery report for a batch that overflowed rings (M:374-391): the device logs (receiver, sequence number)

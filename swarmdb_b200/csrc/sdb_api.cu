@@ -95,6 +95,10 @@ cudaError_t sdb_launch_lease_dl_select(const sdb_lease_buf*, const sdb_lease_scr
 cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_dl_scratch*, uint32_t, uint32_t, uint32_t,
                                      uint32_t, uint32_t, const sdb_compact_args*, uint32_t**, cudaStream_t, sdb_profiler*, int*, int);
 const void* sdb_lease_kernel_anchor();
+cudaError_t sdb_launch_reloc_plan(const sdb_dev_view*, const sdb_reloc_args*, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_reloc_write(const sdb_dev_view*, const sdb_reloc_args*, const sdb_ledger*, uint32_t, cudaStream_t, sdb_profiler*,
+                                   int*, int);
+const void* sdb_relocate_kernel_anchor();
 }
 
 #define SDB_SCAN_TILE 4096u
@@ -227,6 +231,10 @@ struct sdb_ctx {
   uint32_t* rs_agent = nullptr;                          // restore: per-agent tables [6][max_agents] + scan tops, allocated
   unsigned long long* rs_tot = nullptr;                  // on first use; totals [8]
   uint32_t* rs_sort = nullptr;                           // restore: radix-sort keys / values [4][max_recv_records] + digit tables
+  uint32_t* rl_bits = nullptr;                           // relocation: granule bitmap [G / 32 + 2], its word popcounts and
+  uint32_t* rl_cnt = nullptr; uint32_t* rl_pre = nullptr; uint32_t* rl_tops = nullptr;   // their scan (same size) ...
+  uint32_t* rl_sel = nullptr;                            // ... selected agents [max_agents / 32 + 1], totals [8]; allocated on
+  unsigned long long* rl_tot = nullptr;                  // the first sdb_arena_relocate
   // lease store (sdb_lease_reserve): two buffers (a sweep compacts one into the other), scratch, host bookkeeping
   struct LeaseStore {
     sdb_lease_buf buf[2]{}; int cur = 0;
@@ -342,7 +350,7 @@ cudaError_t load_all_kernels() {
     if (q != cudaDriverEntryPointSuccess || !*fp) return cudaErrorNotSupported;
   }
   for (const void* anchor : {sdb_send_kernel_anchor(), sdb_recv_kernel_anchor(), sdb_balance_kernel_anchor(), sdb_xshard_kernel_anchor(),
-                              sdb_restore_kernel_anchor(), sdb_lease_kernel_anchor()}) {
+                              sdb_restore_kernel_anchor(), sdb_lease_kernel_anchor(), sdb_relocate_kernel_anchor()}) {
     cudaFunction_t f = nullptr;
     cudaError_t e = cudaGetFuncBySymbol(&f, anchor);
     if (e != cudaSuccess) return e;
@@ -1027,7 +1035,7 @@ int sdb_destroy(sdb_handle h) {
                  h->be_weight, h->be_load, h->be_scratch, h->be_logtab, h->be_req_cost, h->be_out, h->digest,
                  h->cx.table, h->cx.rec_slot, h->cx.head, h->cx.head_local, h->cx.head_tops, h->cx.gran, h->cx.gran_local,
                  h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out, h->where_bits, h->where_kw,
-                 h->rs_agent, h->rs_tot, h->rs_sort};
+                 h->rs_agent, h->rs_tot, h->rs_sort, h->rl_bits, h->rl_cnt, h->rl_pre, h->rl_tops, h->rl_sel, h->rl_tot};
   for (void* p : dev) if (p) cudaFree(p);
   lease_free(h);
   if (h->descs_host) cudaFreeHost(h->descs_host);
@@ -2146,6 +2154,86 @@ static int restore_staged(sdb_ctx* h, uint32_t n_agents, uint64_t n_entries, uin
     h->dev_stale = true;
   }
   *records_out = records;
+  return SDB_OK;
+}
+
+// ---- relocation of pinned queues -------------------------------------------------------------------------------------
+int sdb_arena_relocate(sdb_handle h, uint64_t floor_bytes, uint32_t flags, sdb_relocate_summary* out) {
+  if (!h) return SDB_EINVAL;
+  if (out) *out = sdb_relocate_summary{};
+  if (flags & ~SDB_RECV_PEEK) return fail(h, SDB_EINVAL, "sdb_arena_relocate accepts SDB_RECV_PEEK only");
+  { int rcc = cursor_to_host(h); if (rcc != SDB_OK) return rcc; }      // a host-placed write, like a send
+  const uint64_t G = h->arena_grans, tail = h->arena_tail;
+  if (!h->rl_bits) {
+    const size_t W = G / 32 + 2, A = h->cfg.max_agents;
+    const int rc = dmalloc_set(h, {{&h->rl_bits, W}, {&h->rl_cnt, W}, {&h->rl_pre, W}, {&h->rl_tops, W / SDB_SCAN_TILE + 2}, {&h->rl_sel, A / 32 + 1},
+                                   {&h->rl_tot, 8}}, "sdb_arena_relocate: device allocation failed");
+    if (rc != SDB_OK) return rc;
+  }
+  // every pending record lies in [arena_floor, tail), at most G granules below the tail
+  const uint64_t lo = std::max<uint64_t>(h->arena_floor, tail > G ? tail - G : 0) & ~31ull;
+  const uint64_t cut = std::min(floor_bytes / SDB_GRANULE + ((floor_bytes % SDB_GRANULE) ? 1u : 0u), tail);
+  sdb_reloc_args r{};
+  r.bits = h->rl_bits; r.cnt = h->rl_cnt; r.pre = h->rl_pre; r.tops = h->rl_tops; r.sel = h->rl_sel; r.tot = h->rl_tot;
+  r.lo = lo; r.tail = tail;
+  r.words = static_cast<uint32_t>((tail - lo) / 32 + 1);
+  r.thr = static_cast<uint32_t>(std::min<uint64_t>(tail - cut, 0xFFFFFFFFull));
+  r.n_agents = h->n_agents;
+  int nl = 0;
+  cudaError_t e = sdb_launch_reloc_plan(&h->view, &r, h->stream, &h->prof, &nl, h->sm_count);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("relocate plan launch: ") + cudaGetErrorString(e));
+  unsigned long long tot[5];
+  static_assert(sizeof(tot) <= TOT_SLOTS * sizeof(unsigned long long), "totals_host holds the relocation plan's totals");
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rl_tot, sizeof(tot), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  std::memcpy(tot, h->totals_host, sizeof(tot));
+  const uint64_t moved = tot[0];
+  const uint64_t floor_now = tail - tot[3];                            // what k_arena_floor would find now
+  uint64_t base = tail;
+  if (moved) {                                                         // arena_reserve's placement and fit test
+    if ((tail & (G - 1)) + moved > G) base = (tail + G - 1) & ~(G - 1);
+    if (moved > G || base + moved - floor_now > G)
+      return fail(h, SDB_EARENA_FULL, "sdb_arena_relocate: the moved records do not fit behind the arena tail (the arena is too "
+                                      "full of live records to relocate them: receive, expire, or choose a lower cut)");
+  }
+  const uint64_t tail_after = base + moved;
+  uint64_t floor_after = tot[4] ? tail - tot[4] : tail_after;          // the unselected agents' oldest records ...
+  if (moved) floor_after = std::min(floor_after, base);                // ... and the moved region
+  sdb_relocate_summary s{};
+  s.agents = tot[1]; s.records = tot[2];
+  s.moved_bytes = moved * SDB_GRANULE; s.skipped_bytes = (base - tail) * SDB_GRANULE;
+  s.floor_before = floor_now * SDB_GRANULE; s.floor_after = floor_after * SDB_GRANULE; s.tail_after = tail_after * SDB_GRANULE;
+  if (flags & SDB_RECV_PEEK) {
+    if (out) *out = s;
+    return SDB_OK;
+  }
+  if (moved) {
+    r.base = base;
+    const sdb_ctx::LeaseStore& L = h->lease;
+    const bool ledger = L.policy && L.led_n;
+    nl = 0;
+    e = sdb_launch_reloc_write(&h->view, &r, ledger ? &L.led : nullptr, static_cast<uint32_t>(ledger ? L.led_n : 0), h->stream,
+                               &h->prof, &nl, h->sm_count);
+    h->launches += nl;
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("relocate write launch: ") + cudaGetErrorString(e));
+    const int pi = sdb_prof_begin(&h->prof, SDB_PK_ARENA_FLOOR, h->stream);
+    e = sdb_launch_arena_floor(&h->view, h->n_agents, static_cast<uint32_t>(tail_after), h->rx_totals + TOT_FLOOR, h->stream);
+    sdb_prof_end(&h->prof, pi, h->stream);
+    h->launches += 1;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->totals_host + TOT_FLOOR, h->rx_totals + TOT_FLOOR, sizeof(unsigned long long),
+                                             cudaMemcpyDeviceToHost, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("relocate: ") + cudaGetErrorString(e));
+    h->arena_tail = tail_after;
+    h->arena_floor = tail_after - h->totals_host[TOT_FLOOR];
+  } else {
+    h->arena_floor = std::max(h->arena_floor, floor_now);
+  }
+  h->dev_stale = true;
+  s.floor_after = h->arena_floor * SDB_GRANULE;
+  if (out) *out = s;
   return SDB_OK;
 }
 

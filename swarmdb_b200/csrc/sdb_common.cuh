@@ -290,6 +290,24 @@ struct sdb_lease_scratch {
 };
 #define SDB_LS_SETTLE_CHUNK (1u << 20)
 
+// ---- relocation of pinned queues (sdb_arena_relocate, sdb_relocate.cu): the marked granules of one call, as a bitmap over
+// arena positions [lo, tail] (bit k = position lo + k, lo a multiple of 32), and the rank of each word (an exclusive scan of
+// their popcounts, block-local part in `pre`, per-tile part in `tops`): a marked granule at position x moves to base + rank(x)
+struct sdb_reloc_args {
+  uint32_t* bits;                  // [words]
+  uint32_t* cnt;                   // [words] popcount of each word
+  uint32_t* pre;                   // [words] its exclusive scan (block-local part)
+  uint32_t* tops;                  // [words / SDB_SCAN_TILE + 1]
+  uint32_t* sel;                   // [ceil(n_agents / 32)] bit a: agent a is selected
+  unsigned long long* tot;         // [0] marked granules [1] agents [2] records [3] largest distance below the tail of an
+                                   // agent's oldest pending record [4] the same over unselected agents (0: none pending)
+  unsigned long long lo, tail;     // granules
+  uint32_t words;                  // (tail - lo) / 32 + 1
+  uint32_t thr;                    // an agent is selected when its oldest pending header lies more than thr below the tail
+  uint32_t n_agents;
+  unsigned long long base;         // write phase: where the first marked granule goes
+};
+
 // ---- asynchronous import (sdb_import_wire_ptrs_async): everything the host used to learn through a sync lives on
 // the device.  `sdb_cursor` is the device-resident twin of the host's arena / sequence counters (whoever advanced
 // them last marks the other side stale); `sdb_batch_base` carries one import's placement from the kernel that

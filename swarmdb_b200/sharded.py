@@ -513,6 +513,9 @@ class ShardedSwarmsDB(SwarmsDB):
         g = dataclasses.replace(g, shard_id=rank, num_shards=world)
         if g.lease_records or g.lease_max_deliveries:
             self._no_leases()
+        if g.arena_relocate:
+            raise NotImplementedError("ShardedSwarmsDB does not retry refused flushes (GpuConfig.arena_relocate): an "
+                                      "asynchronous import that does not fit is dropped whole; call relocate_pinned instead")
         k["gpu_config"] = g
         super().__init__(*a, _shard=shard, **k)
         self.rank, self.world = rank, world
