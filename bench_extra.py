@@ -922,6 +922,88 @@ def deadletter(rounds=3):
     return out
 
 
+def lease_snapshot(rounds=3):
+    """Snapshots of in-flight work on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 records), policy
+    M = 3: the whole backlog leased, half of it nacked and swept back, so the store holds 2,097,152 live leases and the
+    ledger 2,097,152 counts of redelivered records still pending.  Per round:
+      - the export of the whole store into pinned buffers (one call) and the ledger export;
+      - into a fresh handle that was given the pending records (restore, not timed): the ledger import, then the lease
+        import of the exported chunk.
+    Per call: wall clock around the synchronising call and the `lease` kernel time from the profiler; algorithmic bytes of
+    the store calls (the compact output read from the store and written once, or read once and written to the store)
+    over that kernel time, against the H100 SXM's 3.35 TB/s."""
+    import torch
+    from bench import ClockSampler, Workload
+    from swarmdb_b200._native import ENTRY_DTYPE, LEASE_RENEW, META_DTYPE, RECV_PEEK, SEND_DTYPE, Shard, pad32
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py lease_snapshot: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    M = 3
+
+    def shard():
+        x = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+        x.register(np.arange(wl.A, dtype=np.uint32))
+        for g in range(wl.G):
+            x.create_group(g, wl.members(g))
+        x.lease_reserve(rec_cap, rec_cap * pad32(wl.L))
+        x.lease_set_policy(M, rec_cap)
+        return x
+
+    pin = lambda n: torch.empty(n, dtype=torch.uint8, pin_memory=True).numpy()          # noqa: E731
+    pin_ent, pin_snd, pin_pay = pin(rec_cap * 16).view(ENTRY_DTYPE), pin(rec_cap * 32).view(SEND_DTYPE), pin(rec_cap * wl.L)
+    pin_meta = pin(rec_cap * 32).view(META_DTYPE)
+    s = shard()
+    s.send_group_batch(*wl.batch())
+    base = s.receive_leased(None, 1 << 10, 1e300, 0, out_entries=pin_ent, out_sends=pin_snd, out_payload=pin_pay)[4]
+    s.lease_settle(np.arange(base, base + per_step // 2, dtype=np.uint64), LEASE_RENEW, -np.inf)
+    assert s.lease_sweep(0.0)[0] == per_step // 2
+    cnt, ent, snd, pay = (x.copy() for x in s.receive_compact(None, 1 << 10, RECV_PEEK, out_entries=pin_ent,
+                                                              out_sends=pin_snd, out_payload=pin_pay))
+
+    def call(x, fn):
+        x.sync(); x.profile(True)
+        t = time.perf_counter()
+        r = fn()
+        wall = (time.perf_counter() - t) * 1e3
+        prof = x.profile_read(); x.profile(False)
+        return r, {"wall_ms": wall, "lease_kernel_ms": prof["lease"][0]}
+
+    def med(rows):
+        return {k: float(np.median([r[k] for r in rows])) for k in rows[0]} | {"per_round": rows}
+
+    clocks = ClockSampler(0); clocks.start()
+    rows = {k: [] for k in ("export_store", "export_ledger", "import_ledger", "import_store")}
+    for _ in range(rounds):
+        (e, sn, p, m, nxt), t = call(s, lambda: s.lease_export(0, pin_ent, pin_snd, pin_pay, pin_meta))
+        assert len(e) == per_step // 2 and len(s.lease_export(nxt, pin_ent, pin_snd, pin_pay, pin_meta)[0]) == 0
+        moved = 2 * (len(e) * (16 + 32) + len(sn) * 32 + len(p))
+        rows["export_store"].append(t | {"bytes": moved, "tb_per_s": moved / t["lease_kernel_ms"] / 1e9})
+        (la, ls, lc), t = call(s, s.ledger_export)
+        assert len(la) == per_step // 2
+        rows["export_ledger"].append(t)
+        d = shard()
+        assert d.restore_compact(np.arange(len(cnt), dtype=np.uint32), cnt, ent, snd, pay)[0] == per_step // 2
+        n, t = call(d, lambda: d.ledger_import(la, ls, lc))
+        assert n == len(la)
+        rows["import_ledger"].append(t)
+        b, t = call(d, lambda: d.lease_import(e, sn, p, m))
+        rows["import_store"].append(t | {"bytes": moved, "tb_per_s": moved / t["lease_kernel_ms"] / 1e9})
+        assert d.lease_stats()["live"] == per_step // 2
+        d.close()
+    clk = clocks.stop()
+    s.close()
+    out = {k: med(v) for k, v in rows.items()}
+    out.update({"config": f"c2 backlog: {wl.A} agents, {wl.S} group sends x {wl.F} members = {per_step} records, {wl.L}-B "
+                          f"payloads, all leased, half nacked and swept back (M = {M}); pinned host buffers; {rounds} rounds",
+                "leases": per_step // 2, "ledger_counts": per_step // 2, "peak_tb_per_s": 3.35, "clocks": clk})
+    out.update(_gpu_card(0))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", nargs="*", default=["c1", "c4", "c5", "k1", "bcast"])

@@ -421,6 +421,66 @@ int sdb_lease_dead_letters(sdb_handle h, uint32_t n_agents, const uint32_t* agen
                            sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                            uint32_t* deliveries_out, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
 int sdb_lease_policy_stats(sdb_handle h, sdb_lease_policy_summary* out);
+/* ---- snapshots of in-flight work: the lease store and the redelivery ledger read out and put back, so that a restart
+ * keeps at-least-once delivery (leases not yet acked stay owed, dead letters stay parked, delivery counts continue).
+ *   sdb_lease_export  reads only: nothing in the store, ledger, rings or stats moves.  Returns the live leases and the dead
+ *                   letters with id >= start_id, in lease-id order (acked and not yet reclaimed entries are left out), in
+ *                   the compact format (sdb_receive_compact's points 1-3: rows numbered by first appearance, a store row
+ *                   named by several records is one row).  At most rec_cap records per call by sdb_receive_compact's
+ *                   point 4 (no agent grouping: the first rec_cap records); meta_out[total] (nullable, counted against
+ *                   entry_cap) receives each record's sdb_lease_meta.  *next_id_out = the id to pass next (start_id when
+ *                   nothing is returned): loop until *total_out == 0.  flags != 0 or no store: SDB_EINVAL.  It reuses the
+ *                   compact receive's buffers: sdb_digest_fold returns SDB_EINVAL afterwards until the next
+ *                   sdb_receive_batch.
+ *   sdb_lease_import  appends n records, in input order, behind whatever the store holds: record r gets lease id
+ *                   *lease_base_out + r (ids stay ascending) and keeps meta[r].deadline, .state and .deliveries (with a
+ *                   policy, 0 is imported as 1; without one counts are not stored; meta.id is not read).  Counters: live
+ *                   and dead grow by state, entries_used and payload_used grow.  Input in sdb_lease_export's shape; every
+ *                   row is checked and copied.  All or nothing: the input is validated on the device, the call
+ *                   synchronises once, then writes.  Refusals:
+ *                     SDB_EINVAL     NULL arrays with n > 0, entry.send >= n_sends, meta.agent >= max_agents,
+ *                                    entry.receiver neither meta.agent nor SDB_NO_RECEIVER, row len > max_payload_bytes or
+ *                                    prio > 3, payload_off not 16-byte aligned or payload_off + pad32(len) > payload_bytes,
+ *                                    a state other than LIVE or DEAD, a DEAD record on a handle without a policy,
+ *                                    flags != 0, no store;
+ *                     SDB_ECAPACITY  n or n_sends above one compact receive's rec_cap, or payload_bytes above
+ *                                    rec_cap x pad32(max_payload_bytes) (a chunk one export returned always imports in one
+ *                                    call); not enough free store entries, rows or payload ("lease store full").
+ *                   A LIVE lease with deliveries >= max_deliveries of the importing handle becomes a dead letter at its
+ *                   next due sweep.  Like sdb_lease_export it reuses the compact receive's buffers.
+ *   sdb_lease_ledger_export  runs the ledger's collection (the one every leased receive runs), so only entries whose
+ *                   record is still pending are reported, then writes all of them as (agent, seq, count) triples in no
+ *                   particular order; *n_out = their number.  cap below it: SDB_EOUTPUT with *n_out set, nothing written.
+ *                   No policy: SDB_EINVAL.
+ *   sdb_lease_ledger_import  for each triple the oldest pending (not consumed) record of `agent` whose header seq matches
+ *                   gets a ledger entry holding its ring position, its arena handle and `count`: the next leased receive
+ *                   of that record gives it count + 1, as if a sweep had redelivered it.  A triple with no such record
+ *                   is dropped and not counted in *matched_out; for a pair listed twice which entry wins is unspecified.
+ *                   SDB_EINVAL: no policy, agent >= max_agents, count == 0, NULL arrays with n > 0.  SDB_ECAPACITY: n
+ *                   above the ledger's free room after a collection.  Refusals change nothing.
+ * All four are stream-ordered and synchronise; a refused call zeroes its outputs and changes nothing.  Their kernels time
+ * under SDB_PK_LEASE. */
+#define SDB_LEASE_STATE_LIVE 0u
+#define SDB_LEASE_STATE_DEAD 3u
+typedef struct sdb_lease_meta {   /* 32 bytes, one per exported record */
+  uint64_t id;                    /* lease id on the exporting handle */
+  double   deadline;
+  uint32_t agent;
+  uint32_t deliveries;            /* 0 when the exporting handle has no policy */
+  uint32_t state;                 /* SDB_LEASE_STATE_LIVE or SDB_LEASE_STATE_DEAD */
+  uint32_t reserved;              /* 0 */
+} sdb_lease_meta;
+int sdb_lease_export(sdb_handle h, uint64_t start_id, uint32_t flags, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                     sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                     sdb_lease_meta* meta_out, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out,
+                     uint64_t* next_id_out);
+int sdb_lease_import(sdb_handle h, uint64_t n, const sdb_recv_entry* entries, const sdb_recv_send* sends, uint64_t n_sends,
+                     const uint8_t* payload, uint64_t payload_bytes, const sdb_lease_meta* meta, uint32_t flags,
+                     uint64_t* lease_base_out);
+int sdb_lease_ledger_export(sdb_handle h, uint64_t cap, uint32_t* agent_out, uint64_t* seq_out, uint32_t* count_out,
+                            uint64_t* n_out);
+int sdb_lease_ledger_import(sdb_handle h, uint64_t n, const uint32_t* agent, const uint64_t* seq, const uint32_t* count,
+                            uint64_t* matched_out);
 /* Low-latency dequeue server (opt-in): receive_messages (M:521-601) for ONE agent in a few microseconds.
  * enable = 1 starts a persistent single-CTA kernel on its own stream that polls a mailbox in mapped pinned host memory;
  * sdb_receive_batch calls naming exactly one agent with host outputs (what the Python surface's receive_messages makes)

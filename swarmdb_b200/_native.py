@@ -28,6 +28,11 @@ ENTRY_DTYPE = np.dtype([("seq", "<u8"), ("send", "<u4"), ("receiver", "<u4")])
 SEND_DTYPE = np.dtype([("timestamp", "<f8"), ("payload_off", "<u8"), ("sender", "<u4"), ("group", "<u4"),
                        ("len", "<u2"), ("prio", "u1"), ("type", "u1"), ("reserved", "<u4")])
 assert ENTRY_DTYPE.itemsize == 16 and SEND_DTYPE.itemsize == 32
+# one exported lease (sdb_lease_meta): its id on the exporting handle, deadline, agent, delivery count and state
+META_DTYPE = np.dtype([("id", "<u8"), ("deadline", "<f8"), ("agent", "<u4"), ("deliveries", "<u4"), ("state", "<u4"),
+                       ("reserved", "<u4")])
+assert META_DTYPE.itemsize == 32
+LEASE_STATE_LIVE, LEASE_STATE_DEAD = 0, 3
 
 NO_GROUP = 0xFFFFFFFF
 NO_RECEIVER = 0xFFFFFFFF
@@ -149,7 +154,8 @@ EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sd
            "sdb_release_backends", "sdb_select_backend_batch", "sdb_agent_loads", "sdb_queue_stats",
            "sdb_assign_agent_backends", "sdb_backend_loads_from_queues", "sdb_lease_reserve", "sdb_receive_leased",
            "sdb_lease_settle", "sdb_lease_sweep", "sdb_lease_stats", "sdb_lease_set_policy", "sdb_lease_deliveries",
-           "sdb_lease_dead_letters", "sdb_lease_policy_stats", "sdb_arena_relocate"]
+           "sdb_lease_dead_letters", "sdb_lease_policy_stats", "sdb_arena_relocate", "sdb_lease_export",
+           "sdb_lease_import", "sdb_lease_ledger_export", "sdb_lease_ledger_import"]
 
 _lib = None
 
@@ -205,6 +211,11 @@ def load_library() -> C.CDLL:
     L.sdb_lease_dead_letters.restype = i32
     L.sdb_lease_dead_letters.argtypes = [vp, u32, vp, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp, vp]
     L.sdb_lease_policy_stats.restype = i32; L.sdb_lease_policy_stats.argtypes = [vp, C.POINTER(SdbLeasePolicySummary)]
+    L.sdb_lease_export.restype = i32
+    L.sdb_lease_export.argtypes = [vp, u64, u32, vp, u64, vp, u64, vp, u64, vp, vp, vp, vp, vp]
+    L.sdb_lease_import.restype = i32; L.sdb_lease_import.argtypes = [vp, u64, vp, vp, u64, vp, u64, vp, u32, vp]
+    L.sdb_lease_ledger_export.restype = i32; L.sdb_lease_ledger_export.argtypes = [vp, u64, vp, vp, vp, vp]
+    L.sdb_lease_ledger_import.restype = i32; L.sdb_lease_ledger_import.argtypes = [vp, u64, vp, vp, vp, vp]
     L.sdb_arena_relocate.restype = i32; L.sdb_arena_relocate.argtypes = [vp, u64, u32, C.POINTER(SdbRelocateSummary)]
     L.sdb_expire.restype = i32
     L.sdb_expire.argtypes = [vp, u32, vp, C.c_double, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
@@ -684,6 +695,65 @@ class Shard:
         s = SdbLeasePolicySummary()
         self._check(self._L.sdb_lease_policy_stats(self._h, C.byref(s)))
         return {n: int(getattr(s, n)) for n, _ in SdbLeasePolicySummary._fields_}
+
+    def lease_export(self, start_id: int = 0, out_entries: Optional[np.ndarray] = None,
+                     out_sends: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None,
+                     out_meta: Optional[np.ndarray] = None):
+        """One chunk of the store's live leases and dead letters with id >= start_id, in lease-id order, without changing
+        anything (include/swarmdb_b200.h: sdb_lease_export).  Returns (entries, sends, payload, meta META_DTYPE, next_id);
+        loop from next_id until entries is empty.  Views into reusable buffers unless explicit arrays are given; out_meta
+        holds as many records as out_entries."""
+        ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
+        meta = out_meta
+        if meta is None:
+            if len(getattr(self, "_out_meta", ())) < len(ent):
+                self._out_meta = np.zeros(len(ent), META_DTYPE)
+            meta = self._out_meta
+        if len(meta) < len(ent):
+            raise ValueError("out_meta holds fewer records than out_entries")
+        total, n_sends, pbytes, nxt = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_lease_export(self._h, int(start_id), 0, _p(ent), len(ent), _p(snd), len(snd), _p(pay),
+                                             pay.nbytes, _p(meta), C.cast(C.byref(total), C.c_void_p),
+                                             C.cast(C.byref(n_sends), C.c_void_p), C.cast(C.byref(pbytes), C.c_void_p),
+                                             C.cast(C.byref(nxt), C.c_void_p)))
+        return ent[: total.value], snd[: n_sends.value], pay[: pbytes.value], meta[: total.value], int(nxt.value)
+
+    def lease_import(self, entries, sends, payload, meta, flags: int = 0) -> int:
+        """Append exported leases behind what the store holds, with their deadlines, states and counts
+        (include/swarmdb_b200.h: sdb_lease_import).  All or nothing.  Returns the lease id of the first record."""
+        ent, snd = np.ascontiguousarray(entries, ENTRY_DTYPE), np.ascontiguousarray(sends, SEND_DTYPE)
+        pay, met = np.ascontiguousarray(payload, np.uint8), np.ascontiguousarray(meta, META_DTYPE)
+        if len(met) != len(ent):
+            raise ValueError("entries and meta differ in length")
+        base = C.c_uint64(0)
+        self._check(self._L.sdb_lease_import(self._h, len(ent), _p(ent), _p(snd), len(snd), _p(pay), pay.nbytes, _p(met),
+                                             flags, C.cast(C.byref(base), C.c_void_p)))
+        return int(base.value)
+
+    def ledger_export(self) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """The redelivery ledger's counts of records still pending, as (agent uint32, seq uint64, count uint32) arrays in
+        no particular order (include/swarmdb_b200.h: sdb_lease_ledger_export)."""
+        n = C.c_uint64(0)
+        rc = self._L.sdb_lease_ledger_export(self._h, 0, None, None, None, C.cast(C.byref(n), C.c_void_p))
+        if rc not in (0, -8):                                       # -8 (SDB_EOUTPUT): n holds the size
+            self._check(rc)
+        while True:
+            k = int(n.value)
+            a, s, c = np.zeros(k, np.uint32), np.zeros(k, np.uint64), np.zeros(k, np.uint32)
+            rc = self._L.sdb_lease_ledger_export(self._h, k, _p(a), _p(s), _p(c), C.cast(C.byref(n), C.c_void_p))
+            if rc != -8:
+                self._check(rc)
+                return a[: n.value], s[: n.value], c[: n.value]
+
+    def ledger_import(self, agent, seq, count) -> int:
+        """Give each (agent, seq) triple's oldest pending record the delivery count `count` in the ledger, as if a sweep
+        had redelivered it (include/swarmdb_b200.h: sdb_lease_ledger_import).  Returns the triples matched."""
+        a, s, c = _arr(agent, np.uint32), _arr(seq, np.uint64), _arr(count, np.uint32)
+        if not len(a) == len(s) == len(c):
+            raise ValueError("agent, seq and count differ in length")
+        matched = C.c_uint64(0)
+        self._check(self._L.sdb_lease_ledger_import(self._h, len(a), _p(a), _p(s), _p(c), C.cast(C.byref(matched), C.c_void_p)))
+        return int(matched.value)
 
     def relocate(self, floor_bytes: int, peek: bool = False) -> dict:
         """Move the pending records of every agent with one below `floor_bytes` to the arena tail, in place in their

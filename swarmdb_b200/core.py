@@ -1150,17 +1150,25 @@ class SwarmsDB:
 
     # ------------------------------------------------------------------ queue snapshots (restart persistence)
     SNAPSHOT_VERSION = 1
+    SNAPSHOT_VERSION_IN_FLIGHT = 2          # format 1 + the lease store and the redelivery ledger
 
-    def save_queue_snapshot(self, path: Union[str, Path]) -> Path:
+    def save_queue_snapshot(self, path: Union[str, Path], in_flight: bool = False) -> Path:
         """Write every message pending on the device to one .npz file (no pickle) that load_queue_snapshot puts back
         into a fresh instance: the agent and group tables in index order, the id nonce, the sequence counter and the
         pending records as PEEK compact receives in stream order (rows renumbered by smallest seq).  Nothing is
         consumed.  An agent with more pending records than one receive call holds raises: a snapshot is complete or it
         is not written.  Leased messages not yet acked are in flight, not pending, and are not in the snapshot: call
-        redeliver_expired(all=True) first to include them."""
+        redeliver_expired(all=True) first to include them.
+
+        in_flight=True (needs GpuConfig.lease_records) writes format 2 instead: the same, plus every live lease and dead
+        letter with its deadline and delivery count, and the delivery counts of redelivered messages still pending, so a
+        restart keeps at-least-once delivery: leases not yet acked can still be acked or are redelivered when due, dead
+        letters stay parked, and counts continue.  Nothing on the device changes."""
         self.flush()
         g = self.gpu_config
-        if g.lease_records:
+        if in_flight and not g.lease_records:
+            raise ValueError("save_queue_snapshot(in_flight=True) needs a lease store (GpuConfig.lease_records)")
+        if g.lease_records and not in_flight:
             live = self.shard.lease_stats()["live"]
             if live:
                 logger.warning(f"queue snapshot leaves out {live} leased messages in flight "
@@ -1192,9 +1200,10 @@ class SwarmsDB:
         members = [[self._agent_idx[a] for a in (self._group_snapshot[k] or [])] for k in range(len(self._group_name))]
         moff = np.zeros(len(members) + 1, np.uint64)
         moff[1:] = np.cumsum([len(m) for m in members]) if members else []
+        extra = self._in_flight_arrays() if in_flight else {}
         path = Path(path)
         with open(path, "wb") as f:
-            np.savez(f, version=np.uint32(self.SNAPSHOT_VERSION),
+            np.savez(f, version=np.uint32(self.SNAPSHOT_VERSION_IN_FLIGHT if in_flight else self.SNAPSHOT_VERSION), **extra,
                      shard=np.array([g.shard_id, max(1, g.num_shards)], np.uint32),
                      id_nonce=np.uint64(self._id_hi >> 64), next_seq=np.uint64(self._next_seq),
                      agent_names=np.array(self._agent_name, dtype=np.str_),
@@ -1209,13 +1218,95 @@ class SwarmsDB:
                      payload=np.concatenate([p[4] for p in parts]) if parts else np.zeros(0, np.uint8))
         return path
 
+    def _in_flight_arrays(self) -> Dict[str, np.ndarray]:
+        """The lease section (export chunks concatenated, rows and payload rebased per chunk as the pending chunks are)
+        and the ledger section of a format-2 snapshot."""
+        parts: List[Tuple[np.ndarray, ...]] = []
+        start = 0
+        while True:
+            ent, snd, pay, meta, start = self.shard.lease_export(start)
+            if len(ent) == 0:
+                break
+            parts.append((ent.copy(), snd.copy(), pay.copy(), meta.copy()))
+        off = np.zeros((len(parts) + 1, 3), np.uint64)          # chunk k: entries, rows, payload bytes
+        for k, (e, s, p, _) in enumerate(parts):
+            off[k + 1] = off[k] + [len(e), len(s), len(p)]
+        ent_all = np.concatenate([p[0] for p in parts]) if parts else np.zeros(0, _native.ENTRY_DTYPE)
+        snd_all = np.concatenate([p[1] for p in parts]) if parts else np.zeros(0, _native.SEND_DTYPE)
+        if parts:
+            ent_all["send"] += np.repeat(off[:-1, 1], [len(p[0]) for p in parts]).astype(np.uint32)
+            snd_all["payload_off"] += np.repeat(off[:-1, 2], [len(p[1]) for p in parts])
+        M = self.gpu_config.lease_max_deliveries
+        if M:
+            la, ls, lc = self.shard.ledger_export()
+        else:
+            la, ls, lc = np.zeros(0, np.uint32), np.zeros(0, np.uint64), np.zeros(0, np.uint32)
+        return dict(lease_entries=ent_all, lease_sends=snd_all,
+                    lease_payload=np.concatenate([p[2] for p in parts]) if parts else np.zeros(0, np.uint8),
+                    lease_meta=np.concatenate([p[3] for p in parts]) if parts else np.zeros(0, _native.META_DTYPE),
+                    lease_chunk_off=off, ledger_agent=la, ledger_seq=ls, ledger_count=lc,
+                    ledger_max_deliveries=np.uint32(M))
+
     @staticmethod
     def _read_snapshot(path: Union[str, Path]) -> Dict[str, np.ndarray]:
         with np.load(Path(path), allow_pickle=False) as z:
             snap = {k: z[k] for k in z.files}
-        if int(snap["version"]) != SwarmsDB.SNAPSHOT_VERSION:
-            raise ValueError(f"{path}: queue snapshot format {int(snap['version'])}, expected {SwarmsDB.SNAPSHOT_VERSION}")
+        known = (SwarmsDB.SNAPSHOT_VERSION, SwarmsDB.SNAPSHOT_VERSION_IN_FLIGHT)
+        if int(snap["version"]) not in known:
+            raise ValueError(f"{path}: queue snapshot format {int(snap['version'])}, expected one of {known}")
         return snap
+
+    def _lease_parts(self, snap: Dict[str, np.ndarray]) -> List[Tuple[np.ndarray, ...]]:
+        """The lease section as import calls: each chunk split where this instance's receive capacity is smaller, each
+        part with only the rows it names and their payloads packed (entries, sends, payload, meta)."""
+        cap = recv_capacity(self.gpu_config)
+        off = snap["lease_chunk_off"].astype(np.int64)
+        ent, snd, pay, meta = snap["lease_entries"], snap["lease_sends"], snap["lease_payload"], snap["lease_meta"]
+        out = []
+        for k in range(len(off) - 1):
+            for i in range(int(off[k, 0]), int(off[k + 1, 0]), cap):
+                j = min(i + cap, int(off[k + 1, 0]))
+                out.append(_compact_rows(ent[i:j], snd, pay) + (meta[i:j],))
+        return out
+
+    def _check_in_flight_fits(self, snap: Dict[str, np.ndarray], parts) -> None:
+        """Refuse a format-2 snapshot this fresh instance cannot hold, before anything of it is adopted."""
+        g = self.gpu_config
+        if not g.lease_records:
+            raise RuntimeError("snapshot holds in-flight leases: loading it needs a lease store (GpuConfig.lease_records)")
+        meta = snap["lease_meta"]
+        dead = int(np.count_nonzero(meta["state"] == _native.LEASE_STATE_DEAD))
+        counted = len(snap["ledger_agent"]) or int(np.count_nonzero(meta["deliveries"] > 1))
+        if (dead or counted) and not g.lease_max_deliveries:
+            raise RuntimeError(f"snapshot holds {dead} dead letters and delivery counts: loading it needs "
+                               f"GpuConfig.lease_max_deliveries")
+        ls = self.shard.lease_stats()
+        entries, rows = sum(len(p[0]) for p in parts), sum(len(p[1]) for p in parts)
+        pbytes = sum(pad32(len(p[2])) for p in parts)
+        if max(entries, rows) > ls["entries_reserved"] - ls["entries_used"] or pbytes > ls["payload_reserved"] - ls["payload_used"]:
+            raise RuntimeError(f"snapshot holds {entries} leases ({pbytes} payload bytes), more than the lease store's free "
+                               f"room (GpuConfig.lease_records={g.lease_records})")
+        if g.lease_max_deliveries:
+            room = self.shard.lease_policy_stats()["ledger_cap"]
+            if len(snap["ledger_agent"]) > room:
+                raise RuntimeError(f"snapshot holds {len(snap['ledger_agent'])} delivery counts, more than the ledger holds "
+                                   f"({room})")
+
+    def _load_in_flight(self, snap: Dict[str, np.ndarray], parts) -> None:
+        """The ledger (it looks records up in the rings, so after the restore), then the leases; rebuilds the host's
+        lease map and deadline heap so acks, nacks, renewals, sweeps and dead letters work on leases from before."""
+        if len(snap["ledger_agent"]):
+            self.shard.ledger_import(snap["ledger_agent"], snap["ledger_seq"], snap["ledger_count"])
+        deadlines = set()
+        for ent, snd, pay, meta in parts:
+            base = self.shard.lease_import(ent, snd, pay, meta)
+            for k, (seq, a, st, d) in enumerate(zip(ent["seq"].tolist(), meta["agent"].tolist(), meta["state"].tolist(),
+                                                    meta["deadline"].tolist())):
+                self._leases.setdefault(self._make_id(seq), []).append((a, base + k))
+                if st == _native.LEASE_STATE_LIVE:
+                    deadlines.add(d)
+        for d in deadlines:
+            heapq.heappush(self._lease_deadlines, d)
 
     def _check_fresh(self) -> None:
         st = self.shard.stats()
@@ -1289,13 +1380,23 @@ class SwarmsDB:
         equal it) and every pending record is restored with its id, to be delivered as if it had never left.  A snapshot
         this instance cannot hold is refused before anything of it is adopted, and the instance stays fresh: an agent
         with more records than one receive call holds raises RuntimeError (checked first), one with more records than
-        its ring holds raises SdbError (code -4)."""
+        its ring holds raises SdbError (code -4).  A format-2 snapshot (save_queue_snapshot(in_flight=True)) also puts the
+        delivery counts, the leases and the dead letters back, in that order after the pending records; it is refused
+        (RuntimeError) by an instance without a lease store, with too little free store or ledger room, or without
+        GpuConfig.lease_max_deliveries when it holds dead letters or counts.  Leases keep their deadlines, so one that
+        passed during the restart is due at the next sweep; the messages keep their ids."""
         self._check_fresh()
         snap = self._read_snapshot(path)
         self._check_snapshot_fits(snap)
+        in_flight = int(snap["version"]) == self.SNAPSHOT_VERSION_IN_FLIGHT
+        parts = self._lease_parts(snap) if in_flight else []
+        if in_flight:
+            self._check_in_flight_fits(snap, parts)
         self._adopt_tables(snap)
         seq_end = self._restore_chunks(snap)
         self._next_seq = max(self._next_seq, seq_end); self._b_first_seq = self._next_seq
+        if in_flight:
+            self._load_in_flight(snap, parts)
 
     # ------------------------------------------------------------------ LLM backends (M:1281-1325 + real balancer)
     def set_llm_load_balancing(self, enabled: bool = True) -> None:

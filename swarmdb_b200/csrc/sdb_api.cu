@@ -94,6 +94,17 @@ cudaError_t sdb_launch_lease_dl_select(const sdb_lease_buf*, const sdb_lease_scr
                                        uint32_t, cudaStream_t, sdb_profiler*, int*);
 cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_dl_scratch*, uint32_t, uint32_t, uint32_t,
                                      uint32_t, uint32_t, const sdb_compact_args*, uint32_t**, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_x_select(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, unsigned long long, cudaStream_t,
+                                      sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_x_emit(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t, const sdb_compact_args*,
+                                    sdb_lease_meta*, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_import_check(const sdb_lease_scratch*, const sdb_compact_args*, const sdb_lease_meta*, uint32_t, uint32_t,
+                                          unsigned long long, uint32_t, uint32_t, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_import_write(const sdb_lease_buf*, const sdb_compact_args*, const sdb_lease_meta*, const unsigned long long*,
+                                          uint32_t, uint64_t, uint32_t, uint32_t, unsigned long long, unsigned long long, cudaStream_t,
+                                          sdb_profiler*, int*, int);
+cudaError_t sdb_launch_ledger_import(const sdb_dev_view*, const sdb_ledger*, uint32_t, uint32_t, unsigned long long*, cudaStream_t,
+                                     sdb_profiler*, int*, int);
 const void* sdb_lease_kernel_anchor();
 cudaError_t sdb_launch_reloc_plan(const sdb_dev_view*, const sdb_reloc_args*, cudaStream_t, sdb_profiler*, int*, int);
 cudaError_t sdb_launch_reloc_write(const sdb_dev_view*, const sdb_reloc_args*, const sdb_ledger*, uint32_t, cudaStream_t, sdb_profiler*,
@@ -2631,6 +2642,179 @@ int sdb_lease_policy_stats(sdb_handle h, sdb_lease_policy_summary* out) {
   const sdb_ctx::LeaseStore& L = h->lease;
   out->max_deliveries = L.max_deliveries; out->dead = L.dead; out->dead_total = L.dead_total;
   out->ledger_used = L.led_live; out->ledger_cap = L.led_cap; out->held_by_ledger_total = L.held_total;
+  return SDB_OK;
+}
+
+// ---- snapshots of the lease store and the ledger -----------------------------------------------------------------
+int sdb_lease_export(sdb_handle h, uint64_t start_id, uint32_t flags, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                     sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                     sdb_lease_meta* meta_out, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out,
+                     uint64_t* next_id_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (next_id_out) *next_id_out = 0;
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (flags) return fail(h, SDB_EINVAL, "sdb_lease_export: flags must be 0");
+  if (!L.cap) return fail(h, SDB_EINVAL, "sdb_lease_export: no lease store (sdb_lease_reserve)");
+  uint64_t rec_cap = 0;
+  { const int rc = out_rec_cap(h, std::min({room(entry_out, entry_cap), room(meta_out, entry_cap), room(send_out, send_cap)}),
+                               room(payload_out, payload_cap), &rec_cap);
+    if (rc != SDB_OK) return rc; }
+  if (next_id_out) *next_id_out = start_id;
+  if (L.used == 0) return SDB_OK;
+  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  const sdb_lease_buf& b = L.buf[L.cur];
+  const uint32_t used = static_cast<uint32_t>(L.used), rows = static_cast<uint32_t>(L.rows);
+  int nl = 0;
+  cudaError_t e = sdb_launch_lease_x_select(&b, &L.s, used, start_id, h->stream, &h->prof, &nl);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease export launch: ") + cudaGetErrorString(e));
+  { const int rc = lease_totals(h, 0, 1); if (rc != SDB_OK) return rc; }
+  h->stream_busy = false;
+  const uint64_t m = std::min<uint64_t>(L.th[0], rec_cap);
+  if (m == 0) return SDB_OK;
+  sdb_lease_meta* meta_dev = reinterpret_cast<sdb_lease_meta*>(h->rx_hdr);     // [max_recv_records] x 32 bytes
+  nl = 0;
+  e = sdb_launch_lease_x_emit(&b, &L.s, used, rows, static_cast<uint32_t>(m), &h->cx, meta_dev, h->stream, &h->prof, &nl, h->sm_count);
+  h->launches += nl;
+  h->last_rx_valid = false; h->last_rx_compact = true;            // the receive's buffers were reused
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease export launch: ") + cudaGetErrorString(e));
+  { const int rc = lease_totals(h, 6, 3); if (rc != SDB_OK) return rc; }
+  const uint64_t n_sends = L.th[6], pbytes = L.th[7] * SDB_GRANULE, next = L.th[8];
+  if (entry_out) CUDA_TRY(h, cudaMemcpyAsync(entry_out, h->cx.entry_out, m * sizeof(sdb_recv_entry), cudaMemcpyDeviceToHost, h->stream));
+  if (send_out) CUDA_TRY(h, cudaMemcpyAsync(send_out, h->cx.send_out, n_sends * sizeof(sdb_recv_send), cudaMemcpyDeviceToHost, h->stream));
+  if (payload_out && pbytes) CUDA_TRY(h, cudaMemcpyAsync(payload_out, h->cx.payload_out, pbytes, cudaMemcpyDeviceToHost, h->stream));
+  if (meta_out) CUDA_TRY(h, cudaMemcpyAsync(meta_out, meta_dev, m * sizeof(sdb_lease_meta), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  if (total_out) *total_out = m;
+  if (n_sends_out) *n_sends_out = n_sends;
+  if (payload_bytes_out) *payload_bytes_out = pbytes;
+  if (next_id_out) *next_id_out = next;
+  return SDB_OK;
+}
+
+int sdb_lease_import(sdb_handle h, uint64_t n, const sdb_recv_entry* entries, const sdb_recv_send* sends, uint64_t n_sends,
+                     const uint8_t* payload, uint64_t payload_bytes, const sdb_lease_meta* meta, uint32_t flags,
+                     uint64_t* lease_base_out) {
+  if (!h) return SDB_EINVAL;
+  if (lease_base_out) *lease_base_out = 0;
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (flags) return fail(h, SDB_EINVAL, "sdb_lease_import: flags must be 0");
+  if (!L.cap) return fail(h, SDB_EINVAL, "sdb_lease_import: no lease store (sdb_lease_reserve)");
+  if ((n && (!entries || !meta)) || (n_sends && !sends) || (payload_bytes && !payload))
+    return fail(h, SDB_EINVAL, "sdb_lease_import: null input array");
+  const uint64_t rec_cap = recv_rec_cap(h);                  // the input is staged in one compact receive's buffers
+  if (n > rec_cap || n_sends > rec_cap || payload_bytes > rec_cap * pad32(h->cfg.max_payload_bytes))
+    return fail(h, SDB_ECAPACITY, "sdb_lease_import: input larger than one compact receive's capacity");
+  const uint64_t grans = (payload_bytes + SDB_GRANULE - 1) / SDB_GRANULE;
+  if (L.used + n > L.cap || L.rows + n_sends > L.cap || L.pay + grans * SDB_GRANULE > L.pay_cap)
+    return fail(h, SDB_ECAPACITY, "lease store full: settle or sweep");
+  if (n == 0) {
+    if (lease_base_out) *lease_base_out = L.next_id;
+    return SDB_OK;
+  }
+  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  sdb_compact_args& c = h->cx;
+  sdb_lease_meta* meta_dev = reinterpret_cast<sdb_lease_meta*>(h->rx_hdr);
+  h->last_rx_valid = false; h->last_rx_compact = true;            // the receive's buffers are reused
+  CUDA_TRY(h, cudaMemcpyAsync(c.entry_out, entries, n * sizeof(sdb_recv_entry), cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(meta_dev, meta, n * sizeof(sdb_lease_meta), cudaMemcpyHostToDevice, h->stream));
+  if (n_sends) CUDA_TRY(h, cudaMemcpyAsync(c.send_out, sends, n_sends * sizeof(sdb_recv_send), cudaMemcpyHostToDevice, h->stream));
+  if (payload_bytes) CUDA_TRY(h, cudaMemcpyAsync(c.payload_out, payload, payload_bytes, cudaMemcpyHostToDevice, h->stream));
+  int nl = 0;
+  cudaError_t e = sdb_launch_lease_import_check(&L.s, &c, meta_dev, static_cast<uint32_t>(n), static_cast<uint32_t>(n_sends),
+                                                payload_bytes, h->cfg.max_agents, h->cfg.max_payload_bytes, L.policy ? 1u : 0u,
+                                                h->stream, &h->prof, &nl, h->sm_count);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease import launch: ") + cudaGetErrorString(e));
+  { const int rc = lease_totals(h, 0, 1); if (rc != SDB_OK) return rc; }
+  h->stream_busy = false;
+  if (L.th[0])
+    return fail(h, SDB_EINVAL, "sdb_lease_import: bad entry (send index, agent, receiver, state) or row (len, prio, payload_off)");
+  const unsigned long long tot[3] = {n, n_sends, grans};          // the copy kernel reads its counts on the device
+  CUDA_TRY(h, cudaMemcpyAsync(h->rx_totals, tot, sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(c.totals, tot + 1, 2 * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+  nl = 0;
+  e = sdb_launch_lease_import_write(&L.buf[L.cur], &c, meta_dev, h->rx_totals, static_cast<uint32_t>(n),
+                                    std::max({n, n_sends, 2 * grans}), static_cast<uint32_t>(L.used), static_cast<uint32_t>(L.rows),
+                                    L.pay, L.next_id, h->stream, &h->prof, &nl, h->sm_count);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("lease import launch: ") + cudaGetErrorString(e));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  uint64_t dead = 0;
+  for (uint64_t i = 0; i < n; ++i) dead += meta[i].state == SDB_LEASE_STATE_DEAD ? 1 : 0;
+  if (lease_base_out) *lease_base_out = L.next_id;
+  L.used += n; L.rows += n_sends; L.pay += grans * SDB_GRANULE; L.next_id += n;
+  L.live += n - dead; L.dead += dead;
+  return SDB_OK;
+}
+
+// a collection of the ledger, synchronised: afterwards led_n = led_live = entries whose record is still pending
+static int ledger_collect_sync(sdb_ctx* h) {
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (!L.led_n) return SDB_OK;
+  cudaError_t e = ledger_collect(h);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(L.lth, L.led.tot, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream);
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("ledger collection launch: ") + cudaGetErrorString(e));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  L.led_n = L.led_live = L.lth[0];
+  return SDB_OK;
+}
+
+int sdb_lease_ledger_export(sdb_handle h, uint64_t cap, uint32_t* agent_out, uint64_t* seq_out, uint32_t* count_out,
+                            uint64_t* n_out) {
+  if (!h) return SDB_EINVAL;
+  if (n_out) *n_out = 0;
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (!L.policy) return fail(h, SDB_EINVAL, "sdb_lease_ledger_export: no redelivery policy (sdb_lease_set_policy)");
+  { const int rc = ledger_collect_sync(h); if (rc != SDB_OK) return rc; }
+  const uint64_t n = L.led_n;
+  if (n_out) *n_out = n;
+  if (n > cap) return fail(h, SDB_EOUTPUT, "sdb_lease_ledger_export: cap below the ledger's entries (*n_out)");
+  if (n && (!agent_out || !seq_out || !count_out)) {
+    if (n_out) *n_out = 0;
+    return fail(h, SDB_EINVAL, "sdb_lease_ledger_export: null output array");
+  }
+  std::vector<sdb_ledger_ent> ent(n);
+  if (n) {
+    CUDA_TRY(h, cudaMemcpyAsync(ent.data(), L.led.ent, n * sizeof(sdb_ledger_ent), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  for (uint64_t i = 0; i < n; ++i) { agent_out[i] = ent[i].agent; seq_out[i] = ent[i].seq; count_out[i] = ent[i].count; }
+  return SDB_OK;
+}
+
+int sdb_lease_ledger_import(sdb_handle h, uint64_t n, const uint32_t* agent, const uint64_t* seq, const uint32_t* count,
+                            uint64_t* matched_out) {
+  if (!h) return SDB_EINVAL;
+  if (matched_out) *matched_out = 0;
+  sdb_ctx::LeaseStore& L = h->lease;
+  if (!L.policy) return fail(h, SDB_EINVAL, "sdb_lease_ledger_import: no redelivery policy (sdb_lease_set_policy)");
+  if (n && (!agent || !seq || !count)) return fail(h, SDB_EINVAL, "sdb_lease_ledger_import: null input array");
+  for (uint64_t i = 0; i < n; ++i) {
+    if (agent[i] >= h->cfg.max_agents) return fail(h, SDB_EINVAL, "sdb_lease_ledger_import: agent index out of range");
+    if (!count[i]) return fail(h, SDB_EINVAL, "sdb_lease_ledger_import: a count of 0");
+  }
+  { const int rc = ledger_collect_sync(h); if (rc != SDB_OK) return rc; }
+  if (n > L.led_cap - L.led_n) return fail(h, SDB_ECAPACITY, "sdb_lease_ledger_import: more triples than the ledger's free room");
+  if (!n) return SDB_OK;
+  std::vector<sdb_ledger_ent> t(n);                         // staged in the ledger's spare buffer (a collection rewrites it)
+  for (uint64_t i = 0; i < n; ++i) t[i] = sdb_ledger_ent{seq[i], agent[i], count[i], 0u, 0u};
+  CUDA_TRY(h, cudaMemcpyAsync(L.led.alt, t.data(), n * sizeof(sdb_ledger_ent), cudaMemcpyHostToDevice, h->stream));
+  int nl = 0;
+  cudaError_t e = sdb_launch_ledger_import(&h->view, &L.led, static_cast<uint32_t>(n), static_cast<uint32_t>(L.led_n), L.s.tot,
+                                           h->stream, &h->prof, &nl, h->sm_count);
+  h->launches += nl;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("ledger import launch: ") + cudaGetErrorString(e));
+  { const int rc = lease_totals(h, 0, 1); if (rc != SDB_OK) return rc; }
+  h->stream_busy = false;
+  const uint64_t matched = L.th[0];
+  L.led_n += matched; L.led_live += matched;
+  if (matched_out) *matched_out = matched;
   return SDB_OK;
 }
 

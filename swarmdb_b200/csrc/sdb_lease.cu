@@ -23,6 +23,11 @@
 //   (the host then runs restore's plan and write phases on the staged input)
 //   compact  k_lease_mark (staged -> redelivered), k_lease_keep + scans, k_lease_keep_rows + scans, k_lease_copy_entries,
 //            k_lease_copy_rows into the other buffer
+// Snapshots (read out without changing anything, put back behind the tail)
+//   export   k_lease_x_flag + scan (held entries with id >= start), k_lease_x_list, the stage's row kernels over store
+//            order, k_lease_x_emit (entries + sdb_lease_meta)
+//   import   k_lease_import_check (the host synchronises on its verdict), k_lease_import_meta + k_lease_append_copy
+//   ledger   k_ledger_import: one warp per (agent, seq, count) triple finds its record in the agent's ring window
 #include "sdb_common.cuh"
 
 #define SDB_SCAN_TILE 4096u
@@ -731,6 +736,199 @@ extern "C" cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf* b, const sd
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
   return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// ---- snapshots: sdb_lease_export / sdb_lease_import / sdb_lease_ledger_import --------------------------------------
+static_assert(sizeof(sdb_lease_meta) == 32, "lease meta records are 32 bytes");
+// held entries (live or dead) with id >= start_id
+__global__ void __launch_bounds__(256)
+k_lease_x_flag(sdb_lease_buf b, uint32_t used, unsigned long long start_id, uint32_t* __restrict__ flag) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= used) return;
+  const uint32_t st = b.state[e];
+  flag[e] = (st == SDB_LS_LIVE || st == SDB_LS_DEAD) && b.id[e] >= start_id ? 1u : 0u;
+}
+// the first m flagged entries in store (= lease-id) order: staged[p] = store entry, val_a[p] = p (the row kernels' order)
+__global__ void __launch_bounds__(256)
+k_lease_x_list(sdb_lease_scratch s, uint32_t used, uint32_t m) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= used || !s.flag[e]) return;
+  const uint32_t p = ls_scan(s.f_local, s.f_tops, e);
+  if (p < m) { s.staged[p] = e; s.val_a[p] = p; }
+}
+// position p: its entry (send = output row) and its meta; the last position leaves the id to continue from in tot[8]
+__global__ void __launch_bounds__(256)
+k_lease_x_emit(sdb_lease_buf b, sdb_lease_scratch s, uint32_t m, sdb_recv_entry* __restrict__ entry_out,
+               sdb_lease_meta* __restrict__ meta_out) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= m) return;
+  const uint32_t e = s.staged[p];
+  sdb_recv_entry en = b.ent[e];
+  en.send = s.rmap[en.send];
+  entry_out[p] = en;
+  sdb_lease_meta x;
+  x.id = b.id[e]; x.deadline = b.deadline[e]; x.agent = b.agent[e]; x.deliveries = b.deliveries ? b.deliveries[e] : 0u;
+  x.state = b.state[e]; x.reserved = 0u;
+  meta_out[p] = x;
+  if (p == m - 1u) s.tot[8] = x.id + 1ull;
+}
+
+// every entry and row of an import before anything is written; a bad one sets tot[0]
+__global__ void __launch_bounds__(256)
+k_lease_import_check(const sdb_recv_entry* __restrict__ ent, const sdb_lease_meta* __restrict__ meta,
+                     const sdb_recv_send* __restrict__ snd, uint32_t n, uint32_t n_sends, unsigned long long payload_bytes,
+                     uint32_t max_agents, uint32_t max_payload, uint32_t policy, unsigned long long* __restrict__ tot) {
+  const uint32_t m = n > n_sends ? n : n_sends;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+    bool bad = false;
+    if (i < n) {
+      const sdb_recv_entry en = ent[i];
+      const sdb_lease_meta x = meta[i];
+      bad = en.send >= n_sends || x.agent >= max_agents || (en.receiver != x.agent && en.receiver != SDB_NO_RECEIVER) ||
+            !(x.state == SDB_LS_LIVE || (x.state == SDB_LS_DEAD && policy));
+    }
+    if (i < n_sends) {
+      const sdb_recv_send r = snd[i];
+      const unsigned long long pad = 32ull * ls_pg(r.len);
+      bad = bad || r.len > max_payload || r.prio > 3u || (r.payload_off & 15ull) || r.payload_off > payload_bytes ||
+            payload_bytes - r.payload_off < pad;
+    }
+    if (bad) atomicOr(tot, 1ull);
+  }
+}
+// the import's agent, id, deadline, state and count of each entry (entries, rows and payload: k_lease_append_copy)
+__global__ void __launch_bounds__(256)
+k_lease_import_meta(sdb_lease_buf b, const sdb_lease_meta* __restrict__ meta, uint32_t n, uint32_t used,
+                    unsigned long long id_base) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const sdb_lease_meta x = meta[i];
+  const uint32_t e = used + i;
+  b.agent[e] = x.agent; b.id[e] = id_base + i; b.deadline[e] = x.deadline; b.state[e] = x.state;
+  if (b.deliveries) b.deliveries[e] = x.deliveries ? x.deliveries : 1u;
+}
+
+// one warp per triple staged in L.alt[0, n): the oldest pending record of the agent (ring window [head, tail),
+// consumed slots skipped) whose header seq matches takes ledger entry n0 + (matches so far); tot counts them
+__global__ void __launch_bounds__(256)
+k_ledger_import(sdb_dev_view v, sdb_ledger L, uint32_t n, uint32_t n0, unsigned long long* __restrict__ tot) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t q = gw; q < n; q += nw) {
+    const sdb_ledger_ent t = L.alt[q];
+    const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + t.agent);   // {head, tail, ..}
+    const uint2* ring = sdb_ring_of(v, t.agent);
+    const uint32_t w = h.y - h.x;
+    for (uint32_t o = 0; o < w; o += 32) {
+      bool hit = false;
+      uint32_t handle = 0;
+      if (o + lane < w) {
+        const uint2 r = ring[(h.x + o + lane) & (v.ring_slots - 1)];
+        handle = r.x;
+        hit = sdb_meta(r) != SDB_META_TOMB &&
+              *reinterpret_cast<const unsigned long long*>(sdb_arena_ptr(v, r.x)) == t.seq;
+      }
+      const uint32_t m = __ballot_sync(0xFFFFFFFFu, hit);
+      if (!m) continue;
+      if (lane == static_cast<uint32_t>(__ffs(m) - 1)) {
+        const uint32_t k = n0 + static_cast<uint32_t>(atomicAdd(tot, 1ull));
+        sdb_ledger_ent en = t;
+        en.p = h.x + o + lane; en.handle = handle;
+        L.ent[k] = en;
+        lg_index(L, k, t.agent, t.seq);
+      }
+      break;
+    }
+  }
+}
+
+// phase 1: the held entries with id >= start_id are flagged and counted (tot[0]; leaves the flag scan)
+extern "C" cudaError_t sdb_launch_lease_x_select(const sdb_lease_buf* b, const sdb_lease_scratch* s, uint32_t used,
+                                                 unsigned long long start_id, cudaStream_t stream, sdb_profiler* prof,
+                                                 int* n_launches) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  cudaMemsetAsync(s->tot, 0, 16 * sizeof(unsigned long long), stream);
+  LS_LAUNCH(used, k_lease_x_flag, *b, used, start_id, s->flag);
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream);
+  nl += used ? 2 : 0;
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// phase 2: the first m of them in the compact format (rows numbered by first appearance: the sweep's row kernels over
+// store order), entries to cx->entry_out, meta to meta_out.  tot[6] = rows, tot[7] = payload granules, tot[8] = next id
+extern "C" cudaError_t sdb_launch_lease_x_emit(const sdb_lease_buf* b, const sdb_lease_scratch* s, uint32_t used, uint32_t rows_used,
+                                               uint32_t m, const sdb_compact_args* cx, sdb_lease_meta* meta_out,
+                                               cudaStream_t stream, sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  LS_LAUNCH(used, k_lease_x_list, *s, used, m);
+  if (rows_used) cudaMemsetAsync(s->rfirst, 0xFF, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
+  LS_LAUNCH(m, k_lease_row_first, *b, *s, s->val_a, m);
+  LS_LAUNCH(m, k_lease_row_heads, *b, *s, s->val_a, m);
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, m, s->tot + 6, nullptr, stream);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, m, s->tot + 7, nullptr, stream);
+  nl += 4;
+  if (m) {
+    k_lease_stage_rows<<<ls_grid(m, 8, sm_count * 4), 256, 0, stream>>>(*b, *s, s->val_a, m, cx->send_out, cx->payload_out);
+    ++nl;
+  }
+  LS_LAUNCH(m, k_lease_x_emit, *b, *s, m, cx->entry_out, meta_out);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return e == cudaSuccess ? cudaGetLastError() : e;
+}
+
+// import, phase 1: the input staged in cx (entries, rows, payload) and meta; error bits to s->tot[0]
+extern "C" cudaError_t sdb_launch_lease_import_check(const sdb_lease_scratch* s, const sdb_compact_args* cx, const sdb_lease_meta* meta,
+                                                     uint32_t n, uint32_t n_sends, unsigned long long payload_bytes,
+                                                     uint32_t max_agents, uint32_t max_payload, uint32_t policy,
+                                                     cudaStream_t stream, sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  cudaMemsetAsync(s->tot, 0, sizeof(unsigned long long), stream);
+  const uint32_t items = n > n_sends ? n : n_sends;
+  if (items) {
+    k_lease_import_check<<<ls_grid(items, 256, sm_count * 4), 256, 0, stream>>>(cx->entry_out, meta, cx->send_out, n, n_sends,
+                                                                               payload_bytes, max_agents, max_payload, policy,
+                                                                               s->tot);
+    if (n_launches) *n_launches += 1;
+  }
+  sdb_prof_end(prof, pi, stream);
+  return cudaGetLastError();
+}
+
+// import, phase 2: behind the store's tail.  totals = {n} and cx->totals = {n_sends, payload granules} on the device
+extern "C" cudaError_t sdb_launch_lease_import_write(const sdb_lease_buf* b, const sdb_compact_args* cx, const sdb_lease_meta* meta,
+                                                     const unsigned long long* totals, uint32_t n, uint64_t items, uint32_t used,
+                                                     uint32_t rows_used, unsigned long long pay_used, unsigned long long id_base,
+                                                     cudaStream_t stream, sdb_profiler* prof, int* n_launches, int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  int nl = 0;
+  LS_LAUNCH(n, k_lease_import_meta, *b, meta, n, used, id_base);
+  if (items) {
+    k_lease_append_copy<<<ls_grid(items, 256, sm_count * 4), 256, 0, stream>>>(*b, cx->entry_out, cx->send_out, cx->payload_out,
+                                                                               totals, cx->totals, used, rows_used, pay_used);
+    ++nl;
+  }
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += nl;
+  return cudaGetLastError();
+}
+
+// n triples staged in L->alt: matches become entries n0.. of L->ent, *tot counts them (zeroed here)
+extern "C" cudaError_t sdb_launch_ledger_import(const sdb_dev_view* v, const sdb_ledger* L, uint32_t n, uint32_t n0,
+                                                unsigned long long* tot, cudaStream_t stream, sdb_profiler* prof, int* n_launches,
+                                                int sm_count) {
+  const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
+  cudaMemsetAsync(tot, 0, sizeof(unsigned long long), stream);
+  if (n) {
+    k_ledger_import<<<ls_grid(n, 8, sm_count * 4), 256, 0, stream>>>(*v, *L, n, n0, tot);
+    if (n_launches) *n_launches += 1;
+  }
+  sdb_prof_end(prof, pi, stream);
+  return cudaGetLastError();
 }
 
 // any kernel of this file: its module is loaded as a whole before the latency server starts (sdb_api.cu)
