@@ -521,6 +521,58 @@ __device__ __forceinline__ void sdb_st_stream_pol(void* p, const uint4& v, uint6
   asm volatile("st.global.L1::no_allocate.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;"
                :: "l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol) : "memory");
 }
+
+// ---- W consecutive 32-byte headers held one per lane, stored as whole sectors -------------------------------------
+// Lane l of a group of W lanes (W = 8 or 32, groups aligned in the warp) holds header l of a run as (lo, hi).  Stored
+// as held, each 16-byte store instruction writes half of W sectors, and the L2 gets every sector as two partial writes
+// from two instructions (scripts/ubench/stores.cu, header stream mode a).  Here the halves change lanes first: in store
+// s (0, 1) lane l writes half (l & 1) of header s * W/2 + l/2, so lanes 2k and 2k + 1 fill one sector in ONE
+// instruction and the group writes W * 16 contiguous bytes per store.  Two shuffle rounds: lanes below W/2 offer lo in
+// the first round and hi in the second, the others the reverse; lane l reads lane l/2 + (l odd ? W/2 : 0) in the first
+// round and that lane ^ W/2 in the second, which gives an even lane the lo halves of headers l/2 and W/2 + l/2 and an
+// odd lane their hi halves.  A header whose lane passes `valid` false is not written (neither half); all W lanes of
+// the group must call this together.
+struct sdb_hdr_sectors { uint4 x0, x1; bool w0, w1; };    // store 0 / 1 of this lane: value, and whether it is written
+// c ? a : b per component (a select of whole uint4 lvalues can make the compiler address them in local memory)
+__device__ __forceinline__ uint4 sdb_sel4(bool c, uint4 a, uint4 b) {
+  return make_uint4(c ? a.x : b.x, c ? a.y : b.y, c ? a.z : b.z, c ? a.w : b.w);
+}
+template <int W>
+__device__ __forceinline__ sdb_hdr_sectors sdb_pair_headers(uint4 lo, uint4 hi, bool valid, uint32_t lane) {
+  static_assert(W == 8 || W == 16 || W == 32, "header groups are 8 to 32 lanes");
+  constexpr uint32_t H = W / 2;
+  const uint32_t l = lane & (W - 1u), seg = lane & ~(W - 1u);
+  const uint32_t mask = W == 32 ? 0xFFFFFFFFu : ((1u << W) - 1u) << seg;
+  const uint32_t vm = __ballot_sync(mask, valid) >> seg;
+  const bool odd = l & 1u, low = l < H;
+  const uint32_t src = (l >> 1) + (odd ? H : 0u);
+  const uint4 p = sdb_sel4(low, lo, hi), q = sdb_sel4(low, hi, lo);
+  uint4 y0, y1;
+  y0.x = __shfl_sync(mask, p.x, src, W); y0.y = __shfl_sync(mask, p.y, src, W);
+  y0.z = __shfl_sync(mask, p.z, src, W); y0.w = __shfl_sync(mask, p.w, src, W);
+  y1.x = __shfl_sync(mask, q.x, src ^ H, W); y1.y = __shfl_sync(mask, q.y, src ^ H, W);
+  y1.z = __shfl_sync(mask, q.z, src ^ H, W); y1.w = __shfl_sync(mask, q.w, src ^ H, W);
+  sdb_hdr_sectors r;
+  r.x0 = sdb_sel4(odd, y1, y0); r.x1 = sdb_sel4(odd, y0, y1);
+  r.w0 = (vm >> (l >> 1)) & 1u; r.w1 = (vm >> (H + (l >> 1))) & 1u;
+  return r;
+}
+// dst: the group's first header (32-byte aligned)
+template <int W>
+__device__ __forceinline__ void sdb_st_headers(void* dst, uint4 lo, uint4 hi, bool valid, uint32_t lane) {
+  const sdb_hdr_sectors s = sdb_pair_headers<W>(lo, hi, valid, lane);
+  uint4* d = reinterpret_cast<uint4*>(dst) + (lane & (W - 1u));
+  if (s.w0) sdb_st_stream(d, s.x0);
+  if (s.w1) sdb_st_stream(d + W, s.x1);
+}
+template <int W>
+__device__ __forceinline__ void sdb_st_headers_pol(void* dst, uint4 lo, uint4 hi, bool valid, uint32_t lane, uint64_t pol) {
+  const sdb_hdr_sectors s = sdb_pair_headers<W>(lo, hi, valid, lane);
+  uint4* d = reinterpret_cast<uint4*>(dst) + (lane & (W - 1u));
+  if (s.w0) sdb_st_stream_pol(d, s.x0, pol);
+  if (s.w1) sdb_st_stream_pol(d + W, s.x1, pol);
+}
+
 __device__ __forceinline__ void sdb_st_u32_pol(uint32_t* p, uint32_t v, uint64_t pol) {
   asm volatile("st.global.L2::cache_hint.u32 [%0], %1, %2;" :: "l"(p), "r"(v), "l"(pol) : "memory");
 }

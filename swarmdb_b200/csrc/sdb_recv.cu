@@ -743,12 +743,14 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
   __syncwarp();
   const uint32_t gw = blockIdx.x * WARPS + warp, nw = gridDim.x * WARPS;
   uint32_t phase = 0;                                        // bit s = parity of stage s
-  // per-lane state of the two stages.  The 32-byte header travels through registers (two 16-byte loads now, two stores
-  // one step later: the lanes' headers are consecutive in hdr_out, so a warp stores 1 KB contiguous); the payload - right
+  // per-lane state of the two stages.  The 32-byte header travels through registers (two 16-byte loads now, stored one
+  // step later: the lanes' headers are consecutive in hdr_out, and sdb_st_headers swaps halves between lanes so that
+  // each of the warp's two store instructions writes 512 contiguous bytes of whole sectors; stored as loaded, every
+  // sector would reach the L2 as two partial writes, at about half the write bandwidth); the payload - right
   // behind the header, or shared by all recipients of a group send (sdb_common.cuh) - takes ONE bulk load and ONE
   // bulk store.  Two bulk operations per record instead of three: the copy engine, not DRAM, was the limit once the
   // payloads came out of the L2.
-  uint32_t g0 = 0, g1 = 0, rc0 = 0, rc1 = 0; uint64_t po0 = 0, po1 = 0; bool hv0 = false, hv1 = false;
+  uint32_t g0 = 0, g1 = 0; uint64_t po0 = 0, po1 = 0; bool hv0 = false, hv1 = false;
   uint4 ha0 = make_uint4(0, 0, 0, 0), hb0 = ha0, ha1 = ha0, hb1 = ha0;
   uint4 pe_ahead = make_uint4(0, 0, 0, 0);                   // plan entry of the step after the one being requested
   auto issue = [&](uint32_t st, uint32_t r0) {               // all lanes: request step r0 into stage st
@@ -768,8 +770,8 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
       if (bytes) sdb_tma_load(wbase + (static_cast<size_t>(st) * 32u + lane) * slot_bytes, sdb_payload_of(v, pe.x, sdb_entry_dm1(pe.z)), bytes, &s_bar[warp][st]);
     }
     const uint64_t po = static_cast<uint64_t>(pe.y) + ((have && r.plan_tops) ? r.plan_tops[rec / SDB_SCAN_TILE] : 0u);
-    if (st) { g1 = pe.z & 0xFFFFu; rc1 = rec; hv1 = have; po1 = po; ha1 = ha; hb1 = hb; }
-    else { g0 = pe.z & 0xFFFFu; rc0 = rec; hv0 = have; po0 = po; ha0 = ha; hb0 = hb; }
+    if (st) { g1 = pe.z & 0xFFFFu; hv1 = have; po1 = po; ha1 = ha; hb1 = hb; }
+    else { g0 = pe.z & 0xFFFFu; hv0 = have; po0 = po; ha0 = ha; hb0 = hb; }
   };
   uint32_t r0 = gw * 32u;
   if (r0 + lane < total) pe_ahead = __ldg(r.plan + r0 + lane);
@@ -781,10 +783,7 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
     sdb_tma_wait_read<0>();
     __syncwarp();
     if (rn < total) issue(st ^ 1u, rn);
-    if (st ? hv1 : hv0) {
-      uint4* hdst = reinterpret_cast<uint4*>(r.hdr_out + (st ? rc1 : rc0));
-      sdb_st_stream(hdst, st ? ha1 : ha0); sdb_st_stream(hdst + 1, st ? hb1 : hb0);
-    }
+    sdb_st_headers<32>(r.hdr_out + r0, sdb_sel4(st, ha1, ha0), sdb_sel4(st, hb1, hb0), st ? hv1 : hv0, lane);   // whole sectors
     sdb_mbar_wait_bounded(&s_bar[warp][st], (phase >> st) & 1u);
     phase ^= 1u << st;
     {
@@ -821,7 +820,7 @@ k_recv_gather_cpa(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
   const uint32_t wbase_sa = sdb_smem_u32(wbase);
   const uint32_t gw = blockIdx.x * WARPS + warp, nw = gridDim.x * WARPS;
   const uint32_t cpr = slot_bytes >> 4;                      // 16-byte chunks per slot
-  uint32_t g0 = 0, g1 = 0, rc0 = 0, rc1 = 0; uint64_t po0 = 0, po1 = 0; bool hv0 = false, hv1 = false;
+  uint32_t g0 = 0, g1 = 0; uint64_t po0 = 0, po1 = 0; bool hv0 = false, hv1 = false;
   uint4 ha0 = make_uint4(0, 0, 0, 0), hb0 = ha0, ha1 = ha0, hb1 = ha0;
   auto issue = [&](uint32_t st, uint32_t r0) {               // all lanes: request step r0 into stage st
     const uint32_t rec = r0 + lane;
@@ -845,8 +844,8 @@ k_recv_gather_cpa(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
         asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(stage_sa + k * slot_bytes + (c << 4)), "l"(sk + (c << 4)) : "memory");
     }
     const uint64_t po = static_cast<uint64_t>(pe.y) + ((have && r.plan_tops) ? r.plan_tops[rec / SDB_SCAN_TILE] : 0u);
-    if (st) { g1 = pe.z & 0xFFFFu; rc1 = rec; hv1 = have; po1 = po; ha1 = ha; hb1 = hb; }
-    else { g0 = pe.z & 0xFFFFu; rc0 = rec; hv0 = have; po0 = po; ha0 = ha; hb0 = hb; }
+    if (st) { g1 = pe.z & 0xFFFFu; hv1 = have; po1 = po; ha1 = ha; hb1 = hb; }
+    else { g0 = pe.z & 0xFFFFu; hv0 = have; po0 = po; ha0 = ha; hb0 = hb; }
   };
   uint32_t r0 = gw * 32u;
   if (r0 < total) issue(0, r0);
@@ -859,10 +858,7 @@ k_recv_gather_cpa(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
     if (rn < total) issue(st ^ 1u, rn);
     asm volatile("cp.async.commit_group;" ::: "memory");     // one group per step, empty or not: the wait below counts groups
     const bool hv = st ? hv1 : hv0;
-    if (hv) {
-      uint4* hdst = reinterpret_cast<uint4*>(r.hdr_out + (st ? rc1 : rc0));
-      sdb_st_stream(hdst, st ? ha1 : ha0); sdb_st_stream(hdst + 1, st ? hb1 : hb0);
-    }
+    sdb_st_headers<32>(r.hdr_out + r0, sdb_sel4(st, ha1, ha0), sdb_sel4(st, hb1, hb0), hv, lane);
     asm volatile("cp.async.wait_group 1;" ::: "memory");     // everything but the newest group: this stage has landed
     __syncwarp();
     sdb_fence_proxy_async();                                 // copies written through the generic proxy -> visible to the bulk store

@@ -693,18 +693,15 @@ k_group_fanout_shared(sdb_dev_view v, const sdb_send_desc* __restrict__ descs, u
         }
         const bool s0 = j0 < mcount && skip_sender && a0 == sender, s1 = j1 < mcount && skip_sender && a1 == sender;
         n_skip += s0 + s1;
-        if (j0 < mcount && !s0 && a0 < v.max_agents) {
-          uint4 hi = hdr_hi; if (!shared_seq) hi.y = a0;
-          uint4* dst = reinterpret_cast<uint4*>(base + (static_cast<size_t>(j0) << 5));
-          sdb_st_stream_pol(dst, sdb_header_lo(seq0 + (shared_seq ? 0u : p0), ts), pol);
-          sdb_st_stream_pol(dst + 1, hi, pol);
-        }
-        if (j1 < mcount && !s1 && a1 < v.max_agents) {
-          uint4 hi = hdr_hi; if (!shared_seq) hi.y = a1;
-          uint4* dst = reinterpret_cast<uint4*>(base + (static_cast<size_t>(j1) << 5));
-          sdb_st_stream_pol(dst, sdb_header_lo(seq0 + (shared_seq ? 0u : p1), ts), pol);
-          sdb_st_stream_pol(dst + 1, hi, pol);
-        }
+        // headers tile..tile+LPS-1 (one per lane), then the next LPS: each run stored as whole sectors (sdb_st_headers),
+        // skipped senders and out-of-range agents left unwritten
+        uint4 hi0 = hdr_hi, hi1 = hdr_hi;
+        if (!shared_seq) { hi0.y = a0; hi1.y = a1; }
+        uint8_t* const dst = base + (static_cast<size_t>(tile) << 5);
+        sdb_st_headers_pol<LPS>(dst, sdb_header_lo(seq0 + (shared_seq ? 0u : p0), ts), hi0,
+                                j0 < mcount && !s0 && a0 < v.max_agents, lane, pol);
+        sdb_st_headers_pol<LPS>(dst + LPS * 32, sdb_header_lo(seq0 + (shared_seq ? 0u : p1), ts), hi1,
+                                j1 < mcount && !s1 && a1 < v.max_agents, lane, pol);
       }
       // the one payload of the send, behind its mcount headers
       uint8_t* const pdst = base + (static_cast<size_t>(mcount) << 5);
