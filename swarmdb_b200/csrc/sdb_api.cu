@@ -16,104 +16,6 @@
 
 #include "sdb_common.cuh"
 
-extern "C" {
-cudaError_t sdb_launch_p2p(const sdb_dev_view*, const sdb_send_desc*, uint32_t, const uint8_t*, uint64_t, uint64_t, int, cudaStream_t, sdb_profiler*, uint32_t);
-cudaError_t sdb_launch_ovf_resolve(const sdb_dev_view*, uint32_t, unsigned long long*, cudaStream_t);
-cudaError_t sdb_launch_list_index(const sdb_dev_view*, const sdb_send_desc*, const uint32_t*, const uint32_t*, uint32_t, uint32_t, uint64_t,
-                                  cudaStream_t, sdb_profiler*);
-cudaError_t sdb_launch_commit_ranked(const sdb_dev_view*, const sdb_send_desc*, uint32_t, uint32_t, cudaStream_t, sdb_profiler*);
-cudaError_t sdb_send_prepare_device();
-cudaError_t sdb_launch_fanout(const sdb_dev_view*, const sdb_send_desc*, uint32_t, const uint8_t*, const uint32_t*,
-                              uint64_t, uint64_t, uint32_t, int, int, cudaStream_t, sdb_profiler*, const sdb_batch_base*, uint32_t);
-cudaError_t sdb_launch_fanout_shared(const sdb_dev_view*, const sdb_send_desc*, uint32_t, const uint8_t*, uint64_t, uint64_t, uint32_t, int,
-                                     cudaStream_t, sdb_profiler*, const sdb_batch_base*);
-cudaError_t sdb_launch_commit(const sdb_dev_view*, uint32_t, uint32_t, uint32_t*, uint32_t*, int, cudaStream_t, sdb_profiler*,
-                              const sdb_batch_base*);
-cudaError_t sdb_launch_pull(const sdb_dev_view*, const sdb_pull_view*, const sdb_send_desc*, uint32_t, uint32_t, const uint8_t*,
-                            uint32_t, uint32_t, const uint32_t*, const uint32_t*, uint64_t, int, cudaStream_t, sdb_profiler*, int*,
-                            const sdb_batch_base*, uint32_t);
-cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaStream_t, int*, sdb_profiler*, int, uint32_t,
-                               const sdb_compact_args*);
-cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double, uint32_t, const sdb_compact_args*, cudaStream_t,
-                              int*, sdb_profiler*, int);
-cudaError_t sdb_launch_where(const sdb_dev_view*, const sdb_recv_args*, const sdb_where_args*, int, uint32_t, cudaStream_t, int*,
-                             sdb_profiler*, int);
-cudaError_t sdb_recv_prepare_device();
-cudaError_t sdb_balance_prepare_device();
-cudaError_t sdb_launch_receive_small(const sdb_dev_view*, const uint32_t*, uint32_t, uint32_t, uint32_t, uint32_t, uint4*,
-                                     uint8_t*, cudaStream_t, sdb_profiler*);
-cudaError_t sdb_launch_digest(const sdb_recv_args*, uint32_t, unsigned long long*, int, cudaStream_t);
-cudaError_t sdb_launch_arena_floor(const sdb_dev_view*, uint32_t, uint32_t, unsigned long long*, cudaStream_t);
-cudaError_t sdb_launch_latency_server(const sdb_dev_view*, sdb_ls_mailbox*, uint8_t*, uint32_t, uint4*, cudaStream_t);
-const void* sdb_send_kernel_anchor();
-const void* sdb_recv_kernel_anchor();
-const void* sdb_balance_kernel_anchor();
-const void* sdb_xshard_kernel_anchor();
-cudaError_t sdb_launch_pick(int mode, uint32_t n_backends, const uint32_t* weight_dev, unsigned long long* load_dev,
-                            uint32_t n_req, const uint32_t* cost_dev, uint64_t seed, uint32_t* out_dev,
-                            unsigned long long* scratch_dev, const uint32_t* log_tab_dev,
-                            cudaStream_t stream, int* n_launches);
-void sdb_build_log2_table(uint32_t* tab257);
-cudaError_t sdb_launch_agent_loads(const sdb_dev_view*, const uint32_t*, uint32_t, sdb_agent_load*, int, cudaStream_t);
-cudaError_t sdb_launch_queue_stats(const sdb_dev_view*, uint32_t, unsigned long long*, cudaStream_t);
-cudaError_t sdb_launch_backend_loads_from_queues(const sdb_dev_view*, uint32_t, const uint32_t*, uint32_t, unsigned long long*, cudaStream_t);
-cudaError_t sdb_launch_import_measure(const sdb_import_args*, uint32_t, uint32_t*, uint32_t*, uint32_t*, uint32_t*, uint32_t*,
-                                      uint32_t*, uint32_t*, unsigned long long*, cudaStream_t, sdb_profiler*, int*);
-cudaError_t sdb_launch_import_localize(const sdb_import_args*, uint32_t, const uint32_t*, uint32_t*, cudaStream_t, sdb_profiler*, int*);
-cudaError_t sdb_launch_wire_wait(const uint32_t* const*, uint32_t, uint32_t, cudaStream_t, const void* const*, sdb_wire_header*);
-cudaError_t sdb_launch_wire_set(uint32_t*, uint32_t, cudaStream_t);
-cudaError_t sdb_launch_import_fused(const sdb_import2_args*, cudaStream_t, sdb_profiler*, int*);
-cudaError_t sdb_launch_import_place(const sdb_import_totals*, sdb_cursor*, sdb_batch_base*, unsigned long long, uint32_t, uint32_t*, cudaStream_t);
-cudaError_t sdb_launch_arena_floor_cur(const sdb_dev_view*, uint32_t, sdb_cursor*, cudaStream_t);
-cudaError_t sdb_launch_restore_plan(const sdb_dev_view*, const sdb_restore_args*, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_restore_write(const sdb_dev_view*, const sdb_restore_args*, unsigned long long, uint32_t, cudaStream_t,
-                                     sdb_profiler*, int*, int);
-const void* sdb_restore_kernel_anchor();
-cudaError_t sdb_launch_lease_append(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_compact_args*, const uint32_t*,
-                                    const unsigned long long*, const uint32_t*, uint32_t, uint32_t, uint32_t, unsigned long long,
-                                    unsigned long long, double, uint64_t, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_lease_settle(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t, double, cudaStream_t,
-                                    sdb_profiler*, int*);
-cudaError_t sdb_launch_lease_due(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, double, uint32_t, uint32_t, cudaStream_t,
-                                 sdb_profiler*, int*);
-cudaError_t sdb_launch_lease_select(const sdb_dev_view*, const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t,
-                                    uint32_t*, uint32_t*, uint32_t*, cudaStream_t, sdb_profiler*, int*);
-cudaError_t sdb_launch_lease_stage(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, unsigned long long,
-                                   const sdb_compact_args*, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_lease_compact(const sdb_lease_buf*, const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t,
-                                     uint32_t, double, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_ledger_collect(const sdb_dev_view*, const sdb_ledger*, uint32_t, cudaStream_t, sdb_profiler*, int*);
-cudaError_t sdb_launch_ledger_insert(const sdb_dev_view*, const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_ledger*,
-                                     const uint32_t*, const uint32_t*, const uint32_t*, uint32_t, uint32_t, cudaStream_t, sdb_profiler*,
-                                     int*, int);
-cudaError_t sdb_launch_ledger_take(const sdb_lease_buf*, const sdb_ledger*, const sdb_compact_args*, const unsigned long long*, uint32_t,
-                                   uint64_t, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_lease_deliveries(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, cudaStream_t, sdb_profiler*,
-                                        int*);
-cudaError_t sdb_launch_lease_dl_select(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_dl_scratch*, uint32_t, const uint32_t*,
-                                       uint32_t, cudaStream_t, sdb_profiler*, int*);
-cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_dl_scratch*, uint32_t, uint32_t, uint32_t,
-                                     uint32_t, uint32_t, const sdb_compact_args*, uint32_t**, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_lease_x_select(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, unsigned long long, cudaStream_t,
-                                      sdb_profiler*, int*);
-cudaError_t sdb_launch_lease_x_emit(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t, const sdb_compact_args*,
-                                    sdb_lease_meta*, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_lease_import_check(const sdb_lease_scratch*, const sdb_compact_args*, const sdb_lease_meta*, uint32_t, uint32_t,
-                                          unsigned long long, uint32_t, uint32_t, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_lease_import_write(const sdb_lease_buf*, const sdb_compact_args*, const sdb_lease_meta*, const unsigned long long*,
-                                          uint32_t, uint64_t, uint32_t, uint32_t, unsigned long long, unsigned long long, cudaStream_t,
-                                          sdb_profiler*, int*, int);
-cudaError_t sdb_launch_ledger_import(const sdb_dev_view*, const sdb_ledger*, uint32_t, uint32_t, unsigned long long*, cudaStream_t,
-                                     sdb_profiler*, int*, int);
-const void* sdb_lease_kernel_anchor();
-cudaError_t sdb_launch_reloc_plan(const sdb_dev_view*, const sdb_reloc_args*, cudaStream_t, sdb_profiler*, int*, int);
-cudaError_t sdb_launch_reloc_write(const sdb_dev_view*, const sdb_reloc_args*, const sdb_ledger*, uint32_t, cudaStream_t, sdb_profiler*,
-                                   int*, int);
-const void* sdb_relocate_kernel_anchor();
-}
-
-#define SDB_SCAN_TILE 4096u
-
 struct sdb_staged {
   uint32_t kind = 0;          // 0 p2p, 1 group, 2 list
   uint32_t n = 0;
@@ -835,6 +737,16 @@ int send_common(sdb_ctx* h, uint32_t kind, uint32_t n, SendArrays& a, const uint
   return submit(h, s, seq_base_out);
 }
 
+// n elements (at least one) of device memory for *p, recorded in `owned` (the store's or the policy's allocations)
+template <typename T>
+bool lease_alloc(std::vector<void*>& owned, T** p, size_t n) {
+  void* q = nullptr;
+  if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return false;
+  owned.push_back(q);
+  *p = static_cast<T*>(q);
+  return true;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -933,10 +845,10 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
   CUDA_TRY(h, cudaMemsetAsync(h->scratch.payload_dev, 0, c.max_batch_payload + 64, h->stream));
 
   // receive scratch
-  const size_t tiles = (A + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE + 1;
+  const size_t tiles = sdb_scan_tops_len(A);
   CUDA_TRY(h, dmalloc(&h->rx_agent, A)); CUDA_TRY(h, dmalloc(&h->rx_cnt, A));
   CUDA_TRY(h, dmalloc(&h->rx_rec_local, A)); CUDA_TRY(h, dmalloc(&h->rx_rec_tops, tiles));
-  const size_t rtiles = (c.max_recv_records + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE + 1;
+  const size_t rtiles = sdb_scan_tops_len(c.max_recv_records);
   CUDA_TRY(h, dmalloc(&h->rx_plan, c.max_recv_records + 4)); CUDA_TRY(h, dmalloc(&h->rx_rec_off, A));
   CUDA_TRY(h, dmalloc(&h->rx_plan_tops, rtiles));
   CUDA_TRY(h, dmalloc(&h->rx_lb, sdb_lb_words(static_cast<uint32_t>(A / 64 + 2)) + 4));
@@ -979,7 +891,7 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
     h->xs_cap = static_cast<uint32_t>(cap64);
     const size_t n = h->xs_cap, G1 = static_cast<size_t>(c.max_groups) + 1;
     const size_t GB = G1 * c.num_shards + 2;                 // (group, source) pairs
-    const size_t wt = n / SDB_SCAN_TILE + 2, gt = GB / SDB_SCAN_TILE + 2;
+    const size_t wt = sdb_scan_tops_len(n), gt = sdb_scan_tops_len(GB);
     CUDA_TRY(h, dmalloc(&h->xs_w, n)); CUDA_TRY(h, dmalloc(&h->xs_w_local, n)); CUDA_TRY(h, dmalloc(&h->xs_w_tops, wt));
     CUDA_TRY(h, dmalloc(&h->xs_gs_cnt, GB)); CUDA_TRY(h, dmalloc(&h->xs_gs_local, GB)); CUDA_TRY(h, dmalloc(&h->xs_gs_tops, gt));
     CUDA_TRY(h, dmalloc(&h->xs_gs_cur, GB)); CUDA_TRY(h, dmalloc(&h->xs_gs_off, G1)); CUDA_TRY(h, dmalloc(&h->xs_gs_idx, n));
@@ -1970,7 +1882,7 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
 static int compact_ensure(sdb_ctx* h) {
   sdb_compact_args& c = h->cx;
   if (c.table) return SDB_OK;
-  const size_t R = h->cfg.max_recv_records, tiles = (R + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE + 1;
+  const size_t R = h->cfg.max_recv_records, tiles = sdb_scan_tops_len(R);
   uint32_t tbits = 10;
   while ((1ull << tbits) < 2 * R) ++tbits;
   return dmalloc_set(h, {{&c.rec_slot, R}, {&c.head, R}, {&c.head_local, R}, {&c.head_tops, tiles}, {&c.gran, R},
@@ -2102,9 +2014,9 @@ int sdb_restore_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
 static int restore_ensure(sdb_ctx* h) {
   { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
   if (h->rs_agent) return SDB_OK;
-  const size_t A = h->cfg.max_agents, tiles = A / SDB_SCAN_TILE + 2;
+  const size_t A = h->cfg.max_agents, tiles = sdb_scan_tops_len(A);
   const size_t R = h->cfg.max_recv_records, H = 256 * (R / 1024 + 1);
-  return dmalloc_set(h, {{&h->rs_sort, 4 * R + 2 * H + H / SDB_SCAN_TILE + 2}, {&h->rs_tot, 8}, {&h->rs_agent, 6 * A + tiles}},
+  return dmalloc_set(h, {{&h->rs_sort, 4 * R + 2 * H + sdb_scan_tops_len(H)}, {&h->rs_tot, 8}, {&h->rs_agent, 6 * A + tiles}},
                      "restore: device allocation failed");
 }
 
@@ -2177,7 +2089,7 @@ int sdb_arena_relocate(sdb_handle h, uint64_t floor_bytes, uint32_t flags, sdb_r
   const uint64_t G = h->arena_grans, tail = h->arena_tail;
   if (!h->rl_bits) {
     const size_t W = G / 32 + 2, A = h->cfg.max_agents;
-    const int rc = dmalloc_set(h, {{&h->rl_bits, W}, {&h->rl_cnt, W}, {&h->rl_pre, W}, {&h->rl_tops, W / SDB_SCAN_TILE + 2}, {&h->rl_sel, A / 32 + 1},
+    const int rc = dmalloc_set(h, {{&h->rl_bits, W}, {&h->rl_cnt, W}, {&h->rl_pre, W}, {&h->rl_tops, sdb_scan_tops_len(W)}, {&h->rl_sel, A / 32 + 1},
                                    {&h->rl_tot, 8}}, "sdb_arena_relocate: device allocation failed");
     if (rc != SDB_OK) return rc;
   }
@@ -2270,13 +2182,6 @@ static void lease_free(sdb_ctx* h) {
 }
 int sdb_lease_reserve(sdb_handle h, uint64_t max_records, uint64_t max_payload_bytes) {
   if (!h) return SDB_EINVAL;
-  auto lease_alloc = [](sdb_ctx* c, auto** p, size_t n) {
-    void* q = nullptr;
-    if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(**p)) != cudaSuccess) return false;
-    c->lease.mem.push_back(q);
-    *p = static_cast<std::remove_reference_t<decltype(*p)>>(q);
-    return true;
-  };
   sdb_ctx::LeaseStore& L = h->lease;
   if (L.live) return fail(h, SDB_EINVAL, "sdb_lease_reserve: the store holds live leases (ack them or sweep them back first)");
   if (L.dead) return fail(h, SDB_EINVAL, "sdb_lease_reserve: the store holds dead letters (sdb_lease_dead_letters first)");
@@ -2288,26 +2193,27 @@ int sdb_lease_reserve(sdb_handle h, uint64_t max_records, uint64_t max_payload_b
   if (!max_records) return SDB_OK;
   const uint64_t P = (max_payload_bytes + SDB_GRANULE - 1) & ~static_cast<uint64_t>(SDB_GRANULE - 1);
   const size_t cap = max_records, R = h->cfg.max_recv_records, S = std::max(cap, R), A = h->cfg.max_agents;
-  const size_t tS = S / SDB_SCAN_TILE + 2, tR = R / SDB_SCAN_TILE + 2, tC = cap / SDB_SCAN_TILE + 2, tA = A / SDB_SCAN_TILE + 2;
+  const size_t tS = sdb_scan_tops_len(S), tR = sdb_scan_tops_len(R), tC = sdb_scan_tops_len(cap), tA = sdb_scan_tops_len(A);
   const size_t H = 256 * (R / 1024 + 1);
+  std::vector<void*>& m = L.mem;
   bool ok = true;
   for (sdb_lease_buf& b : L.buf)
-    ok = ok && lease_alloc(h, &b.ent, cap) && lease_alloc(h, &b.agent, cap) && lease_alloc(h, &b.id, cap) &&
-         lease_alloc(h, &b.deadline, cap) && lease_alloc(h, &b.state, cap) && lease_alloc(h, &b.rows, cap) &&
-         lease_alloc(h, &b.payload, P);
+    ok = ok && lease_alloc(m, &b.ent, cap) && lease_alloc(m, &b.agent, cap) && lease_alloc(m, &b.id, cap) &&
+         lease_alloc(m, &b.deadline, cap) && lease_alloc(m, &b.state, cap) && lease_alloc(m, &b.rows, cap) &&
+         lease_alloc(m, &b.payload, P);
   sdb_lease_scratch& s = L.s;
-  ok = ok && lease_alloc(h, &s.flag, S) && lease_alloc(h, &s.f_local, S) && lease_alloc(h, &s.f_tops, tS) &&
-       lease_alloc(h, &s.gran, S) && lease_alloc(h, &s.g_local, S) && lease_alloc(h, &s.g_tops, tS) &&
-       lease_alloc(h, &s.rfirst, cap) && lease_alloc(h, &s.rmap, cap) &&
-       lease_alloc(h, &s.rg, cap) && lease_alloc(h, &s.rg_local, cap) && lease_alloc(h, &s.rg_tops, tC) &&
-       lease_alloc(h, &s.chunk, R) && lease_alloc(h, &s.staged, R) && lease_alloc(h, &s.key_a, R) && lease_alloc(h, &s.key_b, R) &&
-       lease_alloc(h, &s.val_a, R) && lease_alloc(h, &s.val_b, R) &&
-       lease_alloc(h, &s.hist, H) && lease_alloc(h, &s.h_local, H) && lease_alloc(h, &s.h_tops, H / SDB_SCAN_TILE + 2) &&
-       lease_alloc(h, &s.run_begin, R + 1) && lease_alloc(h, &s.kcnt, R) && lease_alloc(h, &s.k_local, R) &&
-       lease_alloc(h, &s.k_tops, tR) && lease_alloc(h, &s.kflag, R) && lease_alloc(h, &s.kf_local, R) && lease_alloc(h, &s.kf_tops, tR) &&
-       lease_alloc(h, &s.a_local, A) && lease_alloc(h, &s.a_tops, tA) &&
-       lease_alloc(h, &s.req, SDB_LS_SETTLE_CHUNK) && lease_alloc(h, &s.at, SDB_LS_SETTLE_CHUNK) &&
-       lease_alloc(h, &s.settled, SDB_LS_SETTLE_CHUNK) && lease_alloc(h, &s.tot, 16);
+  ok = ok && lease_alloc(m, &s.flag, S) && lease_alloc(m, &s.f_local, S) && lease_alloc(m, &s.f_tops, tS) &&
+       lease_alloc(m, &s.gran, S) && lease_alloc(m, &s.g_local, S) && lease_alloc(m, &s.g_tops, tS) &&
+       lease_alloc(m, &s.rfirst, cap) && lease_alloc(m, &s.rmap, cap) &&
+       lease_alloc(m, &s.rg, cap) && lease_alloc(m, &s.rg_local, cap) && lease_alloc(m, &s.rg_tops, tC) &&
+       lease_alloc(m, &s.chunk, R) && lease_alloc(m, &s.staged, R) && lease_alloc(m, &s.key_a, R) && lease_alloc(m, &s.key_b, R) &&
+       lease_alloc(m, &s.val_a, R) && lease_alloc(m, &s.val_b, R) &&
+       lease_alloc(m, &s.hist, H) && lease_alloc(m, &s.h_local, H) && lease_alloc(m, &s.h_tops, sdb_scan_tops_len(H)) &&
+       lease_alloc(m, &s.run_begin, R + 1) && lease_alloc(m, &s.kcnt, R) && lease_alloc(m, &s.k_local, R) &&
+       lease_alloc(m, &s.k_tops, tR) && lease_alloc(m, &s.kflag, R) && lease_alloc(m, &s.kf_local, R) && lease_alloc(m, &s.kf_tops, tR) &&
+       lease_alloc(m, &s.a_local, A) && lease_alloc(m, &s.a_tops, tA) &&
+       lease_alloc(m, &s.req, SDB_LS_SETTLE_CHUNK) && lease_alloc(m, &s.at, SDB_LS_SETTLE_CHUNK) &&
+       lease_alloc(m, &s.settled, SDB_LS_SETTLE_CHUNK) && lease_alloc(m, &s.tot, 16);
   ok = ok && cudaHostAlloc(reinterpret_cast<void**>(&L.th), 16 * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
   if (!ok) {
     lease_free(h);
@@ -2518,19 +2424,15 @@ int sdb_lease_set_policy(sdb_handle h, uint32_t max_deliveries, uint64_t ledger_
   h->stream_busy = false;
   lease_policy_free(h);
   if (!max_deliveries) return SDB_OK;
-  auto alloc = [h](auto** p, size_t n) {
-    void* q = nullptr;
-    if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(**p)) != cudaSuccess) return false;
-    h->lease.pmem.push_back(q);
-    *p = static_cast<std::remove_reference_t<decltype(*p)>>(q);
-    return true;
-  };
   const size_t cap = L.cap, N = ledger_entries, A = h->cfg.max_agents, H = 256 * (cap / 1024 + 1);
   sdb_dl_scratch& d = L.dl;
-  bool ok = alloc(&L.buf[0].deliveries, cap) && alloc(&L.buf[1].deliveries, cap) && alloc(&L.led.ent, N) && alloc(&L.led.alt, N) &&
-            alloc(&L.led.index, 2 * N) && alloc(&L.led.tot, 2) &&
-            alloc(&d.key_a, cap) && alloc(&d.key_b, cap) && alloc(&d.val_a, cap) && alloc(&d.val_b, cap) && alloc(&d.staged, cap) &&
-            alloc(&d.hist, H) && alloc(&d.h_local, H) && alloc(&d.h_tops, H / SDB_SCAN_TILE + 2) && alloc(&d.pos, A) && alloc(&d.cnt, A);
+  std::vector<void*>& m = L.pmem;
+  bool ok = lease_alloc(m, &L.buf[0].deliveries, cap) && lease_alloc(m, &L.buf[1].deliveries, cap) && lease_alloc(m, &L.led.ent, N) &&
+            lease_alloc(m, &L.led.alt, N) && lease_alloc(m, &L.led.index, 2 * N) && lease_alloc(m, &L.led.tot, 2) &&
+            lease_alloc(m, &d.key_a, cap) && lease_alloc(m, &d.key_b, cap) && lease_alloc(m, &d.val_a, cap) &&
+            lease_alloc(m, &d.val_b, cap) && lease_alloc(m, &d.staged, cap) && lease_alloc(m, &d.hist, H) &&
+            lease_alloc(m, &d.h_local, H) && lease_alloc(m, &d.h_tops, sdb_scan_tops_len(H)) && lease_alloc(m, &d.pos, A) &&
+            lease_alloc(m, &d.cnt, A);
   ok = ok && cudaHostAlloc(reinterpret_cast<void**>(&L.lth), 2 * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
   ok = ok && cudaMemsetAsync(d.pos, 0xFF, A * sizeof(uint32_t), h->stream) == cudaSuccess &&
        cudaMemsetAsync(L.led.index, 0xFF, 2 * N * sizeof(uint32_t), h->stream) == cudaSuccess &&

@@ -297,7 +297,7 @@ struct sdb_reloc_args {
   uint32_t* bits;                  // [words]
   uint32_t* cnt;                   // [words] popcount of each word
   uint32_t* pre;                   // [words] its exclusive scan (block-local part)
-  uint32_t* tops;                  // [words / SDB_SCAN_TILE + 1]
+  uint32_t* tops;                  // [sdb_scan_tops_len(words)]
   uint32_t* sel;                   // [ceil(n_agents / 32)] bit a: agent a is selected
   unsigned long long* tot;         // [0] marked granules [1] agents [2] records [3] largest distance below the tail of an
                                    // agent's oldest pending record [4] the same over unselected agents (0: none pending)
@@ -429,10 +429,60 @@ static inline void sdb_prof_end(sdb_profiler* p, int i, cudaStream_t s) {
   if (i >= 0) cudaEventRecord(p->ev_b[i], s);
 }
 
+// ---- two-level exclusive scan (sdb_scan_u32): the prefix of element i is local[i] + tops[i / SDB_SCAN_TILE] ----
+#define SDB_SCAN_TILE 4096u   // elements per scan block (1024 threads x 4)
+// words of a `tops` array for a scan of up to n elements
+static inline size_t sdb_scan_tops_len(size_t n) { return n / SDB_SCAN_TILE + 2; }
+
+// blocks for `items` work items at per_block each, between 1 and max_blocks (kernels grid-stride beyond)
+static inline uint32_t sdb_grid(uint64_t items, uint64_t per_block, uint64_t max_blocks) {
+  uint64_t g = (items + per_block - 1) / per_block;
+  if (g > max_blocks) g = max_blocks;
+  return static_cast<uint32_t>(g ? g : 1);
+}
+// radix-sort key width: bits needed for keys 0 .. max_key, at least 1
+static inline uint32_t sdb_key_bits(uint64_t max_key) {
+  uint32_t b = 1;
+  while (b < 32 && (max_key >> b)) ++b;
+  return b;
+}
+
 #ifdef __CUDACC__
 
 __device__ __forceinline__ uint8_t* sdb_arena_ptr(const sdb_dev_view& v, uint64_t apos) {
   return v.arena + ((apos & v.gmask) << 5);
+}
+
+__device__ __forceinline__ uint32_t sdb_scan_at(const uint32_t* local, const uint32_t* tops, uint32_t i) {
+  return local[i] + tops[i / SDB_SCAN_TILE];
+}
+// inclusive scan of x over each aligned group of W lanes (every lane of the warp calls it); lane: the caller's lane in
+// its group
+template <uint32_t W = 32>
+__device__ __forceinline__ uint32_t sdb_warp_incl_scan(uint32_t x, uint32_t lane) {
+#pragma unroll
+  for (uint32_t o = 1; o < W; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o, W);
+    if (lane >= o) x += y;
+  }
+  return x;
+}
+// exclusive scan of one SDB_SCAN_TILE tile held 4 elements per thread by a 1024-thread block (x: zero past the end).
+// Returns the tile-local prefix of this thread's x[0]; one thread writes the tile total to *tile_total.
+__device__ __forceinline__ uint32_t sdb_block_scan_tile(const uint32_t (&x)[4], uint32_t* tile_total) {
+  __shared__ uint32_t s_warp[32];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t tsum = x[0] + x[1] + x[2] + x[3];
+  const uint32_t incl = sdb_warp_incl_scan(tsum, lane);
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t w = s_warp[lane], wi = sdb_warp_incl_scan(w, lane);
+    s_warp[lane] = wi - w;              // exclusive warp offsets
+    if (lane == 31) *tile_total = wi;
+  }
+  __syncthreads();
+  return s_warp[warp] + incl - tsum;
 }
 
 // Claim the next slot of agent a's ring and publish (handle, meta) into it.
@@ -764,3 +814,105 @@ __device__ __forceinline__ void sdb_lb_prefix(unsigned long long* lb, uint32_t t
 }
 
 #endif  // __CUDACC__
+
+// ---- launchers and helpers that one source defines and another calls ----
+extern "C" {
+cudaError_t sdb_launch_p2p(const sdb_dev_view*, const sdb_send_desc*, uint32_t, const uint8_t*, uint64_t, uint64_t, int, cudaStream_t, sdb_profiler*, uint32_t);
+cudaError_t sdb_launch_ovf_resolve(const sdb_dev_view*, uint32_t, unsigned long long*, cudaStream_t);
+cudaError_t sdb_launch_list_index(const sdb_dev_view*, const sdb_send_desc*, const uint32_t*, const uint32_t*, uint32_t, uint32_t, uint64_t,
+                                  cudaStream_t, sdb_profiler*);
+cudaError_t sdb_launch_commit_ranked(const sdb_dev_view*, const sdb_send_desc*, uint32_t, uint32_t, cudaStream_t, sdb_profiler*);
+cudaError_t sdb_send_prepare_device();
+cudaError_t sdb_launch_fanout(const sdb_dev_view*, const sdb_send_desc*, uint32_t, const uint8_t*, const uint32_t*,
+                              uint64_t, uint64_t, uint32_t, int, int, cudaStream_t, sdb_profiler*, const sdb_batch_base*, uint32_t);
+cudaError_t sdb_launch_fanout_shared(const sdb_dev_view*, const sdb_send_desc*, uint32_t, const uint8_t*, uint64_t, uint64_t, uint32_t, int,
+                                     cudaStream_t, sdb_profiler*, const sdb_batch_base*);
+cudaError_t sdb_launch_commit(const sdb_dev_view*, uint32_t, uint32_t, uint32_t*, uint32_t*, int, cudaStream_t, sdb_profiler*,
+                              const sdb_batch_base*);
+cudaError_t sdb_launch_pull(const sdb_dev_view*, const sdb_pull_view*, const sdb_send_desc*, uint32_t, uint32_t, const uint8_t*,
+                            uint32_t, uint32_t, const uint32_t*, const uint32_t*, uint64_t, int, cudaStream_t, sdb_profiler*, int*,
+                            const sdb_batch_base*, uint32_t);
+cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaStream_t, int*, sdb_profiler*, int, uint32_t,
+                               const sdb_compact_args*);
+cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double, uint32_t, const sdb_compact_args*, cudaStream_t,
+                              int*, sdb_profiler*, int);
+cudaError_t sdb_launch_where(const sdb_dev_view*, const sdb_recv_args*, const sdb_where_args*, int, uint32_t, cudaStream_t, int*,
+                             sdb_profiler*, int);
+cudaError_t sdb_recv_prepare_device();
+cudaError_t sdb_balance_prepare_device();
+cudaError_t sdb_launch_receive_small(const sdb_dev_view*, const uint32_t*, uint32_t, uint32_t, uint32_t, uint32_t, uint4*,
+                                     uint8_t*, cudaStream_t, sdb_profiler*);
+cudaError_t sdb_launch_digest(const sdb_recv_args*, uint32_t, unsigned long long*, int, cudaStream_t);
+cudaError_t sdb_launch_arena_floor(const sdb_dev_view*, uint32_t, uint32_t, unsigned long long*, cudaStream_t);
+cudaError_t sdb_launch_latency_server(const sdb_dev_view*, sdb_ls_mailbox*, uint8_t*, uint32_t, uint4*, cudaStream_t);
+const void* sdb_send_kernel_anchor();
+const void* sdb_recv_kernel_anchor();
+const void* sdb_balance_kernel_anchor();
+const void* sdb_xshard_kernel_anchor();
+cudaError_t sdb_launch_pick(int mode, uint32_t n_backends, const uint32_t* weight_dev, unsigned long long* load_dev,
+                            uint32_t n_req, const uint32_t* cost_dev, uint64_t seed, uint32_t* out_dev,
+                            unsigned long long* scratch_dev, const uint32_t* log_tab_dev,
+                            cudaStream_t stream, int* n_launches);
+void sdb_build_log2_table(uint32_t* tab257);
+cudaError_t sdb_launch_agent_loads(const sdb_dev_view*, const uint32_t*, uint32_t, sdb_agent_load*, int, cudaStream_t);
+cudaError_t sdb_launch_queue_stats(const sdb_dev_view*, uint32_t, unsigned long long*, cudaStream_t);
+cudaError_t sdb_launch_backend_loads_from_queues(const sdb_dev_view*, uint32_t, const uint32_t*, uint32_t, unsigned long long*, cudaStream_t);
+cudaError_t sdb_launch_import_measure(const sdb_import_args*, uint32_t, uint32_t*, uint32_t*, uint32_t*, uint32_t*, uint32_t*,
+                                      uint32_t*, uint32_t*, unsigned long long*, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_import_localize(const sdb_import_args*, uint32_t, const uint32_t*, uint32_t*, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_wire_wait(const uint32_t* const*, uint32_t, uint32_t, cudaStream_t, const void* const*, sdb_wire_header*);
+cudaError_t sdb_launch_wire_set(uint32_t*, uint32_t, cudaStream_t);
+cudaError_t sdb_launch_import_fused(const sdb_import2_args*, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_import_place(const sdb_import_totals*, sdb_cursor*, sdb_batch_base*, unsigned long long, uint32_t, uint32_t*, cudaStream_t);
+cudaError_t sdb_launch_arena_floor_cur(const sdb_dev_view*, uint32_t, sdb_cursor*, cudaStream_t);
+cudaError_t sdb_launch_restore_plan(const sdb_dev_view*, const sdb_restore_args*, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_restore_write(const sdb_dev_view*, const sdb_restore_args*, unsigned long long, uint32_t, cudaStream_t,
+                                     sdb_profiler*, int*, int);
+const void* sdb_restore_kernel_anchor();
+cudaError_t sdb_launch_lease_append(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_compact_args*, const uint32_t*,
+                                    const unsigned long long*, const uint32_t*, uint32_t, uint32_t, uint32_t, unsigned long long,
+                                    unsigned long long, double, uint64_t, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_settle(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t, double, cudaStream_t,
+                                    sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_due(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, double, uint32_t, uint32_t, cudaStream_t,
+                                 sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_select(const sdb_dev_view*, const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t,
+                                    uint32_t*, uint32_t*, uint32_t*, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_stage(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, unsigned long long,
+                                   const sdb_compact_args*, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_compact(const sdb_lease_buf*, const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t,
+                                     uint32_t, double, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_ledger_collect(const sdb_dev_view*, const sdb_ledger*, uint32_t, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_ledger_insert(const sdb_dev_view*, const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_ledger*,
+                                     const uint32_t*, const uint32_t*, const uint32_t*, uint32_t, uint32_t, cudaStream_t, sdb_profiler*,
+                                     int*, int);
+cudaError_t sdb_launch_ledger_take(const sdb_lease_buf*, const sdb_ledger*, const sdb_compact_args*, const unsigned long long*, uint32_t,
+                                   uint64_t, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_deliveries(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, cudaStream_t, sdb_profiler*,
+                                        int*);
+cudaError_t sdb_launch_lease_dl_select(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_dl_scratch*, uint32_t, const uint32_t*,
+                                       uint32_t, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf*, const sdb_lease_scratch*, const sdb_dl_scratch*, uint32_t, uint32_t, uint32_t,
+                                     uint32_t, uint32_t, const sdb_compact_args*, uint32_t**, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_x_select(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, unsigned long long, cudaStream_t,
+                                      sdb_profiler*, int*);
+cudaError_t sdb_launch_lease_x_emit(const sdb_lease_buf*, const sdb_lease_scratch*, uint32_t, uint32_t, uint32_t, const sdb_compact_args*,
+                                    sdb_lease_meta*, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_import_check(const sdb_lease_scratch*, const sdb_compact_args*, const sdb_lease_meta*, uint32_t, uint32_t,
+                                          unsigned long long, uint32_t, uint32_t, uint32_t, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_lease_import_write(const sdb_lease_buf*, const sdb_compact_args*, const sdb_lease_meta*, const unsigned long long*,
+                                          uint32_t, uint64_t, uint32_t, uint32_t, unsigned long long, unsigned long long, cudaStream_t,
+                                          sdb_profiler*, int*, int);
+cudaError_t sdb_launch_ledger_import(const sdb_dev_view*, const sdb_ledger*, uint32_t, uint32_t, unsigned long long*, cudaStream_t,
+                                     sdb_profiler*, int*, int);
+const void* sdb_lease_kernel_anchor();
+cudaError_t sdb_launch_reloc_plan(const sdb_dev_view*, const sdb_reloc_args*, cudaStream_t, sdb_profiler*, int*, int);
+cudaError_t sdb_launch_reloc_write(const sdb_dev_view*, const sdb_reloc_args*, const sdb_ledger*, uint32_t, cudaStream_t, sdb_profiler*,
+                                   int*, int);
+const void* sdb_relocate_kernel_anchor();
+cudaError_t sdb_scan_u32(const uint32_t* in, uint32_t* local, uint32_t* tops, uint32_t n, unsigned long long* total_out, uint32_t* out,
+                         cudaStream_t stream, int* n_launches);
+cudaError_t sdb_radix_sort_u32(uint32_t* ka, uint32_t* va, uint32_t* kb, uint32_t* vb, uint32_t n, uint32_t bits, uint32_t* hist,
+                               uint32_t* h_local, uint32_t* h_tops, uint32_t** kres, uint32_t** vres, cudaStream_t stream,
+                               int* n_launches);
+}

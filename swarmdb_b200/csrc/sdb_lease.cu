@@ -30,17 +30,6 @@
 //   ledger   k_ledger_import: one warp per (agent, seq, count) triple finds its record in the agent's ring window
 #include "sdb_common.cuh"
 
-#define SDB_SCAN_TILE 4096u
-
-extern "C" cudaError_t sdb_scan_u32(const uint32_t* in, uint32_t* local, uint32_t* tops, uint32_t n,
-                                    unsigned long long* total_out, uint32_t* out, cudaStream_t stream);
-extern "C" cudaError_t sdb_radix_sort_u32(uint32_t* ka, uint32_t* va, uint32_t* kb, uint32_t* vb, uint32_t n, uint32_t bits,
-                                          uint32_t* hist, uint32_t* h_local, uint32_t* h_tops, uint32_t** kres, uint32_t** vres,
-                                          cudaStream_t stream, int* n_launches);
-
-__device__ __forceinline__ uint32_t ls_scan(const uint32_t* local, const uint32_t* tops, uint32_t i) {
-  return local[i] + tops[i / SDB_SCAN_TILE];
-}
 __device__ __forceinline__ uint32_t ls_pg(uint32_t len) { return ((len + 31u) & ~31u) >> 5; }
 // row i as two 16-byte words: {timestamp, payload_off}, {sender, group, len | prio << 16 | type << 24, reserved}
 __device__ __forceinline__ void ls_row(const sdb_recv_send* rows, uint32_t i, uint4& lo, uint4& hi) {
@@ -60,18 +49,6 @@ __device__ __forceinline__ void ls_copy_payload(const uint8_t* base, const uint4
   for (uint32_t c = lane; c < n; c += 32) d[c] = src[c];
 }
 
-static uint32_t ls_grid(uint64_t items, uint64_t per_block, int sm_count) {
-  uint64_t g = (items + per_block - 1) / per_block;
-  const uint64_t cap = static_cast<uint64_t>(sm_count) * 8;
-  if (g > cap) g = cap;
-  return static_cast<uint32_t>(g ? g : 1);
-}
-static uint32_t ls_bits(uint64_t max_key) {
-  uint32_t b = 1;
-  while (b < 32 && (max_key >> b)) ++b;
-  return b;
-}
-
 // ---- append -----------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 k_lease_append_agents(sdb_lease_buf b, const uint32_t* __restrict__ count, const uint32_t* __restrict__ local,
@@ -82,7 +59,7 @@ k_lease_append_agents(sdb_lease_buf b, const uint32_t* __restrict__ count, const
   for (uint32_t q = gw; q < n; q += nw) {
     const uint32_t c = count[q];
     if (!c) continue;
-    const uint32_t off = ls_scan(local, tops, q), a = agents ? agents[q] : q;
+    const uint32_t off = sdb_scan_at(local, tops, q), a = agents ? agents[q] : q;
     for (uint32_t j = lane; j < c; j += 32) {
       const uint32_t e = used + off + j;
       b.agent[e] = a; b.id[e] = id_base + off + j; b.deadline[e] = deadline; b.state[e] = SDB_LS_LIVE;
@@ -155,7 +132,7 @@ __global__ void __launch_bounds__(256)
 k_lease_chunk(sdb_lease_buf b, uint32_t used, sdb_lease_scratch s, uint32_t C) {
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= used || !s.flag[e]) return;
-  const uint32_t p = ls_scan(s.f_local, s.f_tops, e);
+  const uint32_t p = sdb_scan_at(s.f_local, s.f_tops, e);
   if (p >= C) return;
   s.chunk[p] = e; s.key_a[p] = b.agent[e]; s.val_a[p] = p;
 }
@@ -170,7 +147,7 @@ __global__ void __launch_bounds__(256)
 k_lease_run_begin(sdb_lease_scratch s, uint32_t n) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  if (s.gran[i]) s.run_begin[ls_scan(s.g_local, s.g_tops, i)] = i;
+  if (s.gran[i]) s.run_begin[sdb_scan_at(s.g_local, s.g_tops, i)] = i;
   if (i == 0) s.run_begin[s.tot[1]] = n;
 }
 
@@ -200,13 +177,13 @@ k_lease_stage_list(sdb_lease_scratch s, const uint32_t* __restrict__ key, const 
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t head = s.gran[i];
-  const uint32_t r = ls_scan(s.g_local, s.g_tops, i) + head - 1u;
+  const uint32_t r = sdb_scan_at(s.g_local, s.g_tops, i) + head - 1u;
   const uint32_t c = s.kcnt[r];
   if (!c) return;
-  const uint32_t base = ls_scan(s.k_local, s.k_tops, r);
+  const uint32_t base = sdb_scan_at(s.k_local, s.k_tops, r);
   s.staged[base + i - s.run_begin[r]] = s.chunk[val[i]];
   if (head) {
-    const uint32_t q = ls_scan(s.kf_local, s.kf_tops, r);
+    const uint32_t q = sdb_scan_at(s.kf_local, s.kf_tops, r);
     rs_agent[q] = key[i]; rs_count[q] = c; rs_first[q] = base;
     atomicMax(s.tot + 5, static_cast<unsigned long long>(key[i]) + 1ull);
   }
@@ -253,8 +230,8 @@ k_lease_stage_rows(sdb_lease_buf b, sdb_lease_scratch s, const uint32_t* __restr
   for (uint32_t p = gw; p < n; p += nw) {
     if (!s.flag[p]) continue;
     const uint32_t row = b.ent[s.staged[sv[p]]].send;
-    const uint32_t nr = ls_scan(s.f_local, s.f_tops, p);
-    const unsigned long long off = static_cast<unsigned long long>(ls_scan(s.g_local, s.g_tops, p)) << 5;
+    const uint32_t nr = sdb_scan_at(s.f_local, s.f_tops, p);
+    const unsigned long long off = static_cast<unsigned long long>(sdb_scan_at(s.g_local, s.g_tops, p)) << 5;
     uint4 lo, hi;
     ls_row(b.rows, row, lo, hi);
     ls_copy_payload(b.payload, lo, hi, payload_out + off, lane);
@@ -316,9 +293,9 @@ __global__ void __launch_bounds__(256)
 k_lease_copy_entries(sdb_lease_buf in, sdb_lease_buf out, sdb_lease_scratch s, uint32_t used) {
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= used || !s.flag[e]) return;
-  const uint32_t k = ls_scan(s.f_local, s.f_tops, e);
+  const uint32_t k = sdb_scan_at(s.f_local, s.f_tops, e);
   sdb_recv_entry en = in.ent[e];
-  en.send = ls_scan(s.g_local, s.g_tops, en.send);
+  en.send = sdb_scan_at(s.g_local, s.g_tops, en.send);
   out.ent[k] = en; out.agent[k] = in.agent[e]; out.id[k] = in.id[e]; out.deadline[k] = in.deadline[e];
   out.state[k] = in.state[e];
   if (in.deliveries) out.deliveries[k] = in.deliveries[e];
@@ -331,8 +308,8 @@ k_lease_copy_rows(sdb_lease_buf in, sdb_lease_buf out, sdb_lease_scratch s, uint
   const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t r = gw; r < rows; r += nw) {
     if (!s.gran[r]) continue;
-    const uint32_t k = ls_scan(s.g_local, s.g_tops, r);
-    const unsigned long long off = static_cast<unsigned long long>(ls_scan(s.rg_local, s.rg_tops, r)) << 5;
+    const uint32_t k = sdb_scan_at(s.g_local, s.g_tops, r);
+    const unsigned long long off = static_cast<unsigned long long>(sdb_scan_at(s.rg_local, s.rg_tops, r)) << 5;
     uint4 lo, hi;
     ls_row(in.rows, r, lo, hi);
     ls_copy_payload(in.payload, lo, hi, out.payload + off, lane);
@@ -354,13 +331,12 @@ extern "C" cudaError_t sdb_launch_lease_append(const sdb_lease_buf* b, const sdb
                                                cudaStream_t stream, sdb_profiler* prof, int* n_launches, int sm_count) {
   const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
   int nl = 0;
-  cudaError_t e = sdb_scan_u32(count, s->a_local, s->a_tops, n_agents, nullptr, nullptr, stream);
-  nl += 2;
-  k_lease_append_agents<<<ls_grid(n_agents, 8, sm_count * 4), 256, 0, stream>>>(*b, count, s->a_local, s->a_tops, agents, n_agents,
-                                                                                used, id_base, deadline);
+  cudaError_t e = sdb_scan_u32(count, s->a_local, s->a_tops, n_agents, nullptr, nullptr, stream, &nl);
+  k_lease_append_agents<<<sdb_grid(n_agents, 8, 32 * sm_count), 256, 0, stream>>>(*b, count, s->a_local, s->a_tops, agents, n_agents,
+                                                                                  used, id_base, deadline);
   const uint64_t items = rec_cap * (max_pad / 16u > 1u ? max_pad / 16u : 1u);
-  k_lease_append_copy<<<ls_grid(items, 256, sm_count * 4), 256, 0, stream>>>(*b, cx->entry_out, cx->send_out, cx->payload_out,
-                                                                             rx_totals, cx->totals, used, rows_used, pay_used);
+  k_lease_append_copy<<<sdb_grid(items, 256, 32 * sm_count), 256, 0, stream>>>(*b, cx->entry_out, cx->send_out, cx->payload_out,
+                                                                               rx_totals, cx->totals, used, rows_used, pay_used);
   nl += 2;
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
@@ -389,8 +365,7 @@ extern "C" cudaError_t sdb_launch_lease_due(const sdb_lease_buf* b, const sdb_le
   int nl = 0;
   cudaMemsetAsync(s->tot, 0, 16 * sizeof(unsigned long long), stream);
   LS_LAUNCH(used, k_lease_due, *b, used, now, all, max_deliveries, s->flag);
-  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream);
-  nl += used ? 2 : 0;
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream, &nl);
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
   return e == cudaSuccess ? cudaGetLastError() : e;
@@ -406,16 +381,15 @@ extern "C" cudaError_t sdb_launch_lease_select(const sdb_dev_view* v, const sdb_
   int nl = 0;
   LS_LAUNCH(used, k_lease_chunk, *b, used, *s, n);
   uint32_t *ks = nullptr, *vs = nullptr;
-  cudaError_t e = sdb_radix_sort_u32(s->key_a, s->val_a, s->key_b, s->val_b, n, ls_bits(max_agents - 1u), s->hist, s->h_local,
+  cudaError_t e = sdb_radix_sort_u32(s->key_a, s->val_a, s->key_b, s->val_b, n, sdb_key_bits(max_agents - 1u), s->hist, s->h_local,
                                      s->h_tops, &ks, &vs, stream, &nl);
   LS_LAUNCH(n, k_lease_run_heads, ks, n, s->gran);
-  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, n, s->tot + 1, nullptr, stream);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, n, s->tot + 1, nullptr, stream, &nl);
   LS_LAUNCH(n, k_lease_run_begin, *s, n);
   LS_LAUNCH(n, k_lease_ring_check, *v, *s, ks, n);          // runs <= n: the slots past the run count read 0
-  if (e == cudaSuccess) e = sdb_scan_u32(s->kcnt, s->k_local, s->k_tops, n, s->tot + 2, nullptr, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(s->kflag, s->kf_local, s->kf_tops, n, s->tot + 3, nullptr, stream);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->kcnt, s->k_local, s->k_tops, n, s->tot + 2, nullptr, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->kflag, s->kf_local, s->kf_tops, n, s->tot + 3, nullptr, stream, &nl);
   LS_LAUNCH(n, k_lease_stage_list, *s, ks, vs, n, rs_agent, rs_count, rs_first);
-  nl += 6;
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
   return e == cudaSuccess ? cudaGetLastError() : e;
@@ -430,22 +404,21 @@ extern "C" cudaError_t sdb_launch_lease_stage(const sdb_lease_buf* b, const sdb_
   LS_LAUNCH(n, k_lease_seq_keys, *b, *s, n);
   const unsigned long long top = seq_end ? seq_end - 1ull : 0ull;
   uint32_t *ks = nullptr, *vs = nullptr;
-  cudaError_t e = sdb_radix_sort_u32(s->key_a, s->val_a, s->key_b, s->val_b, n, top >> 32 ? 32u : ls_bits(top), s->hist,
+  cudaError_t e = sdb_radix_sort_u32(s->key_a, s->val_a, s->key_b, s->val_b, n, top >> 32 ? 32u : sdb_key_bits(top), s->hist,
                                      s->h_local, s->h_tops, &ks, &vs, stream, &nl);
   if (e == cudaSuccess && (top >> 32)) {
     uint32_t* kh = ks == s->key_a ? s->key_b : s->key_a;
     uint32_t* vh = vs == s->val_a ? s->val_b : s->val_a;
     LS_LAUNCH(n, k_lease_seq_hi, *b, *s, vs, ks, n);          // the used keys are rewritten in place
-    e = sdb_radix_sort_u32(ks, vs, kh, vh, n, ls_bits(top >> 32), s->hist, s->h_local, s->h_tops, &ks, &vs, stream, &nl);
+    e = sdb_radix_sort_u32(ks, vs, kh, vh, n, sdb_key_bits(top >> 32), s->hist, s->h_local, s->h_tops, &ks, &vs, stream, &nl);
   }
   if (rows_used) cudaMemsetAsync(s->rfirst, 0xFF, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
   LS_LAUNCH(n, k_lease_row_first, *b, *s, vs, n);
   LS_LAUNCH(n, k_lease_row_heads, *b, *s, vs, n);
-  if (e == cudaSuccess) e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, n, s->tot + 6, nullptr, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, n, s->tot + 7, nullptr, stream);
-  nl += 4;
+  if (e == cudaSuccess) e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, n, s->tot + 6, nullptr, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, n, s->tot + 7, nullptr, stream, &nl);
   if (n) {
-    k_lease_stage_rows<<<ls_grid(n, 8, sm_count * 4), 256, 0, stream>>>(*b, *s, vs, n, cx->send_out, cx->payload_out);
+    k_lease_stage_rows<<<sdb_grid(n, 8, 32 * sm_count), 256, 0, stream>>>(*b, *s, vs, n, cx->send_out, cx->payload_out);
     ++nl;
   }
   LS_LAUNCH(n, k_lease_stage_entries, *b, *s, n, cx->entry_out);
@@ -469,13 +442,12 @@ extern "C" cudaError_t sdb_launch_lease_compact(const sdb_lease_buf* in, const s
   if (rows_used) cudaMemsetAsync(s->gran, 0, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
   LS_LAUNCH(used, k_lease_keep, *in, *s, used);
   LS_LAUNCH(rows_used, k_lease_keep_rows, *in, *s, rows_used);
-  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 8, nullptr, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, rows_used, s->tot + 9, nullptr, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(s->rg, s->rg_local, s->rg_tops, rows_used, s->tot + 10, nullptr, stream);
-  nl += (used ? 2 : 0) + (rows_used ? 4 : 0);
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 8, nullptr, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, rows_used, s->tot + 9, nullptr, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->rg, s->rg_local, s->rg_tops, rows_used, s->tot + 10, nullptr, stream, &nl);
   LS_LAUNCH(used, k_lease_copy_entries, *in, *out, *s, used);
   if (rows_used) {
-    k_lease_copy_rows<<<ls_grid(rows_used, 8, sm_count * 4), 256, 0, stream>>>(*in, *out, *s, rows_used);
+    k_lease_copy_rows<<<sdb_grid(rows_used, 8, 32 * sm_count), 256, 0, stream>>>(*in, *out, *s, rows_used);
     ++nl;
   }
   sdb_prof_end(prof, pi, stream);
@@ -615,7 +587,7 @@ k_lease_dl_keys(sdb_lease_buf b, uint32_t used, sdb_lease_scratch s, const uint3
                 uint32_t* __restrict__ staged, uint32_t* __restrict__ key, uint32_t* __restrict__ val) {
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= used || !s.flag[e]) return;
-  const uint32_t k = ls_scan(s.f_local, s.f_tops, e);
+  const uint32_t k = sdb_scan_at(s.f_local, s.f_tops, e);
   key[k] = dl_pos(pos, n_list, b.agent[e]); val[k] = k; staged[k] = e;
 }
 // sorted position p: its entry (send = output row), its count; a take marks the entry for the compaction to drop
@@ -655,7 +627,7 @@ extern "C" cudaError_t sdb_launch_ledger_insert(const sdb_dev_view* v, const sdb
   const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
   int nl = 0;
   if (runs) {
-    k_ledger_insert<<<ls_grid(runs, 8, sm_count * 4), 256, 0, stream>>>(*v, *b, *s, *L, rs_agent, rs_count, rs_first, runs, n0);
+    k_ledger_insert<<<sdb_grid(runs, 8, 32 * sm_count), 256, 0, stream>>>(*v, *b, *s, *L, rs_agent, rs_count, rs_first, runs, n0);
     ++nl;
   }
   sdb_prof_end(prof, pi, stream);
@@ -667,7 +639,7 @@ extern "C" cudaError_t sdb_launch_ledger_take(const sdb_lease_buf* b, const sdb_
                                               const unsigned long long* rx_totals, uint32_t used, uint64_t rec_cap,
                                               cudaStream_t stream, sdb_profiler* prof, int* n_launches, int sm_count) {
   const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
-  k_ledger_take<<<ls_grid(rec_cap, 256, sm_count * 4), 256, 0, stream>>>(*b, *L, cx->entry_out, rx_totals, used);
+  k_ledger_take<<<sdb_grid(rec_cap, 256, 32 * sm_count), 256, 0, stream>>>(*b, *L, cx->entry_out, rx_totals, used);
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += 1;
   return cudaGetLastError();
@@ -696,8 +668,7 @@ extern "C" cudaError_t sdb_launch_lease_dl_select(const sdb_lease_buf* b, const 
   const uint32_t* pos = agents ? d->pos : nullptr;
   if (agents) LS_LAUNCH(n_list, k_lease_dl_pos, agents, n_list, d->pos, 0u);
   LS_LAUNCH(used, k_lease_dl_flag, *b, used, pos, n_list, s->flag, d->cnt);
-  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream);
-  nl += 2;
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream, &nl);
   LS_LAUNCH(used, k_lease_dl_keys, *b, used, *s, pos, n_list, d->staged, d->key_a, d->val_a);
   if (agents) LS_LAUNCH(n_list, k_lease_dl_pos, agents, n_list, d->pos, 1u);
   sdb_prof_end(prof, pi, stream);
@@ -716,7 +687,7 @@ extern "C" cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf* b, const sd
   const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
   int nl = 0;
   uint32_t *ks = nullptr, *vs = nullptr;
-  cudaError_t e = sdb_radix_sort_u32(d->key_a, d->val_a, d->key_b, d->val_b, n, ls_bits(n_list ? n_list - 1u : 0u), d->hist,
+  cudaError_t e = sdb_radix_sort_u32(d->key_a, d->val_a, d->key_b, d->val_b, n, sdb_key_bits(n_list ? n_list - 1u : 0u), d->hist,
                                      d->h_local, d->h_tops, &ks, &vs, stream, &nl);
   uint32_t* dv = ks == d->key_a ? d->key_b : d->key_a;
   *deliveries_dev = dv;
@@ -725,11 +696,10 @@ extern "C" cudaError_t sdb_launch_lease_dl_emit(const sdb_lease_buf* b, const sd
   if (rows_used) cudaMemsetAsync(t.rfirst, 0xFF, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
   LS_LAUNCH(m, k_lease_row_first, *b, t, vs, m);
   LS_LAUNCH(m, k_lease_row_heads, *b, t, vs, m);
-  if (e == cudaSuccess) e = sdb_scan_u32(t.flag, t.f_local, t.f_tops, m, t.tot + 6, nullptr, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(t.gran, t.g_local, t.g_tops, m, t.tot + 7, nullptr, stream);
-  nl += 4;
+  if (e == cudaSuccess) e = sdb_scan_u32(t.flag, t.f_local, t.f_tops, m, t.tot + 6, nullptr, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(t.gran, t.g_local, t.g_tops, m, t.tot + 7, nullptr, stream, &nl);
   if (m) {
-    k_lease_stage_rows<<<ls_grid(m, 8, sm_count * 4), 256, 0, stream>>>(*b, t, vs, m, cx->send_out, cx->payload_out);
+    k_lease_stage_rows<<<sdb_grid(m, 8, 32 * sm_count), 256, 0, stream>>>(*b, t, vs, m, cx->send_out, cx->payload_out);
     ++nl;
   }
   LS_LAUNCH(m, k_lease_dl_emit, *b, t, vs, m, take, cx->entry_out, dv);
@@ -753,7 +723,7 @@ __global__ void __launch_bounds__(256)
 k_lease_x_list(sdb_lease_scratch s, uint32_t used, uint32_t m) {
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= used || !s.flag[e]) return;
-  const uint32_t p = ls_scan(s.f_local, s.f_tops, e);
+  const uint32_t p = sdb_scan_at(s.f_local, s.f_tops, e);
   if (p < m) { s.staged[p] = e; s.val_a[p] = p; }
 }
 // position p: its entry (send = output row) and its meta; the last position leaves the id to continue from in tot[8]
@@ -850,8 +820,7 @@ extern "C" cudaError_t sdb_launch_lease_x_select(const sdb_lease_buf* b, const s
   int nl = 0;
   cudaMemsetAsync(s->tot, 0, 16 * sizeof(unsigned long long), stream);
   LS_LAUNCH(used, k_lease_x_flag, *b, used, start_id, s->flag);
-  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream);
-  nl += used ? 2 : 0;
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, used, s->tot + 0, nullptr, stream, &nl);
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
   return e == cudaSuccess ? cudaGetLastError() : e;
@@ -868,11 +837,10 @@ extern "C" cudaError_t sdb_launch_lease_x_emit(const sdb_lease_buf* b, const sdb
   if (rows_used) cudaMemsetAsync(s->rfirst, 0xFF, static_cast<size_t>(rows_used) * sizeof(uint32_t), stream);
   LS_LAUNCH(m, k_lease_row_first, *b, *s, s->val_a, m);
   LS_LAUNCH(m, k_lease_row_heads, *b, *s, s->val_a, m);
-  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, m, s->tot + 6, nullptr, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, m, s->tot + 7, nullptr, stream);
-  nl += 4;
+  cudaError_t e = sdb_scan_u32(s->flag, s->f_local, s->f_tops, m, s->tot + 6, nullptr, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(s->gran, s->g_local, s->g_tops, m, s->tot + 7, nullptr, stream, &nl);
   if (m) {
-    k_lease_stage_rows<<<ls_grid(m, 8, sm_count * 4), 256, 0, stream>>>(*b, *s, s->val_a, m, cx->send_out, cx->payload_out);
+    k_lease_stage_rows<<<sdb_grid(m, 8, 32 * sm_count), 256, 0, stream>>>(*b, *s, s->val_a, m, cx->send_out, cx->payload_out);
     ++nl;
   }
   LS_LAUNCH(m, k_lease_x_emit, *b, *s, m, cx->entry_out, meta_out);
@@ -890,9 +858,9 @@ extern "C" cudaError_t sdb_launch_lease_import_check(const sdb_lease_scratch* s,
   cudaMemsetAsync(s->tot, 0, sizeof(unsigned long long), stream);
   const uint32_t items = n > n_sends ? n : n_sends;
   if (items) {
-    k_lease_import_check<<<ls_grid(items, 256, sm_count * 4), 256, 0, stream>>>(cx->entry_out, meta, cx->send_out, n, n_sends,
-                                                                               payload_bytes, max_agents, max_payload, policy,
-                                                                               s->tot);
+    k_lease_import_check<<<sdb_grid(items, 256, 32 * sm_count), 256, 0, stream>>>(cx->entry_out, meta, cx->send_out, n, n_sends,
+                                                                                 payload_bytes, max_agents, max_payload, policy,
+                                                                                 s->tot);
     if (n_launches) *n_launches += 1;
   }
   sdb_prof_end(prof, pi, stream);
@@ -908,8 +876,8 @@ extern "C" cudaError_t sdb_launch_lease_import_write(const sdb_lease_buf* b, con
   int nl = 0;
   LS_LAUNCH(n, k_lease_import_meta, *b, meta, n, used, id_base);
   if (items) {
-    k_lease_append_copy<<<ls_grid(items, 256, sm_count * 4), 256, 0, stream>>>(*b, cx->entry_out, cx->send_out, cx->payload_out,
-                                                                               totals, cx->totals, used, rows_used, pay_used);
+    k_lease_append_copy<<<sdb_grid(items, 256, 32 * sm_count), 256, 0, stream>>>(*b, cx->entry_out, cx->send_out, cx->payload_out,
+                                                                                 totals, cx->totals, used, rows_used, pay_used);
     ++nl;
   }
   sdb_prof_end(prof, pi, stream);
@@ -924,7 +892,7 @@ extern "C" cudaError_t sdb_launch_ledger_import(const sdb_dev_view* v, const sdb
   const int pi = sdb_prof_begin(prof, SDB_PK_LEASE, stream);
   cudaMemsetAsync(tot, 0, sizeof(unsigned long long), stream);
   if (n) {
-    k_ledger_import<<<ls_grid(n, 8, sm_count * 4), 256, 0, stream>>>(*v, *L, n, n0, tot);
+    k_ledger_import<<<sdb_grid(n, 8, 32 * sm_count), 256, 0, stream>>>(*v, *L, n, n0, tot);
     if (n_launches) *n_launches += 1;
   }
   sdb_prof_end(prof, pi, stream);

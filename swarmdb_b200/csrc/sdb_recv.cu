@@ -12,7 +12,7 @@
 // Priority order (extension, SURVEY App. A rule 9) keeps the multi-kernel pipeline (all stream-ordered, no host
 // round trip inside):
 //   k_recv_count    cnt[q]   = min(max_messages, live(agent q))
-//   scan            rec_off  = exclusive scan of cnt             (k_scan_local + k_scan_tops)
+//   scan            rec_off  = exclusive scan of cnt             (sdb_scan_u32: k_scan_local + k_scan_tops)
 //   k_recv_select   per agent: choose WHICH pending entries are delivered, write the per-record
 //                   plan (arena handle, payload size) at the record's output index, retire them
 //                     stream order      -> the first cnt live entries (contiguous when the
@@ -32,7 +32,6 @@
 #include <cstdlib>
 #include "sdb_common.cuh"
 
-#define SDB_SCAN_TILE 4096u   // elements per scan block (1024 threads x 4)
 #define SDB_MODE_LIST 0x80000000u
 
 
@@ -40,36 +39,12 @@
 // generic exclusive scan over uint32 (two tiny kernels; consumers add tops[i / TILE])
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024)
-k_scan_local(const uint32_t* __restrict__ in, uint32_t mask, uint32_t* __restrict__ local,
-             uint32_t* __restrict__ tops, uint32_t n) {
-  __shared__ uint32_t s_warp[32];
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t base = blockIdx.x * SDB_SCAN_TILE + tid * 4u;
+k_scan_local(const uint32_t* __restrict__ in, uint32_t* __restrict__ local, uint32_t* __restrict__ tops, uint32_t n) {
+  const uint32_t base = blockIdx.x * SDB_SCAN_TILE + threadIdx.x * 4u;
   uint32_t x[4];
 #pragma unroll
-  for (int k = 0; k < 4; ++k) x[k] = (base + k < n) ? (in[base + k] & mask) : 0u;
-  uint32_t tsum = x[0] + x[1] + x[2] + x[3];
-  uint32_t incl = tsum;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-    if (lane >= o) incl += y;
-  }
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    uint32_t w = s_warp[lane];
-    uint32_t wi = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      uint32_t y = __shfl_up_sync(0xFFFFFFFFu, wi, o);
-      if (lane >= o) wi += y;
-    }
-    s_warp[lane] = wi - w;              // exclusive warp offsets
-    if (lane == 31) tops[blockIdx.x] = wi;
-  }
-  __syncthreads();
-  uint32_t run = s_warp[warp] + incl - tsum;
+  for (int k = 0; k < 4; ++k) x[k] = (base + k < n) ? in[base + k] : 0u;
+  uint32_t run = sdb_block_scan_tile(x, tops + blockIdx.x);
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     if (base + k < n) local[base + k] = run;
@@ -88,22 +63,12 @@ k_scan_tops(uint32_t* __restrict__ tops, uint32_t n_tiles, unsigned long long* _
   for (uint32_t base = 0; base < n_tiles; base += 1024) {
     const uint32_t i = base + tid;
     const uint32_t x = i < n_tiles ? tops[i] : 0u;
-    uint32_t incl = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-      if (lane >= o) incl += y;
-    }
+    const uint32_t incl = sdb_warp_incl_scan(x, lane);
     if (lane == 31) s_warp[warp] = incl;
     __syncthreads();
     if (warp == 0) {
-      uint32_t w = s_warp[lane], wi = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        uint32_t y = __shfl_up_sync(0xFFFFFFFFu, wi, o);
-        if (lane >= o) wi += y;
-      }
-      s_warp[lane] = wi - w;
+      const uint32_t w = s_warp[lane];
+      s_warp[lane] = sdb_warp_incl_scan(w, lane) - w;
     }
     __syncthreads();
     const uint32_t carry = s_carry;
@@ -120,18 +85,20 @@ k_scan_tops(uint32_t* __restrict__ tops, uint32_t n_tiles, unsigned long long* _
 __global__ void __launch_bounds__(256)
 k_scan_apply(const uint32_t* __restrict__ local, const uint32_t* __restrict__ tops, uint32_t* __restrict__ out, uint32_t n) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = local[i] + tops[i / SDB_SCAN_TILE];
+  if (i < n) out[i] = sdb_scan_at(local, tops, i);
 }
 
 // exclusive scan of n uint32 (block-local part in `local`, per-block part in `tops`), optional
-// grand total and optional materialised output; usable from the other translation units
+// grand total and optional materialised output; usable from the other translation units.  Adds its launches to
+// *n_launches (when given).
 extern "C" cudaError_t sdb_scan_u32(const uint32_t* in, uint32_t* local, uint32_t* tops, uint32_t n,
-                                    unsigned long long* total_out, uint32_t* out, cudaStream_t stream) {
+                                    unsigned long long* total_out, uint32_t* out, cudaStream_t stream, int* n_launches) {
   if (n == 0) return cudaSuccess;
   const uint32_t tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
-  k_scan_local<<<tiles, 1024, 0, stream>>>(in, 0xFFFFFFFFu, local, tops, n);
+  k_scan_local<<<tiles, 1024, 0, stream>>>(in, local, tops, n);
   k_scan_tops<<<1, 1024, 0, stream>>>(tops, tiles, total_out);
   if (out) k_scan_apply<<<(n + 255) / 256, 256, 0, stream>>>(local, tops, out, n);
+  if (n_launches) *n_launches += out ? 3 : 2;
   return cudaGetLastError();
 }
 
@@ -293,7 +260,7 @@ k_recv_select(sdb_dev_view v, sdb_recv_args r) {
   if (valid) {
     a = r.agent_idx ? r.agent_idx[q] : q;
     cnt = r.cnt[q];
-    roff = r.rec_local[q] + r.rec_tops[q / SDB_SCAN_TILE];
+    roff = sdb_scan_at(r.rec_local, r.rec_tops, q);
     if (cnt && static_cast<uint64_t>(roff) + cnt > r.rec_cap) {      // does not fit: stays queued ...
       if (roff == 0) cnt = static_cast<uint32_t>(r.rec_cap);          // ... unless first in the output: its first rec_cap records
       else cnt = 0;
@@ -418,7 +385,7 @@ k_recv_select_big(sdb_dev_view v, sdb_recv_args r) {
     const uint32_t q = r.big_list[w];
     const uint32_t a = r.agent_idx ? r.agent_idx[q] : q;
     const uint32_t cnt = r.count_out[q];
-    const uint32_t roff = r.rec_local[q] + r.rec_tops[q / SDB_SCAN_TILE];
+    const uint32_t roff = sdb_scan_at(r.rec_local, r.rec_tops, q);
     const uint4 hd = *reinterpret_cast<const uint4*>(v.ring_hdr + a);
     const uint32_t H = hd.x, T = hd.y, NT = hd.w;
     if (cnt <= SDB_CAND && (prio_mode || NT != 0))
@@ -433,36 +400,13 @@ k_recv_select_big(sdb_dev_view v, sdb_recv_args r) {
 // stored back into plan[].y and the per-tile totals into `tops`.  The element count lives on the device (totals[0]).
 __global__ void __launch_bounds__(1024)
 k_scan_plan(uint4* __restrict__ plan, uint32_t* __restrict__ tops, const unsigned long long* __restrict__ n_dev) {
-  __shared__ uint32_t s_warp[32];
   const uint32_t n = static_cast<uint32_t>(*n_dev);
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const uint32_t base = blockIdx.x * SDB_SCAN_TILE + tid * 4u;
-  if (blockIdx.x * SDB_SCAN_TILE >= n) { if (tid == 0) tops[blockIdx.x] = 0; return; }
+  const uint32_t base = blockIdx.x * SDB_SCAN_TILE + threadIdx.x * 4u;
+  if (blockIdx.x * SDB_SCAN_TILE >= n) { if (threadIdx.x == 0) tops[blockIdx.x] = 0; return; }
   uint32_t x[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) x[k] = (base + k < n) ? (plan[base + k].z & 0xFFFFu) : 0u;
-  const uint32_t tsum = x[0] + x[1] + x[2] + x[3];
-  uint32_t incl = tsum;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-    if (lane >= o) incl += y;
-  }
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    const uint32_t w = s_warp[lane];
-    uint32_t wi = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, wi, o);
-      if (lane >= o) wi += y;
-    }
-    s_warp[lane] = wi - w;
-    if (lane == 31) tops[blockIdx.x] = wi;
-  }
-  __syncthreads();
-  uint32_t run = s_warp[warp] + incl - tsum;
+  uint32_t run = sdb_block_scan_tile(x, tops + blockIdx.x);
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     if (base + k < n) plan[base + k].y = run;
@@ -508,9 +452,7 @@ __device__ __forceinline__ uint32_t fill_offsets_warp(uint4* plan, uint32_t RO, 
   for (uint32_t j0 = 0; j0 < C; j0 += 32) {
     const uint32_t j = j0 + lane;
     const uint32_t g = j < C ? (plan[RO + j].z & 0xFFFFu) : 0u;
-    uint32_t incl = g;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= o) incl += y; }
+    const uint32_t incl = sdb_warp_incl_scan(g, lane);
     if (j < C) plan[RO + j].y = run + incl - g;
     run += __shfl_sync(0xFFFFFFFFu, incl, 31);
   }
@@ -624,9 +566,7 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
   // (per-thread 16-byte stores to scattered places would make the L2 fetch every sector before merging it)
   {
     const uint32_t mycnt = (cnt && simple) ? cnt : 0u;
-    uint32_t winc = mycnt;                                                      // inclusive scan over the warp
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, winc, o); if (lane >= o) winc += y; }
+    const uint32_t winc = sdb_warp_incl_scan(mycnt, lane);                     // inclusive scan over the warp
     const uint32_t wtotal = __shfl_sync(0xFFFFFFFFu, winc, 31);
     // the warp's simple records are NOT contiguous in the plan when it also holds holey or truncated agents; they are
     // contiguous per agent, so stage (destination, entry) pairs: destination index travels in a side array
@@ -945,7 +885,7 @@ k_compact_emit(sdb_dev_view v, sdb_recv_args r, sdb_compact_args c) {
     if (l8 == 0) {
       const uint8_t* src = v.arena + ((static_cast<uint64_t>(pe.x) & v.gmask) << 5);
       const uint4 lo = sdb_ld_stream(src), hi = sdb_ld_stream(src + 16);    // {seq, timestamp}, {sender, receiver, group, len|prio|type}
-      const uint32_t row = c.head_local[own] + c.head_tops[own / SDB_SCAN_TILE];
+      const uint32_t row = sdb_scan_at(c.head_local, c.head_tops, own);
       sdb_st_stream(c.entry_out + rec, make_uint4(lo.x, lo.y, row, hi.y));
       if (head) {
         uint4* dst = reinterpret_cast<uint4*>(c.send_out + row);
@@ -969,22 +909,17 @@ static cudaError_t launch_compact(const sdb_dev_view* v, const sdb_recv_args* r,
   uint32_t tbits = 10;                                         // at least twice as many slots as records: load <= 1/2
   while ((1ull << tbits) < 2 * bound) ++tbits;
   c.tbits = tbits;
-  const uint32_t n = static_cast<uint32_t>(bound), tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
-  uint64_t grid = (bound + 255) / 256;
-  const uint64_t cap = static_cast<uint64_t>(sm_count) * 8;
+  const uint32_t n = static_cast<uint32_t>(bound);
   const int pi = sdb_prof_begin(prof, SDB_PK_RECV_COMPACT, stream);
   cudaMemsetAsync(c.table, 0xFF, (1ull << tbits) * sizeof(unsigned long long), stream);
-  k_compact_owner<<<static_cast<uint32_t>(grid < cap ? grid : cap), 256, 0, stream>>>(*r, packed_inv, c);
-  k_compact_heads<<<static_cast<uint32_t>(grid), 256, 0, stream>>>(*r, c, n);
-  k_scan_local<<<tiles, 1024, 0, stream>>>(c.head, 0xFFFFFFFFu, c.head_local, c.head_tops, n);
-  k_scan_tops<<<1, 1024, 0, stream>>>(c.head_tops, tiles, c.totals);
-  k_scan_local<<<tiles, 1024, 0, stream>>>(c.gran, 0xFFFFFFFFu, c.gran_local, c.gran_tops, n);
-  k_scan_tops<<<1, 1024, 0, stream>>>(c.gran_tops, tiles, c.totals + 1);
-  const uint64_t ewarps = (bound + 3) / 4, eblocks = (ewarps + 7) / 8, ecap = static_cast<uint64_t>(sm_count) * 8 * 4;
-  k_compact_emit<<<static_cast<uint32_t>(eblocks < ecap ? eblocks : ecap), 256, 0, stream>>>(*v, *r, c);
+  k_compact_owner<<<sdb_grid(bound, 256, 8 * sm_count), 256, 0, stream>>>(*r, packed_inv, c);
+  k_compact_heads<<<static_cast<uint32_t>((bound + 255) / 256), 256, 0, stream>>>(*r, c, n);
+  cudaError_t e = sdb_scan_u32(c.head, c.head_local, c.head_tops, n, c.totals, nullptr, stream, n_launches);
+  if (e == cudaSuccess) e = sdb_scan_u32(c.gran, c.gran_local, c.gran_tops, n, c.totals + 1, nullptr, stream, n_launches);
+  k_compact_emit<<<sdb_grid(bound, 32, 32 * sm_count), 256, 0, stream>>>(*v, *r, c);   // 4 records per warp, 8 warps per block
   sdb_prof_end(prof, pi, stream);
-  if (n_launches) *n_launches += 7;
-  return cudaGetLastError();
+  if (n_launches) *n_launches += 3;
+  return e == cudaSuccess ? cudaGetLastError() : e;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1094,9 +1029,7 @@ k_recv_small(sdb_dev_view v, sdb_small_agents ag, uint32_t n, uint32_t max_messa
     for (uint32_t r0 = 0; r0 < total; r0 += 32) {
       const uint32_t r = r0 + lane;
       const uint32_t g = r < total ? (plan[r].z & 0xFFFFu) + 1u : 0u;
-      uint32_t incl = g;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= o) incl += y; }
+      const uint32_t incl = sdb_warp_incl_scan(g, lane);
       if (r < total) s_goff[r] = run + incl - g;
       run += __shfl_sync(0xFFFFFFFFu, incl, 31);
     }
@@ -1170,9 +1103,7 @@ k_latency_server(sdb_dev_view v, sdb_ls_mailbox* mb, uint8_t* out, uint32_t out_
         uint2 e = make_uint2(0u, 1u);
         if (lane < c) e = __ldcv(sdb_ring_of(v, a) + ((head + lane) & (v.ring_slots - 1)));
         const uint32_t g = lane < c ? (sdb_meta(e) & SDB_META_GLEN_MASK) : 0u;       // granules incl. the header
-        uint32_t incl = g;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= o) incl += y; }
+        const uint32_t incl = sdb_warp_incl_scan(g, lane);
         if (lane < c) { s_goff[lane] = incl - g; s_fast[lane] = make_uint2(e.x, (g - 1u) | (e.y & 0xFFFF0000u)); }
         if (lane == c - 1) s_goff[c] = incl;
         if (lane == 0) {
@@ -1197,9 +1128,7 @@ k_latency_server(sdb_dev_view v, sdb_ls_mailbox* mb, uint8_t* out, uint32_t out_
       for (uint32_t r0 = 0; r0 < cnt; r0 += 32) {
         const uint32_t r = r0 + lane;
         const uint32_t g = r < cnt ? (plan[r].z & 0xFFFFu) + 1u : 0u;
-        uint32_t incl = g;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= o) incl += y; }
+        const uint32_t incl = sdb_warp_incl_scan(g, lane);
         if (r < cnt) s_goff[r] = run + incl - g;
         run += __shfl_sync(0xFFFFFFFFu, incl, 31);
       }
@@ -1282,12 +1211,8 @@ static cudaError_t launch_gather(const sdb_dev_view* v, const sdb_recv_args* r, 
     if (use_cpa) k_recv_gather_cpa<WARPS><<<static_cast<uint32_t>(grid), WARPS * 32, smem, stream>>>(*v, *r, packed_inv, slot);
     else k_recv_gather_tma<WARPS><<<static_cast<uint32_t>(grid), WARPS * 32, smem, stream>>>(*v, *r, packed_inv, slot);
   } else {
-    uint64_t gwarps = (bound + 3) / 4;
-    uint64_t gblocks = (gwarps + 7) / 8;
-    const uint64_t cap = static_cast<uint64_t>(sm_count) * 8 * 4;                // grid-stride beyond ~4 waves
-    if (gblocks > cap) gblocks = cap;
-    if (gblocks == 0) gblocks = 1;
-    k_recv_gather<<<static_cast<uint32_t>(gblocks), 256, 0, stream>>>(*v, *r, packed_inv);
+    // 4 records per warp, 8 warps per block; grid-stride beyond ~4 waves
+    k_recv_gather<<<sdb_grid(bound, 32, 32 * sm_count), 256, 0, stream>>>(*v, *r, packed_inv);
   }
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += 1;
@@ -1325,13 +1250,12 @@ extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_
     if (ca) return launch_compact(v, r, ca, r->lb + sdb_lb_words(tiles) - 1, bound, sm_count, stream, prof, n_launches);
     return launch_gather(v, r, r->lb + sdb_lb_words(tiles) - 1, bound, max_rec_bytes, sm_count, stream, prof, n_launches);
   }
-  const uint32_t tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
   pi = sdb_prof_begin(prof, SDB_PK_RECV_COUNT, stream);
   k_recv_count<<<(n + 255) / 256, 256, 0, stream>>>(*v, *r);
   sdb_prof_end(prof, pi, stream);
   pi = sdb_prof_begin(prof, SDB_PK_RECV_SCAN, stream);
-  k_scan_local<<<tiles, 1024, 0, stream>>>(r->cnt, 0xFFFFFFFFu, r->rec_local, r->rec_tops, n);
-  k_scan_tops<<<1, 1024, 0, stream>>>(r->rec_tops, tiles, r->totals);          // totals[0] = records requested
+  // totals[0] = records requested
+  const cudaError_t e = sdb_scan_u32(r->cnt, r->rec_local, r->rec_tops, n, r->totals, nullptr, stream, n_launches);
   sdb_prof_end(prof, pi, stream);
   pi = sdb_prof_begin(prof, SDB_PK_RECV_SELECT, stream);
   cudaMemsetAsync(r->big_count, 0, sizeof(uint32_t), stream);
@@ -1348,7 +1272,8 @@ extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_
   k_scan_plan<<<rtiles, 1024, 0, stream>>>(r->plan, r->plan_tops, r->totals);
   k_scan_tops<<<1, 1024, 0, stream>>>(r->plan_tops, rtiles, r->totals + 1);    // totals[1] = payload granules
   sdb_prof_end(prof, pi, stream);
-  if (n_launches) *n_launches += 7;
+  if (n_launches) *n_launches += 5;
+  if (e != cudaSuccess) return e;
   if (ca) return launch_compact(v, r, ca, nullptr, bound, sm_count, stream, prof, n_launches);
   return launch_gather(v, r, nullptr, bound, max_rec_bytes, sm_count, stream, prof, n_launches);
 }
@@ -1392,7 +1317,7 @@ k_expire(sdb_dev_view v, sdb_recv_args r, double older_than, uint32_t all) {
     uint32_t limit = 0xFFFFFFFFu, RO = 0;
     if (MODE == SDB_EXP_SELECT && valid) {
       uint32_t c = r.cnt[q];
-      RO = r.rec_local[q] + r.rec_tops[q / SDB_SCAN_TILE];
+      RO = sdb_scan_at(r.rec_local, r.rec_tops, q);
       if (c && static_cast<uint64_t>(RO) + c > r.rec_cap) {     // does not fit: stays queued ...
         c = RO == 0 ? static_cast<uint32_t>(r.rec_cap) : 0u;    // ... unless first in the output: its first rec_cap matches
         if (l8 == 0) atomicMin(r.totals, static_cast<unsigned long long>(RO) + c);
@@ -1460,24 +1385,22 @@ extern "C" cudaError_t sdb_launch_expire(const sdb_dev_view* v, const sdb_recv_a
                                          int sm_count) {
   if (r->n == 0) return cudaSuccess;
   const uint32_t n = r->n;
-  uint64_t blocks = (static_cast<uint64_t>(n) + 31) / 32;                    // 4 slots per warp, 8 warps per block
-  const uint64_t bcap = static_cast<uint64_t>(sm_count) * 8 * 4;             // grid-stride beyond ~4 waves
-  if (blocks > bcap) blocks = bcap;
+  const uint32_t blocks = sdb_grid(n, 32, 32 * sm_count);                    // 4 slots per warp, 8 warps per block
   const int pi = sdb_prof_begin(prof, SDB_PK_EXPIRE, stream);
   if (!ca) {
     cudaMemsetAsync(r->totals, 0, sizeof(unsigned long long), stream);
-    k_expire<SDB_EXP_DROP><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, older_than, all);
+    k_expire<SDB_EXP_DROP><<<blocks, 256, 0, stream>>>(*v, *r, older_than, all);
     sdb_prof_end(prof, pi, stream);
     if (n_launches) *n_launches += 1;
     return cudaGetLastError();
   }
-  const uint32_t tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
-  k_expire<SDB_EXP_COUNT><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, older_than, all);
-  k_scan_local<<<tiles, 1024, 0, stream>>>(r->cnt, 0xFFFFFFFFu, r->rec_local, r->rec_tops, n);
-  k_scan_tops<<<1, 1024, 0, stream>>>(r->rec_tops, tiles, r->totals);       // totals[0] = matches; the cut may lower it
-  k_expire<SDB_EXP_SELECT><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, older_than, all);
+  k_expire<SDB_EXP_COUNT><<<blocks, 256, 0, stream>>>(*v, *r, older_than, all);
+  // totals[0] = matches; the cut may lower it
+  const cudaError_t e = sdb_scan_u32(r->cnt, r->rec_local, r->rec_tops, n, r->totals, nullptr, stream, n_launches);
+  k_expire<SDB_EXP_SELECT><<<blocks, 256, 0, stream>>>(*v, *r, older_than, all);
   sdb_prof_end(prof, pi, stream);
-  if (n_launches) *n_launches += 4;
+  if (n_launches) *n_launches += 2;
+  if (e != cudaSuccess) return e;
   uint64_t bound = static_cast<uint64_t>(n) * v->ring_slots;               // upper bound on the records planned
   if (bound > r->rec_cap) bound = r->rec_cap;
   return launch_compact(v, r, ca, nullptr, bound, sm_count, stream, prof, n_launches);
@@ -1491,7 +1414,7 @@ extern "C" cudaError_t sdb_launch_expire(const sdb_dev_view* v, const sdb_recv_a
 //   k_where_kw      with a keyword: one warp per request slot, a lane per entry for the header clauses, then every
 //                   record that passes gets a warp-cooperative substring search of its content bytes
 //   both            write the verdict words and cnt[q] = min(matches, max_messages)
-//   scan            k_scan_local / k_scan_tops over cnt (take mode)
+//   scan            sdb_scan_u32 over cnt (take mode)
 //   k_where_select  capacity cut of k_recv_select, then the first count_out[q] set bits in delivery order (priority
 //                   order: one walk per level 3..0 over the entries' meta) are planned {handle, -, plan z, slot} and
 //                   tombstoned; head / ntomb by select_agent_warp's rule, the ring header stored at most once.  Take
@@ -1674,7 +1597,7 @@ k_where_select(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
       a = r.agent_idx ? r.agent_idx[q] : q;
       c = r.cnt[q];
       if (PLAN) {
-        RO = r.rec_local[q] + r.rec_tops[q / SDB_SCAN_TILE];
+        RO = sdb_scan_at(r.rec_local, r.rec_tops, q);
         if (c && static_cast<uint64_t>(RO) + c > r.rec_cap) {   // does not fit: stays queued ...
           c = RO == 0 ? static_cast<uint32_t>(r.rec_cap) : 0u;  // ... unless first in the output: its first rec_cap matches
           if (l8 == 0) atomicMin(r.totals, static_cast<unsigned long long>(RO) + c);
@@ -1756,36 +1679,31 @@ extern "C" cudaError_t sdb_launch_where(const sdb_dev_view* v, const sdb_recv_ar
                                         int sm_count) {
   if (r->n == 0) return cudaSuccess;
   const uint32_t n = r->n;
-  uint64_t blocks = (static_cast<uint64_t>(n) + 31) / 32;                    // 4 slots per warp, 8 warps per block
-  const uint64_t bcap = static_cast<uint64_t>(sm_count) * 8 * 4;             // grid-stride beyond ~4 waves
-  if (blocks > bcap) blocks = bcap;
+  const uint32_t blocks = sdb_grid(n, 32, 32 * sm_count);                    // 4 slots per warp, 8 warps per block
   const int pi = sdb_prof_begin(prof, SDB_PK_WHERE, stream);
   if (f->fields & SDB_FILTER_KEYWORD) {
-    uint64_t kb = (static_cast<uint64_t>(n) + 7) / 8;                        // a warp per slot, 8 warps per block
-    const uint64_t kcap = static_cast<uint64_t>(sm_count) * 8;
-    if (kb > kcap) kb = kcap;
-    k_where_kw<<<static_cast<uint32_t>(kb), 256, 0, stream>>>(*v, *r, *f);
+    k_where_kw<<<sdb_grid(n, 8, 8 * sm_count), 256, 0, stream>>>(*v, *r, *f);   // a warp per slot, 8 warps per block
   } else {
-    k_where_eval<<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, *f);
+    k_where_eval<<<blocks, 256, 0, stream>>>(*v, *r, *f);
   }
   if (drop) {
     cudaMemsetAsync(r->totals, 0, 2 * sizeof(unsigned long long), stream);
-    k_where_select<false><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, *f);
+    k_where_select<false><<<blocks, 256, 0, stream>>>(*v, *r, *f);
     sdb_prof_end(prof, pi, stream);
     if (n_launches) *n_launches += 2;
     return cudaGetLastError();
   }
-  const uint32_t tiles = (n + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE;
-  k_scan_local<<<tiles, 1024, 0, stream>>>(r->cnt, 0xFFFFFFFFu, r->rec_local, r->rec_tops, n);
-  k_scan_tops<<<1, 1024, 0, stream>>>(r->rec_tops, tiles, r->totals);       // totals[0] = matches; the cut may lower it
-  k_where_select<true><<<static_cast<uint32_t>(blocks), 256, 0, stream>>>(*v, *r, *f);
+  // totals[0] = matches; the cut may lower it
+  const cudaError_t e = sdb_scan_u32(r->cnt, r->rec_local, r->rec_tops, n, r->totals, nullptr, stream, n_launches);
+  k_where_select<true><<<blocks, 256, 0, stream>>>(*v, *r, *f);
   uint64_t bound = static_cast<uint64_t>(n) * (r->max_messages < v->ring_slots ? r->max_messages : v->ring_slots);   // records planned, at most
   if (bound > r->rec_cap) bound = r->rec_cap;
   const uint32_t rtiles = static_cast<uint32_t>((bound + SDB_SCAN_TILE - 1) / SDB_SCAN_TILE);
   k_scan_plan<<<rtiles, 1024, 0, stream>>>(r->plan, r->plan_tops, r->totals);
   k_scan_tops<<<1, 1024, 0, stream>>>(r->plan_tops, rtiles, r->totals + 1);  // totals[1] = payload granules
   sdb_prof_end(prof, pi, stream);
-  if (n_launches) *n_launches += 6;
+  if (n_launches) *n_launches += 4;
+  if (e != cudaSuccess) return e;
   return launch_gather(v, r, nullptr, bound, max_rec_bytes, sm_count, stream, prof, n_launches);
 }
 

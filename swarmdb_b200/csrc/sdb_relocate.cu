@@ -24,11 +24,7 @@
 // Every kernel is timed under SDB_PK_ARENA_FLOOR.
 #include "sdb_common.cuh"
 
-#define SDB_SCAN_TILE 4096u
 #define SDB_RL_G 8u            // lanes per agent
-
-extern "C" cudaError_t sdb_scan_u32(const uint32_t* in, uint32_t* local, uint32_t* tops, uint32_t n,
-                                    unsigned long long* total_out, uint32_t* out, cudaStream_t stream);
 
 // arena position of a 32-bit ring handle: handles are positions mod 2^32 and every pending one lies below the tail
 __device__ __forceinline__ unsigned long long rl_pos(const sdb_reloc_args& r, uint32_t handle) {
@@ -47,7 +43,7 @@ __device__ __forceinline__ void rl_mark_run(const sdb_reloc_args& r, unsigned lo
 __device__ __forceinline__ uint32_t rl_rank(const sdb_reloc_args& r, unsigned long long pos) {
   const unsigned long long k = pos - r.lo;
   const uint32_t w = static_cast<uint32_t>(k >> 5);
-  return r.pre[w] + r.tops[w / SDB_SCAN_TILE] + __popc(r.bits[w] & ((1u << (k & 31u)) - 1u));
+  return sdb_scan_at(r.pre, r.tops, w) + __popc(r.bits[w] & ((1u << (k & 31u)) - 1u));
 }
 __device__ __forceinline__ bool rl_selected(const sdb_reloc_args& r, uint32_t a) { return (r.sel[a >> 5] >> (a & 31u)) & 1u; }
 
@@ -129,7 +125,7 @@ k_reloc_copy(sdb_dev_view v, sdb_reloc_args r) {
   for (uint32_t w = gw; w < r.words; w += nw) {                         // warp-uniform
     const uint32_t m = r.bits[w];
     if (!m) continue;
-    const uint32_t r0 = r.pre[w] + r.tops[w / SDB_SCAN_TILE];
+    const uint32_t r0 = sdb_scan_at(r.pre, r.tops, w);
     const unsigned long long p0 = r.lo + (static_cast<unsigned long long>(w) << 5);
 #pragma unroll
     for (uint32_t c = lane; c < 64u; c += 32u) {                         // 16-byte chunk c of granule c / 2
@@ -180,13 +176,6 @@ k_reloc_ring(sdb_dev_view v, sdb_reloc_args r) {
   }
 }
 
-static uint32_t rl_grid(uint64_t items, uint64_t per_block, int sm_count) {
-  uint64_t g = (items + per_block - 1) / per_block;
-  const uint64_t cap = static_cast<uint64_t>(sm_count) * 8 * 4;
-  if (g > cap) g = cap;
-  return static_cast<uint32_t>(g ? g : 1);
-}
-
 // plan phase: r->tot ends with the totals the host reads (tot[0] = marked granules)
 extern "C" cudaError_t sdb_launch_reloc_plan(const sdb_dev_view* v, const sdb_reloc_args* r, cudaStream_t stream, sdb_profiler* prof,
                                              int* n_launches, int sm_count) {
@@ -198,12 +187,12 @@ extern "C" cudaError_t sdb_launch_reloc_plan(const sdb_dev_view* v, const sdb_re
   int nl = 0;
   if (e == cudaSuccess) {
     if (r->n_agents) {
-      k_reloc_mark<<<rl_grid(r->n_agents, 32, sm_count), 256, 0, stream>>>(*v, *r);
+      k_reloc_mark<<<sdb_grid(r->n_agents, 32, 32 * sm_count), 256, 0, stream>>>(*v, *r);
       ++nl;
     }
     k_reloc_count<<<(r->words + 255) / 256, 256, 0, stream>>>(*r);
-    e = sdb_scan_u32(r->cnt, r->pre, r->tops, r->words, r->tot, nullptr, stream);
-    nl += 3;
+    ++nl;
+    e = sdb_scan_u32(r->cnt, r->pre, r->tops, r->words, r->tot, nullptr, stream, &nl);
   }
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
@@ -216,10 +205,10 @@ extern "C" cudaError_t sdb_launch_reloc_write(const sdb_dev_view* v, const sdb_r
                                               int sm_count) {
   const int pi = sdb_prof_begin(prof, SDB_PK_ARENA_FLOOR, stream);
   int nl = 0;
-  k_reloc_copy<<<rl_grid(r->words, 8, sm_count), 256, 0, stream>>>(*v, *r);
+  k_reloc_copy<<<sdb_grid(r->words, 8, 32 * sm_count), 256, 0, stream>>>(*v, *r);
   ++nl;
   if (ledger && n_ledger) { k_reloc_ledger<<<(n_ledger + 255) / 256, 256, 0, stream>>>(*v, *ledger, n_ledger, *r); ++nl; }
-  if (r->n_agents) { k_reloc_ring<<<rl_grid(r->n_agents, 32, sm_count), 256, 0, stream>>>(*v, *r); ++nl; }
+  if (r->n_agents) { k_reloc_ring<<<sdb_grid(r->n_agents, 32, 32 * sm_count), 256, 0, stream>>>(*v, *r); ++nl; }
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
   return cudaGetLastError();

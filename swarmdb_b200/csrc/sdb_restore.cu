@@ -21,17 +21,10 @@
 //   k_restore_ring      8 lanes per agent: private images, ring entries in order, tail = ctail
 #include "sdb_common.cuh"
 
-#define SDB_SCAN_TILE 4096u
 #define SDB_RS_G 8u            // lanes per agent
 #define SDB_RS_HDRS 65535u     // headers per payload copy (dm1 = headers - 1 - j must fit 16 bits)
 
-extern "C" cudaError_t sdb_scan_u32(const uint32_t* in, uint32_t* local, uint32_t* tops, uint32_t n,
-                                    unsigned long long* total_out, uint32_t* out, cudaStream_t stream);
-
 __device__ __forceinline__ uint32_t rs_pg(uint32_t len) { return ((len + 31u) & ~31u) >> 5; }   // payload granules
-__device__ __forceinline__ uint32_t rs_scan(const uint32_t* local, const uint32_t* tops, uint32_t i) {
-  return local[i] + tops[i / SDB_SCAN_TILE];
-}
 // row i: {timestamp, payload_off}, {sender, group, len | prio << 16 | type << 24, reserved}
 __device__ __forceinline__ void rs_row(const sdb_recv_send* s, uint32_t i, uint4& lo, uint4& hi) {
   const uint4* p = reinterpret_cast<const uint4*>(s + i);
@@ -166,7 +159,7 @@ k_rs_scatter(const uint32_t* __restrict__ kin, const uint32_t* __restrict__ vin,
              const uint32_t* __restrict__ ht, uint32_t tiles) {
   __shared__ uint32_t s[256];
   const uint32_t lane = threadIdx.x;
-  for (uint32_t d = lane; d < 256; d += 32) s[d] = rs_scan(hl, ht, d * tiles + blockIdx.x);
+  for (uint32_t d = lane; d < 256; d += 32) s[d] = sdb_scan_at(hl, ht, d * tiles + blockIdx.x);
   __syncwarp();
   const uint32_t base = blockIdx.x * SDB_RS_TILE;
   for (uint32_t k = 0; k < SDB_RS_TILE; k += 32) {
@@ -195,8 +188,8 @@ k_restore_headers(sdb_dev_view v, sdb_restore_args r, const uint32_t* __restrict
     const uint32_t e = sorted[p];
     const uint32_t row = r.e_row[e];
     const uint32_t n = r.row_cnt[row];
-    const uint32_t rank = p - rs_scan(r.rc_local, r.rc_tops, row);
-    const unsigned long long rb = r.base + rs_scan(r.rg_local, r.rg_tops, row);
+    const uint32_t rank = p - sdb_scan_at(r.rc_local, r.rc_tops, row);
+    const unsigned long long rb = r.base + sdb_scan_at(r.rg_local, r.rg_tops, row);
     uint4 lo, hi;
     rs_row(r.snd, row, lo, hi);
     const uint32_t pg = rs_pg(hi.z & 0xFFFFu);
@@ -219,7 +212,7 @@ k_restore_payloads(sdb_dev_view v, sdb_restore_args r) {
   for (uint32_t row = gw; row < r.n_sends; row += nw) {
     const uint32_t n = r.row_cnt[row];
     if (n == 0) continue;
-    const unsigned long long rb = r.base + rs_scan(r.rg_local, r.rg_tops, row);
+    const unsigned long long rb = r.base + sdb_scan_at(r.rg_local, r.rg_tops, row);
     uint4 lo, hi;
     rs_row(r.snd, row, lo, hi);
     const uint32_t pg = rs_pg(hi.z & 0xFFFFu);
@@ -255,7 +248,7 @@ k_restore_ring(sdb_dev_view v, sdb_restore_args r, unsigned long long priv_base)
       W = skip ? 0u : r.count[q];
       e0 = r.first[q];
       nsh = r.nsh[q];
-      pbase = priv_base + rs_scan(r.p_local, r.p_tops, q);
+      pbase = priv_base + sdb_scan_at(r.p_local, r.p_tops, q);
       if (W) T = v.ring_hdr[a].tail;
     }
     const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
@@ -273,12 +266,7 @@ k_restore_ring(sdb_dev_view v, sdb_restore_args r, unsigned long long priv_base)
         rs_row(r.snd, en.z, lo, hi);
         g = 1u + rs_pg(hi.z & 0xFFFFu);
       }
-      uint32_t incl = g;
-#pragma unroll
-      for (uint32_t o = 1; o < SDB_RS_G; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o, SDB_RS_G);
-        if (l8 >= o) incl += t;
-      }
+      const uint32_t incl = sdb_warp_incl_scan<SDB_RS_G>(g, l8);
       const unsigned long long apos = pbase + pcarry + incl - g;
       pcarry += __shfl_sync(0xFFFFFFFFu, incl, SDB_RS_G - 1, SDB_RS_G);
       if (priv) {
@@ -312,13 +300,6 @@ k_restore_ring(sdb_dev_view v, sdb_restore_args r, unsigned long long priv_base)
   if (lane == 0 && wrec) atomicAdd(&v.ctr->enqueued, wrec);
 }
 
-static uint32_t rs_grid(uint64_t items, uint64_t per_block, int sm_count) {
-  uint64_t g = (items + per_block - 1) / per_block;
-  const uint64_t cap = static_cast<uint64_t>(sm_count) * 8 * 4;
-  if (g > cap) g = cap;
-  return static_cast<uint32_t>(g ? g : 1);
-}
-
 // plan phase: validation, row counts, the three scans; r->tot ends with the totals the host reads
 extern "C" cudaError_t sdb_launch_restore_plan(const sdb_dev_view* v, const sdb_restore_args* r, cudaStream_t stream,
                                                sdb_profiler* prof, int* n_launches, int sm_count) {
@@ -327,12 +308,11 @@ extern "C" cudaError_t sdb_launch_restore_plan(const sdb_dev_view* v, const sdb_
   if (r->n_entries) cudaMemsetAsync(r->e_row, 0xFF, static_cast<size_t>(r->n_entries) * sizeof(uint32_t), stream);
   if (r->n_sends) cudaMemsetAsync(r->row_cnt, 0, static_cast<size_t>(r->n_sends) * sizeof(uint32_t), stream);
   int nl = 0;
-  if (r->n) { k_restore_plan<<<rs_grid(r->n, 32, sm_count), 256, 0, stream>>>(*v, *r); ++nl; }
+  if (r->n) { k_restore_plan<<<sdb_grid(r->n, 32, 32 * sm_count), 256, 0, stream>>>(*v, *r); ++nl; }
   if (r->n_sends) { k_restore_rows_gran<<<(r->n_sends + 255) / 256, 256, 0, stream>>>(*r); ++nl; }
-  cudaError_t e = sdb_scan_u32(r->row_cnt, r->rc_local, r->rc_tops, r->n_sends, r->tot + 5, nullptr, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(r->row_gran, r->rg_local, r->rg_tops, r->n_sends, r->tot + 0, nullptr, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(r->pgran, r->p_local, r->p_tops, r->n, r->tot + 1, nullptr, stream);
-  nl += (r->n_sends ? 4 : 0) + (r->n ? 2 : 0);
+  cudaError_t e = sdb_scan_u32(r->row_cnt, r->rc_local, r->rc_tops, r->n_sends, r->tot + 5, nullptr, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(r->row_gran, r->rg_local, r->rg_tops, r->n_sends, r->tot + 0, nullptr, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(r->pgran, r->p_local, r->p_tops, r->n, r->tot + 1, nullptr, stream, &nl);
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
   return e == cudaSuccess ? cudaGetLastError() : e;
@@ -347,31 +327,22 @@ extern "C" cudaError_t sdb_launch_restore_write(const sdb_dev_view* v, const sdb
   int nl = 0;
   cudaError_t e = cudaSuccess;
   if (n_shared) {
-    const uint32_t n = r->n_entries, tiles = (n + SDB_RS_TILE - 1) / SDB_RS_TILE;
-    uint32_t bits = 1;
-    while (bits < 32 && (r->n_sends >> bits)) ++bits;                     // keys are 0 .. n_sends
-    k_rs_init<<<(n + 255) / 256, 256, 0, stream>>>(*r);
+    k_rs_init<<<(r->n_entries + 255) / 256, 256, 0, stream>>>(*r);
     ++nl;
-    uint32_t *kin = r->key_a, *vin = r->val_a, *kout = r->key_b, *vout = r->val_b;
-    for (uint32_t shift = 0; shift < bits && e == cudaSuccess; shift += 8) {
-      k_rs_hist<<<tiles, 32, 0, stream>>>(kin, n, shift, r->hist, tiles);
-      e = sdb_scan_u32(r->hist, r->h_local, r->h_tops, 256u * tiles, nullptr, nullptr, stream);
-      k_rs_scatter<<<tiles, 32, 0, stream>>>(kin, vin, kout, vout, n, shift, r->h_local, r->h_tops, tiles);
-      nl += 4;
-      uint32_t* t = kin; kin = kout; kout = t;
-      t = vin; vin = vout; vout = t;
-    }
-    k_restore_headers<<<rs_grid(n_shared, 256, sm_count), 256, 0, stream>>>(*v, *r, vin, n_shared);
-    k_restore_payloads<<<rs_grid(r->n_sends, 8, sm_count), 256, 0, stream>>>(*v, *r);
+    uint32_t *ks = nullptr, *vs = nullptr;                               // keys are 0 .. n_sends
+    e = sdb_radix_sort_u32(r->key_a, r->val_a, r->key_b, r->val_b, r->n_entries, sdb_key_bits(r->n_sends), r->hist, r->h_local,
+                           r->h_tops, &ks, &vs, stream, &nl);
+    k_restore_headers<<<sdb_grid(n_shared, 256, 32 * sm_count), 256, 0, stream>>>(*v, *r, vs, n_shared);
+    k_restore_payloads<<<sdb_grid(r->n_sends, 8, 32 * sm_count), 256, 0, stream>>>(*v, *r);
     nl += 2;
   }
-  if (r->n) { k_restore_ring<<<rs_grid(r->n, 32, sm_count), 256, 0, stream>>>(*v, *r, r->base + row_grans); ++nl; }
+  if (r->n) { k_restore_ring<<<sdb_grid(r->n, 32, 32 * sm_count), 256, 0, stream>>>(*v, *r, r->base + row_grans); ++nl; }
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += nl;
   return e == cudaSuccess ? cudaGetLastError() : e;
 }
 
-// The radix sort above for other callers (the lease sweep): stable sort of n (key, value) pairs by the low `bits` bits of
+// The radix sort above, for the restore and the lease sweep: stable sort of n (key, value) pairs by the low `bits` bits of
 // the keys.  hist / h_local take 256 x ceil(n / 1024) words, h_tops that / 4096 + 1.  *kres / *vres name the buffers
 // holding the result: the a pair or the b pair.
 extern "C" cudaError_t sdb_radix_sort_u32(uint32_t* ka, uint32_t* va, uint32_t* kb, uint32_t* vb, uint32_t n, uint32_t bits,
@@ -383,9 +354,9 @@ extern "C" cudaError_t sdb_radix_sort_u32(uint32_t* ka, uint32_t* va, uint32_t* 
   int nl = 0;
   for (uint32_t shift = 0; n && shift < bits && e == cudaSuccess; shift += 8) {
     k_rs_hist<<<tiles, 32, 0, stream>>>(kin, n, shift, hist, tiles);
-    e = sdb_scan_u32(hist, h_local, h_tops, 256u * tiles, nullptr, nullptr, stream);
+    e = sdb_scan_u32(hist, h_local, h_tops, 256u * tiles, nullptr, nullptr, stream, &nl);
     k_rs_scatter<<<tiles, 32, 0, stream>>>(kin, vin, kout, vout, n, shift, h_local, h_tops, tiles);
-    nl += 4;
+    nl += 2;
     uint32_t* t = kin; kin = kout; kout = t;
     t = vin; vin = vout; vout = t;
   }

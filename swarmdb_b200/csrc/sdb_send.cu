@@ -998,9 +998,7 @@ k_pull_index_group(sdb_dev_view v, sdb_pull_view pv, const sdb_send_desc* __rest
       f = pv.first ? pv.first[lane] : 0u;
     }
     const uint32_t mstart = __ldg(lstart + g), mcount = __ldg(lcount + g);
-    uint32_t incl = e - o;                                   // prefix over sources: where each source's sends start in the bucket
-#pragma unroll
-    for (int d = 1; d < SDB_MAX_SRC; d <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= static_cast<uint32_t>(d)) incl += y; }
+    const uint32_t incl = sdb_warp_incl_scan<SDB_MAX_SRC>(e - o, lane);   // prefix over sources: where each source's sends start in the bucket
     const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, SDB_MAX_SRC - 1 < 31 ? SDB_MAX_SRC - 1 : 31);
     const uint32_t excl = incl - (e - o);
     if (total && mcount) {
@@ -1403,10 +1401,8 @@ extern "C" cudaError_t sdb_launch_p2p(const sdb_dev_view* v, const sdb_send_desc
                                       const uint8_t* payload, uint64_t seq_base, uint64_t arena_base,
                                       int sm_count, cudaStream_t stream, sdb_profiler* prof, uint32_t max_padlen) {
   if (n == 0) return cudaSuccess;
-  const uint32_t recs_per_cta = 8 * 4;                            // 8 warps x 4 records per step
-  uint32_t grid = (n + recs_per_cta - 1) / recs_per_cta;
-  const uint32_t cap = static_cast<uint32_t>(sm_count) * 8u * 4u;   // ~4 waves of 8 CTAs/SM, grid-stride beyond
-  if (grid > cap) grid = cap;
+  // 8 warps x 4 records per step; ~4 waves of 8 CTAs/SM, grid-stride beyond
+  const uint32_t grid = sdb_grid(n, 8 * 4, 32 * sm_count);
   const int pi = sdb_prof_begin(prof, SDB_PK_P2P, stream);
   static const bool use_tma = !(getenv("SDB_P2P_TMA") && atoi(getenv("SDB_P2P_TMA")) == 0);
   if (use_tma && max_padlen <= 512u) {
@@ -1516,11 +1512,9 @@ extern "C" cudaError_t sdb_launch_fanout_shared(const sdb_dev_view* v, const sdb
   if (n == 0) return cudaSuccess;
   const int pi = sdb_prof_begin(prof, SDB_PK_FANOUT, stream);
   const uint32_t lps = narrow ? 8u : 32u;
-  uint64_t grid = (static_cast<uint64_t>(n) * lps + 255) / 256;
-  const uint64_t cap = static_cast<uint64_t>(sm_count) * 8u * 4u;
-  if (grid > cap) grid = cap;
-  if (narrow) k_group_fanout_shared<8><<<static_cast<uint32_t>(grid), 256, 0, stream>>>(*v, descs, n, payload, seq_base, arena_base, bb);
-  else k_group_fanout_shared<32><<<static_cast<uint32_t>(grid), 256, 0, stream>>>(*v, descs, n, payload, seq_base, arena_base, bb);
+  const uint32_t grid = sdb_grid(static_cast<uint64_t>(n) * lps, 256, 32 * sm_count);
+  if (narrow) k_group_fanout_shared<8><<<grid, 256, 0, stream>>>(*v, descs, n, payload, seq_base, arena_base, bb);
+  else k_group_fanout_shared<32><<<grid, 256, 0, stream>>>(*v, descs, n, payload, seq_base, arena_base, bb);
   sdb_prof_end(prof, pi, stream);
   return cudaGetLastError();
 }

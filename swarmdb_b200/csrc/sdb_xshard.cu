@@ -24,9 +24,6 @@
 // pulls the sends it has recipients for.
 #include "sdb_common.cuh"
 
-#define SDB_SCAN_TILE 4096u
-
-
 __device__ __forceinline__ const sdb_wire_header* wire_hdr(const sdb_import_args& a, uint32_t src) {
   return reinterpret_cast<const sdb_wire_header*>(a.meta[src]);
 }
@@ -116,13 +113,13 @@ k_wire_localize(sdb_import_args a, uint32_t n_total) {
   // absolute address (the fan-out kernel is launched with a null payload base): the payload stays where the
   // source rank exported it - possibly in a peer GPU's memory - and is pulled by the fan-out's TMA loads
   out.payload_off = reinterpret_cast<uint64_t>(a.wire[src]) + a.tab->payload_off[src] + d->payload_off;
-  out.gran0 = a.w_local[gi] + a.w_tops[gi / SDB_SCAN_TILE];
+  out.gran0 = sdb_scan_at(a.w_local, a.w_tops, gi);
   out.rec0 = static_cast<uint32_t>(rb + d->rec0);
   const bool abs_seq = a.tab->explicit_seq[src] != 0;
   out.seq_abs = abs_seq ? rb + d->rec0 : 0ull;
   if (d->flags & (SDB_DESC_P2P | SDB_DESC_LIST_TEMP)) {
     const uint32_t own = a.lw[gi];
-    uint32_t lo = a.lw_local[gi] + a.lw_tops[gi / SDB_SCAN_TILE];
+    uint32_t lo = sdb_scan_at(a.lw_local, a.lw_tops, gi);
     const bool fits = static_cast<uint64_t>(lo) + own <= a.list_cap;      // checked on the host before launch
     out.mstart = lo; out.mcount = fits ? own : 0u; out.group = SDB_NO_GROUP;
     if (d->flags & SDB_DESC_P2P) {
@@ -180,9 +177,6 @@ k_bucket_fill(sdb_import_args a, const uint32_t* __restrict__ goff, uint32_t* __
   for (uint32_t k = b; k < e; ++k) a.gs_idx[dst + (k - b)] = first + ix[k];
 }
 
-extern "C" cudaError_t sdb_scan_u32(const uint32_t* in, uint32_t* local, uint32_t* tops, uint32_t n,
-                                    unsigned long long* total_out, uint32_t* out, cudaStream_t stream);
-
 // phase 1: measure + scans.  totals_dev[0] receives the arena granules this import will write.
 extern "C" cudaError_t sdb_launch_import_measure(const sdb_import_args* a, uint32_t n_cap, uint32_t* w_local,
                                                  uint32_t* w_tops, uint32_t* gs_local, uint32_t* gs_tops,
@@ -192,14 +186,15 @@ extern "C" cudaError_t sdb_launch_import_measure(const sdb_import_args* a, uint3
   const int pi = sdb_prof_begin(prof, SDB_PK_XSHARD, stream);
   k_wire_table<<<1, 32, 0, stream>>>(*a, const_cast<sdb_src_tab*>(a->tab));
   k_wire_measure<<<(n_cap + 255) / 256, 256, 0, stream>>>(*a, n_cap);
-  cudaError_t e = sdb_scan_u32(a->w, w_local, w_tops, n_cap, totals_dev, nullptr, stream);
+  int nl = 3;                                                  // k_wire_table, k_wire_measure, k_bucket_sizes
+  cudaError_t e = sdb_scan_u32(a->w, w_local, w_tops, n_cap, totals_dev, nullptr, stream, &nl);
   const uint32_t nb = a->max_groups * a->n_src + 1;
   k_bucket_sizes<<<(nb + 255) / 256, 256, 0, stream>>>(*a);
   // gs_off_out here is the materialised scan over (group, source) pairs ("goff", nb entries)
-  if (e == cudaSuccess) e = sdb_scan_u32(a->gs_cnt, gs_local, gs_tops, nb, nullptr, gs_off_out, stream);
-  if (e == cudaSuccess) e = sdb_scan_u32(a->lw, lw_local, lw_tops, n_cap, totals_dev + 1, nullptr, stream);   // owned recipients
+  if (e == cudaSuccess) e = sdb_scan_u32(a->gs_cnt, gs_local, gs_tops, nb, nullptr, gs_off_out, stream, &nl);
+  if (e == cudaSuccess) e = sdb_scan_u32(a->lw, lw_local, lw_tops, n_cap, totals_dev + 1, nullptr, stream, &nl);   // owned recipients
   sdb_prof_end(prof, pi, stream);
-  if (n_launches) *n_launches += 9;
+  if (n_launches) *n_launches += nl;
   return e != cudaSuccess ? e : cudaGetLastError();
 }
 

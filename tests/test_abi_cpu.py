@@ -119,3 +119,60 @@ def test_every_environment_switch_of_the_library_is_documented():
     finally:
         if old is not None:
             os.environ["SDB_SHARED_PAYLOAD"] = old
+
+
+def _extern_c(text):
+    """(name, has_body) of every function declared with C linkage in C++ source text: after an extern "C" specifier, or
+    at the top level of an extern "C" { } block."""
+    text = re.sub(r"/\*.*?\*/", "", re.sub(r"//[^\n]*", "", text), flags=re.S)
+    text = re.sub(r"^\s*#[^\n]*", "", text, flags=re.M)
+
+    def close(i, o, c):                                      # index of the bracket closing the one at i
+        depth = 0
+        for k in range(i, len(text)):
+            depth += (text[k] == o) - (text[k] == c)
+            if depth == 0:
+                return k
+
+    def decl(i):                                             # the declaration whose parameter list opens at i
+        head = re.split(r"[;{}]", text[:i])[-1]
+        k = close(i, "(", ")") + 1
+        return re.findall(r"\w+", head)[-1], text[k:].lstrip()[:1] == "{", k, re.search(r"\bstatic\b", head)
+
+    out = []
+    for m in re.finditer(r'extern\s+"C"\s*', text):
+        i = m.end()
+        if text[i] != "{":
+            out.append(decl(text.index("(", i))[:2])
+            continue
+        k, end = i + 1, close(i, "{", "}")
+        while k < end:
+            if text[k] == "{":
+                k = close(k, "{", "}") + 1
+            elif text[k] == "(":
+                name, body, k, internal = decl(k)
+                if not internal:                             # static functions have no linkage to check
+                    out.append((name, body))
+            else:
+                k += 1
+    return out
+
+
+def test_launchers_are_declared_once_where_their_definitions_see_them():
+    """The two-level scan layout is defined once, and every extern "C" function one source defines for another is declared
+    in sdb_common.cuh, which every source includes: C linkage has no name mangling, so a prototype the defining file
+    never sees would let a changed signature link and pass wrong arguments."""
+    csrc = ROOT / "swarmdb_b200" / "csrc"
+    files = sorted(csrc.glob("*.cu")) + sorted(csrc.glob("*.cuh"))
+    assert sum(p.read_text().count("#define SDB_SCAN_TILE") for p in files) == 1
+    common = (csrc / "sdb_common.cuh").read_text()
+    block = re.search(r'extern "C" \{(.*?)\n\}', common, flags=re.S).group(1)
+    declared = set(re.findall(r"(\w+)\s*\(", re.sub(r"//[^\n]*", "", block)))
+    public = set(_declared())
+    defined = set()
+    for p in sorted(csrc.glob("*.cu")):
+        fns = _extern_c(p.read_text())
+        assert all(body for _, body in fns), (p.name, [n for n, body in fns if not body])
+        defined |= {n for n, _ in fns}
+    assert len(defined) > 60
+    assert sorted(defined - public - declared) == []
