@@ -1004,6 +1004,111 @@ def lease_snapshot(rounds=3):
     return out
 
 
+def budget(rounds=2, per_agent=2):
+    """Receive by byte budget (sdb_receive_compact_budget).
+    drain: GpuConfig's default caps (32 KB max_payload_bytes, 64 MB and 65536 records per call) and a backlog of
+      256-byte messages, `per_agent` per agent over 1 M agents, drained into pinned buffers by receive_compact (sized
+      for the worst case: 2048 records per call) and by the budget call without a per-agent limit (sized by the bytes
+      selected), alternated; calls, wall time per record drained and D2H bytes.
+    plan: the c2 backlog (bench.py's step, 4,194,304 records over 1 M agents) received with a per-agent limit of two
+      padded payloads (half of each queue) against the plain receive; the plan kernel's time from the library profiler
+      (PEEK calls: the backlog stays)."""
+    import torch
+    from bench import Workload
+    from swarmdb_b200._native import ENTRY_DTYPE, RECV_PEEK, SEND_DTYPE, Shard, pad32
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py budget: no CUDA device - swarmdb_b200 has no CPU fallback")
+
+    def pinned(nbytes):
+        return torch.empty(nbytes, dtype=torch.uint8, pin_memory=True).numpy()
+
+    # ---- drain at the default caps
+    A, L, P = 1 << 20, 256, 32768
+    n = A * per_agent
+    shard = Shard(max_agents=A, ring_slots=64, arena_bytes=1 << 31, max_payload_bytes=P, max_batch_sends=1 << 16,
+                  max_batch_payload=(1 << 16) * L, max_recv_records=1 << 16, max_recv_payload=1 << 26)
+    shard.register(np.arange(A, dtype=np.uint32))
+    rng = np.random.default_rng(7)
+    B = 1 << 16
+    recv_all = np.tile(np.arange(A, dtype=np.uint32), per_agent)
+    pay_in = rng.integers(0, 256, B * L, dtype=np.uint8)
+    off = (np.arange(B, dtype=np.uint64) * L)
+    lens, z8, ts = np.full(B, L, np.uint16), np.zeros(B, np.uint8), np.zeros(B)
+
+    def fill():
+        for i in range(0, n, B):
+            shard.send_batch(recv_all[i:i + B] ^ 1, recv_all[i:i + B], z8, z8, lens, off, pay_in, ts)
+        shard.sync()
+
+    pin_ent = pinned((1 << 16) * 16).view(ENTRY_DTYPE)
+    pin_snd = pinned((1 << 16) * 32).view(SEND_DTYPE)
+    pin_pay = pinned(1 << 26)
+    seqs = {}
+
+    def drain(name):
+        calls, recs, d2h = 0, 0, 0
+        got = []
+        t = time.perf_counter()
+        while True:
+            kw = {} if name == "compact" else {"max_agent_bytes": 0}
+            cnt, ent, snd, pay = shard.receive_compact(None, 100, 0, out_entries=pin_ent, out_sends=pin_snd,
+                                                       out_payload=pin_pay, **kw)
+            calls += 1
+            d2h += len(cnt) * 4 + len(ent) * 16 + len(snd) * 32 + len(pay) + 24
+            if len(ent) == 0:
+                break
+            recs += len(ent)
+            got.append(ent["seq"].copy())
+        sec = time.perf_counter() - t
+        seqs[name] = np.sort(np.concatenate(got))
+        return {"calls": calls, "records": recs, "s": sec, "ns_per_record": sec * 1e9 / recs, "d2h_bytes": d2h}
+
+    res = {"compact": [], "budget": []}
+    for r in range(rounds):
+        for name in (("compact", "budget") if r % 2 == 0 else ("budget", "compact")):
+            fill()
+            res[name].append(drain(name))
+    assert all(np.array_equal(s - s[0], np.arange(n)) for s in seqs.values())     # both drains took every message once
+    st = shard.stats()
+    assert st["ring_overflow"] == 0 and st["delivered"] == st["enqueued"]
+    shard.close()
+    out = {"drain_config": f"{A} agents x {per_agent} messages of {L} B, max_payload_bytes {P}, 64 MB / 65536 records "
+                           f"per call, pinned outputs; {rounds} rounds, order alternated",
+           "drain": {k: {"runs": v, "ns_per_record": float(np.median([x["ns_per_record"] for x in v])),
+                         "calls": v[-1]["calls"], "d2h_bytes": v[-1]["d2h_bytes"]} for k, v in res.items()}}
+
+    # ---- plan kernel on the c2 backlog, per-agent limit of half of each queue
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    shard = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+    shard.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        shard.create_group(g, wl.members(g))
+    shard.send_group_batch(*wl.batch())
+    shard.sync()
+    limit = 2 * pad32(wl.L)
+    reps = 20
+    kern, recs = {}, {}
+    for name, kw in (("plain", {}), ("budget", {"max_agent_bytes": limit})) * 2:
+        shard.receive_compact(None, 100, RECV_PEEK, **kw)                     # warm-up
+        shard.profile(True)
+        for _ in range(reps):
+            cnt, ent, _, _ = shard.receive_compact(None, 100, RECV_PEEK, **kw)
+        prof = shard.profile_read()
+        shard.profile(False)
+        kern.setdefault(name, []).append(prof["recv_select"][0] / reps)
+        recs[name] = len(ent)
+    shard.close()
+    out["plan_config"] = (f"c2 backlog: {per_step} records over {wl.A} agents, {wl.L}-B payloads; per-agent limit "
+                          f"{limit} B; PEEK compact receives, {reps} per block, blocks alternated")
+    out["plan"] = {k: {"plan_ms_blocks": v, "plan_ms": float(np.median(v)), "records": recs[k]} for k, v in kern.items()}
+    out.update(_gpu_card(0))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", nargs="*", default=["c1", "c4", "c5", "k1", "bcast"])

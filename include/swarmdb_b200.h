@@ -225,6 +225,8 @@ int sdb_free_staged(sdb_handle h, sdb_staged_t s);
  * dropped.  The only exception is an agent that is first in the output (nothing placed
  * before it): it gets its first rec_cap records, in the call's delivery order, and keeps
  * the rest queued.  So every call on a non-empty queue makes progress.
+ * sdb_receive_budget (below) bounds each agent's take by bytes and sizes a call by the bytes
+ * it actually selects instead of the worst case.
  */
 #define SDB_RECV_PRIORITY 1u
 #define SDB_RECV_PEEK 2u                /* return what a receive would deliver, retire nothing (history snapshots, M:852-892) */
@@ -284,6 +286,36 @@ int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
                         uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
                         sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                         uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
+/* Receive by byte budget (Kafka's max.partition.fetch.bytes per agent and fetch.max.bytes per call): the arguments of
+ * sdb_receive_batch / sdb_receive_compact plus max_agent_bytes.
+ *   1. Per-agent take: the longest prefix of the agent's delivery order (stream order, or priority order with
+ *      SDB_RECV_PRIORITY) with at most max_messages records and sum(pad32(len)) <= max_agent_bytes (0: no byte limit).
+ *      An agent whose first record alone is larger takes that one record, so an oversized message never blocks its queue.
+ *   2. Call capacity, exact in bytes: rec_cap = min(max_recv_records, hdr_cap) (full format) or min(max_recv_records,
+ *      entry_cap, send_cap) (compact format), with no division by pad32(max_payload_bytes); byte capacity
+ *      min(max_recv_payload, payload_cap), compared against sum(pad32(len)) of the records selected (each caller cap
+ *      counts only when its pointer is given).  Truncation as in sdb_receive_batch: agents in list order, an agent whose
+ *      take does not fit either cap stays queued together with every later agent; an agent first in the output takes the
+ *      longest prefix of its take that fits both caps.
+ *   3. Progress: payload_cap (when payload_out is given) below pad32(max_payload_bytes) is refused (SDB_EINVAL), so every
+ *      call on a non-empty queue makes progress.
+ *   4. Compact format: bytes are counted per record as in the full format, never per distinct row, so which records a
+ *      call takes does not depend on how much they share; the compact payload output is never larger than that count.
+ *   5. Equivalence: the result (records, order, bytes, retirement, counters, rings and, after a full-format call,
+ *      sdb_digest_fold) is exactly what sdb_receive_batch / sdb_receive_compact return when each agent's max_messages is
+ *      its take.  SDB_RECV_PRIORITY, SDB_RECV_PEEK and SDB_RECV_OWNED as there; SDB_RECV_ASYNC is refused (SDB_EINVAL).
+ *      Refused calls leave every queue untouched.  A budget call always runs the bulk plan (never the few-agent or
+ *      latency-server paths). */
+int sdb_receive_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                       uint64_t max_agent_bytes, uint32_t flags,
+                       uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
+                       uint8_t* payload_out, uint64_t payload_cap,
+                       uint64_t* total_out, uint64_t* payload_bytes_out);
+int sdb_receive_compact_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                               uint64_t max_agent_bytes, uint32_t flags,
+                               uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                               sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                               uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
 /* Restore: put records in the compact format back on the device - a queue snapshot (a PEEK compact receive) after a
  * restart, or what a compact receive just took when its consumer failed (requeue).  Input in exactly the shape
  * sdb_receive_compact and sdb_expire's archive mode return: listed agent i owns the next count[i] entries.

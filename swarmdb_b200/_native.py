@@ -147,7 +147,7 @@ class SdbRelocateSummary(C.Structure):
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_profile_read_n", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
-           "sdb_receive_batch", "sdb_receive_compact", "sdb_restore_compact", "sdb_expire", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
+           "sdb_receive_batch", "sdb_receive_compact", "sdb_receive_budget", "sdb_receive_compact_budget", "sdb_restore_compact", "sdb_expire", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
@@ -198,6 +198,10 @@ def load_library() -> C.CDLL:
     L.sdb_receive_batch.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, vp]
     L.sdb_receive_compact.restype = i32
     L.sdb_receive_compact.argtypes = [vp, u32, vp, u32, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    L.sdb_receive_budget.restype = i32
+    L.sdb_receive_budget.argtypes = [vp, u32, vp, u32, u64, u32, vp, vp, u64, vp, u64, vp, vp]
+    L.sdb_receive_compact_budget.restype = i32
+    L.sdb_receive_compact_budget.argtypes = [vp, u32, vp, u32, u64, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_restore_compact.restype = i32
     L.sdb_restore_compact.argtypes = [vp, u32, vp, vp, vp, u64, vp, u64, vp, u64, u32, vp, vp]
     L.sdb_lease_reserve.restype = i32; L.sdb_lease_reserve.argtypes = [vp, u64, u64]
@@ -588,19 +592,40 @@ class Shard:
             counts = self._served_counts(counts, flags)
         return counts, hdr[: total.value], pay[: pbytes.value]
 
+    def receive_budget(self, agents, max_messages: int, max_agent_bytes: int, flags: int = 0,
+                       out_hdr: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+        """receive_batch by byte budget (include/swarmdb_b200.h: sdb_receive_budget): each agent takes the longest prefix
+        of its delivery order with at most max_messages records and sum(pad32(len)) <= max_agent_bytes (0: no byte
+        limit; an oversized first record is taken alone), and the call fills its buffers exactly by bytes instead of
+        by max_payload_bytes.  Returns (counts[n_agents], headers[total], payload bytes) as receive_batch does."""
+        a, n, counts = self._agents_arg(agents)
+        hdr = out_hdr if out_hdr is not None else self._grow_hdr()
+        pay = out_payload if out_payload is not None else self._grow_pay()
+        total, pbytes = C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_receive_budget(self._h, n, _p(a), max_messages, int(max_agent_bytes), flags, _p(counts),
+                                               _p(hdr), len(hdr), _p(pay), pay.nbytes, C.cast(C.byref(total), C.c_void_p),
+                                               C.cast(C.byref(pbytes), C.c_void_p)))
+        if agents is None:
+            counts = self._served_counts(counts, flags)
+        return counts, hdr[: total.value], pay[: pbytes.value]
+
     def receive_compact(self, agents, max_messages: int, flags: int = 0, out_entries: Optional[np.ndarray] = None,
-                        out_sends: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+                        out_sends: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None,
+                        max_agent_bytes: Optional[int] = None):
         """The records receive_batch would return, in the compact format (include/swarmdb_b200.h:
         sdb_receive_compact): (counts[n_agents], entries[total] ENTRY_DTYPE, sends[n_sends] SEND_DTYPE, payload bytes),
         each distinct payload once.  Views into reusable buffers unless explicit (e.g. pinned) arrays are given;
-        expand_compact() turns them into receive_batch's (headers, payload)."""
+        expand_compact() turns them into receive_batch's (headers, payload).  With max_agent_bytes (0: no per-agent
+        limit) the call takes receive_budget's records (sdb_receive_compact_budget)."""
         a, n, counts = self._agents_arg(agents)
         ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
         total, n_sends, pbytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-        self._check(self._L.sdb_receive_compact(self._h, n, _p(a), max_messages, flags, _p(counts), _p(ent), len(ent),
-                                                _p(snd), len(snd), _p(pay), pay.nbytes,
-                                                C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
-                                                C.cast(C.byref(pbytes), C.c_void_p)))
+        tail = (_p(counts), _p(ent), len(ent), _p(snd), len(snd), _p(pay), pay.nbytes, C.cast(C.byref(total), C.c_void_p),
+                C.cast(C.byref(n_sends), C.c_void_p), C.cast(C.byref(pbytes), C.c_void_p))
+        if max_agent_bytes is None:
+            self._check(self._L.sdb_receive_compact(self._h, n, _p(a), max_messages, flags, *tail))
+        else:
+            self._check(self._L.sdb_receive_compact_budget(self._h, n, _p(a), max_messages, int(max_agent_bytes), flags, *tail))
         if agents is None:
             counts = self._served_counts(counts, flags)
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]

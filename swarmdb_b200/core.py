@@ -723,12 +723,17 @@ class SwarmsDB:
         return ids
 
     # ------------------------------------------------------------------ receive
-    def receive_messages(self, agent_id: str, max_messages: int = 100, timeout: float = 1.0) -> List[Message]:
+    def receive_messages(self, agent_id: str, max_messages: int = 100, timeout: float = 1.0,
+                         max_bytes: Optional[int] = None) -> List[Message]:
         """Pop up to `max_messages` pending messages for `agent_id` in stream order (or priority
         order with GpuConfig.priority_dequeue).  Never blocks: `timeout` is accepted for
-        compatibility (the reference spins up to `timeout` when fewer are available, M:553-556)."""
+        compatibility (the reference spins up to `timeout` when fewer are available, M:553-556).
+        max_bytes bounds the encoded payload bytes returned: the longest run of pending messages, in delivery order,
+        whose encoded payloads (each rounded up to 32 bytes) fit max_bytes, or the first message alone when it is
+        larger.  A byte budget is the device's stand-in for a token budget (as many messages as fit N bytes of
+        context).  One such call returns at most GpuConfig.max_recv_records messages and max_recv_payload bytes."""
         self._prepare_receive(agent_id)
-        return self._receive_local(agent_id, max_messages)
+        return self._receive_local(agent_id, max_messages, max_bytes)
 
     def _prepare_receive(self, agent_id: str) -> bool:
         """Before a receive for `agent_id`: register it if needed and push buffered sends (a sharded front-end checks
@@ -739,10 +744,22 @@ class SwarmsDB:
         self.flush()
         return True
 
-    def _receive_local(self, agent_id: str, max_messages: int) -> List[Message]:
+    def _receive_budget_one(self, agent_id: str, max_messages: int, max_bytes: int, flags: int):
+        """(headers, payload) of one byte-budget receive for one agent (Shard.receive_budget)."""
+        if max_bytes < 0:
+            raise ValueError("max_bytes must be >= 0")
+        k = min(max_messages, self.shard.max_recv_records)
+        # the device reads 0 as "no limit"; a 1-byte limit takes the same records as a 0-byte one (sizes are multiples of 32)
+        _, hdr, pay = self.shard.receive_budget([self._index(agent_id)], k, max(int(max_bytes), 1), flags)
+        return hdr, pay
+
+    def _receive_local(self, agent_id: str, max_messages: int, max_bytes: Optional[int] = None) -> List[Message]:
         if max_messages <= 0:
             return []
         flags = RECV_PRIORITY if self.gpu_config.priority_dequeue else 0
+        if max_bytes is not None:
+            hdr, pay = self._receive_budget_one(agent_id, max_messages, max_bytes, flags)
+            return self._decode(hdr, pay, agent_id)
         out: List[Message] = []
         a = self._index(agent_id)
         remaining = max_messages
@@ -934,11 +951,17 @@ class SwarmsDB:
         flushes delivered, so it overrides this with a no-op)."""
         self.flush()
 
-    def peek_messages(self, agent_id: str, max_messages: int = 100) -> List[Message]:
-        """What `receive_messages` would return next, without consuming it (device PEEK receive)."""
+    def peek_messages(self, agent_id: str, max_messages: int = 100, max_bytes: Optional[int] = None) -> List[Message]:
+        """What `receive_messages` (with the same max_bytes) would return next, without consuming it (device PEEK
+        receive)."""
         self._pre_read()
         flags = RECV_PEEK | (RECV_PRIORITY if self.gpu_config.priority_dequeue else 0)
-        hdr, pay, _ = self.shard.receive_one(self._index(agent_id), max_messages, flags)
+        if max_bytes is not None:
+            if max_messages <= 0:
+                return []
+            hdr, pay = self._receive_budget_one(agent_id, max_messages, max_bytes, flags)
+        else:
+            hdr, pay, _ = self.shard.receive_one(self._index(agent_id), max_messages, flags)
         return self._decode(hdr, pay, agent_id, record=False, status=MessageStatus.DELIVERED)
 
     def _where_filter(self, sender_id=None, receiver_idx=None, message_type=None, min_priority=None, group_name=None,
@@ -1125,17 +1148,26 @@ class SwarmsDB:
         self._next_seq = self.shard.stats()["next_seq"]; self._b_first_seq = self._next_seq
         return base
 
-    def receive_batch(self, agent_idx=None, max_messages: int = 100, priority: Optional[bool] = None, **kw):
+    def receive_batch(self, agent_idx=None, max_messages: int = 100, priority: Optional[bool] = None,
+                      max_bytes: Optional[int] = None, **kw):
+        """max_bytes: each agent takes at most that many encoded payload bytes (each payload rounded up to 32 bytes; an
+        oversized first message alone; 0: no per-agent limit) and the call is sized by the bytes it selects
+        (Shard.receive_budget).  None keeps the plain receive."""
         self.flush()
         pr = self.gpu_config.priority_dequeue if priority is None else priority
+        if max_bytes is not None:
+            return self.shard.receive_budget(agent_idx, max_messages, int(max_bytes), RECV_PRIORITY if pr else 0, **kw)
         return self.shard.receive_batch(agent_idx, max_messages, RECV_PRIORITY if pr else 0, **kw)
 
-    def receive_batch_compact(self, agent_idx=None, max_messages: int = 100, priority: Optional[bool] = None, **kw):
+    def receive_batch_compact(self, agent_idx=None, max_messages: int = 100, priority: Optional[bool] = None,
+                              max_bytes: Optional[int] = None, **kw):
         """receive_batch's records in the compact format: (counts, entries, sends, payload) with each distinct
-        payload once (Shard.receive_compact; _native.expand_compact gives receive_batch's (headers, payload))."""
+        payload once (Shard.receive_compact; _native.expand_compact gives receive_batch's (headers, payload)).
+        max_bytes as in receive_batch; bytes are counted per message, shared payloads included."""
         self.flush()
         pr = self.gpu_config.priority_dequeue if priority is None else priority
-        return self.shard.receive_compact(agent_idx, max_messages, RECV_PRIORITY if pr else 0, **kw)
+        return self.shard.receive_compact(agent_idx, max_messages, RECV_PRIORITY if pr else 0,
+                                          max_agent_bytes=None if max_bytes is None else int(max_bytes), **kw)
 
     def requeue_batch_compact(self, counts, entries, sends, payload, agent_idx) -> int:
         """The nack of receive_batch_compact: put what a compact receive took (or any input of that shape: agent_idx[i]

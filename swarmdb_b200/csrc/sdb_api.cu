@@ -1869,7 +1869,7 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   if (async && (count_out || hdr_out || payload_out)) return fail(h, SDB_EINVAL, "SDB_RECV_ASYNC takes no host output buffers");
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
-                                     nullptr);
+                                     nullptr, nullptr);
   h->launches += nl;
   if (!(r.flags & SDB_RECV_PRIORITY)) r.plan_tops = nullptr;       // single-pass path: plan offsets are absolute
   h->last_rx = r; h->last_rx_valid = (e == cudaSuccess); h->last_rx_compact = false;
@@ -1914,10 +1914,83 @@ int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
     if (rc != SDB_OK) return rc; }
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
-                                     &h->cx);
+                                     &h->cx, nullptr);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = true;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("compact receive launch: ") + cudaGetErrorString(e));
+  return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
+}
+
+// Capacity of a byte-budget receive (include/swarmdb_b200.h: sdb_receive_budget), exact in bytes: `rec_room` records and
+// the payload buffer's granules, which must hold one record of the maximum size.  budget = {per-agent limit, call
+// capacity} in payload granules.
+static int budget_caps(sdb_ctx* h, uint64_t rec_room, const void* payload_out, uint64_t payload_cap, uint64_t max_agent_bytes,
+                       uint64_t* rec_cap, uint2* budget) {
+  const uint64_t P = pad32(h->cfg.max_payload_bytes);
+  if (payload_out && payload_cap < P) return fail(h, SDB_EINVAL, "payload_cap below pad32(max_payload_bytes): a call could not make progress");
+  const uint64_t gran_cap = std::min<uint64_t>(h->pay_cap_gran, room(payload_out, payload_cap) / SDB_GRANULE);
+  *rec_cap = std::min<uint64_t>(h->cfg.max_recv_records, rec_room);
+  if (*rec_cap == 0 || gran_cap * SDB_GRANULE < P) return fail(h, SDB_EOUTPUT, "output buffers cannot hold a single maximum-size record");
+  const uint64_t agent_gran = max_agent_bytes ? max_agent_bytes / SDB_GRANULE : ~0ull;     // sum(pad32(len)) <= max_agent_bytes
+  *budget = make_uint2(static_cast<uint32_t>(std::min<uint64_t>(agent_gran, 0xFFFFFFFFull)), static_cast<uint32_t>(gran_cap));
+  return SDB_OK;
+}
+
+int sdb_receive_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint64_t max_agent_bytes,
+                       uint32_t flags, uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
+                       uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_budget returns host results: SDB_RECV_ASYNC is not accepted");
+  uint64_t rec_cap = 0;
+  uint2 budget;
+  { const int rc = budget_caps(h, room(hdr_out, hdr_cap), payload_out, payload_cap, max_agent_bytes, &rec_cap, &budget);
+    if (rc != SDB_OK) return rc; }
+  const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
+  if (n_agents == 0 || max_messages == 0) return SDB_OK;
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
+  sdb_recv_args r{};
+  { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK), rec_cap, &r);
+    if (rc != SDB_OK) return rc; }
+  int nl = 0;
+  cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
+                                     nullptr, &budget);
+  h->launches += nl;
+  r.plan_tops = nullptr;                                        // single-pass plan in both orders: offsets are absolute
+  h->last_rx = r; h->last_rx_valid = (e == cudaSuccess); h->last_rx_compact = false;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("budget receive launch: ") + cudaGetErrorString(e));
+  return copy_full(h, n_agents, count_out, hdr_out, payload_out, total_out, payload_bytes_out);
+}
+
+int sdb_receive_compact_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                               uint64_t max_agent_bytes, uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out,
+                               uint64_t entry_cap, sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out,
+                               uint64_t payload_cap, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_compact_budget returns host results: SDB_RECV_ASYNC is not accepted");
+  // bytes are counted per record, so the compact payload (one copy per distinct image) never exceeds the count
+  uint64_t rec_cap = 0;
+  uint2 budget;
+  { const int rc = budget_caps(h, std::min(room(entry_out, entry_cap), room(send_out, send_cap)), payload_out, payload_cap,
+                               max_agent_bytes, &rec_cap, &budget);
+    if (rc != SDB_OK) return rc; }
+  const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
+  if (n_agents == 0 || max_messages == 0) return SDB_OK;
+  { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
+  { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
+  sdb_recv_args r{};
+  { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK), rec_cap, &r);
+    if (rc != SDB_OK) return rc; }
+  int nl = 0;
+  cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
+                                     &h->cx, &budget);
+  h->launches += nl;
+  h->last_rx_valid = false; h->last_rx_compact = true;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("compact budget receive launch: ") + cudaGetErrorString(e));
   return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
 }
 
@@ -2263,7 +2336,7 @@ int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_id
   int nl = 0;
   const bool ledger = L.policy && L.led_n;      // the ledger holds entries: collect before anything is retired, look up after
   cudaError_t e = ledger ? ledger_collect(h) : cudaSuccess;
-  if (e == cudaSuccess) e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx);
+  if (e == cudaSuccess) e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx, nullptr);
   h->last_rx_valid = false; h->last_rx_compact = true;
   if (e == cudaSuccess)
     e = sdb_launch_lease_append(&L.buf[L.cur], &L.s, &h->cx, h->rx_count, h->rx_totals, r.agent_idx, n_agents,

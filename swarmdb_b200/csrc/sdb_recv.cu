@@ -26,6 +26,8 @@
 //   k_recv_gather   flat over records: copy header + payload from the arena to the packed output
 // A compact receive (sdb_receive_compact) runs either plan and replaces the gather with the compact kernels (below):
 // 16-byte entries per record and one row + payload per distinct payload image.
+// A byte-budget receive (sdb_receive_budget) runs the single-pass plan in either order (k_recv_plan<SDB_PLAN_BUDGET>,
+// <SDB_PLAN_BUDGET_PRIO>), then the gather or the compact kernels.
 //
 // Roofline: HBM-bound.  Algorithmic bytes per agent-call: P*1 priority bytes scanned (we scan
 // 2-byte ring_meta entries) + 2*k*(L+H) gather+emit (SURVEY 8d).
@@ -459,10 +461,82 @@ __device__ __forceinline__ uint32_t fill_offsets_warp(uint4* plan, uint32_t RO, 
   return run;
 }
 
+// Byte budgets (sdb_receive_budget): an agent's take is the longest prefix of its delivery order with at most C records
+// and at most `lim` payload granules, or its first record alone when that one is larger.
+// Whole warp over the window [H, T): {records, granules} of the take.  Stream order stops at the first entry that does
+// not fit; priority order (PRIO) first counts {records, granules} per level, takes whole levels from the top while they
+// fit, then the arrival-order prefix of the level where the limit falls.
+template <bool PRIO>
+__device__ __forceinline__ uint2 budget_take_warp(const uint2* rs, uint32_t mask, uint32_t H, uint32_t T, uint32_t C,
+                                                  uint32_t lim, uint32_t lane) {
+  uint32_t acc_c = 0, acc_g = 0, cut = 0;
+  if (PRIO) {
+    // per level: live records (nc) and their payload granules (hg)
+    uint32_t hg0 = 0, hg1 = 0, hg2 = 0, hg3 = 0;
+    uint32_t nc0 = 0, nc1 = 0, nc2 = 0, nc3 = 0;
+    for (uint32_t p0 = H; static_cast<int32_t>(T - p0) > 0; p0 += 32) {
+      const uint32_t p = p0 + lane;
+      const uint32_t m = static_cast<int32_t>(T - p) > 0 ? (rs[p & mask].y & 0xFFFFu) : SDB_META_TOMB;
+      const bool live = m != SDB_META_TOMB;
+      const uint32_t L = m >> 14, g = (m & SDB_META_GLEN_MASK) - 1u;
+      nc0 += live && L == 0; nc1 += live && L == 1; nc2 += live && L == 2; nc3 += live && L == 3;
+      hg0 += (live && L == 0) ? g : 0u; hg1 += (live && L == 1) ? g : 0u;
+      hg2 += (live && L == 2) ? g : 0u; hg3 += (live && L == 3) ? g : 0u;
+    }
+    cut = 4;                                                  // 4: every level fits
+    auto level = [&](uint32_t L, uint32_t nc, uint32_t hg) {
+      const uint32_t c = __reduce_add_sync(0xFFFFFFFFu, nc), g = __reduce_add_sync(0xFFFFFFFFu, hg);
+      if (cut == 4) {
+        if (acc_c + c <= C && acc_g + g <= lim) { acc_c += c; acc_g += g; }
+        else cut = L;
+      }
+    };
+    level(3, nc3, hg3); level(2, nc2, hg2); level(1, nc1, hg1); level(0, nc0, hg0);
+    if (cut == 4) return make_uint2(acc_c, acc_g);
+  }
+  uint32_t taken = 0, sum = 0;
+  for (uint32_t p0 = H; static_cast<int32_t>(T - p0) > 0 && acc_c + taken < C; p0 += 32) {
+    const uint32_t p = p0 + lane;
+    const uint32_t m = static_cast<int32_t>(T - p) > 0 ? (rs[p & mask].y & 0xFFFFu) : SDB_META_TOMB;
+    const bool sel = m != SDB_META_TOMB && (!PRIO || (m >> 14) == cut);
+    const uint32_t g = sel ? (m & SDB_META_GLEN_MASK) - 1u : 0u;
+    const uint32_t b = __ballot_sync(0xFFFFFFFFu, sel);
+    const uint32_t k = acc_c + taken + lane_prefix(b, lane);                   // rank in the delivery order
+    const uint32_t run = acc_g + sum + sdb_warp_incl_scan(g, lane);
+    const bool ok = sel && k < C && (run <= lim || k == 0);
+    const uint32_t bo = __ballot_sync(0xFFFFFFFFu, ok);
+    sum += __reduce_add_sync(0xFFFFFFFFu, ok ? g : 0u);
+    taken += __popc(bo);
+    if (bo != b) break;                                        // an entry did not fit: the take ends before it
+  }
+  return make_uint2(acc_c + taken, acc_g + sum);
+}
+// one thread, the first n (<= 8) entries of a window without holes held in registers: records of the take, granules in gsum
+__device__ __forceinline__ uint32_t budget_take_regs(const uint64_t (&ev)[8], uint32_t n, uint32_t lim, uint32_t& gsum) {
+  uint32_t take = 0, sum = 0;
+  bool open = true;
+#pragma unroll
+  for (uint32_t j = 0; j < 8; ++j) {
+    if (open && j < n) {
+      const uint32_t g = (static_cast<uint32_t>(ev[j] >> 32) & SDB_META_GLEN_MASK) - 1u;
+      if (j == 0 || sum + g <= lim) { sum += g; take = j + 1; }
+      else open = false;
+    }
+  }
+  gsum = sum;
+  return take;
+}
+
+// MODE: SDB_PLAN_PLAIN (sdb_receive_batch, stream order), SDB_PLAN_BUDGET (byte budgets, stream order),
+// SDB_PLAN_BUDGET_PRIO (byte budgets, priority order: every agent is walked and selected by its warp).
+// budget = {per-agent limit, call capacity} in payload granules, read by the budget modes only.
+enum { SDB_PLAN_PLAIN = 0, SDB_PLAN_BUDGET = 1, SDB_PLAN_BUDGET_PRIO = 2 };
 // at most 64 registers (4 CTAs per SM, the shared-memory limit allows 5): with 80, which the compiler picks otherwise,
 // the c2 plan ran 13 % slower on an H100 (400 W power limit)
+template <int MODE>
 __global__ void __launch_bounds__(SDB_PLAN_TILE, 4)
-k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) {
+k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed, uint2 budget) {
+  constexpr bool BUDGET = MODE != SDB_PLAN_PLAIN, PRIO = MODE == SDB_PLAN_BUDGET_PRIO;
   __shared__ uint32_t s_tile;
   __shared__ unsigned long long s_wr[SDB_PLAN_WARPS], s_wg[SDB_PLAN_WARPS];
   __shared__ unsigned long long s_br, s_bg;
@@ -493,9 +567,10 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
       cnt = min(tail - head - nt, r.max_messages);
     }
   }
-  const bool holey = cnt && nt != 0;
+  const bool holey = cnt && (PRIO || nt != 0);      // planned by the warp (select_agent_warp)
   const bool simple = cnt && !holey;
   const bool in_regs = simple && cnt <= KEEP;       // entries held in ev[] (decided before any capacity truncation)
+  const bool walked = BUDGET ? cnt && !in_regs : holey;   // sized by the warp (long windows too under a byte budget)
   const uint2* rs = sdb_ring_of(v, valid && a < v.max_agents ? a : 0u);
   uint64_t ev[KEEP];
   uint32_t gsum = 0;
@@ -504,20 +579,29 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
 #pragma unroll
       for (uint32_t j = 0; j < KEEP; ++j)
         if (j < cnt) ev[j] = sdb_ld_u64_pol(reinterpret_cast<const uint64_t*>(rs + ((head + j) & mask)), pol);
+      if constexpr (BUDGET) {
+        cnt = budget_take_regs(ev, cnt, budget.x, gsum);
+      } else {
 #pragma unroll
-      for (uint32_t j = 0; j < KEEP; ++j)
-        if (j < cnt) gsum += (static_cast<uint32_t>(ev[j] >> 32) & SDB_META_GLEN_MASK) - 1u;
-    } else {
+        for (uint32_t j = 0; j < KEEP; ++j)
+          if (j < cnt) gsum += (static_cast<uint32_t>(ev[j] >> 32) & SDB_META_GLEN_MASK) - 1u;
+      }
+    } else if (!BUDGET) {
       for (uint32_t j = 0; j < cnt; ++j) gsum += (rs[(head + j) & mask].y & SDB_META_GLEN_MASK) - 1u;
     }
   }
   // agents with holes: their warp walks the window (rare: stream-order receive after priority receives)
-  for (uint32_t hb = __ballot_sync(0xFFFFFFFFu, holey); hb; hb &= hb - 1) {
+  for (uint32_t hb = __ballot_sync(0xFFFFFFFFu, walked); hb; hb &= hb - 1) {
     const uint32_t src = __ffs(hb) - 1;
     const uint32_t A_ = __shfl_sync(0xFFFFFFFFu, a, src), H_ = __shfl_sync(0xFFFFFFFFu, head, src);
     const uint32_t T_ = __shfl_sync(0xFFFFFFFFu, tail, src), C_ = __shfl_sync(0xFFFFFFFFu, cnt, src);
-    const uint32_t sum = holey_sum_warp(sdb_ring_of(v, A_), mask, H_, T_, C_, lane);
-    if (lane == src) gsum = sum;
+    if constexpr (BUDGET) {
+      const uint2 t = budget_take_warp<PRIO>(sdb_ring_of(v, A_), mask, H_, T_, C_, budget.x, lane);
+      if (lane == src) { cnt = t.x; gsum = t.y; }
+    } else {
+      const uint32_t sum = holey_sum_warp(sdb_ring_of(v, A_), mask, H_, T_, C_, lane);
+      if (lane == src) gsum = sum;
+    }
   }
 
   // ---- tile scan of {records, granules} (two 64-bit sums: a pathological tile may exceed 32 bits before truncation)
@@ -552,12 +636,26 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
   const unsigned long long pr = s_br + s_wr[warp] + ir - cnt, pg = s_bg + s_wg[warp] + ig - gsum;   // exclusive prefix of this slot
   const uint32_t roff = static_cast<uint32_t>(min(pr, 0xFFFFFFFFull));
   const uint32_t goff = static_cast<uint32_t>(min(pg, 0xFFFFFFFFull));
-  const bool over = cnt && pr + cnt > r.rec_cap;                                // does not fit: stays queued ...
+  const bool over = cnt && (pr + cnt > r.rec_cap || (BUDGET && pg + gsum > budget.y));   // does not fit: stays queued ...
   const bool lead = over && pr == 0;                                            // ... unless first in the output: then it
-  if (lead) cnt = static_cast<uint32_t>(r.rec_cap);                             // takes its first rec_cap records (their
-  else if (over) {                                                              // granules are summed while they are planned)
+  if (lead) {                                                                   // takes its first rec_cap records (their
+    if constexpr (BUDGET) {                                                     // granules are summed while they are planned)
+      cnt = static_cast<uint32_t>(min(static_cast<uint64_t>(cnt), r.rec_cap));  // or, under a byte budget, the longest
+    } else {                                                                    // prefix of its take that fits both caps
+      cnt = static_cast<uint32_t>(r.rec_cap);
+    }
+  } else if (over) {
     atomicMax(r.lb + totals_at, ~((static_cast<unsigned long long>(roff) << 32) | goff));
     cnt = 0;
+  }
+  if constexpr (BUDGET) {
+    for (uint32_t hb = __ballot_sync(0xFFFFFFFFu, lead); hb; hb &= hb - 1) {    // at most one in the call
+      const uint32_t src = __ffs(hb) - 1;
+      const uint32_t A_ = __shfl_sync(0xFFFFFFFFu, a, src), H_ = __shfl_sync(0xFFFFFFFFu, head, src);
+      const uint32_t T_ = __shfl_sync(0xFFFFFFFFu, tail, src), C_ = __shfl_sync(0xFFFFFFFFu, cnt, src);
+      const uint2 t = budget_take_warp<PRIO>(sdb_ring_of(v, A_), mask, H_, T_, C_, budget.y, lane);
+      if (lane == src) cnt = t.x;
+    }
   }
   if (valid) { r.count_out[q] = cnt; r.rec_off[q] = roff; }
 
@@ -609,7 +707,7 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed) 
     const uint32_t T_ = __shfl_sync(0xFFFFFFFFu, tail, src), C_ = __shfl_sync(0xFFFFFFFFu, cnt, src);
     const uint32_t N_ = __shfl_sync(0xFFFFFFFFu, nt, src), RO_ = __shfl_sync(0xFFFFFFFFu, roff, src);
     const uint32_t G_ = __shfl_sync(0xFFFFFFFFu, goff, src), Q_ = __shfl_sync(0xFFFFFFFFu, q, src);
-    select_agent_warp(v, r.plan, Q_, false, A_, H_, T_, N_, C_, RO_, lane, retire);
+    select_agent_warp(v, r.plan, Q_, PRIO, A_, H_, T_, N_, C_, RO_, lane, retire);
     __threadfence_block();
     __syncwarp();
     const uint32_t end = fill_offsets_warp(r.plan, RO_, C_, G_, lane);
@@ -1226,9 +1324,11 @@ extern "C" cudaError_t sdb_recv_prepare_device() {
 }
 
 // ca != nullptr: a compact receive (the same plan; the compact kernels replace the gather)
+// budget != nullptr: byte budgets (sdb_receive_budget), {per-agent limit, call capacity} in payload granules; both orders
+// take the single-pass plan
 extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_args* r0, cudaStream_t stream,
                                           int* n_launches, sdb_profiler* prof, int sm_count, uint32_t max_rec_bytes,
-                                          const sdb_compact_args* ca) {
+                                          const sdb_compact_args* ca, const uint2* budget) {
   if (r0->n == 0) return cudaSuccess;
   sdb_recv_args ra = *r0;
   sdb_recv_args* r = &ra;
@@ -1237,14 +1337,19 @@ extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_
   uint64_t bound = static_cast<uint64_t>(n) * r->max_messages;
   if (bound > r->rec_cap) bound = r->rec_cap;
   int pi;
-  if (!(r->flags & SDB_RECV_PRIORITY)) {
-    // ---- stream order: single-pass plan + gather
+  if (!(r->flags & SDB_RECV_PRIORITY) || budget) {
+    // ---- stream order (and byte budgets): single-pass plan + gather
     const uint32_t tiles = (n + SDB_PLAN_TILE - 1) / SDB_PLAN_TILE;
     r->plan_tops = nullptr;
     pi = sdb_prof_begin(prof, SDB_PK_RECV_SELECT, stream);
     cudaMemsetAsync(r->lb, 0, sdb_lb_words(tiles) * sizeof(unsigned long long), stream);
     static const uint32_t ticketed = (getenv("SDB_PLAN_TICKET") && atoi(getenv("SDB_PLAN_TICKET")) == 0) ? 0u : 1u;
-    k_recv_plan<<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, ticketed);
+    if (!budget)
+      k_recv_plan<SDB_PLAN_PLAIN><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, ticketed, make_uint2(0u, 0u));
+    else if (r->flags & SDB_RECV_PRIORITY)
+      k_recv_plan<SDB_PLAN_BUDGET_PRIO><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, ticketed, *budget);
+    else
+      k_recv_plan<SDB_PLAN_BUDGET><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, ticketed, *budget);
     sdb_prof_end(prof, pi, stream);
     if (n_launches) *n_launches += 1;
     if (ca) return launch_compact(v, r, ca, r->lb + sdb_lb_words(tiles) - 1, bound, sm_count, stream, prof, n_launches);
