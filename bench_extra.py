@@ -587,6 +587,156 @@ def where(rounds=3, block=4):
     return out
 
 
+def ids(rounds=3):
+    """The id clause of sdb_receive_where (SDB_FILTER_IDS) on the c2 backlog (1M agents, 65,536 group sends x 64 =
+    4,194,304 pending records, one seq per record): (a) one drop call for 65,536 random pending ids with id_hits (the
+    device call of SwarmsDB.delete_messages), each on a fresh backlog; (b) the per-id path delete_message used before,
+    one SDB_FILTER_SEQ [s, s + 1) drop over every agent per id, for 64 of those ids, every call timed; (c) the calls of
+    get_messages for 1,024 ids and of get_message for one: a DROP | PEEK count with id_agent over every agent, then a
+    PEEK of the agents that hold them; (d) id_hits of one broadcast queued at every agent, the contention worst case.
+    Outside the timed region the outputs are checked: every listed id is hit once, the 64 per-id drops remove one
+    record each, the lookups return the listed seqs and the broadcast counts every agent."""
+    import torch
+    from bench import ClockSampler, Workload
+    from swarmdb_b200._native import NO_RECEIVER, RECV_PEEK, WHERE_DROP, Shard, make_filter
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py ids: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    stream = torch.cuda.Stream()
+    shard = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L, list_pool_entries=wl.A + 1024)
+    shard.set_stream(stream.cuda_stream)
+    shard.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        shard.create_group(g, wl.members(g))
+    batch = wl.batch()
+    rng = np.random.default_rng(17)
+    state = {}
+
+    def backlog():
+        while shard.receive_batch(None, 1 << 10, copy_out=False)[1]:
+            pass
+        state["base"] = shard.send_group_batch(*batch)
+        shard.sync()
+
+    def timed(fn):
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        t = time.perf_counter()
+        r = fn()
+        wall = (time.perf_counter() - t) * 1e3
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return wall, e0.elapsed_time(e1), r
+
+    def profiled(fn):
+        shard.profile(True)
+        fn()
+        prof = shard.profile_read()
+        shard.profile(False)
+        return {k: v[0] for k, v in prof.items() if v[1]}
+
+    out = {"config": f"c2 backlog: {wl.A} agents, {wl.S} group sends x {wl.F} members = {per_step} pending records, "
+                     f"{wl.L}-B payloads, one seq per record"}
+    checks = {}
+    with torch.cuda.stream(stream):
+        backlog()
+        seqs = lambda n: (state["base"] + rng.choice(per_step, n, replace=False)).astype(np.uint64)
+        # (a) one bulk drop of 65,536 ids
+        n_a = 1 << 16
+        hits = np.zeros(n_a, np.uint32)
+        bulk = lambda ids: shard.receive_where(None, n_a, WHERE_DROP, make_filter(ids=ids), drop=True, id_hits=hits)
+        timed(lambda: bulk(seqs(n_a)))                                      # warm-up: allocates the id table
+        a_ms, a_ev, a_kern = [], [], []
+        for _ in range(rounds):
+            backlog()
+            ids_a = seqs(n_a)
+            wall, ev, (_, dropped) = timed(lambda: bulk(ids_a))
+            a_ms.append(wall); a_ev.append(ev)
+            checks["bulk_drop_hits_one_each"] = bool((hits == 1).all()) and dropped == n_a
+            backlog()
+            ids_a = seqs(n_a)
+            a_kern.append(profiled(lambda: bulk(ids_a)))
+        # (b) the per-id seq-range drop, 64 calls
+        backlog()
+        one = lambda s: shard.receive_where(None, 1, WHERE_DROP, make_filter(seq=(int(s), int(s) + 1)), drop=True)
+        timed(lambda: one(seqs(1)[0]))
+        b_ms, b_ev, b_drop = [], [], 0
+        for s in seqs(64):
+            wall, ev, (_, d) = timed(lambda: one(s))
+            b_ms.append(wall); b_ev.append(ev); b_drop += d
+        checks["per_id_drops_one_each"] = b_drop == 64
+        b_kern = profiled(lambda: one(seqs(1)[0]))
+        # (c) get_messages (1,024 ids) and get_message (1 id): count with id_agent, then PEEK the holders
+        backlog()
+
+        def lookup(ids):
+            where = np.zeros(len(ids), np.uint32)
+            f = make_filter(ids=ids)
+            shard.receive_where(None, 1, WHERE_DROP | RECV_PEEK, f, drop=True, id_agent=where)
+            holders = np.unique(where[where != NO_RECEIVER]).astype(np.uint32)
+            return shard.receive_where(holders, 1 << 20, RECV_PEEK, f)[1]
+        look = {}
+        for name, n in (("get_messages_1024", 1024), ("get_message_1", 1)):
+            lookup(seqs(n))
+            ms, ev = [], []
+            for _ in range(rounds * 4):
+                ids_c = seqs(n)
+                wall, e, hdr = timed(lambda: lookup(ids_c))
+                ms.append(wall); ev.append(e)
+                checks[name + "_found"] = sorted(hdr["seq"].tolist()) == sorted(ids_c.tolist())
+            look[name] = {"ms_per_call": float(np.median(ms)), "event_ms_per_call": float(np.median(ev)),
+                          "kernel_ms": profiled(lambda: lookup(seqs(n)))}
+        # (d) one broadcast queued at every agent: every record of the backlog is checked, all hits go to one slot
+        backlog()
+        shard.send_list_batch([0], np.array([0, wl.A], np.uint64), np.arange(wl.A, dtype=np.uint32), [1], [0], [16], [0],
+                              np.zeros(64, np.uint8))
+        shard.sync()
+        bc = shard.stats()["next_seq"] - 1
+        bh = np.zeros(1, np.uint32)
+        count = lambda: shard.receive_where(None, 1, WHERE_DROP | RECV_PEEK, make_filter(ids=[bc]), drop=True, id_hits=bh)
+        count()
+        d_ms = [timed(count)[0] for _ in range(rounds * 4)]
+        checks["broadcast_hits_every_agent"] = int(bh[0]) == wl.A
+        d_kern = profiled(count)
+        clocks = ClockSampler(0); clocks.start()
+        clk_probe = [timed(count)[0] for _ in range(8)]
+        clk = clocks.stop()
+    shard.close()
+    assert all(checks.values()), checks
+
+    peak = 3.35e12                                        # H100 SXM data sheet, HBM3
+    # algorithmic bytes of the where kernels: 16-B ring header per agent and, per pending record, its 8-B ring entry and
+    # 32-B header sector, plus one 8-B key read per probe of the id table (one probe per record)
+    scan = 16 * wl.A + per_step * (40 + 8)
+
+    def rate(kern, nbytes):
+        k = kern.get("where", 0.0)
+        return {"where_kernel_ms": k, "algorithmic_bytes": nbytes, "where_gb_per_s": nbytes / (k * 1e-3) / 1e9 if k else None,
+                "frac_of_3.35TB_s": nbytes / (k * 1e-3) / peak if k else None}
+    a_k = [k.get("where", 0.0) for k in a_kern]
+    out["bulk_drop_65536"] = {"ids": n_a, "records_dropped": n_a, "ms_per_call": float(np.median(a_ms)),
+                              "event_ms_per_call": float(np.median(a_ev)), "kernel_ms": a_kern[-1],
+                              **rate({"where": float(np.median(a_k))}, scan), "call_ms": a_ms}
+    b_med = float(np.median(b_ms))
+    out["per_id_drop"] = {"calls": 64, "ms_per_call": b_med, "event_ms_per_call": float(np.median(b_ev)),
+                          "ms_64_calls_measured": float(np.sum(b_ms)), "kernel_ms": b_kern,
+                          **rate(b_kern, 16 * wl.A + per_step * 40), "call_ms": b_ms}
+    out["bulk_vs_per_id_per_message"] = {"bulk_us_per_id": float(np.median(a_ms)) * 1e3 / n_a, "per_id_us": b_med * 1e3}
+    out.update(look)
+    out["broadcast_every_agent"] = {"agents": wl.A, "ms_per_call": float(np.median(d_ms)), "kernel_ms": d_kern,
+                                    **rate(d_kern, scan + 16 * wl.A + 40 * wl.A)}
+    out["oracle_checks"] = checks
+    out.update(_gpu_card(0))
+    out["clocks"] = clk
+    out["clock_probe_ms"] = clk_probe
+    return out
+
+
 def restore(rounds=3):
     """sdb_restore_compact on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 pending records): a
     snapshot (PEEK compact receive into pinned host buffers), its restore into a fresh handle from those buffers, and the

@@ -777,11 +777,28 @@ int sdb_arena_relocate(sdb_handle h, uint64_t floor_bytes, uint32_t flags, sdb_r
  *                 drop mode) and *payload_bytes_out reads 0.  DROP | PEEK is a dry-run count.
  *              7. SDB_EINVAL: a NULL filter or a wrong struct_bytes, unknown bits in fields or flags, SDB_RECV_ASYNC, a
  *                 NULL keyword with keyword_len > 0, keyword_len > SDB_FILTER_MAX_KEYWORD, drop mode with output
- *                 buffers, an agent listed twice or out of range.  SDB_EOUTPUT as in sdb_receive_batch.
+ *                 buffers, an agent listed twice or out of range; SDB_FILTER_IDS with the old struct_bytes, NULL ids (even
+ *                 with n_ids == 0), n_ids > SDB_FILTER_MAX_IDS, id_hits or id_agent without SDB_FILTER_IDS.  SDB_EOUTPUT as
+ *                 in sdb_receive_batch.
  *              8. The call always runs the bulk kernels (never the few-agent or latency-server paths); sdb_digest_fold
  *                 after it returns SDB_EINVAL until the next sdb_receive_batch.
+ *   Ids        SDB_FILTER_IDS matches the records whose seq is one of ids[0, n_ids): get_message / delete_message by id
+ *              on the device queue, many ids in one call.  ids is never NULL; duplicates are allowed, n_ids == 0 and id 0
+ *              (never a seq) match nothing.  The call builds an open-addressing hash table of the ids on the device (next power of two
+ *              >= 2 x n_ids slots of 16 bytes), and every record that passes the other header clauses costs one probe,
+ *              O(1) expected reads.  Per-id outputs (host arrays of n_ids, each nullable, only with the clause):
+ *                id_hits[i]   pending records of the listed agents with seq == ids[i] that pass every clause, counted
+ *                             when the records are evaluated: before max_messages and the capacity cut.  In drop mode
+ *                             with max_messages >= ring_slots it is the number of copies dropped.
+ *                id_agent[i]  the smallest agent index holding such a record, else SDB_NO_RECEIVER.
+ *              Duplicate ids read the same values.  A call that returns before running (no agents, max_messages == 0)
+ *              writes 0 and SDB_NO_RECEIVER.  Only pending records are found: a leased (in flight) or dead-lettered
+ *              record is not, and a deleted id that is leased elsewhere comes back only through its lease.
+ *              struct_bytes == offsetof(sdb_filter, n_ids), the size before this block, is still accepted, without
+ *              SDB_FILTER_IDS.
  *   Memory     one verdict bit per ring slot (max_agents x ring_slots bits) and a 256-byte keyword buffer, allocated on
- *              the first call. */
+ *              the first call; with SDB_FILTER_IDS the id table, the ids and the per-id outputs (at most 80 bytes per id
+ *              at the largest n_ids so far), allocated on the first call that needs them and grown on demand. */
 #define SDB_FILTER_SENDER   1u          /* header.sender == sender */
 #define SDB_FILTER_RECEIVER 2u          /* header.receiver == receiver (SDB_NO_RECEIVER: broadcast copies) */
 #define SDB_FILTER_GROUP    4u          /* header.group == group (SDB_NO_GROUP: non-group sends) */
@@ -791,10 +808,12 @@ int sdb_arena_relocate(sdb_handle h, uint64_t floor_bytes, uint32_t flags, sdb_r
 #define SDB_FILTER_SEQ      64u         /* seq_lo <= seq < seq_hi */
 #define SDB_FILTER_KEYWORD  128u        /* keyword occurs in the content bytes */
 #define SDB_FILTER_ICASE    256u        /* keyword compare folds ASCII A-Z/a-z only; every other byte is compared exactly */
+#define SDB_FILTER_IDS      512u        /* seq is one of ids[0, n_ids) */
 #define SDB_FILTER_MAX_KEYWORD 256u
+#define SDB_FILTER_MAX_IDS  4194304u    /* n_ids at most */
 #define SDB_WHERE_DROP 32u              /* flag: retire the matches without returning them */
 typedef struct sdb_filter {
-  uint32_t struct_bytes;    /* sizeof(sdb_filter) */
+  uint32_t struct_bytes;    /* sizeof(sdb_filter), or offsetof(sdb_filter, n_ids) without SDB_FILTER_IDS */
   uint32_t fields;          /* SDB_FILTER_* clauses that apply (ANDed); 0 matches every pending record */
   uint32_t sender;          /* SDB_FILTER_SENDER */
   uint32_t receiver;        /* SDB_FILTER_RECEIVER */
@@ -805,6 +824,10 @@ typedef struct sdb_filter {
   double   after, before;   /* SDB_FILTER_TIME */
   uint64_t seq_lo, seq_hi;  /* SDB_FILTER_SEQ */
   const uint8_t* keyword;   /* host pointer */
+  uint64_t n_ids;           /* SDB_FILTER_IDS: 0 .. SDB_FILTER_MAX_IDS */
+  const uint64_t* ids;      /* host pointers, [n_ids] each */
+  uint32_t* id_hits;
+  uint32_t* id_agent;
 } sdb_filter;
 int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
                       const sdb_filter* filter,

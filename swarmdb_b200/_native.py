@@ -46,8 +46,9 @@ LEASE_ACK = 0                   # sdb_lease_settle ops
 LEASE_RENEW = 1
 LEASE_ALL = 1                   # sdb_lease_sweep flag: every live lease is due
 FILTER_SENDER, FILTER_RECEIVER, FILTER_GROUP, FILTER_TYPE = 1, 2, 4, 8
-FILTER_PRIO, FILTER_TIME, FILTER_SEQ, FILTER_KEYWORD, FILTER_ICASE = 16, 32, 64, 128, 256
+FILTER_PRIO, FILTER_TIME, FILTER_SEQ, FILTER_KEYWORD, FILTER_ICASE, FILTER_IDS = 16, 32, 64, 128, 256, 512
 FILTER_MAX_KEYWORD = 256
+FILTER_MAX_IDS = 1 << 22
 TYPEF_JSON = 0x08
 TYPEF_EXTRAS = 0x10
 TYPE_MASK = 0x07
@@ -82,16 +83,18 @@ class SdbFilter(C.Structure):
     _fields_ = [("struct_bytes", C.c_uint32), ("fields", C.c_uint32), ("sender", C.c_uint32), ("receiver", C.c_uint32),
                 ("group", C.c_uint32), ("type_mask", C.c_uint8), ("prio_mask", C.c_uint8), ("keyword_len", C.c_uint16),
                 ("after", C.c_double), ("before", C.c_double), ("seq_lo", C.c_uint64), ("seq_hi", C.c_uint64),
-                ("keyword", C.c_void_p)]
+                ("keyword", C.c_void_p), ("n_ids", C.c_uint64), ("ids", C.c_void_p), ("id_hits", C.c_void_p),
+                ("id_agent", C.c_void_p)]
 
 
 def make_filter(sender=None, receiver=None, group=None, types=None, prios=None, after=None, before=None, seq=None,
-                keyword=None, icase=False) -> SdbFilter:
+                keyword=None, icase=False, ids=None) -> SdbFilter:
     """A filter for Shard.receive_where.  Each argument that is not None adds its clause: sender / receiver / group are
     indices (NO_RECEIVER selects broadcast copies, NO_GROUP non-group sends); types / prios are iterables of type codes
     (0..7) and priorities (0..3); after / before bound the timestamp strictly (either may be None: unbounded); seq is a
     half-open range (lo, hi); keyword (bytes or str, UTF-8) must occur in the content bytes, ASCII case folded with
-    icase.  The keyword bytes are kept alive by the returned object."""
+    icase; ids (an iterable of sequence numbers or a u64 array; duplicates allowed, empty matches nothing) selects the
+    records whose seq is listed.  The keyword bytes and the id array are kept alive by the returned object."""
     f = SdbFilter()
     f.struct_bytes = C.sizeof(SdbFilter)
     fields = 0
@@ -119,6 +122,14 @@ def make_filter(sender=None, receiver=None, group=None, types=None, prios=None, 
         f.keyword_len = len(kw) if len(kw) <= 0xFFFF else 0xFFFF
     if icase:
         fields |= FILTER_ICASE
+    if ids is not None:
+        a = ids if isinstance(ids, np.ndarray) else np.fromiter((int(x) for x in ids), np.uint64)
+        f._ids = np.ascontiguousarray(a, np.uint64)
+        if f._ids.ndim != 1:
+            raise ValueError("ids must be one-dimensional")
+        fields |= FILTER_IDS
+        f.n_ids = len(f._ids)
+        f.ids = f._ids.ctypes.data                                 # never NULL: the library refuses NULL ids
     f.fields = fields
     return f
 
@@ -811,13 +822,21 @@ class Shard:
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
 
     def receive_where(self, agents, max_messages: int, flags: int = 0, filt: Optional[SdbFilter] = None,
-                      drop: bool = False, out_hdr: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+                      drop: bool = False, out_hdr: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None,
+                      id_hits: Optional[np.ndarray] = None, id_agent: Optional[np.ndarray] = None):
         """Take (or with RECV_PEEK, only look at) the first max_messages pending records per agent that match `filt`
         (make_filter(); None matches every record), in delivery order (include/swarmdb_b200.h: sdb_receive_where).
         Returns receive_batch's (counts, headers, payload); what does not fit stays queued, so loop until nothing
-        comes back.  drop=True retires the matches on the device without returning them: (counts, total)."""
+        comes back.  drop=True retires the matches on the device without returning them: (counts, total).
+        With an id clause (make_filter(ids=...)), id_hits / id_agent (u32 arrays, one per listed id) receive each id's
+        matching records, counted before max_messages and the capacity cut, and the smallest agent holding one
+        (NO_RECEIVER: none)."""
         if filt is None:
             filt = make_filter()
+        n_ids = int(filt.n_ids) if filt.fields & FILTER_IDS else 0
+        for name, out in (("id_hits", id_hits), ("id_agent", id_agent)):
+            if out is not None and (out.dtype != np.uint32 or out.shape != (n_ids,) or not out.flags.c_contiguous):
+                raise ValueError(f"{name} must be a contiguous uint32 array of one entry per id ({n_ids})")
         a, n, counts = self._agents_arg(agents)
         total, pbytes = C.c_uint64(0), C.c_uint64(0)
         hdr = pay = None
@@ -826,9 +845,14 @@ class Shard:
         else:
             hdr = out_hdr if out_hdr is not None else self._grow_hdr()
             pay = out_payload if out_payload is not None else self._grow_pay()
-        self._check(self._L.sdb_receive_where(self._h, n, _p(a), max_messages, flags, C.byref(filt), _p(counts), _p(hdr),
-                                              0 if hdr is None else len(hdr), _p(pay), 0 if pay is None else pay.nbytes,
-                                              C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(pbytes), C.c_void_p)))
+        filt.id_hits, filt.id_agent = _p(id_hits), _p(id_agent)
+        try:
+            self._check(self._L.sdb_receive_where(self._h, n, _p(a), max_messages, flags, C.byref(filt), _p(counts),
+                                                  _p(hdr), 0 if hdr is None else len(hdr), _p(pay),
+                                                  0 if pay is None else pay.nbytes, C.cast(C.byref(total), C.c_void_p),
+                                                  C.cast(C.byref(pbytes), C.c_void_p)))
+        finally:
+            filt.id_hits = filt.id_agent = None                    # the filter does not keep the caller's arrays
         if agents is None:
             counts = self._served_counts(counts, flags)
         if drop:

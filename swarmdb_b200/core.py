@@ -39,7 +39,7 @@ import numpy as np
 from pydantic import BaseModel, Field
 
 from . import _native
-from ._native import (EXPIRE_ALL, FILTER_MAX_KEYWORD, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON,
+from ._native import (EXPIRE_ALL, FILTER_MAX_IDS, FILTER_MAX_KEYWORD, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON,
                       SdbError, Shard, make_filter, pad32, recv_capacity)
 
 
@@ -965,10 +965,15 @@ class SwarmsDB:
         return self._decode(hdr, pay, agent_id, record=False, status=MessageStatus.DELIVERED)
 
     def _where_filter(self, sender_id=None, receiver_idx=None, message_type=None, min_priority=None, group_name=None,
-                      after_timestamp=None, before_timestamp=None, keyword=None, case_sensitive=True):
-        """The device filter (make_filter) for these host-level clauses, or None when an unknown sender or group makes
-        it match nothing."""
+                      after_timestamp=None, before_timestamp=None, keyword=None, case_sensitive=True, message_ids=None):
+        """The device filter (make_filter) for these host-level clauses, or None when an unknown sender or group, or
+        message ids none of which this instance issued, make it match nothing."""
         kw = {}
+        if message_ids is not None:
+            seqs = [s for s in map(self._seq_of_id, message_ids) if s is not None]
+            if not seqs:
+                return None
+            kw["ids"] = np.array(seqs, np.uint64)
         if sender_id is not None:
             if sender_id not in self._agent_idx:
                 return None
@@ -993,18 +998,23 @@ class SwarmsDB:
                          message_type: Optional[MessageType] = None, min_priority: Optional[MessagePriority] = None,
                          group_name: Optional[str] = None, after_timestamp: Optional[float] = None,
                          before_timestamp: Optional[float] = None, keyword: Optional[str] = None,
-                         case_sensitive: bool = False) -> List[Message]:
+                         case_sensitive: bool = False, message_ids: Optional[Iterable[str]] = None) -> List[Message]:
         """A selective receive_messages: pop up to `max_messages` of the agent's pending messages that match every
         given clause, in stream order (priority order with GpuConfig.priority_dequeue), with receive_messages'
         bookkeeping; the other messages stay queued in their order.  The timestamp bounds are strict.  `keyword` must
         occur in the message content (its UTF-8 text; JSON content as json.dumps gives it), at most 256 bytes; the
-        case-insensitive compare folds ASCII letters only."""
+        case-insensitive compare folds ASCII letters only.  `message_ids` takes those specific messages (ids this
+        instance did not issue match nothing)."""
+        if message_ids is not None:
+            message_ids = list(message_ids)
+            if len(message_ids) > FILTER_MAX_IDS:
+                raise ValueError(f"more than {FILTER_MAX_IDS} message ids")
         if keyword is not None and len(keyword.encode("utf-8")) > FILTER_MAX_KEYWORD:
             raise ValueError(f"keyword longer than {FILTER_MAX_KEYWORD} bytes")     # taken records cannot be re-checked
         if not self._prepare_receive(agent_id):
             return []
         filt = self._where_filter(sender_id, None, message_type, min_priority, group_name, after_timestamp,
-                                  before_timestamp, keyword, case_sensitive)
+                                  before_timestamp, keyword, case_sensitive, message_ids)
         if max_messages <= 0 or filt is None:
             return []
         flags = RECV_PRIORITY if self.gpu_config.priority_dequeue else 0
@@ -1483,8 +1493,49 @@ class SwarmsDB:
         return {b: int(l) for b, l in zip(self._backend_name, self.shard.backend_loads())}
 
     # ------------------------------------------------------------------ host-side bookkeeping (M:603-808, 973-1206)
-    def get_message(self, message_id: str) -> Optional[Message]:
-        return self.messages.get(message_id)
+    def get_message(self, message_id: str, include_device: bool = False) -> Optional[Message]:
+        """The host record of `message_id` (M:603-613).  include_device=True also looks the id up on the device queue
+        when there is no host record (bulk sends, other ranks' traffic, messages sent before a load_message_history,
+        restored or redelivered records): one counting pass over every agent's queue finds the first agent holding
+        it, then one PEEK of that agent returns it, status DELIVERED.  Only pending messages are found (not leased or
+        dead-lettered ones), and only ids this instance issued."""
+        m = self.messages.get(message_id)
+        if m is not None or not include_device:
+            return m
+        return self.get_messages([message_id], include_device=True)[0]
+
+    def get_messages(self, message_ids: Iterable[str], include_device: bool = False) -> List[Optional[Message]]:
+        """get_message for many ids, in input order (None: not found).  With include_device=True the ids without a host
+        record are looked up on the device in one counting pass over every agent's queue, then one PEEK per part of
+        the agents that hold them; a host record wins over its device copy."""
+        ids = list(message_ids)
+        out: List[Optional[Message]] = [self.messages.get(mid) for mid in ids]
+        if not include_device:
+            return out
+        want = {}
+        for k, mid in enumerate(ids):
+            seq = self._seq_of_id(mid) if out[k] is None else None
+            if seq is not None:
+                want.setdefault(seq, []).append(k)
+        if not want:
+            return out
+        if len(want) > FILTER_MAX_IDS:
+            raise ValueError(f"more than {FILTER_MAX_IDS} distinct message ids")
+        self._pre_read()
+        filt = make_filter(ids=np.fromiter(want, np.uint64, count=len(want)))
+        where = np.empty(len(want), np.uint32)
+        agents, flags = self._expire_scope(None)
+        self.shard.receive_where(agents, 1, flags | RECV_PEEK, filt, drop=True, id_agent=where)
+        holders = np.unique(where[where != _native.NO_RECEIVER])
+        found: Dict[int, Message] = {}
+        for part, cap in self._pending_chunks(holders.astype(np.uint32), 1 << 31):
+            _, hdr, pay = self.shard.receive_where(part, cap, RECV_PEEK, filt)
+            for m, seq in zip(self._decode(hdr, pay, "", record=False, status=MessageStatus.DELIVERED), hdr["seq"].tolist()):
+                found.setdefault(seq, m)
+        for seq, ks in want.items():
+            for k in ks:
+                out[k] = found.get(seq)
+        return out
 
     def get_agent_messages(self, agent_id: str, status: Optional[MessageStatus] = None, limit: int = 100,
                            skip: int = 0) -> List[Message]:
@@ -1637,19 +1688,43 @@ class SwarmsDB:
         """Delete the host record (M:1132-1157).  include_device=True also drops every device-queued copy of the
         message (all copies of a broadcast), so it is never delivered; only ids this instance issued are looked up
         there.  True when anything was deleted."""
-        found = self.messages.pop(message_id, None) is not None
-        if found:
-            for inbox in self.agent_inbox.values():
-                if message_id in inbox:
-                    inbox.remove(message_id)
-        if include_device:
-            seq = self._seq_of_id(message_id)
-            if seq is not None:
-                self._pre_read()
-                agents, flags = self._expire_scope(None)
-                _, n = self.shard.receive_where(agents, 1, flags, make_filter(seq=(seq, seq + 1)), drop=True)
-                found = found or n > 0
-        return found
+        return self.delete_messages([message_id], include_device)[0]
+
+    def delete_messages(self, message_ids: Iterable[str], include_device: bool = False) -> List[bool]:
+        """delete_message for many ids, in input order: True where anything of that id was deleted.  With
+        include_device=True one device call drops every pending copy of every listed id (only ids this instance
+        issued are looked up there).  A leased (in flight) or dead-lettered copy is not pending and stays: a deleted
+        id that is leased elsewhere comes back only through its lease."""
+        ids = list(message_ids)
+        host = {}
+        for mid in dict.fromkeys(ids):
+            host[mid] = self.messages.pop(mid, None) is not None
+            if host[mid]:
+                for inbox in self.agent_inbox.values():
+                    if mid in inbox:
+                        inbox.remove(mid)
+        out = [host[mid] for mid in ids]
+        if not include_device:
+            return out
+        seq_of = {mid: self._seq_of_id(mid) for mid in host}
+        seqs = list(dict.fromkeys(s for s in seq_of.values() if s is not None))
+        if not seqs:
+            return out
+        if len(seqs) > FILTER_MAX_IDS:
+            raise ValueError(f"more than {FILTER_MAX_IDS} distinct message ids")
+        self._pre_read()
+        agents, flags = self._expire_scope(None)
+        # at most one copy per id and agent, as a send leaves it.  One id is the range [seq, seq + 1): the call's total
+        # answers it, with no id table to build; several ids take the id clause and its per-id hit counts.
+        if len(seqs) == 1:
+            _, n = self.shard.receive_where(agents, 1, flags, make_filter(seq=(seqs[0], seqs[0] + 1)), drop=True)
+            dropped = set(seqs) if n else set()
+        else:
+            hits = np.empty(len(seqs), np.uint32)
+            self.shard.receive_where(agents, len(seqs), flags, make_filter(ids=np.array(seqs, np.uint64)), drop=True,
+                                     id_hits=hits)
+            dropped = {s for s, h in zip(seqs, hits.tolist()) if h}
+        return [o or seq_of[mid] in dropped for o, mid in zip(out, ids)]
 
     def _seq_of_id(self, message_id: str) -> Optional[int]:
         """The sequence number behind an id this instance issued (_make_id), else None."""

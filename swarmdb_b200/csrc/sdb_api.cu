@@ -140,6 +140,10 @@ struct sdb_ctx {
   sdb_compact_args cx{};                                 // compact receive scratch + outputs, allocated on first use
   uint32_t* where_bits = nullptr;                        // filtered receive: verdict bitmap [max_agents][ceil(R / 32)] ...
   uint8_t* where_kw = nullptr;                           // ... and the keyword [SDB_FILTER_MAX_KEYWORD], allocated on first use
+  sdb_id_slot* id_tab = nullptr;                         // SDB_FILTER_IDS: id table [id_slots], the ids [id_cap] and the
+  unsigned long long* id_in = nullptr;                   // per-id outputs [2 x id_cap], allocated on the first call with
+  uint32_t* id_out = nullptr;                            // the clause and grown on demand
+  uint64_t id_cap = 0, id_slots = 0;
   unsigned long long* digest = nullptr;                  // [max_agents] stream digests, allocated on first use
   uint32_t* rs_agent = nullptr;                          // restore: per-agent tables [6][max_agents] + scan tops, allocated
   unsigned long long* rs_tot = nullptr;                  // on first use; totals [8]
@@ -958,6 +962,7 @@ int sdb_destroy(sdb_handle h) {
                  h->be_weight, h->be_load, h->be_scratch, h->be_logtab, h->be_req_cost, h->be_out, h->digest,
                  h->cx.table, h->cx.rec_slot, h->cx.head, h->cx.head_local, h->cx.head_tops, h->cx.gran, h->cx.gran_local,
                  h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out, h->where_bits, h->where_kw,
+                 h->id_tab, h->id_in, h->id_out,
                  h->rs_agent, h->rs_tot, h->rs_sort, h->rl_bits, h->rl_cnt, h->rl_pre, h->rl_tops, h->rl_sel, h->rl_tot};
   for (void* p : dev) if (p) cudaFree(p);
   lease_free(h);
@@ -2800,9 +2805,23 @@ int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   if (total_out) *total_out = 0;
   if (payload_bytes_out) *payload_bytes_out = 0;
   constexpr uint32_t all_fields = SDB_FILTER_SENDER | SDB_FILTER_RECEIVER | SDB_FILTER_GROUP | SDB_FILTER_TYPE | SDB_FILTER_PRIO |
-                                  SDB_FILTER_TIME | SDB_FILTER_SEQ | SDB_FILTER_KEYWORD | SDB_FILTER_ICASE;
-  if (!filter || filter->struct_bytes != sizeof(sdb_filter)) return fail(h, SDB_EINVAL, "sdb_receive_where: struct_bytes != sizeof(sdb_filter)");
+                                  SDB_FILTER_TIME | SDB_FILTER_SEQ | SDB_FILTER_KEYWORD | SDB_FILTER_ICASE | SDB_FILTER_IDS;
+  constexpr uint32_t v1_bytes = offsetof(sdb_filter, n_ids);  // the struct before the id block: callers built against it
+  if (!filter || (filter->struct_bytes != sizeof(sdb_filter) && filter->struct_bytes != v1_bytes))
+    return fail(h, SDB_EINVAL, "sdb_receive_where: struct_bytes is neither sizeof(sdb_filter) nor offsetof(sdb_filter, n_ids)");
   if (filter->fields & ~all_fields) return fail(h, SDB_EINVAL, "sdb_receive_where: unknown filter fields");
+  // the id block is read only with the full struct_bytes
+  const bool use_ids = (filter->fields & SDB_FILTER_IDS) != 0;
+  const uint64_t n_ids = use_ids ? filter->n_ids : 0;
+  uint32_t* const id_hits = filter->struct_bytes == v1_bytes ? nullptr : filter->id_hits;
+  uint32_t* const id_agent = filter->struct_bytes == v1_bytes ? nullptr : filter->id_agent;
+  if (use_ids) {
+    if (filter->struct_bytes == v1_bytes) return fail(h, SDB_EINVAL, "sdb_receive_where: SDB_FILTER_IDS needs struct_bytes == sizeof(sdb_filter)");
+    if (n_ids > SDB_FILTER_MAX_IDS) return fail(h, SDB_EINVAL, "sdb_receive_where: n_ids > SDB_FILTER_MAX_IDS");
+    if (!filter->ids) return fail(h, SDB_EINVAL, "sdb_receive_where: NULL ids (an empty set takes any other pointer)");
+  } else if (id_hits || id_agent) {
+    return fail(h, SDB_EINVAL, "sdb_receive_where: id_hits / id_agent without SDB_FILTER_IDS");
+  }
   if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_where returns host results: SDB_RECV_ASYNC is not accepted");
   if (flags & ~(SDB_RECV_PRIORITY | SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_WHERE_DROP))
     return fail(h, SDB_EINVAL, "sdb_receive_where accepts SDB_RECV_PRIORITY, SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_WHERE_DROP only");
@@ -2814,6 +2833,8 @@ int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   const bool drop = (flags & SDB_WHERE_DROP) != 0;
   if (drop && (hdr_out || payload_out)) return fail(h, SDB_EINVAL, "sdb_receive_where: drop mode takes no output buffers but count_out");
   const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
+  if (id_hits) std::fill(id_hits, id_hits + n_ids, 0u);
+  if (id_agent) std::fill(id_agent, id_agent + n_ids, SDB_NO_RECEIVER);
   if (n_agents == 0 || max_messages == 0) return SDB_OK;
   { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
   uint64_t rec_cap = ~0ull;
@@ -2831,19 +2852,44 @@ int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK), rec_cap, &r);
     if (rc != SDB_OK) return rc; }
   if (use_kw) CUDA_TRY(h, cudaMemcpyAsync(h->where_kw, filter->keyword, filter->keyword_len, cudaMemcpyHostToDevice, h->stream));
+  uint64_t id_slots = 64;                                     // a power of two >= 2 x n_ids (an empty table matches nothing)
+  while (id_slots < 2 * n_ids) id_slots <<= 1;
+  int nl = 0;
+  if (use_ids) {
+    if (id_slots > h->id_slots || n_ids > h->id_cap) {
+      const uint64_t cap = std::max(n_ids, h->id_cap), slots = std::max(id_slots, h->id_slots);
+      { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }   // cudaFree waits for the kernels on the device
+      for (void* p : {static_cast<void*>(h->id_tab), static_cast<void*>(h->id_in), static_cast<void*>(h->id_out)}) if (p) cudaFree(p);
+      h->id_tab = nullptr; h->id_in = nullptr; h->id_out = nullptr; h->id_cap = h->id_slots = 0;
+      const int rc = dmalloc_set(h, {{&h->id_tab, slots}, {&h->id_in, cap}, {&h->id_out, 2 * cap}},
+                                 "filtered receive: id table allocation failed");
+      if (rc != SDB_OK) return rc;
+      h->id_cap = cap; h->id_slots = slots;
+    }
+    CUDA_TRY(h, cudaMemsetAsync(h->id_tab, 0, id_slots * sizeof(sdb_id_slot), h->stream));
+    if (n_ids) CUDA_TRY(h, cudaMemcpyAsync(h->id_in, filter->ids, n_ids * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+    const cudaError_t e = sdb_launch_id_table(h->id_in, static_cast<uint32_t>(n_ids), h->id_tab, static_cast<uint32_t>(id_slots - 1),
+                                              h->stream, &nl);
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("id table launch: ") + cudaGetErrorString(e));
+  }
   sdb_where_args f{};
   f.fields = use_kw ? filter->fields : (filter->fields & ~SDB_FILTER_KEYWORD);
   f.sender = filter->sender; f.receiver = filter->receiver; f.group = filter->group;
   f.type_mask = filter->type_mask; f.prio_mask = filter->prio_mask; f.kw_len = use_kw ? filter->keyword_len : 0u;
   f.after = filter->after; f.before = filter->before; f.seq_lo = filter->seq_lo; f.seq_hi = filter->seq_hi;
   f.kw = h->where_kw; f.bits = h->where_bits; f.stride = stride;
-  int nl = 0;
+  f.id_tab = h->id_tab; f.id_mask = static_cast<uint32_t>(id_slots - 1); f.id_count = (id_hits || id_agent) && n_ids ? 1u : 0u;
   cudaError_t e = sdb_launch_where(&h->view, &r, &f, drop ? 1 : 0, 32u + pad32(h->cfg.max_payload_bytes), h->stream, &nl,
                                    &h->prof, h->sm_count);
+  if (e == cudaSuccess && f.id_count)
+    e = sdb_launch_id_out(h->id_in, static_cast<uint32_t>(n_ids), h->id_tab, f.id_mask, h->id_out, h->stream, &nl);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = false;       // no full receive to fold: the plan belongs to a filtered call
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("filtered receive launch: ") + cudaGetErrorString(e));
-  // drop mode has no output buffers, and its payload byte count stays 0
+  if (id_hits && f.id_count) CUDA_TRY(h, cudaMemcpyAsync(id_hits, h->id_out, n_ids * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  if (id_agent && f.id_count)
+    CUDA_TRY(h, cudaMemcpyAsync(id_agent, h->id_out + n_ids, n_ids * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  // drop mode has no output buffers, and its payload byte count stays 0; the synchronisation covers the id outputs
   return copy_full(h, n_agents, count_out, hdr_out, payload_out, total_out, drop ? nullptr : payload_bytes_out);
 }
 

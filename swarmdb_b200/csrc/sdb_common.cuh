@@ -193,6 +193,16 @@ struct sdb_where_args {
   const uint8_t* kw;           // [kw_len] device copy of the keyword (unfolded)
   uint32_t* bits;              // [max_agents][stride] bit j of agent a: the record at head + j matches
   uint32_t stride;             // words per agent = ceil(ring_slots / 32)
+  struct sdb_id_slot* id_tab;  // SDB_FILTER_IDS: open-addressing table [id_mask + 1] of the listed ids
+  uint32_t id_mask;            // table slots - 1 (a power of two >= 2 x the ids)
+  uint32_t id_count;           // 1: every match adds to its id's hit counter and first agent
+};
+
+// one slot of the id table of SDB_FILTER_IDS: key 0 is an empty slot (seq 0 is never assigned).  nagent holds ~agent so
+// that the zeroed table reads SDB_NO_RECEIVER and atomicMax keeps the smallest agent.
+struct __align__(16) sdb_id_slot {
+  unsigned long long key;
+  uint32_t hits, nagent;
 };
 
 // arguments of one restore (sdb_restore_compact): the compact-format input staged in the compact receive's buffers, the
@@ -838,6 +848,8 @@ cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double,
                               int*, sdb_profiler*, int);
 cudaError_t sdb_launch_where(const sdb_dev_view*, const sdb_recv_args*, const sdb_where_args*, int, uint32_t, cudaStream_t, int*,
                              sdb_profiler*, int);
+cudaError_t sdb_launch_id_table(const unsigned long long*, uint32_t, sdb_id_slot*, uint32_t, cudaStream_t, int*);
+cudaError_t sdb_launch_id_out(const unsigned long long*, uint32_t, const sdb_id_slot*, uint32_t, uint32_t*, cudaStream_t, int*);
 cudaError_t sdb_recv_prepare_device();
 cudaError_t sdb_balance_prepare_device();
 cudaError_t sdb_launch_receive_small(const sdb_dev_view*, const uint32_t*, uint32_t, uint32_t, uint32_t, uint32_t, uint4*,

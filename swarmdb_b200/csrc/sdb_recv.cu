@@ -1518,7 +1518,9 @@ extern "C" cudaError_t sdb_launch_expire(const sdb_dev_view* v, const sdb_recv_a
 //                   entries coalesced, the 32-byte header sector of every live entry with 4 loads per lane in flight
 //   k_where_kw      with a keyword: one warp per request slot, a lane per entry for the header clauses, then every
 //                   record that passes gets a warp-cooperative substring search of its content bytes
-//   both            write the verdict words and cnt[q] = min(matches, max_messages)
+//   both            write the verdict words and cnt[q] = min(matches, max_messages); with SDB_FILTER_IDS the seq of every
+//                   record that passes the other header clauses is probed in the id table (k_id_table), and with
+//                   per-id outputs every final match adds to its slot, once per warp and slot (k_id_out reads them out)
 //   scan            sdb_scan_u32 over cnt (take mode)
 //   k_where_select  capacity cut of k_recv_select, then the first count_out[q] set bits in delivery order (priority
 //                   order: one walk per level 3..0 over the entries' meta) are planned {handle, -, plan z, slot} and
@@ -1527,11 +1529,63 @@ extern "C" cudaError_t sdb_launch_expire(const sdb_dev_view* v, const sdb_recv_a
 //   back end        k_scan_plan + k_scan_tops, then the receive gather unchanged
 // ------------------------------------------------------------------------------------------
 #define SDB_WHERE_HDR_FIELDS (SDB_FILTER_SENDER | SDB_FILTER_RECEIVER | SDB_FILTER_GROUP | SDB_FILTER_TYPE | SDB_FILTER_PRIO | \
-                              SDB_FILTER_TIME | SDB_FILTER_SEQ)
+                              SDB_FILTER_TIME | SDB_FILTER_SEQ | SDB_FILTER_IDS)
 #define SDB_WHERE_STAGE 1024u     // content bytes staged per warp and step of the keyword search
+#define SDB_ID_NONE 0xFFFFFFFFu   // "no slot": the record is not a match of the id clause
 
-// lo = {seq lo, seq hi, timestamp lo, timestamp hi}, hi = {sender, receiver, group, len | prio << 16 | type << 24}
-__device__ __forceinline__ bool where_header(const sdb_where_args& f, const uint4& lo, const uint4& hi) {
+// id table of SDB_FILTER_IDS: linear probing from a 64-bit mix of the seq (sequence numbers are dense, so the low bits
+// alone would fill runs of neighbouring slots).  At most half the slots are used, so a probe ends at an empty slot.
+__device__ __forceinline__ uint32_t id_hash(unsigned long long k) {
+  k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
+  return static_cast<uint32_t>(k);
+}
+// the slot holding key s, or SDB_ID_NONE
+__device__ __forceinline__ uint32_t id_find(const sdb_id_slot* tab, uint32_t mask, unsigned long long s) {
+  if (s == 0) return SDB_ID_NONE;
+  for (uint32_t i = id_hash(s) & mask;; i = (i + 1) & mask) {
+    const unsigned long long k = __ldg(&tab[i].key);
+    if (k == s) return i;
+    if (k == 0) return SDB_ID_NONE;
+  }
+}
+
+// one kernel inserts every id with a 64-bit CAS; duplicates meet in one slot, id 0 (never a seq) is left out
+__global__ void __launch_bounds__(256)
+k_id_table(const unsigned long long* ids, uint32_t n, sdb_id_slot* tab, uint32_t mask) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n || ids[t] == 0) return;
+  const unsigned long long s = ids[t];
+  for (uint32_t i = id_hash(s) & mask;; i = (i + 1) & mask) {
+    const unsigned long long k = atomicCAS(&tab[i].key, 0ull, s);
+    if (k == 0 || k == s) return;
+  }
+}
+
+// the slots' values in input order: out[0, n) hits, out[n, 2n) first agent
+__global__ void __launch_bounds__(256)
+k_id_out(const unsigned long long* ids, uint32_t n, const sdb_id_slot* tab, uint32_t mask, uint32_t* out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const uint32_t i = id_find(tab, mask, ids[t]);
+  out[t] = i == SDB_ID_NONE ? 0u : tab[i].hits;
+  out[n + t] = i == SDB_ID_NONE ? SDB_NO_RECEIVER : ~tab[i].nagent;
+}
+
+// a match of agent a in id slot `slot` (SDB_ID_NONE: no match); whole warp.  The lanes that hit one slot add once: a
+// broadcast queued at every agent sends all its hits to one slot.
+__device__ __forceinline__ void where_count_id(const sdb_where_args& f, uint32_t slot, uint32_t a) {
+  const uint32_t grp = __match_any_sync(0xFFFFFFFFu, slot);
+  if (slot == SDB_ID_NONE) return;
+  const uint32_t na = __reduce_max_sync(grp, ~a);
+  if ((threadIdx.x & 31) == static_cast<uint32_t>(__ffs(grp) - 1)) {
+    atomicAdd(&f.id_tab[slot].hits, static_cast<uint32_t>(__popc(grp)));
+    atomicMax(&f.id_tab[slot].nagent, na);
+  }
+}
+
+// lo = {seq lo, seq hi, timestamp lo, timestamp hi}, hi = {sender, receiver, group, len | prio << 16 | type << 24};
+// *slot: the record's id-table slot when the id clause was tested (left alone otherwise)
+__device__ __forceinline__ bool where_header(const sdb_where_args& f, const uint4& lo, const uint4& hi, uint32_t* slot) {
   const uint32_t fl = f.fields;
   bool ok = true;
   if (fl & SDB_FILTER_SENDER) ok = ok && hi.x == f.sender;
@@ -1546,6 +1600,10 @@ __device__ __forceinline__ bool where_header(const sdb_where_args& f, const uint
   if (fl & SDB_FILTER_SEQ) {
     const unsigned long long s = (static_cast<unsigned long long>(lo.y) << 32) | lo.x;
     ok = ok && s >= f.seq_lo && s < f.seq_hi;
+  }
+  if ((fl & SDB_FILTER_IDS) && ok) {                          // last: one probe only for records every other clause passed
+    *slot = id_find(f.id_tab, f.id_mask, (static_cast<unsigned long long>(lo.y) << 32) | lo.x);
+    ok = *slot != SDB_ID_NONE;
   }
   return ok;
 }
@@ -1592,8 +1650,10 @@ k_where_eval(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
       uint32_t word = 0;
 #pragma unroll
       for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
-        const bool match = sdb_meta(e[u]) != SDB_META_TOMB && (!need_hdr || where_header(f, lo[u], hi[u]));
+        uint32_t slot = SDB_ID_NONE;
+        const bool match = sdb_meta(e[u]) != SDB_META_TOMB && (!need_hdr || where_header(f, lo[u], hi[u], &slot));
         word |= ((__ballot_sync(0xFFFFFFFFu, match) >> gsh) & 0xFFu) << (u * SDB_EXP_G);
+        if (f.id_count) where_count_id(f, match ? slot : SDB_ID_NONE, a);
       }
       if (l8 == 0 && j0 < W) bits[j0 >> 5] = word;
       got += __popc(word);
@@ -1663,7 +1723,8 @@ k_where_kw(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
         const uint4* src = reinterpret_cast<const uint4*>(v.arena + ((static_cast<uint64_t>(e.x) & v.gmask) << 5));
         lo = __ldg(src); hi = __ldg(src + 1);
       }
-      uint32_t word = __ballot_sync(0xFFFFFFFFu, lv && where_header(f, lo, hi));
+      uint32_t slot = SDB_ID_NONE;
+      uint32_t word = __ballot_sync(0xFFFFFFFFu, lv && where_header(f, lo, hi, &slot));
       for (uint32_t c = word; c; c &= c - 1) {
         const uint32_t src = __ffs(c) - 1;
         const uint32_t hx = __shfl_sync(0xFFFFFFFFu, e.x, src), hy = __shfl_sync(0xFFFFFFFFu, e.y, src);
@@ -1677,6 +1738,7 @@ k_where_kw(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
         }
         if (!where_find(p, (len + 31u) & ~31u, cs, ce, s_kw, K, icase, s_buf[warp], lane)) word &= ~(1u << src);
       }
+      if (f.id_count) where_count_id(f, ((word >> lane) & 1u) ? slot : SDB_ID_NONE, a);
       if (lane == 0) bits[j0 >> 5] = word;
       got += __popc(word);
     }
@@ -1810,6 +1872,26 @@ extern "C" cudaError_t sdb_launch_where(const sdb_dev_view* v, const sdb_recv_ar
   if (n_launches) *n_launches += 4;
   if (e != cudaSuccess) return e;
   return launch_gather(v, r, nullptr, bound, max_rec_bytes, sm_count, stream, prof, n_launches);
+}
+
+// the id table of SDB_FILTER_IDS from ids[0, n) into the zeroed tab[mask + 1]
+extern "C" cudaError_t sdb_launch_id_table(const unsigned long long* ids, uint32_t n, sdb_id_slot* tab, uint32_t mask,
+                                           cudaStream_t stream, int* n_launches) {
+  if (n) {
+    k_id_table<<<(n + 255) / 256, 256, 0, stream>>>(ids, n, tab, mask);
+    if (n_launches) ++*n_launches;
+  }
+  return cudaGetLastError();
+}
+
+// per input id, after the filtered receive: out[0, n) hits, out[n, 2n) first agent
+extern "C" cudaError_t sdb_launch_id_out(const unsigned long long* ids, uint32_t n, const sdb_id_slot* tab, uint32_t mask,
+                                         uint32_t* out, cudaStream_t stream, int* n_launches) {
+  if (n) {
+    k_id_out<<<(n + 255) / 256, 256, 0, stream>>>(ids, n, tab, mask, out);
+    if (n_launches) ++*n_launches;
+  }
+  return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------

@@ -286,8 +286,9 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
             agent_id=who, max_messages=max_messages, timeout=timeout))]
 
     @app.get("/messages/{message_id}", response_model=MessageOut)
-    def get_message(message_id: str, who: str = Depends(caller)):
-        m = db.get_message(message_id)
+    def get_message(message_id: str, include_device: bool = False, who: str = Depends(caller)):
+        # include_device: a message still queued on the device without a host record is found there too
+        m = guarded("get message", lambda: db.get_message(message_id, include_device))
         if m is None:
             raise HTTPException(status_code=http.HTTP_404_NOT_FOUND, detail=f"Message {message_id} not found")
         may_see = who == "admin" or who in (m.sender_id, m.receiver_id) or not m.visible_to or who in m.visible_to   # A:554-562

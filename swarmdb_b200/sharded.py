@@ -503,7 +503,10 @@ class ShardedSwarmsDB(SwarmsDB):
         traffic and returns message ids immediately (composite sequence numbers);
       * `flush()` is COLLECTIVE - every rank calls it; wire batches are exchanged and imported;
       * `receive_messages(agent)` is LOCAL to the rank that owns the agent
-        (`shard_of_agent(agent_id, world)`), and returns what earlier flushes delivered.
+        (`shard_of_agent(agent_id, world)`), and returns what earlier flushes delivered;
+      * device lookups by id (`get_message` / `get_messages` / `delete_message(s)` with include_device=True,
+        `receive_matching(..., message_ids=)`) are LOCAL, with no collective: each rank reads the queues of the agents
+        it owns, so a message queued for an agent of another rank is found (or deleted) on that rank.
     """
 
     def __init__(self, rank: int, world: int, *a, exchange_factory=None, shard=None, **k):
