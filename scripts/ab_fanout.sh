@@ -3,18 +3,16 @@
 OUT=${OUT:-bench_outputs}
 mkdir -p $OUT
 timeout 200 python -m pytest tests/test_gpu_xshard.py tests/test_gpu_parity.py -m gpu -x -q 2>&1 | tail -4
-run() {  # variant waves
-  SDB_FANOUT_VARIANT=$1 SDB_FANOUT_WAVES=$2 timeout 60 python scripts/proxy_import8.py 2>&1 | tail -1 | sed "s/^/v$1 w$2 proxy: /"
+run() {  # variant
+  SDB_FANOUT_VARIANT=$1 timeout 60 python scripts/proxy_import8.py 2>&1 | tail -1 | sed "s/^/v$1 proxy: /"
 }
 bench() {
-  SDB_FANOUT_WAVES=$2 timeout 100 python bench.py --steps 32 --warmup 4 --variant $1 --cpu-budget 0 > $OUT/ab.json 2> $OUT/ab.err
+  timeout 100 python bench.py --steps 32 --warmup 4 --variant $1 --cpu-budget 0 > $OUT/ab.json 2> $OUT/ab.err
   python - <<PY
 import json
 d=json.loads(open("$OUT/ab.json").read().strip().splitlines()[-1])
-print("v$1 w$2 bench:", round(d["value"]/1e9,3), round(d["ms_per_step"],4), {k:round(x["ms_per_launch"],4) for k,x in d["kernels"].items()}, round(d["roofline"]["frac"],4))
+print("v$1 bench:", round(d["value"]/1e9,3), round(d["ms_per_step"],4), {k:round(x["ms_per_launch"],4) for k,x in d["kernels"].items()}, round(d["roofline"]["frac"],4))
 PY
 }
-run 3 2
-run 3 4
-bench 3 2
-bench 3 4
+for v in 0 1 2 3; do run $v; done
+for v in 0 1 2 3; do bench $v; done

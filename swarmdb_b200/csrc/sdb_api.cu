@@ -118,8 +118,6 @@ struct sdb_ctx {
   uint8_t* wire_host = nullptr;                // pinned: header + descriptors of an export
   sdb_wire_header* hdrs_host = nullptr;        // pinned [num_shards]
   cudaEvent_t staging_free = nullptr;    // previous H2D of pinned staging has completed
-  cudaStream_t side = nullptr;           // the index build of a pure group batch runs beside the fan-out
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   // receive scratch + outputs
   uint32_t* rx_agent = nullptr; uint32_t* rx_cnt = nullptr; uint32_t* rx_rec_local = nullptr; uint32_t* rx_rec_tops = nullptr;
   uint4* rx_plan = nullptr; uint32_t* rx_rec_off = nullptr; unsigned long long* rx_lb = nullptr;
@@ -617,24 +615,6 @@ int submit(sdb_ctx* h, const sdb_staged* s, uint64_t* seq_base_out) {
   int rc = arena_reserve(h, s->total_grans, &base);
   if (rc != SDB_OK) return rc;
   cudaError_t e;
-  // a pure group batch has two independent halves: the payload fan-out (arena) and the index build (rings);
-  // the latter is latency-bound and runs on a side stream beside the former
-  // only when SDB_OVERLAP_INDEX is set: the two kernels contend for issue slots and HBM.  On an H100 (400 W) the c2
-  // step measured 1.234 ms with the overlap and 1.246 ms without, while the fan-out took 12 % and the index 53 % longer;
-  // it stays opt-in because that 1 % has not been measured at other power limits
-  static const bool allow_overlap = getenv("SDB_OVERLAP_INDEX") != nullptr;
-  const bool overlap = allow_overlap && s->has_pull && !s->has_atomic && s->kind != 0;
-  if (overlap) {
-    CUDA_TRY(h, cudaEventRecord(h->ev_fork, h->stream));
-    CUDA_TRY(h, cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-    sdb_pull_view pv{h->memb_off_dev, h->memb_grp_dev, h->memb_pos_dev, s->gs_off_dev, s->gs_idx_dev, 1u, 0u, 0u, nullptr};
-    int nlp = 0;
-    e = sdb_launch_pull(&h->view, &pv, s->descs_dev, h->n_agents, h->cfg.max_groups, h->gexcl_dev, h->n_excl_groups,
-                        h->n_shared_agents, h->lstart_dev, h->lcount_dev, base, 1, h->side, &h->prof, &nlp, nullptr, s->shared ? 1u : 0u);
-    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("index launch: ") + cudaGetErrorString(e));
-    CUDA_TRY(h, cudaEventRecord(h->ev_join, h->side));
-    h->launches += nlp;
-  }
   if (s->kind == 0) {
     e = sdb_launch_p2p(&h->view, s->descs_dev, s->n, s->payload_dev, h->next_seq, base, h->sm_count, h->stream, &h->prof, s->max_padlen);
     if (e == cudaSuccess && s->ranked) {      // entries are in send order already: publish them, nothing to sort
@@ -648,9 +628,10 @@ int submit(sdb_ctx* h, const sdb_staged* s, uint64_t* seq_base_out) {
                           s->max_padlen, static_cast<int>(h->cfg.fanout_variant), h->sm_count, h->stream, &h->prof, nullptr, 0u);
   }
   h->launches += 1;
-  if (e == cudaSuccess && overlap) {
-    CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_join, 0));
-  } else if (e == cudaSuccess && s->has_pull) {
+  // the index build (rings) follows the payload fan-out (arena) on the same stream.  Beside it on a second stream the
+  // two contend for issue slots and HBM: on an H100 (400 W) the fan-out took 12 % and the index 53 % longer, and the
+  // c2 step was only 1 % shorter (1.234 against 1.246 ms)
+  if (e == cudaSuccess && s->has_pull) {
     sdb_pull_view pv{h->memb_off_dev, h->memb_grp_dev, h->memb_pos_dev, s->gs_off_dev, s->gs_idx_dev, 1u, 0u, 0u, nullptr};
     int nlp = 0;
     e = sdb_launch_pull(&h->view, &pv, s->descs_dev, h->n_agents, h->cfg.max_groups, h->gexcl_dev, h->n_excl_groups,
@@ -791,15 +772,11 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
     return fail(h, SDB_ECUDA, "no CUDA device: swarmdb_b200 has no CPU fallback");
   if (c.device < 0 || c.device >= ndev) return fail(h, SDB_EINVAL, "device ordinal out of range");
   CUDA_TRY(h, cudaSetDevice(c.device));
-  {
-    // L2 fetch granularity 64 bytes (device-wide limit of this process; SDB_L2_FETCH=128 restores the default, 0 leaves
-    // the limit alone).  The receive gather reads 288-byte records at 32-byte alignment in receiver order: with the
-    // default 128-byte granularity every record costs three full lines (1.37x its bytes).  On an H100 (700 W) the c2
-    // step measured the same with 64 and 128 (1.229 ms); 64 is kept because it never moves more bytes.
-    const char* fg = getenv("SDB_L2_FETCH");
-    const int gran = fg ? atoi(fg) : 64;
-    if (gran > 0) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, static_cast<size_t>(gran));
-  }
+  // L2 fetch granularity 64 bytes (device-wide limit of this process).  The receive gather reads 288-byte records at
+  // 32-byte alignment in receiver order: with the default 128-byte granularity every record costs three full lines
+  // (1.37x its bytes).  On an H100 (700 W) the c2 step measured the same with 64 and 128 (1.229 ms); 64 is kept
+  // because it never moves more bytes.
+  cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 64);
   {
     // shared payloads for group sends above the pull threshold (sdb_common.cuh): SDB_SHARED_PAYLOAD=0 keeps one
     // payload copy per recipient in the arena log
@@ -815,9 +792,6 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
   CUDA_TRY(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   h->own_stream = true;
   CUDA_TRY(h, cudaEventCreateWithFlags(&h->staging_free, cudaEventDisableTiming));
-  CUDA_TRY(h, cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
-  CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-  CUDA_TRY(h, cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
 
   const size_t A = c.max_agents, R = c.ring_slots;
   h->arena_grans = c.arena_bytes / SDB_GRANULE;
@@ -980,9 +954,6 @@ int sdb_destroy(sdb_handle h) {
   if (h->small_host) cudaFreeHost(h->small_host);
   if (h->rx_small) cudaFree(h->rx_small);
   if (h->staging_free) cudaEventDestroy(h->staging_free);
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  if (h->ev_join) cudaEventDestroy(h->ev_join);
-  if (h->side) { cudaStreamSynchronize(h->side); cudaStreamDestroy(h->side); }
   if (h->prof.cap) {
     for (int i = 0; i < h->prof.cap; ++i) { cudaEventDestroy(h->prof.ev_a[i]); cudaEventDestroy(h->prof.ev_b[i]); }
     delete[] h->prof.kind; delete[] h->prof.ev_a; delete[] h->prof.ev_b;
@@ -1376,22 +1347,10 @@ int sdb_import_wire_ptrs(sdb_handle h, uint32_t n_src, const void* const* wire_p
   int rc = arena_reserve(h, total_grans, &base);
   if (rc != SDB_OK) return rc;
   e = sdb_launch_import_localize(&a, n_cap, h->xs_gs_cur /* goff */, h->xs_gs_off, h->stream, &h->prof, &nl);
-  static const bool allow_overlap_x = getenv("SDB_OVERLAP_INDEX") != nullptr;
-  const bool overlap = allow_overlap_x && n_other == 0;   // pure group traffic: index build beside the fan-out (off by default)
-  if (e == cudaSuccess && overlap) {
-    CUDA_TRY(h, cudaEventRecord(h->ev_fork, h->stream));
-    CUDA_TRY(h, cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-    sdb_pull_view pv{h->memb_off_dev, h->memb_grp_dev, h->memb_pos_dev, h->xs_gs_off, h->xs_gs_idx, 1u, 0u, 0u, nullptr};
-    e = sdb_launch_pull(&h->view, &pv, h->xs_descs, h->n_agents, h->cfg.max_groups, h->gexcl_dev, h->n_excl_groups,
-                        h->n_shared_agents, h->lstart_dev, h->lcount_dev, base, 1, h->side, &h->prof, &nl, nullptr, 0u);
-    if (e == cudaSuccess) CUDA_TRY(h, cudaEventRecord(h->ev_join, h->side));
-  }
   if (e == cudaSuccess)
     e = sdb_launch_fanout(&h->view, h->xs_descs, n_cap, nullptr, h->scratch.list_dev, h->next_seq, base, max_padlen,
                           h->cfg.fanout_variant >= 2 ? 3 : static_cast<int>(h->cfg.fanout_variant), h->sm_count, h->stream, &h->prof, nullptr, 0u);
-  if (e == cudaSuccess && overlap) {
-    CUDA_TRY(h, cudaStreamWaitEvent(h->stream, h->ev_join, 0));
-  } else if (e == cudaSuccess) {
+  if (e == cudaSuccess) {
     sdb_pull_view pv{h->memb_off_dev, h->memb_grp_dev, h->memb_pos_dev, h->xs_gs_off, h->xs_gs_idx, 1u, 0u, 0u, nullptr};
     e = sdb_launch_pull(&h->view, &pv, h->xs_descs, h->n_agents, h->cfg.max_groups, h->gexcl_dev, h->n_excl_groups,
                         h->n_shared_agents, h->lstart_dev, h->lcount_dev, base, n_other ? 0 : 1, h->stream, &h->prof, &nl, nullptr, 0u);

@@ -535,7 +535,7 @@ enum { SDB_PLAN_PLAIN = 0, SDB_PLAN_BUDGET = 1, SDB_PLAN_BUDGET_PRIO = 2 };
 // the c2 plan ran 13 % slower on an H100 (400 W power limit)
 template <int MODE>
 __global__ void __launch_bounds__(SDB_PLAN_TILE, 4)
-k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed, uint2 budget) {
+k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint2 budget) {
   constexpr bool BUDGET = MODE != SDB_PLAN_PLAIN, PRIO = MODE == SDB_PLAN_BUDGET_PRIO;
   __shared__ uint32_t s_tile;
   __shared__ unsigned long long s_wr[SDB_PLAN_WARPS], s_wg[SDB_PLAN_WARPS];
@@ -543,13 +543,11 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint32_t ticketed, 
   __shared__ uint4 s_stage[SDB_PLAN_WARPS][SDB_PLAN_STAGE];                // per warp: plan entries on their way out (32 KB)
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const size_t ticket_at = static_cast<size_t>(tiles) + 3 * ((tiles + 31) / 32), totals_at = ticket_at + 1;
-  // tile id: a ticket (dispatch order by construction) or, SDB_PLAN_TICKET=0, the block index (the hardware dispatches
-  // the blocks of a 1-D grid in index order, so earlier tiles are resident or finished: saves one L2 round trip)
-  if (ticketed) {
-    if (tid == 0) s_tile = atomicAdd(reinterpret_cast<unsigned int*>(r.lb + ticket_at), 1u);
-    __syncthreads();
-  }
-  const uint32_t tile = ticketed ? s_tile : blockIdx.x;
+  // tile id from a ticket: tiles start in ticket order by construction, so every earlier tile the look-back waits on is
+  // resident or finished
+  if (tid == 0) s_tile = atomicAdd(reinterpret_cast<unsigned int*>(r.lb + ticket_at), 1u);
+  __syncthreads();
+  const uint32_t tile = s_tile;
   const uint32_t q = tile * SDB_PLAN_TILE + tid;
   const bool valid = q < r.n;
   const bool retire = !(r.flags & SDB_RECV_PEEK);
@@ -769,6 +767,9 @@ k_recv_gather(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __restr
 // stream).  Two stages per warp: while step i is being stored, step i + 1 is already in flight.  A lane never touches
 // the bytes, so the kernel needs few registers, and a CTA keeps stage_bytes x 32 lanes x 2 stages x warps in flight -
 // several times what 16-byte loads held in registers can.  Used when a record fits the per-lane slot.
+// A per-lane bulk copy costs the warp ~12 issue slots (the copy engine takes its operands from uniform registers), which
+// looked like the limit with the payloads coming out of the L2.  It is not: a form with the whole warp moving the
+// payloads by 16-byte cp.async copies ran the c2 gather in the same 0.775 ms on an H100 (700 W) and was removed.
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
 k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __restrict__ packed_inv, uint32_t slot_bytes) {
@@ -834,77 +835,6 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
       } else if (hv && g) {
         sdb_tma_store(r.payload_out + ((st ? po1 : po0) << 5), wbase + (static_cast<size_t>(st) * 32u + lane) * slot_bytes, g << 5);
       }
-    }
-    sdb_tma_commit();
-  }
-  sdb_tma_wait_all<0>();
-}
-
-// The same gather with the payloads brought in by the whole warp with 16-byte asynchronous copies (cp.async, LDGSTS)
-// instead of one bulk load per lane.  A per-lane bulk copy costs the warp ~12 issue slots (the copy engine takes its
-// operands from uniform registers, so the 32 lanes issue one after the other); with the payloads coming out of the L2
-// that issue loop - not memory - looked like the limit.  It is not: on an H100 (700 W) this form runs the c2 gather
-// in the same time as the bulk-load form, 0.775 ms (SDB_GATHER_LDGSTS=1 selects it; both pass the whole parity suite).  Here one warp instruction
-// moves 512 bytes: lane l copies chunk (flat % cpr) of record (flat / cpr), flat = 32 f + l, the records' source
-// addresses travelling by shuffle.  Completion by cp.async groups (one per step, also when the step is empty), then a
-// proxy fence, then ONE bulk store of the warp's 32 slots when they are all full (else one per lane).
-template <int WARPS>
-__global__ void __launch_bounds__(WARPS * 32)
-k_recv_gather_cpa(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __restrict__ packed_inv, uint32_t slot_bytes) {
-  extern __shared__ __align__(128) uint8_t s_dyn[];          // [WARPS][2][32][slot_bytes]
-  const uint32_t total = gather_total(r, packed_inv);
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint8_t* const wbase = s_dyn + static_cast<size_t>(warp) * 2u * 32u * slot_bytes;
-  const uint32_t wbase_sa = sdb_smem_u32(wbase);
-  const uint32_t gw = blockIdx.x * WARPS + warp, nw = gridDim.x * WARPS;
-  const uint32_t cpr = slot_bytes >> 4;                      // 16-byte chunks per slot
-  uint32_t g0 = 0, g1 = 0; uint64_t po0 = 0, po1 = 0; bool hv0 = false, hv1 = false;
-  uint4 ha0 = make_uint4(0, 0, 0, 0), hb0 = ha0, ha1 = ha0, hb1 = ha0;
-  auto issue = [&](uint32_t st, uint32_t r0) {               // all lanes: request step r0 into stage st
-    const uint32_t rec = r0 + lane;
-    const bool have = rec < total;
-    uint32_t bytes = 0; uint4 pe = make_uint4(0, 0, 0, 0);
-    if (have) { pe = __ldg(r.plan + rec); bytes = (pe.z & 0xFFFFu) << 5; }
-    uint4 ha = make_uint4(0, 0, 0, 0), hb = ha;
-    unsigned long long psrc = 0;
-    if (have) {
-      const uint8_t* src = v.arena + ((static_cast<uint64_t>(pe.x) & v.gmask) << 5);
-      ha = sdb_ld_stream(src); hb = sdb_ld_stream(src + 16);
-      psrc = reinterpret_cast<unsigned long long>(sdb_payload_of(v, pe.x, sdb_entry_dm1(pe.z)));
-    }
-    const uint32_t stage_sa = wbase_sa + st * 32u * slot_bytes;
-    for (uint32_t f = 0; f < cpr; ++f) {
-      const uint32_t flat = (f << 5) + lane;
-      const uint32_t k = flat / cpr, c = flat - k * cpr;     // record of the step, chunk of its payload
-      const unsigned long long sk = __shfl_sync(0xFFFFFFFFu, psrc, k);
-      const uint32_t bk = __shfl_sync(0xFFFFFFFFu, bytes, k);
-      if ((c << 4) < bk)
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(stage_sa + k * slot_bytes + (c << 4)), "l"(sk + (c << 4)) : "memory");
-    }
-    const uint64_t po = static_cast<uint64_t>(pe.y) + ((have && r.plan_tops) ? r.plan_tops[rec / SDB_SCAN_TILE] : 0u);
-    if (st) { g1 = pe.z & 0xFFFFu; hv1 = have; po1 = po; ha1 = ha; hb1 = hb; }
-    else { g0 = pe.z & 0xFFFFu; hv0 = have; po0 = po; ha0 = ha; hb0 = hb; }
-  };
-  uint32_t r0 = gw * 32u;
-  if (r0 < total) issue(0, r0);
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  uint32_t st = 0;
-  for (; r0 < total; r0 += nw * 32u, st ^= 1u) {
-    const uint32_t rn = r0 + nw * 32u;
-    sdb_tma_wait_read<0>();                                  // the other stage's bulk stores have finished reading it
-    __syncwarp();
-    if (rn < total) issue(st ^ 1u, rn);
-    asm volatile("cp.async.commit_group;" ::: "memory");     // one group per step, empty or not: the wait below counts groups
-    const bool hv = st ? hv1 : hv0;
-    sdb_st_headers<32>(r.hdr_out + r0, sdb_sel4(st, ha1, ha0), sdb_sel4(st, hb1, hb0), hv, lane);
-    asm volatile("cp.async.wait_group 1;" ::: "memory");     // everything but the newest group: this stage has landed
-    __syncwarp();
-    sdb_fence_proxy_async();                                 // copies written through the generic proxy -> visible to the bulk store
-    const uint32_t g = st ? g1 : g0;
-    if (__all_sync(0xFFFFFFFFu, hv && (g << 5) == slot_bytes)) {
-      if (lane == 0) sdb_tma_store(r.payload_out + ((st ? po1 : po0) << 5), wbase + static_cast<size_t>(st) * 32u * slot_bytes, 32u * slot_bytes);
-    } else if (hv && g) {
-      sdb_tma_store(r.payload_out + ((st ? po1 : po0) << 5), wbase + (static_cast<size_t>(st) * 32u + lane) * slot_bytes, g << 5);
     }
     sdb_tma_commit();
   }
@@ -1289,25 +1219,18 @@ extern "C" cudaError_t sdb_launch_receive_small(const sdb_dev_view* v, const uin
 static cudaError_t launch_gather(const sdb_dev_view* v, const sdb_recv_args* r, const unsigned long long* packed_inv,
                                  uint64_t bound, uint32_t max_rec_bytes, int sm_count, cudaStream_t stream,
                                  sdb_profiler* prof, int* n_launches) {
-  static int use_tma = -1;
-  if (use_tma < 0) { const char* e = getenv("SDB_GATHER_TMA"); use_tma = e ? atoi(e) : 1; }
   const int pi = sdb_prof_begin(prof, SDB_PK_RECV_GATHER, stream);
-  if (use_tma && max_rec_bytes <= 544 && bound >= 4096) {
+  if (max_rec_bytes <= 544 && bound >= 4096) {
     constexpr int WARPS = 4;
     const uint32_t slot = max_rec_bytes > 64u ? max_rec_bytes - 32u : 32u;          // a slot stages the payload only
     const size_t smem = static_cast<size_t>(WARPS) * 2u * 32u * slot;
     uint32_t per_sm = static_cast<uint32_t>((226u * 1024u) / (smem + 1024 + 128));
     if (per_sm < 1) per_sm = 1;
     if (per_sm > 8) per_sm = 8;
-    static int waves = -1;
-    if (waves < 0) { const char* e = getenv("SDB_GATHER_WAVES"); waves = e ? atoi(e) : 8; if (waves < 1) waves = 1; }
-    uint64_t grid = static_cast<uint64_t>(sm_count) * per_sm * waves;              // a few waves: the tail evens out
+    uint64_t grid = static_cast<uint64_t>(sm_count) * per_sm * 8u;                 // 8 waves: the tail evens out
     const uint64_t need = (bound + WARPS * 32 - 1) / (WARPS * 32);
     if (grid > need) grid = need;
-    static int use_cpa = -1;
-    if (use_cpa < 0) { const char* e = getenv("SDB_GATHER_LDGSTS"); use_cpa = e ? atoi(e) : 0; }   // no faster: off
-    if (use_cpa) k_recv_gather_cpa<WARPS><<<static_cast<uint32_t>(grid), WARPS * 32, smem, stream>>>(*v, *r, packed_inv, slot);
-    else k_recv_gather_tma<WARPS><<<static_cast<uint32_t>(grid), WARPS * 32, smem, stream>>>(*v, *r, packed_inv, slot);
+    k_recv_gather_tma<WARPS><<<static_cast<uint32_t>(grid), WARPS * 32, smem, stream>>>(*v, *r, packed_inv, slot);
   } else {
     // 4 records per warp, 8 warps per block; grid-stride beyond ~4 waves
     k_recv_gather<<<sdb_grid(bound, 32, 32 * sm_count), 256, 0, stream>>>(*v, *r, packed_inv);
@@ -1318,8 +1241,6 @@ static cudaError_t launch_gather(const sdb_dev_view* v, const sdb_recv_args* r, 
 }
 
 extern "C" cudaError_t sdb_recv_prepare_device() {
-  cudaError_t e = cudaFuncSetAttribute(k_recv_gather_cpa<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2 * 32 * 544);
-  if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(k_recv_gather_tma<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2 * 32 * 544);
 }
 
@@ -1343,13 +1264,12 @@ extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_
     r->plan_tops = nullptr;
     pi = sdb_prof_begin(prof, SDB_PK_RECV_SELECT, stream);
     cudaMemsetAsync(r->lb, 0, sdb_lb_words(tiles) * sizeof(unsigned long long), stream);
-    static const uint32_t ticketed = (getenv("SDB_PLAN_TICKET") && atoi(getenv("SDB_PLAN_TICKET")) == 0) ? 0u : 1u;
     if (!budget)
-      k_recv_plan<SDB_PLAN_PLAIN><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, ticketed, make_uint2(0u, 0u));
+      k_recv_plan<SDB_PLAN_PLAIN><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, make_uint2(0u, 0u));
     else if (r->flags & SDB_RECV_PRIORITY)
-      k_recv_plan<SDB_PLAN_BUDGET_PRIO><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, ticketed, *budget);
+      k_recv_plan<SDB_PLAN_BUDGET_PRIO><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, *budget);
     else
-      k_recv_plan<SDB_PLAN_BUDGET><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, ticketed, *budget);
+      k_recv_plan<SDB_PLAN_BUDGET><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, *budget);
     sdb_prof_end(prof, pi, stream);
     if (n_launches) *n_launches += 1;
     if (ca) return launch_compact(v, r, ca, r->lb + sdb_lb_words(tiles) - 1, bound, sm_count, stream, prof, n_launches);

@@ -1404,8 +1404,7 @@ extern "C" cudaError_t sdb_launch_p2p(const sdb_dev_view* v, const sdb_send_desc
   // 8 warps x 4 records per step; ~4 waves of 8 CTAs/SM, grid-stride beyond
   const uint32_t grid = sdb_grid(n, 8 * 4, 32 * sm_count);
   const int pi = sdb_prof_begin(prof, SDB_PK_P2P, stream);
-  static const bool use_tma = !(getenv("SDB_P2P_TMA") && atoi(getenv("SDB_P2P_TMA")) == 0);
-  if (use_tma && max_padlen <= 512u) {
+  if (max_padlen <= 512u) {
     constexpr int WARPS = 4;
     const uint32_t slot = max_padlen < 32u ? 32u : max_padlen;
     const size_t smem = static_cast<size_t>(WARPS) * 2u * 32u * slot;
@@ -1469,9 +1468,8 @@ extern "C" cudaError_t sdb_launch_fanout(const sdb_dev_view* v, const sdb_send_d
     const size_t smem = static_cast<size_t>(WARPS) * (SDB_SPAN_DESC * sizeof(sdb_send_desc) + SDB_SPAN_TABLES + static_cast<size_t>(SDB_SPAN_PAY) * stage);
     uint32_t per_sm = 8;
     while (per_sm > 1 && per_sm * (smem + 1024) > 200 * 1024) --per_sm;
-    static int mult = 0;                                    // CTA waves per SM slot: > 1 lets the block scheduler even out the tail
-    if (!mult) { const char* e = getenv("SDB_FANOUT_WAVES"); mult = e ? atoi(e) : 4; if (mult < 1) mult = 1; }
-    uint32_t grid = static_cast<uint32_t>(sm_count) * per_sm * static_cast<uint32_t>(mult);
+    // 4 CTA waves per SM slot: more than one lets the block scheduler even out the tail
+    uint32_t grid = static_cast<uint32_t>(sm_count) * per_sm * 4u;
     const uint32_t need = (n + WARPS - 1) / WARPS;
     if (grid > need) grid = need;
     k_group_fanout_span<WARPS><<<grid, WARPS * 32, smem, stream>>>(*v, descs, n, payload, tmp_list, seq_base, arena_base, stage, bb, skip_pull);

@@ -3,19 +3,13 @@ halves so that two lanes write one header in one instruction (sdb_st_headers).  
 (the sender itself, skipped) stays unwritten, and the last warp step of a receive gather holds fewer than 32 records.
 These tests put skipped senders at every tile position of groups whose sizes are not multiples of the tile (the wide
 fan-out, 32 lanes per send, and the narrow one, 8 lanes per send, that imports use at 4 shards and more) and drain
-through the bulk-copy gathers with totals that leave a partial last step, against the CPU oracle.
+through the bulk-copy gather with totals that leave a partial last step, against the CPU oracle.
 """
-import os
-import subprocess
-import sys
-from pathlib import Path
-
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
-ROOT = Path(__file__).resolve().parents[1]
 # tails of 1..31 records after whole tiles of 8, 16, 32 and 64 headers
 SIZES = [1, 2, 7, 9, 31, 32, 33, 63, 64, 65, 97, 131]
 EXTRA = 64                       # agents in no group: they send too
@@ -146,11 +140,3 @@ def test_skipped_senders_narrow_fanout_four_shards():
             s.close()
         oracle.close()
 
-
-def test_cp_async_gather_stores_the_same_headers():
-    """The same single-shard drain through the cp.async gather (SDB_GATHER_LDGSTS=1 is read once per process)."""
-    env = dict(os.environ, SDB_GATHER_LDGSTS="1")
-    cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider",
-           "tests/test_gpu_header_sectors.py::test_skipped_senders_and_partial_gather_steps_one_shard"]
-    p = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=600)
-    assert p.returncode == 0, p.stdout[-3000:] + p.stderr[-3000:]
