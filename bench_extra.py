@@ -1259,6 +1259,116 @@ def budget(rounds=2, per_agent=2):
     return out
 
 
+def dedup(rounds=2, batch=1 << 16, n=1 << 20, L=256):
+    """Deduplicated sends (sdb_send_mixed_batch_dedup) against plain sdb_send_mixed_batch of the same batches.
+    send: n point-to-point sends of L bytes (one per agent), in batches of `batch`, host clock to a synchronise, each
+      mode alternated with a plain run: zero keys (the table is consulted by nobody: the probe and its one
+      synchronisation alone), explicit keys without duplicates, content keys, and content keys where the second half
+      of every batch repeats the first (half duplicates).
+    kernels: from torch.profiler in a run of its own: the content-key kernel's payload bytes per second against the
+      H100 SXM data sheet's 3.35 TB/s, and a rebuild of a table of n entries of which half have expired."""
+    import torch
+    from swarmdb_b200._native import Shard
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py dedup: no CUDA device - swarmdb_b200 has no CPU fallback")
+    A = n
+    shard = Shard(max_agents=A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=L, max_batch_sends=batch,
+                  max_batch_payload=batch * L + 64)
+    shard.register(np.arange(A, dtype=np.uint32))
+    shard.dedup_reserve(4 * n, 1e9)
+    rng = np.random.default_rng(9)
+    pay = torch.empty(batch * L + 64, dtype=torch.uint8, pin_memory=True).numpy()
+    pay[:] = rng.integers(0, 256, len(pay), dtype=np.uint8)
+    half = pay.copy()
+    half[batch // 2 * L: batch * L] = half[: batch // 2 * L]
+    half_pin = torch.empty(len(half), dtype=torch.uint8, pin_memory=True).numpy()
+    half_pin[:] = half
+    off = np.arange(batch, dtype=np.uint64) * L
+    lens, kind, z8, ts = np.full(batch, L, np.uint16), np.zeros(batch, np.uint8), np.zeros(batch, np.uint8), np.zeros(batch)
+    lo = np.zeros(1, np.uint64)
+    key_ctr = [1]
+
+    def run(mode):
+        shard.dedup_reserve(4 * n, 1e9)                               # a cleared table for every run
+        ndup = 0
+        shard.sync()
+        t = time.perf_counter()
+        for b in range(0, n, batch):
+            recv = np.arange(b, b + batch, dtype=np.uint32)
+            snd = recv ^ 1
+            p = half_pin if mode == "content_half_dup" else pay
+            if mode == "plain":
+                shard.send_mixed_batch(snd, kind, recv, lo, None, z8, z8, lens, off, p, ts)
+                continue
+            keys = None
+            if mode == "keys":
+                k = np.arange(key_ctr[0], key_ctr[0] + batch, dtype=np.uint64)
+                key_ctr[0] += batch
+                keys = np.stack([k, k], 1)
+            if mode == "content_half_dup":
+                snd = snd.copy(); snd[batch // 2:] = snd[: batch // 2]
+                recv = recv.copy(); recv[batch // 2:] = recv[: batch // 2]
+            _, dup, _ = shard.send_mixed_batch_dedup(snd, kind, recv, lo, None, z8, z8, lens, off, p, ts, keys=keys,
+                                                     content=mode.startswith("content"), now=1.0)
+            ndup += int((dup != 0).sum())
+        shard.sync()
+        return time.perf_counter() - t, ndup
+
+    modes = ("zero_keys", "keys", "content", "content_half_dup")
+    res = {m: [] for m in modes}
+    res["plain"] = []
+    for r in range(rounds):
+        for m in modes:
+            for name in (("plain", m) if r % 2 == 0 else (m, "plain")):
+                sec, ndup = run(name)
+                res[name].append({"s": sec, "ns_per_send": sec * 1e9 / n, "duplicates": ndup})
+        shard.receive_compact(None, 1 << 10, 0)          # keep the rings clear between rounds
+    out = {"send_config": f"{n} point-to-point {L}-B sends in batches of {batch}, one per agent over {A} agents; "
+                          f"{rounds} rounds, each mode alternated with plain",
+           "send": {k: {"runs": v, "ns_per_send": float(np.median([x["ns_per_send"] for x in v]))} for k, v in res.items()}}
+    shard.close()
+
+    # ---- kernel times: the content-key kernel, and a rebuild with half of the entries expired
+    from torch.profiler import ProfilerActivity, profile
+    shard = Shard(max_agents=A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=L, max_batch_sends=batch,
+                  max_batch_payload=batch * L + 64)
+    shard.register(np.arange(A, dtype=np.uint32))
+    recv = np.arange(batch, dtype=np.uint32)
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        shard.dedup_reserve(4 * n, 1e9)
+        for _ in range(4):
+            shard.send_mixed_batch_dedup(recv ^ 1, kind, recv, lo, None, z8, z8, lens, off, pay, ts, content=True, now=6.0)
+            shard.receive_compact(None, 1 << 10, 0)
+        shard.dedup_reserve(n, 10.0)
+        for b in range(0, n, batch):                               # n keys: half at now = 0, half at now = 5
+            k = np.arange(b + 1, b + batch + 1, dtype=np.uint64)
+            shard.send_mixed_batch_dedup(recv ^ 1, kind, recv, lo, None, z8, z8, lens, off, pay, ts,
+                                         keys=np.stack([k, k], 1), now=0.0 if b < n // 2 else 5.0)
+            shard.receive_compact(None, 1 << 10, 0)
+        # the table is full and half of it expired at now = 10: the next new keys rebuild it
+        k = np.arange(n + 1, n + 1 + batch, dtype=np.uint64)
+        shard.send_mixed_batch_dedup(recv ^ 1, kind, recv, lo, None, z8, z8, lens, off, pay, ts,
+                                     keys=np.stack([k, k], 1), now=10.0)
+        shard.sync()
+    ds = shard.dedup_stats()
+    shard.close()
+    ev = {}
+    for e in prof.key_averages():
+        for name in ("k_dedup_content", "k_dedup_rebuild", "k_dedup_probe", "k_dedup_verdict", "k_dedup_insert"):
+            if name in e.key:
+                ev[name] = {"us_avg": e.device_time_total / max(e.count, 1), "count": e.count}
+    hash_bytes = batch * L
+    if "k_dedup_content" in ev:
+        bps = hash_bytes / (ev["k_dedup_content"]["us_avg"] * 1e-6)
+        ev["k_dedup_content"]["payload_bytes"] = hash_bytes
+        ev["k_dedup_content"]["bytes_per_s"] = bps
+        ev["k_dedup_content"]["share_of_3_35_TBps"] = bps / 3.35e12
+    out["kernels"] = ev
+    out["rebuild"] = {"table_entries": n, "expired_before": n // 2, "stats_after": ds}
+    out.update(_gpu_card(0))
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", nargs="*", default=["c1", "c4", "c5", "k1", "bcast"])

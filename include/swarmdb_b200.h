@@ -133,10 +133,13 @@ enum { SDB_PK_P2P = 0, SDB_PK_FANOUT, SDB_PK_COMMIT, SDB_PK_RECV_COUNT, SDB_PK_R
        SDB_PK_RECV_COMPACT = 12, SDB_PK_EXPIRE = 13, SDB_PK_WHERE = 14, SDB_PK_RESTORE = 15, SDB_PK_N = 16,
        /* classes past SDB_PK_N: sdb_profile_read fills SDB_PK_N entries (the array size of every ABI-1 caller), so
           these are read with sdb_profile_read_n only */
-       SDB_PK_LEASE = 16, SDB_PK_ALL = 17 };
+       SDB_PK_LEASE = 16, SDB_PK_ALL = 17,
+       /* classes past SDB_PK_ALL (the array size of callers written before them): read with sdb_profile_read_n, whose
+          n asks for them; SDB_PK_CLASSES counts every class */
+       SDB_PK_DEDUP = 17, SDB_PK_CLASSES = 18 };
 int sdb_profile(sdb_handle h, int enable);
 int sdb_profile_read(sdb_handle h, double* ms_out /* [SDB_PK_N] */, uint64_t* count_out /* [SDB_PK_N] */);
-/* The same for the first min(n, SDB_PK_ALL) classes (entries from there to n are zeroed); like sdb_profile_read it
+/* The same for the first min(n, SDB_PK_CLASSES) classes (entries from there to n are zeroed); like sdb_profile_read it
  * consumes the recorded intervals. */
 int sdb_profile_read_n(sdb_handle h, uint32_t n, double* ms_out /* [n] */, uint64_t* count_out /* [n] */);
 
@@ -861,6 +864,57 @@ int sdb_select_backend_batch(sdb_handle h, uint32_t n_req, const uint32_t* cost,
  * backlog.  Call it before sdb_select_backend_batch whenever the loads should track the queues. */
 int sdb_assign_agent_backends(sdb_handle h, uint32_t n, const uint32_t* agent_idx, const uint32_t* backend_idx);
 int sdb_backend_loads_from_queues(sdb_handle h);
+
+/* ---- deduplicated sends: a producer names a message with a 128-bit key, and a second send with a key the table holds
+ * as a live entry is not written (SQS MessageDeduplicationId, NATS Msg-Id).  Off until sdb_dedup_reserve.
+ *   sdb_dedup_reserve           a table of `entries` keys (load factor at most 1/2, 32 bytes a slot, two buffers) with
+ *                               the given window (> 0 s); 0 entries frees it.  Either clears the table.
+ *   sdb_send_mixed_batch_dedup  sdb_send_mixed_batch's arguments up to timestamp, then one key per send (NULL: every key
+ *                               {0,0}), and seq_base_out last.  A send
+ *                               with key {0,0} bypasses the table unless SDB_DEDUP_CONTENT gives it its content key (the
+ *                               hash of sender, kind, target or the list's recipients, len, prio, type and payload; not
+ *                               the timestamp; INTEGRATION.md §3.9).  A send is a duplicate when the table holds its key
+ *                               as an entry live at `now` (now < inserted_at + window), or when an earlier send of the
+ *                               batch has the key.  Accepted sends are written exactly as sdb_send_mixed_batch writes the
+ *                               batch without the duplicates, with the sequence numbers the whole batch gives them; a
+ *                               duplicate's numbers stay unused, and it writes nothing and is not counted in `enqueued`.
+ *                               dup_of_out[i]: the first seq of the original send (0: accepted); key_out[i]: the key
+ *                               used; *n_dup_out: duplicates.  Then every accepted keyed send stores (key, its first seq,
+ *                               now); when the new keys would take the occupied slots past `entries`, a rebuild first
+ *                               drops the entries not live at `now`.  Refusals leave rings, arena, the seq counter, the
+ *                               table and sdb_dedup_stats unchanged, and sdb_stats too except kernel_launches, which
+ *                               counts the probe (and counting) kernels a refused call ran: SDB_EARENA_FULL,
+ *                               SDB_ECAPACITY (the new keys do not fit beside the live entries), SDB_EINVAL (no table, a
+ *                               non-finite now, unknown flags, a non-zero key or SDB_DEDUP_CONTENT on a sharded handle,
+ *                               or any argument sdb_send_mixed_batch refuses).
+ *   sdb_dedup_forget            kill the entries of the given keys; removed_out[i] = 1 where the entry was live at the
+ *                               `now` of the last send call.
+ *   sdb_dedup_stats             capacity, entries live at the last send call's `now`, occupied slots and totals.
+ * Restores, requeues, lease redeliveries, redrives and cross-shard imports neither consult nor fill the table, and
+ * expiry or delete-by-id remove no key.  Snapshots do not carry it.  Kernels are timed under SDB_PK_DEDUP. */
+typedef struct sdb_dedup_key { uint64_t lo, hi; } sdb_dedup_key;      /* {0,0}: not deduplicated */
+#define SDB_DEDUP_CONTENT 1u          /* sends whose key is {0,0} (all of them when key == NULL) get the content key */
+typedef struct sdb_dedup_summary {
+  uint64_t capacity;            /* entries the table takes */
+  uint64_t live;                /* entries live at the last send call's now */
+  uint64_t used;                /* occupied slots: live, expired and forgotten entries until a rebuild drops them */
+  double window;                /* seconds */
+  uint64_t accepted_total;      /* keyed sends accepted (entries stored) */
+  uint64_t duplicate_total;     /* sends refused as duplicates */
+  uint64_t expired_total;       /* entries dropped by rebuilds (expired or forgotten) */
+  uint64_t forgotten_total;     /* entries killed by sdb_dedup_forget */
+  uint64_t rebuilds;
+} sdb_dedup_summary;
+int sdb_dedup_reserve(sdb_handle h, uint64_t entries, double window_seconds);
+int sdb_send_mixed_batch_dedup(sdb_handle h, uint32_t n, const uint32_t* sender, const uint8_t* kind, const uint32_t* target,
+                               uint32_t n_lists, const uint64_t* list_off, const uint32_t* list_idx, const uint8_t* prio,
+                               const uint8_t* type, const uint16_t* len, const uint64_t* payload_off, const uint8_t* payload,
+                               uint64_t payload_bytes, const double* timestamp,
+                               const sdb_dedup_key* key /* [n], nullable */, uint32_t flags, double now,
+                               sdb_dedup_key* key_out /* [n], nullable */, uint64_t* dup_of_out /* [n], nullable */,
+                               uint32_t* n_dup_out, uint64_t* seq_base_out);
+int sdb_dedup_forget(sdb_handle h, uint64_t n, const sdb_dedup_key* key, uint8_t* removed_out /* [n], nullable */);
+int sdb_dedup_stats(sdb_handle h, sdb_dedup_summary* out);
 
 #ifdef __cplusplus
 }

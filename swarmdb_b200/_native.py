@@ -150,6 +150,15 @@ class SdbLeasePolicySummary(C.Structure):
                                           "held_by_ledger_total")]
 
 
+class SdbDedupSummary(C.Structure):
+    _fields_ = [("capacity", C.c_uint64), ("live", C.c_uint64), ("used", C.c_uint64), ("window", C.c_double)] + \
+        [(n, C.c_uint64) for n in ("accepted_total", "duplicate_total", "expired_total", "forgotten_total", "rebuilds")]
+
+
+DEDUP_CONTENT = 1
+KEY_DTYPE = np.dtype([("lo", "<u8"), ("hi", "<u8")])     # sdb_dedup_key; {0,0}: not deduplicated
+
+
 class SdbRelocateSummary(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("agents", "records", "moved_bytes", "skipped_bytes", "floor_before", "floor_after",
                                           "tail_after")]
@@ -166,9 +175,21 @@ EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sd
            "sdb_assign_agent_backends", "sdb_backend_loads_from_queues", "sdb_lease_reserve", "sdb_receive_leased",
            "sdb_lease_settle", "sdb_lease_sweep", "sdb_lease_stats", "sdb_lease_set_policy", "sdb_lease_deliveries",
            "sdb_lease_dead_letters", "sdb_lease_policy_stats", "sdb_arena_relocate", "sdb_lease_export",
-           "sdb_lease_import", "sdb_lease_ledger_export", "sdb_lease_ledger_import"]
+           "sdb_lease_import", "sdb_lease_ledger_export", "sdb_lease_ledger_import", "sdb_dedup_reserve",
+           "sdb_send_mixed_batch_dedup", "sdb_dedup_forget", "sdb_dedup_stats"]
 
 _lib = None
+
+
+def _keys(keys, n: Optional[int]) -> np.ndarray:
+    """Keys as a contiguous KEY_DTYPE array: from KEY_DTYPE or an (n, 2) array of (lo, hi)."""
+    k = np.asarray(keys)
+    if k.dtype != KEY_DTYPE:
+        k = np.ascontiguousarray(np.asarray(keys, np.uint64).reshape(-1, 2)).view(KEY_DTYPE).reshape(-1)
+    k = np.ascontiguousarray(k)
+    if n is not None and len(k) != n:
+        raise ValueError(f"{len(k)} keys for {n} sends")
+    return k
 
 
 def load_library() -> C.CDLL:
@@ -202,6 +223,11 @@ def load_library() -> C.CDLL:
     L.sdb_send_list_batch.restype = i32; L.sdb_send_list_batch.argtypes = [vp, u32] + [vp] * 8 + [u64, vp, vp]
     L.sdb_send_mixed_batch.restype = i32
     L.sdb_send_mixed_batch.argtypes = [vp, u32, vp, vp, vp, u32] + [vp] * 7 + [u64, vp, vp]
+    L.sdb_send_mixed_batch_dedup.restype = i32
+    L.sdb_send_mixed_batch_dedup.argtypes = [vp, u32, vp, vp, vp, u32] + [vp] * 7 + [u64, vp, vp, u32, C.c_double, vp, vp, vp, vp]
+    L.sdb_dedup_reserve.restype = i32; L.sdb_dedup_reserve.argtypes = [vp, u64, C.c_double]
+    L.sdb_dedup_forget.restype = i32; L.sdb_dedup_forget.argtypes = [vp, u64, vp, vp]
+    L.sdb_dedup_stats.restype = i32; L.sdb_dedup_stats.argtypes = [vp, C.POINTER(SdbDedupSummary)]
     L.sdb_stage_batch.restype = i32; L.sdb_stage_batch.argtypes = [vp, u32, u32] + [vp] * 7 + [u64, vp, C.POINTER(vp)]
     L.sdb_submit_staged.restype = i32; L.sdb_submit_staged.argtypes = [vp, vp, vp]
     L.sdb_free_staged.restype = i32; L.sdb_free_staged.argtypes = [vp, vp]
@@ -376,17 +402,18 @@ class Shard:
     PROFILE_KINDS = ["p2p", "fanout", "commit", "recv_count", "recv_scan", "recv_select", "recv_gather",
                      "arena_floor", "pick", "xshard", "index", "xwait", "recv_compact", "expire", "where", "restore"]
     PROFILE_KINDS_ALL = PROFILE_KINDS + ["lease"]
+    PROFILE_CLASSES = PROFILE_KINDS_ALL + ["dedup"]      # SDB_PK_CLASSES: every class sdb_profile_read_n reports
 
     def profile(self, enable: bool) -> None:
         self._check(self._L.sdb_profile(self._h, 1 if enable else 0))
 
     def profile_read(self) -> dict:
-        """{kernel class: (total ms, launches)} over PROFILE_KINDS_ALL, measured with CUDA events on the launching stream."""
-        n = len(self.PROFILE_KINDS_ALL)
+        """{kernel class: (total ms, launches)} over PROFILE_CLASSES, measured with CUDA events on the launching stream."""
+        n = len(self.PROFILE_CLASSES)
         ms = np.zeros(n, np.float64)
         cnt = np.zeros(n, np.uint64)
         self._check(self._L.sdb_profile_read_n(self._h, n, _p(ms), _p(cnt)))
-        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.PROFILE_KINDS_ALL)}
+        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.PROFILE_CLASSES)}
 
     # ------------------------------------------------------------------ registry / groups
     def register(self, idx) -> None:
@@ -454,6 +481,42 @@ class Shard:
                                                  _p(prio), _p(typ), _p(lens), _p(po), _p(pl), pl.nbytes, _p(ts),
                                                  C.cast(C.byref(base), C.c_void_p)))
         return base.value
+
+    def send_mixed_batch_dedup(self, sender, kind, target, list_off, list_idx, prio, typ, lens, payload_off, payload,
+                               ts=None, keys=None, content: bool = False, now: float = 0.0):
+        """send_mixed_batch with deduplication (include/swarmdb_b200.h "deduplicated sends").  keys: KEY_DTYPE[n] or a
+        (n, 2) uint64 array of (lo, hi), None for all {0,0}.  Returns (seq_base, dup_of uint64[n], keys KEY_DTYPE[n]):
+        dup_of[i] is the first seq of the send i duplicates (0: accepted), keys the keys used."""
+        s, k, t = _arr(sender, np.uint32), _arr(kind, np.uint8), _arr(target, np.uint32)
+        lo = _arr(list_off if list_off is not None else [0], np.uint64)
+        li = _arr(list_idx if list_idx is not None else [], np.uint32)
+        prio, typ, lens, po, pl, ts = self._common(len(s), prio, typ, lens, payload_off, payload, ts)
+        kin = None if keys is None else _keys(keys, len(s))
+        kout = np.zeros(len(s), KEY_DTYPE)
+        dup = np.zeros(len(s), np.uint64)
+        base, ndup = C.c_uint64(0), C.c_uint32(0)
+        self._keep = pl
+        self._check(self._L.sdb_send_mixed_batch_dedup(
+            self._h, len(s), _p(s), _p(k), _p(t), len(lo) - 1, _p(lo), _p(li), _p(prio), _p(typ), _p(lens), _p(po), _p(pl),
+            pl.nbytes, _p(ts), None if kin is None else _p(kin), DEDUP_CONTENT if content else 0, float(now), _p(kout),
+            _p(dup), C.cast(C.byref(ndup), C.c_void_p), C.cast(C.byref(base), C.c_void_p)))
+        return base.value, dup, kout
+
+    def dedup_reserve(self, entries: int, window: float = 300.0) -> None:
+        """Allocate (or clear) the deduplication table; 0 entries frees it."""
+        self._check(self._L.sdb_dedup_reserve(self._h, int(entries), float(window)))
+
+    def dedup_forget(self, keys) -> np.ndarray:
+        """Kill the entries of the given keys; returns removed uint8[n] (1 where the entry was live)."""
+        kin = _keys(keys, None)
+        out = np.zeros(len(kin), np.uint8)
+        self._check(self._L.sdb_dedup_forget(self._h, len(kin), _p(kin), _p(out)))
+        return out
+
+    def dedup_stats(self) -> dict:
+        st = SdbDedupSummary()
+        self._check(self._L.sdb_dedup_stats(self._h, C.byref(st)))
+        return {n: (float(getattr(st, n)) if n == "window" else int(getattr(st, n))) for n, _ in SdbDedupSummary._fields_}
 
     def stage(self, kind: int, sender, second, prio, typ, lens, payload_off, payload, ts=None) -> int:
         """Copy a p2p (kind 0) or group (kind 1) batch to device memory; returns a staged handle."""

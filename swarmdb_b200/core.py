@@ -23,7 +23,9 @@ Bulk entry points for index-level traffic (`send_to_group_batch`, `send_batch`,
 """
 from __future__ import annotations
 
+import bisect
 import datetime
+import hashlib
 import heapq
 import json
 import os
@@ -165,6 +167,9 @@ class GpuConfig:
                                           # no counts); needs lease_records
     lease_ledger_entries: int = 0         # ... and the device ledger of redelivered records' counts (0: lease_records)
     arena_relocate: bool = False          # a flush the arena refuses relocates the agents that pin the log and retries once
+    dedup_entries: int = 0                # deduplicated sends: device table of this many keys (0: off, no memory)
+    dedup_window: float = 300.0           # ... seconds a key stays live after its send
+    dedup_content: bool = False           # ... sends without a dedup_id are keyed by their content
 
 
 def _check_lease_policy(g: GpuConfig) -> None:
@@ -296,6 +301,13 @@ class SwarmsDB:
             self.shard.lease_reserve(g.lease_records, g.lease_payload_bytes or g.lease_records * pad32(g.max_payload_bytes))
         if g.lease_max_deliveries:
             self.shard.lease_set_policy(g.lease_max_deliveries, g.lease_ledger_entries or g.lease_records)
+        # deduplicated sends: duplicate id -> the id of the message it matched, and the dedup_id of each keyed message
+        self._dup_of: Dict[str, str] = {}
+        self._dedup_ids: Dict[str, str] = {}
+        if g.dedup_entries:
+            if not g.dedup_window > 0:
+                raise ValueError(f"GpuConfig.dedup_window={g.dedup_window} must be > 0 seconds")
+            self.shard.dedup_reserve(g.dedup_entries, g.dedup_window)
         self._reset_buffer()
         self._closed = False
         self.admin_client = _TransportAdmin(self)          # M:202-204: callers only list topics through it
@@ -315,6 +327,8 @@ class SwarmsDB:
         self._b_list_off: List[int] = [0]
         self._b_list_idx: List[int] = []
         self._b_msgs: List[Message] = []
+        self._b_key: List[Tuple[int, int]] = []          # dedup key of each send, (0, 0): none
+        self._b_seq0: List[int] = []                     # first seq of each send
         self._b_first_seq = self._next_seq
 
     def _index(self, agent_id: str) -> int:
@@ -341,10 +355,12 @@ class SwarmsDB:
         text = json.dumps(content) if isinstance(content, (dict, list)) else str(content)
         return self.token_counter(text)
 
-    def _stage(self, kind: int, sender: int, target: int, prio: int, type_code: int, payload: bytes, ts: float) -> None:
+    def _stage(self, kind: int, sender: int, target: int, prio: int, type_code: int, payload: bytes, ts: float,
+               key: Tuple[int, int] = (0, 0)) -> None:
         if len(payload) > self.gpu_config.max_payload_bytes:
             raise ValueError(f"encoded message is {len(payload)} bytes; GpuConfig.max_payload_bytes="
                              f"{self.gpu_config.max_payload_bytes}")
+        self._b_key.append(key); self._b_seq0.append(self._next_seq)
         self._b_sender.append(sender); self._b_kind.append(kind); self._b_target.append(target)
         self._b_prio.append(prio); self._b_type.append(type_code); self._b_len.append(len(payload))
         self._b_off.append(len(self._b_payload)); self._b_ts.append(ts)
@@ -357,6 +373,7 @@ class SwarmsDB:
         if n == 0:
             return
         msgs = self._b_msgs
+        keys = None                             # the keys the device used (deduplicated sends only)
         try:
             payload = np.frombuffer(bytes(self._b_payload) + b"\0" * 32, dtype=np.uint8)
             batch = (np.asarray(self._b_sender, np.uint32), np.asarray(self._b_kind, np.uint8),
@@ -364,16 +381,27 @@ class SwarmsDB:
                      np.asarray(self._b_list_idx, np.uint32), np.asarray(self._b_prio, np.uint8),
                      np.asarray(self._b_type, np.uint8), np.asarray(self._b_len, np.uint16),
                      np.asarray(self._b_off, np.uint64), payload, np.asarray(self._b_ts, np.float64))
+            g = self.gpu_config
+            now = time.time()
+
+            def send():
+                if not g.dedup_entries:
+                    return self.shard.send_mixed_batch(*batch), None, None
+                return self.shard.send_mixed_batch_dedup(*batch, keys=np.asarray(self._b_key, np.uint64).reshape(-1, 2),
+                                                         content=g.dedup_content, now=now)
             try:
-                base = self.shard.send_mixed_batch(*batch)
+                base, dup_of, keys = send()
             except SdbError as e:
-                # a refused batch takes no sequence numbers and writes nothing, so it can be sent again as it is
+                # a refused batch takes no sequence numbers and writes nothing (nor stores a key), so it can be sent
+                # again as it is and gets the same verdicts
                 if e.code != -5 or not self.gpu_config.arena_relocate:
                     raise
                 self.relocate_pinned(self._batch_bound())
-                base = self.shard.send_mixed_batch(*batch)
+                base, dup_of, keys = send()
             if base != self._b_first_seq:
                 raise RuntimeError(f"sequence mirror out of step: device {base}, host {self._b_first_seq}")
+            if dup_of is not None:
+                self._settle_duplicates(msgs, dup_of)
             st = self.shard.stats()
             if st["ring_overflow"] > getattr(self, "_seen_overflow", 0):
                 lost = st["ring_overflow"] - getattr(self, "_seen_overflow", 0)
@@ -387,11 +415,55 @@ class SwarmsDB:
                 for m in msgs:
                     m.status = MessageStatus.FAILED
                     m.metadata["error"] = str(e)
+            if keys is not None:                # forget the keys of failed sends, so that a resend is accepted
+                self._forget_failed(msgs, keys, dup_of)
             # ids already handed out stay used: the device counter moves up to the host's, never the other way
             self.shard.advance_seq(self._next_seq)
             self._reset_buffer()
             raise
         self._reset_buffer()
+
+    def _dedup_key(self, sender_id: str, dedup_id: Optional[str]) -> Tuple[int, int]:
+        """The device key of a send: a 128-bit blake2b of sender_id NUL dedup_id (a dedup_id is scoped to its sender)."""
+        if dedup_id is None:
+            return (0, 0)
+        if not self.gpu_config.dedup_entries:
+            raise ValueError("dedup_id needs deduplication (GpuConfig.dedup_entries > 0)")
+        d = hashlib.blake2b(f"{sender_id}\0{dedup_id}".encode("utf-8"), digest_size=16).digest()
+        lo, hi = int.from_bytes(d[:8], "little"), int.from_bytes(d[8:], "little")
+        return (lo, hi) if lo or hi else (1, 0)
+
+    def _send_of(self, m: Message) -> int:
+        """Index in the flushed batch of the send that carries message m."""
+        return bisect.bisect_right(self._b_seq0, self._seq_of_id(m.id)) - 1
+
+    def _settle_duplicates(self, msgs: List[Message], dup_of: np.ndarray) -> None:
+        """The device wrote nothing for a duplicate send: its messages leave `messages` and the inboxes, and each names
+        the message it matched (member j of a group send matches member j of the original)."""
+        for m in msgs:
+            i = self._send_of(m)
+            d = int(dup_of[i])
+            if not d:
+                continue
+            orig = self._make_id(d + self._seq_of_id(m.id) - self._b_seq0[i])
+            self._dup_of[m.id] = orig
+            m.metadata["duplicate_of"] = orig
+            if self.messages.pop(m.id, None) is not None:
+                self.message_count -= 1
+            for a in ([m.receiver_id] if m.receiver_id is not None else list(self.agent_inbox)):
+                inbox = self.agent_inbox.get(a)
+                if inbox and m.id in inbox:
+                    inbox.remove(m.id)
+
+    def _forget_failed(self, msgs: List[Message], keys: np.ndarray, dup_of: np.ndarray) -> None:
+        failed = sorted({self._send_of(m) for m in msgs if m.status == MessageStatus.FAILED})
+        sel = [i for i in failed if not dup_of[i] and (keys["lo"][i] or keys["hi"][i])]
+        if sel:
+            self.shard.dedup_forget(keys[sel])
+
+    def original_id(self, message_id: str) -> Optional[str]:
+        """The id of the message a duplicate send matched (GpuConfig.dedup_entries), else None."""
+        return self._dup_of.get(message_id)
 
     def _batch_bound(self) -> int:
         """Arena bytes the buffered batch can take at most: one header and one padded payload per copy."""
@@ -505,7 +577,11 @@ class SwarmsDB:
         metadata: Optional[Dict[str, Any]] = None,
         visible_to: Optional[List[str]] = None,
         _group: int = NO_GROUP,
+        dedup_id: Optional[str] = None,
     ) -> str:
+        """dedup_id: with GpuConfig.dedup_entries, a second send of the same sender with the same dedup_id inside the
+        window is not queued; after the flush, original_id() names the message it matched."""
+        key = self._dedup_key(sender_id, dedup_id)
         if sender_id not in self.registered_agents:
             self.register_agent(sender_id)
         if receiver_id is not None and receiver_id not in self.registered_agents:
@@ -557,9 +633,9 @@ class SwarmsDB:
             if receiver_id is not None:
                 deliverable = (not message.visible_to) or (receiver_id in message.visible_to)    # M:579-585
                 if deliverable:
-                    self._stage(0, sender, self._index(receiver_id), prio, type_code, payload, message.timestamp)
+                    self._stage(0, sender, self._index(receiver_id), prio, type_code, payload, message.timestamp, key)
                 else:      # in the log, matched by no consumer: an empty recipient list
-                    self._stage_list(sender, [], prio, type_code, payload, message.timestamp)
+                    self._stage_list(sender, [], prio, type_code, payload, message.timestamp, key)
             else:
                 seen: Set[int] = set()
                 recips = []
@@ -567,13 +643,15 @@ class SwarmsDB:
                     i = self._index(a)
                     if i not in seen:
                         seen.add(i); recips.append(i)
-                self._stage_list(sender, recips, prio, type_code, payload, message.timestamp)
+                self._stage_list(sender, recips, prio, type_code, payload, message.timestamp, key)
         except Exception as e:
             message.status = MessageStatus.FAILED
             message.metadata["error"] = str(e)
             raise
         self._next_seq += 1
         self._b_msgs.append(message)
+        if dedup_id is not None:
+            self._dedup_ids[message.id] = dedup_id
         message.status = MessageStatus.DELIVERED                          # delivery report, M:374-391
         self._after_send()
         return message.id
@@ -602,12 +680,13 @@ class SwarmsDB:
             return [self._agent_name[i] for i in range(min(n, len(self._agent_name))) if i not in skip]
         return list(extras.get("v", []))
 
-    def _stage_list(self, sender: int, recips: List[int], prio: int, type_code: int, payload: bytes, ts: float) -> None:
+    def _stage_list(self, sender: int, recips: List[int], prio: int, type_code: int, payload: bytes, ts: float,
+                    key: Tuple[int, int] = (0, 0)) -> None:
         # recipient lists (and the one-entry lists of buffered point-to-point sends) share the device's per-batch
         # list pool: flush first if this list would not fit beside what is already buffered
         if self._b_sender and len(self._b_list_idx) + len(recips) + len(self._b_sender) + 1 > self._list_cap:
             self.flush()
-        self._stage(2, sender, len(self._b_list_off) - 1, prio, type_code, payload, ts)
+        self._stage(2, sender, len(self._b_list_off) - 1, prio, type_code, payload, ts, key)
         self._b_list_idx.extend(recips)
         self._b_list_off.append(len(self._b_list_idx))
 
@@ -626,11 +705,12 @@ class SwarmsDB:
         priority: MessagePriority = MessagePriority.NORMAL,
         metadata: Optional[Dict[str, Any]] = None,
         exclude_agents: Optional[List[str]] = None,
+        dedup_id: Optional[str] = None,
     ) -> str:
         excluded = set(exclude_agents or [])
         visible = [a for a in self.registered_agents if a != sender_id and a not in excluded]
         return self.send_message(sender_id=sender_id, content=content, receiver_id=None, message_type=message_type,
-                                 priority=priority, metadata=metadata, visible_to=visible)
+                                 priority=priority, metadata=metadata, visible_to=visible, dedup_id=dedup_id)
 
     # ------------------------------------------------------------------ groups
     def add_agent_group(self, group_name: str, agent_ids: List[str]) -> None:
@@ -667,7 +747,9 @@ class SwarmsDB:
         message_type: MessageType = MessageType.CHAT,
         priority: MessagePriority = MessagePriority.NORMAL,
         metadata: Optional[Dict[str, Any]] = None,
+        dedup_id: Optional[str] = None,
     ) -> List[str]:
+        key = self._dedup_key(sender_id, dedup_id)
         groups = self.metadata.get("agent_groups", {})
         if group_name not in groups:
             logger.warning(f"Agent group '{group_name}' not found")
@@ -716,7 +798,7 @@ class SwarmsDB:
             staged = True
         if staged or members:
             self._stage(1, self._index(sender_id), g, int(MessagePriority(priority)),
-                        _TYPE_CODE[MessageType(message_type)] | flags, payload, now)
+                        _TYPE_CODE[MessageType(message_type)] | flags, payload, now, key)
             self._next_seq += len(members)
         if ids:
             self._after_send()
@@ -1500,6 +1582,8 @@ class SwarmsDB:
         it, then one PEEK of that agent returns it, status DELIVERED.  Only pending messages are found (not leased or
         dead-lettered ones), and only ids this instance issued."""
         m = self.messages.get(message_id)
+        if m is None and message_id in self._dup_of:           # a duplicate send: the message it matched
+            m = self.messages.get(self._dup_of[message_id])
         if m is not None or not include_device:
             return m
         return self.get_messages([message_id], include_device=True)[0]
@@ -1672,6 +1756,8 @@ class SwarmsDB:
             out["leases"] = self.shard.lease_stats()
         if self.gpu_config.lease_max_deliveries:
             out["dead_letters"] = self.shard.lease_policy_stats()["dead"]
+        if self.gpu_config.dedup_entries:
+            out["dedup"] = self.shard.dedup_stats()
         return out
 
     def resend_failed_messages(self) -> List[str]:
@@ -1679,7 +1765,7 @@ class SwarmsDB:
         for m in [x for x in self.messages.values() if x.status == MessageStatus.FAILED]:
             new_id = self.send_message(sender_id=m.sender_id, content=m.content, receiver_id=m.receiver_id,
                                        message_type=m.type, priority=m.priority, metadata=m.metadata,
-                                       visible_to=m.visible_to)
+                                       visible_to=m.visible_to, dedup_id=self._dedup_ids.get(m.id))
             self.messages[new_id].metadata["resent_from"] = m.id
             resent.append(new_id)
         return resent

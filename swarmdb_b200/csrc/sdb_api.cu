@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <new>
@@ -187,6 +188,22 @@ struct sdb_ctx {
   uint64_t launches = 0;
   uint64_t picks = 0;
   uint64_t seen_overflow = 0;
+  // deduplication table (sdb_dedup_reserve): two buffers (a rebuild copies the live entries into the other), per-batch
+  // scratch for max_batch_sends sends, pinned mirrors, host bookkeeping
+  struct Dedup {
+    sdb_dedup_entry* tab[2] = {nullptr, nullptr}; int cur = 0;
+    sdb_dedup_args a{};
+    sdb_dedup_send* snd_dev = nullptr;
+    uint32_t* lists_dev = nullptr; uint64_t lists_cap = 0;
+    std::vector<void*> mem;                              // every device allocation but lists_dev
+    sdb_dedup_key* key_host = nullptr; sdb_dedup_send* snd_host = nullptr;      // pinned [max_batch_sends]
+    unsigned long long* verdict_host = nullptr; unsigned long long* seq_host = nullptr;
+    unsigned long long* ctr_host = nullptr;              // pinned [SDB_DD_CTRS]
+    std::vector<uint8_t> keep;
+    uint64_t entries = 0, used = 0;
+    double last_now = -INFINITY;
+    uint64_t accepted = 0, dups = 0, expired = 0, forgotten = 0, rebuilds = 0;
+  } dd;
   sdb_profiler prof{};
   std::string err;
 };
@@ -366,6 +383,7 @@ struct SendArrays {
   const uint64_t* lbegin = nullptr; const uint64_t* lend = nullptr;
   const uint32_t* list_pool = nullptr;
   uint32_t* lp_out = nullptr; uint64_t lp_cap = 0;     // staging of the list-parallel index tables (nullptr: not offered)
+  const uint8_t* keep = nullptr;      // mixed batches: keep[i] == 0 leaves send i out, its sequence numbers unused
 };
 
 // Build descriptors into `out` (host).  kind 0: second = receiver; 1: second = group idx;
@@ -385,6 +403,7 @@ int build_descs(sdb_ctx* h, uint32_t batch_kind, uint32_t n, SendArrays& a, cons
   uint64_t o = 0;                      // output cursor (descriptors emitted)
   uint32_t max_padlen = 0;
   uint32_t n_group_sends = 0, n_other = 0;
+  uint32_t n_kept = n;                 // sends written (all but the duplicates a.keep leaves out)
   const uint32_t A = h->cfg.max_agents;
   if (h->sharded) return fail(h, SDB_EINVAL, "sharded handle: sends go through sdb_export_*_batch + sdb_import_wire_*");
   // shared payloads (pure group batches above the pull threshold, exclusive groups, payloads <= 512 bytes, groups of at
@@ -427,6 +446,17 @@ int build_descs(sdb_ctx* h, uint32_t batch_kind, uint32_t n, SendArrays& a, cons
     if (batch_kind == 3) {
       kind = a.kind[i];
       if (kind > 2) return fail(h, SDB_EINVAL, "kind must be 0, 1 or 2");
+      if (a.keep && !a.keep[i]) {     // a duplicate: it takes its sequence numbers and writes nothing
+        if (kind == 1) {
+          const uint32_t g = a.second[i];
+          if (g >= h->cfg.max_groups || !h->gdefined[g]) return fail(h, SDB_ENOTFOUND, "unknown group index");
+          rec += h->gcount[g];
+        } else {
+          rec += 1;
+        }
+        --n_kept;
+        continue;
+      }
       if (kind == 0) {      // p2p inside a mixed batch: a one-entry temporary list through the fan-out kernel
         if (a.second[i] >= A) return fail(h, SDB_EINVAL, "receiver index out of range");
         if (a.p2p_list_used >= a.p2p_list_cap) return fail(h, SDB_ECAPACITY, "recipient lists exceed list_pool_entries");
@@ -484,12 +514,17 @@ int build_descs(sdb_ctx* h, uint32_t batch_kind, uint32_t n, SendArrays& a, cons
   const uint32_t n_out = static_cast<uint32_t>(o);
   s->kind = batch_kind; s->n = n_out; s->total_recs = rec; s->total_grans = gran; s->max_padlen = max_padlen;
   s->has_pull = false; s->has_atomic = true; s->ranked = false; s->list_pull = false; s->shared = shared;
-  if (n_list_sends == n && n && list_copies >= SDB_PULL_THRESHOLD && a.lp_out && a.lbegin && a.list_pool) {
+  if (n_list_sends == n_kept && n_kept && list_copies >= SDB_PULL_THRESHOLD && a.lp_out && a.lbegin && a.list_pool) {
     // pure broadcast batch: if the lists it names are pairwise disjoint (and free of repeats), every member of a list
     // receives exactly the sends naming it, in send order -> owner-computes index build (k_list_index), no atomics.
     // Lists are identified by where they start in the pool (identical lists were stored once by the caller).
-    std::vector<std::pair<uint64_t, uint32_t>> key(n);                    // (list begin, send)
-    for (uint32_t i = 0; i < n; ++i) { const uint32_t li = batch_kind == 3 ? a.second[i] : i; key[i] = {a.lbegin[li], i}; }
+    std::vector<std::pair<uint64_t, uint32_t>> key;                       // (list begin, send)
+    key.reserve(n_kept);
+    for (uint32_t i = 0; i < n; ++i) {
+      if (a.keep && !a.keep[i]) continue;
+      const uint32_t li = batch_kind == 3 ? a.second[i] : i; key.push_back({a.lbegin[li], i});
+    }
+    const uint32_t n = n_kept;
     std::stable_sort(key.begin(), key.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
     uint32_t nd = 0;
     for (uint32_t k = 0; k < n; ++k) if (k == 0 || key[k].first != key[k - 1].first) ++nd;
@@ -655,8 +690,10 @@ int submit(sdb_ctx* h, const sdb_staged* s, uint64_t* seq_base_out) {
   return SDB_OK;
 }
 
+// payload_staged: the payload is in the handle's payload staging already (deduplicated sends hash it first)
 int send_common(sdb_ctx* h, uint32_t kind, uint32_t n, SendArrays& a, const uint64_t* list_off,
-                const uint32_t* list_idx, const uint8_t* payload, uint64_t payload_bytes, uint64_t* seq_base_out) {
+                const uint32_t* list_idx, const uint8_t* payload, uint64_t payload_bytes, uint64_t* seq_base_out,
+                bool payload_staged = false) {
   if (!h) return SDB_EINVAL;
   if (n == 0) { int rcc = cursor_to_host(h); if (seq_base_out) *seq_base_out = h->next_seq; return rcc; }
   if (!a.sender || !a.len || (kind != 2 && !a.second) || (kind == 3 && !a.kind)) return fail(h, SDB_EINVAL, "null array");
@@ -716,7 +753,7 @@ int send_common(sdb_ctx* h, uint32_t kind, uint32_t n, SendArrays& a, const uint
     CUDA_TRY(h, cudaMemcpyAsync(s->list_dev, h->list_host, list_total * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaMemcpyAsync(s->descs_dev, h->descs_host, static_cast<size_t>(s->n) * sizeof(sdb_send_desc),
                               cudaMemcpyHostToDevice, h->stream));
-  if (payload_bytes)   // straight from the caller's buffer (pinned memory makes this a true async DMA)
+  if (payload_bytes && !payload_staged)   // straight from the caller's buffer (pinned memory makes this a true async DMA)
     CUDA_TRY(h, cudaMemcpyAsync(s->payload_dev, payload, payload_bytes, cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaEventRecord(h->staging_free, h->stream));
   return submit(h, s, seq_base_out);
@@ -906,6 +943,7 @@ int sdb_create(const sdb_config* cfg, sdb_handle* out) {
 }
 
 static void lease_free(sdb_ctx* h);
+static void dedup_free(sdb_ctx* h);
 
 int sdb_destroy(sdb_handle h) {
   if (!h) return SDB_EINVAL;
@@ -940,6 +978,7 @@ int sdb_destroy(sdb_handle h) {
                  h->rs_agent, h->rs_tot, h->rs_sort, h->rl_bits, h->rl_cnt, h->rl_pre, h->rl_tops, h->rl_sel, h->rl_tot};
   for (void* p : dev) if (p) cudaFree(p);
   lease_free(h);
+  dedup_free(h);
   if (h->descs_host) cudaFreeHost(h->descs_host);
   if (h->list_host) cudaFreeHost(h->list_host);
   if (h->lp_host) cudaFreeHost(h->lp_host);
@@ -995,7 +1034,7 @@ int sdb_profile_read_n(sdb_handle h, uint32_t n, double* ms_out, uint64_t* count
   if (!h || !ms_out || !count_out) return SDB_EINVAL;
   for (uint32_t k = 0; k < n; ++k) { ms_out[k] = 0.0; count_out[k] = 0; }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  const int classes = static_cast<int>(std::min<uint32_t>(n, SDB_PK_ALL));
+  const int classes = static_cast<int>(std::min<uint32_t>(n, SDB_PK_CLASSES));
   sdb_profiler& p = h->prof;
   for (int i = 0; i < p.n; ++i) {
     float ms = 0.f;
@@ -1581,6 +1620,237 @@ int sdb_send_mixed_batch(sdb_handle h, uint32_t n, const uint32_t* sender, const
   SendArrays a{sender, target, prio, type, len, payload_off, timestamp};
   a.kind = kind; a.n_lists = n_lists;
   return send_common(h, 3, n, a, list_off, list_idx, payload, payload_bytes, seq_base_out);
+}
+
+// ---- deduplicated sends (include/swarmdb_b200.h "deduplicated sends", kernels in sdb_dedup.cu)
+static void dedup_free(sdb_ctx* h) {
+  sdb_ctx::Dedup& D = h->dd;
+  for (void* p : D.mem) cudaFree(p);
+  if (D.lists_dev) cudaFree(D.lists_dev);
+  for (void* p : {static_cast<void*>(D.key_host), static_cast<void*>(D.snd_host), static_cast<void*>(D.verdict_host),
+                  static_cast<void*>(D.seq_host), static_cast<void*>(D.ctr_host)})
+    if (p) cudaFreeHost(p);
+  D = sdb_ctx::Dedup{};
+}
+
+static uint64_t pow2_at_least(uint64_t x) {
+  uint64_t p = 64;
+  while (p < x) p <<= 1;
+  return p;
+}
+
+int sdb_dedup_reserve(sdb_handle h, uint64_t entries, double window_seconds) {
+  if (!h) return SDB_EINVAL;
+  if (entries && !(window_seconds > 0.0)) return fail(h, SDB_EINVAL, "sdb_dedup_reserve: the window must be > 0 seconds");
+  if (entries > (1ull << 31)) return fail(h, SDB_EINVAL, "sdb_dedup_reserve: more than 2^31 entries");
+  { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }        // cudaFree / cudaMalloc wait for running kernels
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  dedup_free(h);
+  if (!entries) return SDB_OK;
+  sdb_ctx::Dedup& D = h->dd;
+  const size_t slots = pow2_at_least(2 * entries), B = h->cfg.max_batch_sends, bslots = pow2_at_least(2ull * B);
+  std::vector<void*>& m = D.mem;
+  sdb_dedup_args& a = D.a;
+  unsigned long long* seq_of = nullptr;
+  bool ok = lease_alloc(m, &D.tab[0], slots) && lease_alloc(m, &D.tab[1], slots) && lease_alloc(m, &a.key, B) &&
+            lease_alloc(m, &D.snd_dev, B) && lease_alloc(m, &a.btab, bslots) && lease_alloc(m, &a.bmin, bslots) &&
+            lease_alloc(m, &a.bslot, B) && lease_alloc(m, &a.verdict, B) && lease_alloc(m, &seq_of, B) &&
+            lease_alloc(m, &a.ctr, SDB_DD_CTRS);
+  ok = ok && cudaHostAlloc(reinterpret_cast<void**>(&D.key_host), B * sizeof(sdb_dedup_key), cudaHostAllocDefault) == cudaSuccess &&
+       cudaHostAlloc(reinterpret_cast<void**>(&D.snd_host), B * sizeof(sdb_dedup_send), cudaHostAllocDefault) == cudaSuccess &&
+       cudaHostAlloc(reinterpret_cast<void**>(&D.verdict_host), B * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess &&
+       cudaHostAlloc(reinterpret_cast<void**>(&D.seq_host), B * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess &&
+       cudaHostAlloc(reinterpret_cast<void**>(&D.ctr_host), SDB_DD_CTRS * sizeof(unsigned long long), cudaHostAllocDefault) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(D.tab[0], 0, slots * sizeof(sdb_dedup_entry), h->stream) == cudaSuccess &&
+       cudaMemsetAsync(a.ctr, 0, SDB_DD_CTRS * sizeof(unsigned long long), h->stream) == cudaSuccess &&
+       cudaStreamSynchronize(h->stream) == cudaSuccess;
+  if (!ok) {
+    dedup_free(h);
+    cudaGetLastError();
+    return fail(h, SDB_ENOMEM, "sdb_dedup_reserve: allocation failed");
+  }
+  a.tab = D.tab[0]; a.mask = slots - 1; a.window = window_seconds; a.snd = D.snd_dev; a.bmask = bslots - 1; a.seq_of = seq_of;
+  D.entries = entries;
+  D.keep.assign(B, 1);
+  return SDB_OK;
+}
+
+// Entries live at `now` (a counting pass, one synchronisation); the table is not touched
+static int dedup_count_live(sdb_ctx* h, double now, uint64_t* live) {
+  sdb_ctx::Dedup& D = h->dd;
+  cudaError_t e = sdb_launch_dedup_rebuild(&D.a, nullptr, now, h->stream, &h->prof);
+  h->launches += 1;
+  if (e == cudaSuccess) e = cudaMemcpyAsync(D.ctr_host, D.a.ctr, SDB_DD_CTRS * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dedup count: ") + cudaGetErrorString(e));
+  *live = D.ctr_host[SDB_DD_LIVE];
+  return SDB_OK;
+}
+
+int sdb_send_mixed_batch_dedup(sdb_handle h, uint32_t n, const uint32_t* sender, const uint8_t* kind, const uint32_t* target,
+                               uint32_t n_lists, const uint64_t* list_off, const uint32_t* list_idx, const uint8_t* prio,
+                               const uint8_t* type, const uint16_t* len, const uint64_t* payload_off, const uint8_t* payload,
+                               uint64_t payload_bytes, const double* timestamp, const sdb_dedup_key* key, uint32_t flags,
+                               double now, sdb_dedup_key* key_out, uint64_t* dup_of_out, uint32_t* n_dup_out,
+                               uint64_t* seq_base_out) {
+  if (!h) return SDB_EINVAL;
+  sdb_ctx::Dedup& D = h->dd;
+  if (n_dup_out) *n_dup_out = 0;
+  if (!D.entries) return fail(h, SDB_EINVAL, "no deduplication table (sdb_dedup_reserve)");
+  if (!std::isfinite(now)) return fail(h, SDB_EINVAL, "now must be finite");
+  if (flags & ~SDB_DEDUP_CONTENT) return fail(h, SDB_EINVAL, "unknown deduplication flags");
+  const bool content = (flags & SDB_DEDUP_CONTENT) != 0;
+  if (h->sharded) {
+    if (content) return fail(h, SDB_EINVAL, "sharded handle: no content deduplication");
+    for (uint32_t i = 0; key && i < n; ++i)
+      if (key[i].lo | key[i].hi) return fail(h, SDB_EINVAL, "sharded handle: no deduplication keys");
+  }
+  if (n == 0 || h->sharded)
+    return sdb_send_mixed_batch(h, n, sender, kind, target, n_lists, list_off, list_idx, prio, type, len, payload_off, payload,
+                                payload_bytes, timestamp, seq_base_out);
+  if (!sender || !len || !target || !kind) return fail(h, SDB_EINVAL, "null array");
+  if (n > h->cfg.max_batch_sends) return fail(h, SDB_ECAPACITY, "n exceeds max_batch_sends");
+  if (payload_bytes > h->cfg.max_batch_payload) return fail(h, SDB_ECAPACITY, "payload_bytes exceeds max_batch_payload");
+  if (payload_bytes && !payload) return fail(h, SDB_EINVAL, "null payload");
+  if (n_lists && (!list_off || (list_off[n_lists] && !list_idx))) return fail(h, SDB_EINVAL, "null list arrays");
+  // what the content key and the sequence numbers read is checked before anything is staged
+  { int rcc = cursor_to_host(h); if (rcc != SDB_OK) return rcc; }
+  CUDA_TRY(h, cudaEventSynchronize(h->staging_free));
+  uint64_t rec = h->next_seq;
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t k = kind[i], l = len[i];
+    const uint64_t off = payload_off ? payload_off[i] : 0;
+    if (k > 2) return fail(h, SDB_EINVAL, "kind must be 0, 1 or 2");
+    if (l > h->cfg.max_payload_bytes) return fail(h, SDB_EINVAL, "payload longer than max_payload_bytes");
+    if ((off & 15u) || off + l > payload_bytes) return fail(h, SDB_EINVAL, "bad payload_off");
+    if (sender[i] >= h->cfg.max_agents) return fail(h, SDB_EINVAL, "sender index out of range");
+    sdb_dedup_send& d = D.snd_host[i];
+    d.payload_off = off; d.list_b = 0; d.sender = sender[i]; d.target = target[i]; d.kind = k;
+    d.lpt = l | static_cast<uint32_t>(prio ? prio[i] : 1) << 16 | static_cast<uint32_t>(type ? type[i] : 0) << 24;
+    D.seq_host[i] = rec;
+    if (k == 1) {
+      if (target[i] >= h->cfg.max_groups || !h->gdefined[target[i]]) return fail(h, SDB_ENOTFOUND, "unknown group index");
+      rec += h->gcount[target[i]];
+    } else {
+      if (k == 2) {
+        if (target[i] >= n_lists || list_off[target[i] + 1] < list_off[target[i]] || list_off[target[i] + 1] > list_off[n_lists])
+          return fail(h, SDB_EINVAL, "bad list number or list_off");
+        d.list_b = list_off[target[i]]; d.target = static_cast<uint32_t>(list_off[target[i] + 1] - list_off[target[i]]);
+      }
+      rec += 1;
+    }
+  }
+  if (key) std::memcpy(D.key_host, key, n * sizeof(sdb_dedup_key));
+  else std::memset(D.key_host, 0, n * sizeof(sdb_dedup_key));
+  CUDA_TRY(h, cudaMemcpyAsync(D.a.key, D.key_host, n * sizeof(sdb_dedup_key), cudaMemcpyHostToDevice, h->stream));
+  if (content) {
+    const uint64_t nl = n_lists ? list_off[n_lists] : 0;
+    if (nl > D.lists_cap) {
+      if (D.lists_dev) { CUDA_TRY(h, cudaStreamSynchronize(h->stream)); cudaFree(D.lists_dev); D.lists_dev = nullptr; D.lists_cap = 0; }
+      CUDA_TRY(h, dmalloc(&D.lists_dev, nl));
+      D.lists_cap = nl;
+    }
+    if (nl) CUDA_TRY(h, cudaMemcpyAsync(D.lists_dev, list_idx, nl * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(D.snd_dev, D.snd_host, n * sizeof(sdb_dedup_send), cudaMemcpyHostToDevice, h->stream));
+    if (payload_bytes)
+      CUDA_TRY(h, cudaMemcpyAsync(h->scratch.payload_dev, payload, payload_bytes, cudaMemcpyHostToDevice, h->stream));
+    D.a.payload = h->scratch.payload_dev; D.a.lists = D.lists_dev;
+  }
+  int nl = 0;
+  cudaError_t e = sdb_launch_dedup_probe(&D.a, n, content ? 1u : 0u, now, h->sm_count, h->stream, &h->prof, &nl);
+  h->launches += nl;
+  if (e == cudaSuccess) e = cudaMemcpyAsync(D.verdict_host, D.a.verdict, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(D.ctr_host, D.a.ctr, SDB_DD_CTRS * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess && key_out) e = cudaMemcpyAsync(key_out, D.a.key, n * sizeof(sdb_dedup_key), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);       // the one synchronisation: verdicts to the host
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dedup probe: ") + cudaGetErrorString(e));
+  const uint64_t n_new = D.ctr_host[SDB_DD_NEW];
+  D.used = D.ctr_host[SDB_DD_USED];
+  uint32_t n_dup = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    const unsigned long long v = D.verdict_host[i];
+    const uint64_t dup_of = (v & SDB_DD_BATCH) ? D.seq_host[v & ~SDB_DD_BATCH] : v;
+    D.keep[i] = dup_of == 0;
+    n_dup += dup_of != 0;
+    if (dup_of_out) dup_of_out[i] = dup_of;
+  }
+  // the new keys must fit beside the occupied slots; when they do not, the entries that are not live at `now` are
+  // dropped by a rebuild, which runs only once the enqueue is accepted (a refused call leaves the table as it was)
+  uint64_t live = D.used;
+  const bool rebuild = D.used + n_new > D.entries;
+  if (rebuild) {
+    int rc = dedup_count_live(h, now, &live);
+    if (rc != SDB_OK) return rc;
+    if (live + n_new > D.entries) return fail(h, SDB_ECAPACITY, "deduplication table full of live entries");
+  }
+  CUDA_TRY(h, cudaMemcpyAsync(const_cast<unsigned long long*>(D.a.seq_of), D.seq_host, n * sizeof(unsigned long long),
+                              cudaMemcpyHostToDevice, h->stream));
+  SendArrays a{sender, target, prio, type, len, payload_off, timestamp};
+  a.kind = kind; a.n_lists = n_lists; a.keep = D.keep.data();
+  uint64_t base = 0;
+  int rc = send_common(h, 3, n, a, list_off, list_idx, payload, payload_bytes, &base, content);
+  if (rc != SDB_OK) return rc;
+  if (h->scratch.n == 0) {             // every send was a duplicate: the batch still takes its sequence numbers
+    h->next_seq += h->scratch.total_recs;
+    h->dev_stale = true;
+  }
+  if (rebuild) {                       // stream-ordered before the insert; keeps exactly the `live` entries counted above
+    e = sdb_launch_dedup_rebuild(&D.a, D.tab[D.cur ^ 1], now, h->stream, &h->prof);
+    h->launches += 1;
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dedup rebuild: ") + cudaGetErrorString(e));
+    D.cur ^= 1; D.a.tab = D.tab[D.cur];
+    D.expired += D.used - live; D.used = live; D.rebuilds += 1;
+  }
+  e = sdb_launch_dedup_insert(&D.a, n, now, h->stream, &h->prof);
+  h->launches += 1;
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dedup insert: ") + cudaGetErrorString(e));
+  h->stream_busy = true;
+  D.used += n_new;                     // at most; the next probe reads the exact count
+  D.accepted += n_new; D.dups += n_dup; D.last_now = now;
+  if (n_dup_out) *n_dup_out = n_dup;
+  if (seq_base_out) *seq_base_out = base;
+  return SDB_OK;
+}
+
+int sdb_dedup_forget(sdb_handle h, uint64_t n, const sdb_dedup_key* key, uint8_t* removed_out) {
+  if (!h) return SDB_EINVAL;
+  sdb_ctx::Dedup& D = h->dd;
+  if (!D.entries) return fail(h, SDB_EINVAL, "no deduplication table (sdb_dedup_reserve)");
+  if (n && !key) return fail(h, SDB_EINVAL, "null keys");
+  CUDA_TRY(h, cudaEventSynchronize(h->staging_free));
+  const uint64_t B = h->cfg.max_batch_sends;
+  uint8_t* removed_dev = reinterpret_cast<uint8_t*>(D.a.bslot);       // [B] bytes of the batch scratch
+  for (uint64_t c = 0; c < n; c += B) {
+    const uint32_t m = static_cast<uint32_t>(std::min(B, n - c));
+    std::memcpy(D.key_host, key + c, m * sizeof(sdb_dedup_key));
+    cudaError_t e = cudaMemcpyAsync(D.a.key, D.key_host, m * sizeof(sdb_dedup_key), cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = sdb_launch_dedup_forget(&D.a, m, D.last_now, removed_dev, h->stream, &h->prof);
+    h->launches += 1;
+    if (e == cudaSuccess && removed_out) e = cudaMemcpyAsync(removed_out + c, removed_dev, m, cudaMemcpyDeviceToHost, h->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(D.ctr_host, D.a.ctr, SDB_DD_CTRS * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dedup forget: ") + cudaGetErrorString(e));
+    D.forgotten += D.ctr_host[SDB_DD_FORGOT];
+  }
+  return SDB_OK;
+}
+
+int sdb_dedup_stats(sdb_handle h, sdb_dedup_summary* out) {
+  if (!h || !out) return SDB_EINVAL;
+  std::memset(out, 0, sizeof(*out));
+  sdb_ctx::Dedup& D = h->dd;
+  if (!D.entries) return SDB_OK;
+  cudaError_t e = sdb_launch_dedup_rebuild(&D.a, nullptr, D.last_now, h->stream, &h->prof);      // count only
+  h->launches += 1;
+  if (e == cudaSuccess) e = cudaMemcpyAsync(D.ctr_host, D.a.ctr, SDB_DD_CTRS * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("dedup stats: ") + cudaGetErrorString(e));
+  D.used = D.ctr_host[SDB_DD_USED];
+  out->capacity = D.entries; out->live = D.ctr_host[SDB_DD_LIVE]; out->used = D.used; out->window = D.a.window;
+  out->accepted_total = D.accepted; out->duplicate_total = D.dups; out->expired_total = D.expired;
+  out->forgotten_total = D.forgotten; out->rebuilds = D.rebuilds;
+  return SDB_OK;
 }
 
 int sdb_stage_batch(sdb_handle h, uint32_t kind, uint32_t n, const uint32_t* sender, const uint32_t* second,

@@ -239,6 +239,41 @@ struct sdb_restore_args {
 #define SDB_RS_EINVAL 1ull         // tot[3]: a bad entry or row
 #define SDB_RS_ERING 2ull          // tot[3]: some agent's ring cannot take its records
 
+// ---- deduplication table (sdb_dedup.cu): one 32-byte entry per key, key {0,0} = empty slot
+struct __align__(32) sdb_dedup_entry {
+  sdb_dedup_key key;
+  unsigned long long seq;          // first seq of the send that stored the key
+  double at;                       // inserted_at; -inf once forgotten
+};
+static_assert(sizeof(sdb_dedup_entry) == 32, "dedup entry must be one 32-byte sector");
+// what the content key reads of a send (staged by the host, 32 bytes)
+struct __align__(16) sdb_dedup_send {
+  uint64_t payload_off;
+  uint64_t list_b;                 // kind 2: first recipient in `lists`
+  uint32_t sender;
+  uint32_t target;                 // receiver (kind 0), group (kind 1) or the list's length (kind 2)
+  uint32_t lpt;                    // len | prio << 16 | type << 24
+  uint32_t kind;
+};
+#define SDB_DD_BATCH (1ull << 63)  // verdict: SDB_DD_BATCH | index of the earlier send of the batch with the same key
+enum : uint32_t { SDB_DD_USED = 0, SDB_DD_NEW = 1, SDB_DD_FORGOT = 2, SDB_DD_LIVE = 3, SDB_DD_CTRS = 4 };
+struct sdb_dedup_args {
+  sdb_dedup_entry* tab;            // [mask + 1] the current buffer
+  unsigned long long mask;
+  double window;
+  sdb_dedup_key* key;              // [max_batch_sends] keys of the call (content keys filled in on the device)
+  const sdb_dedup_send* snd;       // [max_batch_sends]
+  const uint8_t* payload;          // the batch payload
+  const uint32_t* lists;           // the batch's recipient lists
+  sdb_dedup_key* btab;             // [bmask + 1] keys of the batch ...
+  uint32_t* bmin;                  // ... and the lowest send index holding each
+  unsigned long long bmask;
+  uint32_t* bslot;                 // [max_batch_sends] batch-table slot of each send
+  unsigned long long* verdict;     // [max_batch_sends]
+  const unsigned long long* seq_of;  // [max_batch_sends] first seq of each send (insert)
+  unsigned long long* ctr;         // [SDB_DD_CTRS]
+};
+
 // ---- lease store (sdb_receive_leased / sdb_lease_settle / sdb_lease_sweep, sdb_lease.cu): one of its two buffers.  Entries
 // are in lease-id order (append-only, then stable compaction); rows and payloads in the compact receive format.
 #define SDB_LS_LIVE 0u
@@ -927,4 +962,8 @@ cudaError_t sdb_scan_u32(const uint32_t* in, uint32_t* local, uint32_t* tops, ui
 cudaError_t sdb_radix_sort_u32(uint32_t* ka, uint32_t* va, uint32_t* kb, uint32_t* vb, uint32_t n, uint32_t bits, uint32_t* hist,
                                uint32_t* h_local, uint32_t* h_tops, uint32_t** kres, uint32_t** vres, cudaStream_t stream,
                                int* n_launches);
+cudaError_t sdb_launch_dedup_probe(const sdb_dedup_args*, uint32_t, uint32_t, double, int, cudaStream_t, sdb_profiler*, int*);
+cudaError_t sdb_launch_dedup_insert(const sdb_dedup_args*, uint32_t, double, cudaStream_t, sdb_profiler*);
+cudaError_t sdb_launch_dedup_forget(const sdb_dedup_args*, uint32_t, double, uint8_t*, cudaStream_t, sdb_profiler*);
+cudaError_t sdb_launch_dedup_rebuild(const sdb_dedup_args*, sdb_dedup_entry*, double, cudaStream_t, sdb_profiler*);
 }

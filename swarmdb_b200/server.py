@@ -26,7 +26,7 @@ from dataclasses import dataclass, field
 from datetime import datetime, timedelta, timezone
 from typing import Any, Deque, Dict, List, Optional, Union
 
-from fastapi import Depends, FastAPI, HTTPException, Query, Request
+from fastapi import Depends, FastAPI, Header, HTTPException, Query, Request
 from fastapi import status as http
 from fastapi.middleware.cors import CORSMiddleware
 from fastapi.responses import JSONResponse
@@ -251,20 +251,30 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
         return {"status": "success", "agent_id": agent_id}
 
     # ---- send -------------------------------------------------------------------------------------------------
+    # An Idempotency-Key header is the send's dedup_id (GpuConfig.dedup_entries): the route flushes, so that a retried
+    # request whose first attempt was queued answers with the original message instead of queueing a second copy.
+    def settled(mid: str, key: Optional[str]) -> str:
+        if key is None:
+            return mid
+        db.flush()
+        return db.original_id(mid) or mid
+
     @app.post("/messages", response_model=MessageOut)
-    def send(body: SendIn, who: str = Depends(caller)):
+    def send(body: SendIn, who: str = Depends(caller),
+             idempotency_key: Optional[str] = Header(None, alias="Idempotency-Key")):
         def go():
             mid = db.send_message(sender_id=who, content=body.content, receiver_id=body.receiver_id,
                                   message_type=body.message_type, priority=body.priority, metadata=body.metadata,
-                                  visible_to=body.visible_to)
-            return MessageOut.of(db.get_message(mid))
+                                  visible_to=body.visible_to, dedup_id=idempotency_key)
+            return MessageOut.of(db.get_message(settled(mid, idempotency_key)))
         return guarded("send message", go)
 
     @app.post("/messages/broadcast", response_model=BroadcastOut)
-    def broadcast(body: BroadcastIn, who: str = Depends(caller)):
-        mid = guarded("broadcast message", lambda: db.broadcast_message(
+    def broadcast(body: BroadcastIn, who: str = Depends(caller),
+                  idempotency_key: Optional[str] = Header(None, alias="Idempotency-Key")):
+        mid = guarded("broadcast message", lambda: settled(db.broadcast_message(
             sender_id=who, content=body.content, message_type=body.message_type, priority=body.priority,
-            metadata=body.metadata, exclude_agents=body.exclude_agents))
+            metadata=body.metadata, exclude_agents=body.exclude_agents, dedup_id=idempotency_key), idempotency_key))
         return BroadcastOut(status="success", message_id=mid)
 
     @app.post("/groups", status_code=http.HTTP_201_CREATED)
@@ -273,11 +283,14 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
         return {"status": "success", "group_name": body.group_name}
 
     @app.post("/groups/message", response_model=GroupSendOut)
-    def send_group(body: GroupSendIn, who: str = Depends(caller)):
-        ids = guarded("send group message", lambda: db.send_to_group(
-            sender_id=who, group_name=body.group_name, content=body.content, message_type=body.message_type,
-            priority=body.priority, metadata=body.metadata))
-        return GroupSendOut(status="success", message_ids=ids)
+    def send_group(body: GroupSendIn, who: str = Depends(caller),
+                   idempotency_key: Optional[str] = Header(None, alias="Idempotency-Key")):
+        def go():
+            ids = db.send_to_group(sender_id=who, group_name=body.group_name, content=body.content,
+                                   message_type=body.message_type, priority=body.priority, metadata=body.metadata,
+                                   dedup_id=idempotency_key)
+            return [settled(mid, idempotency_key) for mid in ids]
+        return GroupSendOut(status="success", message_ids=guarded("send group message", go))
 
     # ---- read -------------------------------------------------------------------------------------------------
     @app.post("/agents/receive", response_model=List[MessageOut])

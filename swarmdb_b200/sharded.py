@@ -516,6 +516,8 @@ class ShardedSwarmsDB(SwarmsDB):
         g = dataclasses.replace(g, shard_id=rank, num_shards=world)
         if g.lease_records or g.lease_max_deliveries:
             self._no_leases()
+        if g.dedup_entries:
+            self._no_dedup()
         if g.arena_relocate:
             raise NotImplementedError("ShardedSwarmsDB does not retry refused flushes (GpuConfig.arena_relocate): an "
                                       "asynchronous import that does not fit is dropped whole; call relocate_pinned instead")
@@ -593,11 +595,21 @@ class ShardedSwarmsDB(SwarmsDB):
 
     def send_message(self, sender_id, content, receiver_id=None, message_type=None, priority=None, metadata=None,
                      visible_to=None, **kw):
+        if kw.get("dedup_id") is not None:
+            self._no_dedup()
         self._require_known(sender_id, receiver_id, *(visible_to or []))
         return super().send_message(sender_id, content, receiver_id, message_type or MessageType.CHAT,
                                     priority if priority is not None else MessagePriority.NORMAL, metadata, visible_to, **kw)
 
-    def send_to_group(self, sender_id, group_name, content, message_type=None, priority=None, metadata=None):
+    def broadcast_message(self, sender_id, content, *a, dedup_id=None, **kw):
+        if dedup_id is not None:
+            self._no_dedup()
+        return super().broadcast_message(sender_id, content, *a, **kw)
+
+    def send_to_group(self, sender_id, group_name, content, message_type=None, priority=None, metadata=None,
+                      dedup_id=None):
+        if dedup_id is not None:
+            self._no_dedup()
         self._require_known(sender_id)
         return super().send_to_group(sender_id, group_name, content, message_type or MessageType.CHAT,
                                      priority if priority is not None else MessagePriority.NORMAL, metadata)
@@ -740,6 +752,10 @@ class ShardedSwarmsDB(SwarmsDB):
                                   "sequence numbers of later rounds")
 
     # ---- leased receives redeliver with the original ids, which meets the composite-round numbering as requeue does
+    def _no_dedup(self):
+        raise NotImplementedError("ShardedSwarmsDB does not deduplicate sends yet (GpuConfig.dedup_entries, dedup_id): "
+                                  "a key must be checked on the rank that numbers the send, before the exchange")
+
     def _no_leases(self, *args, **kwargs):
         raise NotImplementedError("ShardedSwarmsDB does not lease yet: redelivered ids must stay below the composite "
                                   "sequence numbers of later rounds (see requeue_batch_compact)")
