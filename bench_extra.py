@@ -7,6 +7,8 @@
   k1  point-to-point enqueue kernel roofline (1M records x 256 B)
   compact  the c2 step with host buffers out: full receive format against the compact format (sdb_receive_compact)
   expire   retention on the c2 backlog (sdb_expire): drop mode at the median cutoff, SDB_EXPIRE_ALL, archive mode
+  trim     bounded queues on the c2 backlog (sdb_trim): count cap 2, byte cap 512 B, byte cap with priority, archive mode;
+           and a SwarmsDB flush of 4,096 sends with and without GpuConfig.queue_max_messages
   where    filtered receive on the c2 backlog (sdb_receive_where): header-clause and keyword PEEKs, a take of one group's
            records, and keyword counts over deep queues
   restore  restore on the c2 backlog (sdb_restore_compact): snapshot, restore into a fresh handle, requeue
@@ -422,6 +424,135 @@ def expire(rounds=3, block=4):
                      "records_per_s": n / (ms * 1e-3), "kernel_ms": kern[name], "kernel_ms_total": kms,
                      "algorithmic_bytes": nbytes, "algorithmic_gb_per_s_kernel": nbytes / (kms * 1e-3) / 1e9 if kms else None,
                      "call_ms_blocks": res[name]["call_ms"]}
+    out.update(_gpu_card(0))
+    out["clocks"] = clk
+    return out
+
+
+def trim(rounds=3, block=4):
+    """sdb_trim on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 pending records): drop mode with a
+    count cap of 2, a byte cap of 512 B, the byte cap with SDB_RECV_PRIORITY, and the count cap in archive mode into
+    pinned host buffers, alternated in blocks in one process.  Every timed call starts from a fresh backlog (drain +
+    resend, untimed).  Then a SwarmsDB flush of 4,096 point-to-point sends over 1,024 agents (max_agents = 4,096, so the
+    host's recipient-list pool holds the batch), with and without
+    GpuConfig.queue_max_messages = 2, alternated (the queues are drained after every flush, untimed)."""
+    import torch
+    import swarmdb_b200 as sdb
+    from bench import ClockSampler, Workload
+    from swarmdb_b200._native import ENTRY_DTYPE, RECV_PRIORITY, SEND_DTYPE, Shard
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py trim: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    stream = torch.cuda.Stream()
+    shard = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+    shard.set_stream(stream.cuda_stream)
+    shard.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        shard.create_group(g, wl.members(g))
+    batch = wl.batch()
+
+    def pinned(nbytes):
+        return torch.empty(nbytes, dtype=torch.uint8, pin_memory=True).numpy()
+    pin_ent, pin_snd, pin_pay = pinned(rec_cap * 16).view(ENTRY_DTYPE), pinned(rec_cap * 32).view(SEND_DTYPE), pinned(rec_cap * wl.L)
+
+    def backlog():
+        while shard.receive_batch(None, 1 << 10, copy_out=False)[1]:
+            pass
+        shard.send_group_batch(*batch)
+        shard.sync()
+
+    # name: (call, walks over the ring entries per kernel, kernels)
+    calls = {"drop_count2": (lambda: shard.trim(None, 2, 0, archive=False)[1], 1, 1),
+             "drop_bytes512": (lambda: shard.trim(None, 0, 512, archive=False)[1], 2, 1),
+             "drop_bytes512_priority": (lambda: shard.trim(None, 0, 512, RECV_PRIORITY, archive=False)[1], 2, 1),
+             "archive_count2": (lambda: len(shard.trim(None, 2, 0, out_entries=pin_ent, out_sends=pin_snd,
+                                                       out_payload=pin_pay)[1]), 1, 2)}
+
+    def timed(fn):
+        backlog()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        t = time.perf_counter()
+        n = fn()                                         # synchronises: it returns totals
+        wall = (time.perf_counter() - t) * 1e3
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return wall, e0.elapsed_time(e1), n
+
+    res = {k: {"call_ms": [], "event_ms": []} for k in calls}
+    trimmed = {}
+    with torch.cuda.stream(stream):
+        for fn, _, _ in calls.values():                  # warm-up: every shape once
+            timed(fn)
+        clocks = ClockSampler(0); clocks.start()
+        for _ in range(rounds):
+            for name, (fn, _, _) in calls.items():
+                for _ in range(block):
+                    wall, ev, n = timed(fn)
+                    res[name]["call_ms"].append(wall); res[name]["event_ms"].append(ev)
+                    trimmed[name] = n
+        clk = clocks.stop()
+        kern = {}
+        for name, (fn, _, _) in calls.items():
+            backlog()
+            shard.profile(True)
+            fn()
+            prof = shard.profile_read()
+            shard.profile(False)
+            kern[name] = {k: v[0] for k, v in prof.items() if v[1]}
+    shard.close()
+    out = {"config": f"c2 backlog: {wl.A} agents, {wl.S} group sends x {wl.F} members = {per_step} pending records, "
+                     f"{wl.L}-B payloads; {rounds} rounds of {block} calls per mode, each on a fresh backlog"}
+    for name, (_, walks, kernels) in calls.items():
+        ms = float(np.median(res[name]["call_ms"]))
+        n = trimmed[name]
+        # algorithmic bytes: per kernel a 16-B ring header per agent and 8 B per ring entry per walk, plus an 8-B
+        # tombstone per trimmed record (archive mode: the count and select kernels; the compact back end is not counted)
+        nbytes = kernels * (16 * wl.A + 8 * per_step * walks) + 8 * n
+        kms = kern[name].get("expire", sum(kern[name].values()))
+        out[name] = {"records_trimmed": n, "ms_per_call": ms, "event_ms_per_call": float(np.median(res[name]["event_ms"])),
+                     "kernel_ms": kern[name], "trim_kernel_ms": kms, "algorithmic_bytes": nbytes,
+                     "algorithmic_gb_per_s_kernel": nbytes / (kms * 1e-3) / 1e9 if kms else None,
+                     "share_of_3_35_TBps": nbytes / (kms * 1e-3) / 3.35e12 if kms else None,
+                     "call_ms_blocks": res[name]["call_ms"]}
+    # SwarmsDB flush of 4,096 sends, with and without the automatic cap
+    import tempfile
+    n_agents, n_sends = 1024, 4096
+    rng = np.random.default_rng(5)
+    recv = rng.integers(0, n_agents, n_sends).tolist()
+    flush_ms = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        dbs = {name: sdb.SwarmsDB(save_dir=tmp, auto_save=False,
+                                  gpu_config=sdb.GpuConfig(max_agents=n_sends, flush_threshold=n_sends + 1,
+                                                           deterministic_ids=True, queue_max_messages=cap))
+               for name, cap in (("flush_no_cap", 0), ("flush_cap2", 2))}
+        names = [f"a{i}" for i in range(n_agents)]
+        for db in dbs.values():
+            for a in names:
+                db.register_agent(a)
+        flush_ms = {name: [] for name in dbs}
+        for r in range(2 + rounds * block):
+            for name, db in (dbs.items() if r % 2 == 0 else reversed(list(dbs.items()))):
+                for i, a in enumerate(recv):
+                    db.send_message(names[i % n_agents], "x" * 100, receiver_id=names[a])
+                torch.cuda.synchronize()
+                t = time.perf_counter()
+                db.flush()
+                db.shard.sync()
+                if r >= 2:
+                    flush_ms[name].append((time.perf_counter() - t) * 1e3)
+                db.shard.receive_batch(None, 1 << 10, copy_out=False)
+                db.messages.clear(); db.agent_inbox.clear()
+        trimmed_db = dbs["flush_cap2"].get_stats()["trimmed"]
+        for db in dbs.values():
+            db.close()
+    for name, v in flush_ms.items():
+        out[name] = {"ms_per_flush": float(np.median(v)), "ms_blocks": v, "sends": n_sends, "agents": n_agents}
+    out["flush_cap2"]["records_trimmed_total"] = trimmed_db
     out.update(_gpu_card(0))
     out["clocks"] = clk
     return out

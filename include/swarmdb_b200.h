@@ -417,7 +417,7 @@ int sdb_lease_stats(sdb_handle h, sdb_lease_summary* out);
  * max_deliveries times, then parked).  Off by default; nothing below allocates or launches anything until it is set.
  *   Delivery count  a record returned by a leased receive has deliveries = 1, except when a sweep redelivered it from a
  *                   lease with count k and it stayed pending since (no plain, priority, filtered or compact receive took
- *                   it, no expiry or purge retired it): then the next leased receive that returns it gives it k + 1.
+ *                   it, no expiry, purge or trim retired it): then the next leased receive that returns it gives it k + 1.
  *                   Records put back by sdb_restore_compact (requeue, redrive) start again at 1.  Records are identified by
  *                   (agent, seq); when two pending copies share both, which one inherits the count is unspecified.
  *   Ledger          the counts of redelivered records wait in a device table keyed by (agent, seq) holding the ring
@@ -704,6 +704,40 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
                uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
                sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
+
+/* ---- bounded queues: x-max-length / x-max-length-bytes with overflow=drop-head, XTRIM MAXLEN, retention.bytes -------
+ * sdb_trim caps each listed agent's pending queue by count and bytes and retires what is over the cap, oldest (or
+ * lowest priority) first, without delivering it.  It reads ring entries only, never the arena.
+ *   1. Limits     max_records caps an agent's live pending records (0: no count limit).  max_agent_bytes caps the sum of
+ *                 pad32(len) over them - the units of sdb_receive_budget and of sdb_agent_load.pending_granules x 32 -
+ *                 rounded down to granules (0: no byte limit).  Both 0 is SDB_EINVAL (purging is SDB_EXPIRE_ALL's job).
+ *   2. Eviction   default: stream order, oldest first.  SDB_RECV_PRIORITY: the lowest level first (0, then 1, 2, 3),
+ *      order      oldest first within a level.  Records are retired in eviction order until the agent's remaining live
+ *                 records meet both limits: the shortest prefix of the eviction order that does it.  A record larger
+ *                 than the byte limit on its own goes.  An agent already within both limits is not written at all.
+ *   3. Scope      only pending ring records are counted or retired; in-flight leases and dead letters are neither
+ *                 counted nor touched.  agent_idx == NULL and SDB_RECV_OWNED as in sdb_expire; an agent listed twice or
+ *                 out of range is SDB_EINVAL.
+ *   4. Effect     that of sdb_expire: every later receive (any order, any path, digests included) delivers what it would
+ *                 have delivered had the trimmed records never been enqueued.  sdb_stats does not move; in
+ *                 sdb_agent_loads `pending` and `pending_granules` fall and `received` stays.  Ring capacity is freed
+ *                 (head moves to the first live entry, ntomb stays exact); the next send that needs room recomputes the
+ *                 arena floor.  Ledger entries of trimmed records (sdb_lease_set_policy) are collected as expired ones.
+ *   5. Archive    (any of entry_out / send_out / payload_out given) the trimmed records come back in the compact receive
+ *      mode       format with sdb_expire's capacity rule: agents in list order, stream order within an agent.  An agent
+ *                 whose trimmed records do not fit stays whole, except the first agent of the output, which gives the
+ *                 first rec_cap records of its eviction order.  Calls repeated until *total_out == 0 retire exactly the
+ *                 records one drop-mode call retires.  No usable output capacity: SDB_EOUTPUT.
+ *   6. Drop mode  (all three output pointers NULL) no capacity limit: count_out[n_agents] (nullable) and *total_out are
+ *                 filled, *n_sends_out and *payload_bytes_out read 0.
+ *   7. Flags      SDB_RECV_PEEK (dry run: select and report, retire nothing), SDB_RECV_OWNED, SDB_RECV_PRIORITY; any
+ *                 other bit is SDB_EINVAL.
+ *   8. Ordering   as sdb_expire: stream-ordered, synchronising, rings only (so it may sit inside an import prefetch
+ *                 window).  Kernels are timed under SDB_PK_EXPIRE. */
+int sdb_trim(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_records, uint64_t max_agent_bytes,
+             uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+             sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+             uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
 
 /* ---- relocation of pinned queues: the other remedy for an agent that pins the log.  Where sdb_expire drops its records,
  * sdb_arena_relocate keeps them: it copies the live records of the agents pinning the log to the tail of the arena and

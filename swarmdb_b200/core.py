@@ -170,6 +170,10 @@ class GpuConfig:
     dedup_entries: int = 0                # deduplicated sends: device table of this many keys (0: off, no memory)
     dedup_window: float = 300.0           # ... seconds a key stays live after its send
     dedup_content: bool = False           # ... sends without a dedup_id are keyed by their content
+    queue_max_messages: int = 0           # bounded queues: after every flush each agent keeps its newest this many
+                                          # pending messages (0: no count cap)
+    queue_max_bytes: int = 0              # ... and pending payload bytes, sum of pad32(len) (0: no byte cap)
+    queue_trim_priority: bool = False     # ... dropping the lowest priority first (oldest first within a level)
 
 
 def _check_lease_policy(g: GpuConfig) -> None:
@@ -182,6 +186,27 @@ def _check_lease_policy(g: GpuConfig) -> None:
         raise ValueError("GpuConfig.lease_max_deliveries needs a lease store (GpuConfig.lease_records)")
     if g.lease_ledger_entries and not g.lease_max_deliveries:
         raise ValueError("GpuConfig.lease_ledger_entries is used only with GpuConfig.lease_max_deliveries")
+
+
+def _check_queue_caps(g: GpuConfig) -> None:
+    """The bounded-queue settings of a GpuConfig, checked before any device work."""
+    if not isinstance(g.queue_max_messages, int) or not 0 <= g.queue_max_messages <= 0xFFFFFFFF:
+        raise ValueError(f"GpuConfig.queue_max_messages={g.queue_max_messages!r} is not an integer in [0, 2^32 - 1]")
+    if not isinstance(g.queue_max_bytes, int) or not 0 <= g.queue_max_bytes < (1 << 64):
+        raise ValueError(f"GpuConfig.queue_max_bytes={g.queue_max_bytes!r} is not an integer in [0, 2^64)")
+    if not isinstance(g.queue_trim_priority, bool):
+        raise ValueError(f"GpuConfig.queue_trim_priority={g.queue_trim_priority!r} is not a bool")
+
+
+def _trim_limits(max_messages: Optional[int], max_bytes: Optional[int]) -> Tuple[int, int]:
+    """The (max_records, max_agent_bytes) of sdb_trim for trim_queues' arguments (None: no limit)."""
+    for name, v, top in (("max_messages", max_messages, 0xFFFFFFFF), ("max_bytes", max_bytes, (1 << 64) - 1)):
+        if v is not None and (isinstance(v, bool) or not isinstance(v, int) or not 1 <= v <= top):
+            raise ValueError(f"{name}={v!r} is not None or an integer in [1, {top}]")
+    if max_messages is None and max_bytes is None:
+        raise ValueError("trim_queues needs max_messages or max_bytes (expire_pending or deregister_agent(purge=True) "
+                         "empties queues)")
+    return max_messages or 0, max_bytes or 0
 
 
 def _encode_content(content: Any) -> (bytes, int):
@@ -256,6 +281,7 @@ class SwarmsDB:
         self.gpu_config = gpu_config or GpuConfig()
         g = self.gpu_config
         _check_lease_policy(g)
+        _check_queue_caps(g)
         # the transport: constructing it fails loudly when the CUDA library or a device is missing
         self.shard = _shard if _shard is not None else Shard(
             max_agents=g.max_agents, ring_slots=g.ring_slots, arena_bytes=g.arena_bytes,
@@ -308,6 +334,7 @@ class SwarmsDB:
             if not g.dedup_window > 0:
                 raise ValueError(f"GpuConfig.dedup_window={g.dedup_window} must be > 0 seconds")
             self.shard.dedup_reserve(g.dedup_entries, g.dedup_window)
+        self._trimmed = 0                       # records the automatic queue caps dropped (get_stats()["trimmed"])
         self._reset_buffer()
         self._closed = False
         self.admin_client = _TransportAdmin(self)          # M:202-204: callers only list topics through it
@@ -422,6 +449,15 @@ class SwarmsDB:
             self._reset_buffer()
             raise
         self._reset_buffer()
+        self._apply_queue_caps()
+
+    def _apply_queue_caps(self) -> None:
+        """GpuConfig.queue_max_messages / queue_max_bytes: one drop-mode trim of every agent this instance serves."""
+        g = self.gpu_config
+        if g.queue_max_messages or g.queue_max_bytes:
+            agents, flags = self._expire_scope(None)
+            flags |= RECV_PRIORITY if g.queue_trim_priority else 0
+            self._trimmed += self.shard.trim(agents, g.queue_max_messages, g.queue_max_bytes, flags, archive=False)[1]
 
     def _dedup_key(self, sender_id: str, dedup_id: Optional[str]) -> Tuple[int, int]:
         """The device key of a send: a 128-bit blake2b of sender_id NUL dedup_id (a dedup_id is scoped to its sender)."""
@@ -1758,6 +1794,8 @@ class SwarmsDB:
             out["dead_letters"] = self.shard.lease_policy_stats()["dead"]
         if self.gpu_config.dedup_entries:
             out["dedup"] = self.shard.dedup_stats()
+        if self.gpu_config.queue_max_messages or self.gpu_config.queue_max_bytes:
+            out["trimmed"] = self._trimmed                 # messages the queue caps dropped, never delivered
         return out
 
     def resend_failed_messages(self) -> List[str]:
@@ -1861,6 +1899,19 @@ class SwarmsDB:
         if agents is not None and len(agents) == 0:
             return 0
         return self.shard.expire(agents, cutoff, flags, archive=False)[1]
+
+    def trim_queues(self, max_messages: Optional[int] = None, max_bytes: Optional[int] = None,
+                    agent_ids: Optional[Iterable[str]] = None, by_priority: bool = False) -> int:
+        """Cap the device queues: each agent (default: every agent) keeps at most max_messages pending messages and
+        max_bytes pending payload bytes (sum of pad32(len)); None is no limit.  The oldest messages go first, or with
+        by_priority=True the lowest priority first (oldest first within a level); they are dropped without being
+        delivered.  Returns the number of records dropped.  Host records are not touched, as in expire_pending."""
+        limits = _trim_limits(max_messages, max_bytes)
+        self._pre_read()
+        agents, flags = self._expire_scope(agent_ids)
+        if agents is not None and len(agents) == 0:
+            return 0
+        return self.shard.trim(agents, *limits, flags | (RECV_PRIORITY if by_priority else 0), archive=False)[1]
 
     def _expire_device_archive(self, cutoff: float) -> List[Message]:
         """Expire the device-queued records older than the cutoff in archive mode, call after call until none is left,

@@ -2228,16 +2228,12 @@ int sdb_receive_compact_budget(sdb_handle h, uint32_t n_agents, const uint32_t* 
   return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
 }
 
-int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, double older_than, uint32_t flags,
-               uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
-               sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
-               uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
-  if (!h) return SDB_EINVAL;
-  if (total_out) *total_out = 0;
-  if (n_sends_out) *n_sends_out = 0;
-  if (payload_bytes_out) *payload_bytes_out = 0;
-  if (flags & ~(SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_EXPIRE_ALL))
-    return fail(h, SDB_EINVAL, "sdb_expire accepts SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_EXPIRE_ALL only");
+// The body of sdb_expire and sdb_trim: `flags` were checked by the caller, trim == nullptr is an expiry.  Archive mode
+// takes sdb_receive_compact's capacity rule and copy-out; drop mode returns the count and the per-agent counts.
+static int retire_call(sdb_ctx* h, uint32_t n_agents, const uint32_t* agent_idx, double older_than, const uint2* trim,
+                       uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                       sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                       uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
   const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
   const bool archive = entry_out || send_out || payload_out;
   uint64_t rec_cap = 0;
@@ -2249,16 +2245,17 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
   { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
   if (archive) { const int rc = compact_ensure(h); if (rc != SDB_OK) return rc; }
   sdb_recv_args r{};
-  { const int rc = recv_args(h, n_agents, agent_idx, owned, 0, flags & SDB_RECV_PEEK, rec_cap, &r); if (rc != SDB_OK) return rc; }
+  { const int rc = recv_args(h, n_agents, agent_idx, owned, 0, flags & (SDB_RECV_PEEK | SDB_RECV_PRIORITY), rec_cap, &r);
+    if (rc != SDB_OK) return rc; }
   if (!archive && !count_out) r.count_out = nullptr;           // nobody reads the counts
   int nl = 0;
-  cudaError_t e = sdb_launch_expire(&h->view, &r, older_than, (flags & SDB_EXPIRE_ALL) ? 1u : 0u, archive ? &h->cx : nullptr,
+  cudaError_t e = sdb_launch_expire(&h->view, &r, older_than, (flags & SDB_EXPIRE_ALL) ? 1u : 0u, trim, archive ? &h->cx : nullptr,
                                     h->stream, &nl, &h->prof, h->sm_count);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = false;       // the receive scratch was reused: nothing left to fold
-  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("expire launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string(trim ? "trim" : "expire") + " launch: " + cudaGetErrorString(e));
   if (archive) return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
-  // drop mode: the number of records expired and the counts
+  // drop mode: the number of records retired and the counts
   CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
   if (count_out)
     CUDA_TRY(h, cudaMemcpyAsync(count_out, h->rx_count, static_cast<size_t>(n_agents) * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
@@ -2266,6 +2263,40 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
   h->stream_busy = false;
   if (total_out) *total_out = h->totals_host[TOT_RECORDS];
   return SDB_OK;
+}
+
+int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, double older_than, uint32_t flags,
+               uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+               sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+               uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (flags & ~(SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_EXPIRE_ALL))
+    return fail(h, SDB_EINVAL, "sdb_expire accepts SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_EXPIRE_ALL only");
+  return retire_call(h, n_agents, agent_idx, older_than, nullptr, flags, count_out, entry_out, entry_cap, send_out, send_cap,
+                     payload_out, payload_cap, total_out, n_sends_out, payload_bytes_out);
+}
+
+int sdb_trim(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_records, uint64_t max_agent_bytes,
+             uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+             sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+             uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (flags & ~(SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_RECV_PRIORITY))
+    return fail(h, SDB_EINVAL, "sdb_trim accepts SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_RECV_PRIORITY only");
+  if (max_records == 0 && max_agent_bytes == 0)
+    return fail(h, SDB_EINVAL, "sdb_trim: max_records and max_agent_bytes are both 0 (SDB_EXPIRE_ALL purges a queue)");
+  // limits in records and payload granules, ~0 for none (a queue's granules are counted in 32 bits, as in sdb_agent_loads)
+  const uint2 lim = make_uint2(max_records ? max_records : 0xFFFFFFFFu,
+                               max_agent_bytes ? static_cast<uint32_t>(std::min<uint64_t>(max_agent_bytes / SDB_GRANULE, 0xFFFFFFFEull))
+                                               : 0xFFFFFFFFu);
+  return retire_call(h, n_agents, agent_idx, 0.0, &lim, flags, count_out, entry_out, entry_cap, send_out, send_cap,
+                     payload_out, payload_cap, total_out, n_sends_out, payload_bytes_out);
 }
 
 static int restore_ensure(sdb_ctx* h);

@@ -879,8 +879,8 @@ cudaError_t sdb_launch_pull(const sdb_dev_view*, const sdb_pull_view*, const sdb
                             const sdb_batch_base*, uint32_t);
 cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaStream_t, int*, sdb_profiler*, int, uint32_t,
                                const sdb_compact_args*, const uint2*);
-cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double, uint32_t, const sdb_compact_args*, cudaStream_t,
-                              int*, sdb_profiler*, int);
+cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double, uint32_t, const uint2*, const sdb_compact_args*,
+                              cudaStream_t, int*, sdb_profiler*, int);
 cudaError_t sdb_launch_where(const sdb_dev_view*, const sdb_recv_args*, const sdb_where_args*, int, uint32_t, cudaStream_t, int*,
                              sdb_profiler*, int);
 cudaError_t sdb_launch_id_table(const unsigned long long*, uint32_t, sdb_id_slot*, uint32_t, cudaStream_t, int*);

@@ -1320,6 +1320,62 @@ enum { SDB_EXP_DROP = 0, SDB_EXP_COUNT = 1, SDB_EXP_SELECT = 2 };
 #define SDB_EXP_G 8u     // lanes per request slot
 #define SDB_EXP_U 4u     // entries per lane in flight
 
+// The parts of a retiring walk that expiry and trimming share.  exp_cut: in EXP_SELECT, the capacity cut of
+// k_recv_select on the scanned counts (an agent that does not fit stays queued, unless it is first in the output: then
+// its first rec_cap selections); returns how many the slot may retire, RO = its first output record.
+template <int MODE>
+__device__ __forceinline__ uint32_t exp_cut(const sdb_recv_args& r, bool valid, uint32_t q, uint32_t l8, uint32_t* RO) {
+  *RO = 0;
+  if (MODE != SDB_EXP_SELECT || !valid) return 0xFFFFFFFFu;
+  uint32_t c = r.cnt[q];
+  *RO = sdb_scan_at(r.rec_local, r.rec_tops, q);
+  if (c && static_cast<uint64_t>(*RO) + c > r.rec_cap) {
+    c = *RO == 0 ? static_cast<uint32_t>(r.rec_cap) : 0u;
+    if (l8 == 0) atomicMin(r.totals, static_cast<unsigned long long>(*RO) + c);
+  }
+  if (l8 == 0) r.count_out[q] = c;
+  return c;
+}
+
+// exp_retire: one step of 8 entries per slot (entry e at ring position pos).  A selected entry is planned at its stream
+// rank among the slot's selections {handle, 0, plan z, slot} (EXP_SELECT) and tombstoned; `got` counts the selections and
+// `nh` becomes the first live entry not selected (T while there is none), the head by select_agent_warp's rule.
+template <int MODE>
+__device__ __forceinline__ void exp_retire(const sdb_recv_args& r, uint2* rs, uint32_t mask, uint2 e, uint32_t pos, bool lv,
+                                           bool sel, bool retire, uint32_t q, uint32_t RO, uint32_t l8, uint32_t gsh,
+                                           uint32_t T, uint32_t& got, uint32_t& nh) {
+  const uint32_t bs = (__ballot_sync(0xFFFFFFFFu, sel) >> gsh) & 0xFFu;
+  const uint32_t bk = (__ballot_sync(0xFFFFFFFFu, lv && !sel) >> gsh) & 0xFFu;
+  if (sel) {
+    if (MODE == SDB_EXP_SELECT) r.plan[RO + got + __popc(bs & ((1u << l8) - 1u))] = make_uint4(e.x, 0u, sdb_plan_z(e.y), q);
+    if (retire) rs[pos & mask].y = SDB_META_TOMB;
+  }
+  got += __popc(bs);
+  if (bk && nh == T) nh = pos - l8 + (__ffs(bk) - 1);
+}
+
+// exp_store: the end of a slot.  The ring header is stored once, and only when something was retired (ntomb stays
+// exact); the count goes to cnt (EXP_COUNT) or count_out and the warp's total (EXP_DROP).
+template <int MODE>
+__device__ __forceinline__ void exp_store(const sdb_dev_view& v, const sdb_recv_args& r, bool valid, bool retire, uint32_t l8,
+                                          uint32_t q, uint32_t a, uint32_t H, uint32_t NT, uint32_t got, uint32_t nh,
+                                          unsigned long long& wsum) {
+  if (l8 != 0 || !valid) return;
+  if (retire && got) {
+    v.ring_hdr[a].head = nh;
+    v.ring_hdr[a].ntomb = NT + got - (nh - H);
+  }
+  if (MODE == SDB_EXP_COUNT) r.cnt[q] = got;
+  if (MODE == SDB_EXP_DROP) { if (r.count_out) r.count_out[q] = got; wsum += got; }
+}
+
+template <int MODE>
+__device__ __forceinline__ void exp_total(const sdb_recv_args& r, uint32_t lane, unsigned long long wsum) {
+  if (MODE != SDB_EXP_DROP) return;
+  for (int o = 16; o; o >>= 1) wsum += __shfl_xor_sync(0xFFFFFFFFu, wsum, o);
+  if (lane == 0 && wsum) atomicAdd(r.totals, wsum);
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(256)
 k_expire(sdb_dev_view v, sdb_recv_args r, double older_than, uint32_t all) {
@@ -1339,17 +1395,8 @@ k_expire(sdb_dev_view v, sdb_recv_args r, double older_than, uint32_t all) {
       H = h.x; T = h.y; NT = h.w;
     }
     const uint32_t live = T - H - NT;
-    uint32_t limit = 0xFFFFFFFFu, RO = 0;
-    if (MODE == SDB_EXP_SELECT && valid) {
-      uint32_t c = r.cnt[q];
-      RO = sdb_scan_at(r.rec_local, r.rec_tops, q);
-      if (c && static_cast<uint64_t>(RO) + c > r.rec_cap) {     // does not fit: stays queued ...
-        c = RO == 0 ? static_cast<uint32_t>(r.rec_cap) : 0u;    // ... unless first in the output: its first rec_cap matches
-        if (l8 == 0) atomicMin(r.totals, static_cast<unsigned long long>(RO) + c);
-      }
-      if (l8 == 0) r.count_out[q] = c;
-      limit = c;
-    }
+    uint32_t RO;
+    const uint32_t limit = exp_cut<MODE>(r, valid, q, l8, &RO);
     // entries are walked unless ALL makes the count alone enough (a selection always needs the handles)
     const bool walk = valid && live && (MODE == SDB_EXP_SELECT ? limit != 0 : !all);
     const uint32_t W = walk ? T - H : 0u;
@@ -1376,53 +1423,167 @@ k_expire(sdb_dev_view v, sdb_recv_args r, double older_than, uint32_t all) {
         const bool lv = sdb_meta(e[u]) != SDB_META_TOMB;
         const bool match = lv && (all || ts[u] < older_than);           // NaN never compares below: never expires
         const uint32_t bm = (__ballot_sync(0xFFFFFFFFu, match) >> gsh) & 0xFFu;
-        const uint32_t k = got + __popc(bm & ((1u << l8) - 1u));
-        const bool sel = match && k < limit;
-        if (sel) {
-          if (MODE == SDB_EXP_SELECT) r.plan[RO + k] = make_uint4(e[u].x, 0u, sdb_plan_z(e[u].y), q);
-          if (retire) rs[(H + j) & mask].y = SDB_META_TOMB;
-        }
-        const uint32_t bs = (__ballot_sync(0xFFFFFFFFu, sel) >> gsh) & 0xFFu;
-        const uint32_t bk = (__ballot_sync(0xFFFFFFFFu, lv && !sel) >> gsh) & 0xFFu;
-        got += __popc(bs);
-        if (bk && nh == T) nh = H + j0 + u * SDB_EXP_G + (__ffs(bk) - 1);
+        const bool sel = match && got + __popc(bm & ((1u << l8) - 1u)) < limit;
+        exp_retire<MODE>(r, rs, mask, e[u], H + j, lv, sel, retire, q, RO, l8, gsh, T, got, nh);
       }
     }
-    if (l8 == 0 && valid) {
-      if (retire && got) {                                      // the ring header, once
-        v.ring_hdr[a].head = nh;
-        v.ring_hdr[a].ntomb = NT + got - (nh - H);
-      }
-      if (MODE == SDB_EXP_COUNT) r.cnt[q] = got;
-      if (MODE == SDB_EXP_DROP) { if (r.count_out) r.count_out[q] = got; wsum += got; }
-    }
+    exp_store<MODE>(v, r, valid, retire, l8, q, a, H, NT, got, nh, wsum);
   }
-  if (MODE == SDB_EXP_DROP) {
-    for (int o = 16; o; o >>= 1) wsum += __shfl_xor_sync(0xFFFFFFFFu, wsum, o);
-    if (lane == 0 && wsum) atomicAdd(r.totals, wsum);
-  }
+  exp_total<MODE>(r, lane, wsum);
 }
 
-// drop mode (ca == nullptr): one launch; totals[0] = records expired.  Archive mode: count, scan, select, then the compact
+// ------------------------------------------------------------------------------------------
+// trimming (sdb_trim): retire the records that take an agent's pending queue past max_records records or max_gran
+// payload granules (~0: no limit), in eviction order: stream order (NL = 1), or with SDB_RECV_PRIORITY level 0 first,
+// then 1, 2, 3, stream order within a level (NL = 4).  k_expire's shape and modes, and no arena reads: the ring meta
+// holds the priority (bits 14-15) and the record's granules (1 + payload granules).
+//   walk 1  per level: live records L and payload granules G (8-lane reductions).  Skipped when the header decides:
+//           stream order without a byte limit has L = tail - head - ntomb; an agent within both limits has no walk 2.
+//   walk 2  record i of level p (in-level rank i, in-level granule prefix pg) is retired iff what is left after every
+//           record before it in eviction order is gone still breaks a limit: sum_{l>=p} L_l - i > max_records or
+//           sum_{l>=p} G_l - pg > max_gran.  Both sides fall along the order, so the retired records are a prefix of it;
+//           the eviction rank of a retired record is sum_{l<p} L_l + i, which the capacity cut of EXP_SELECT compares
+//           with the slot's limit.  Ranks come from ballots, granule prefixes from 8-lane shuffle scans.
+// ------------------------------------------------------------------------------------------
+template <int NL>
+__device__ __forceinline__ uint32_t trim_pick(const uint32_t (&x)[NL], uint32_t p) {
+  uint32_t y = x[0];
+#pragma unroll
+  for (int l = 1; l < NL; ++l) if (p == static_cast<uint32_t>(l)) y = x[l];
+  return y;
+}
+
+template <int MODE, int NL>
+__global__ void __launch_bounds__(256)
+k_trim(sdb_dev_view v, sdb_recv_args r, uint32_t max_records, uint32_t max_gran) {
+  const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_EXP_G - 1), gsh = lane & ~(SDB_EXP_G - 1);
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1, below = (1u << l8) - 1u;
+  const bool retire = MODE != SDB_EXP_COUNT && !(r.flags & SDB_RECV_PEEK);
+  const bool bytes = max_gran != 0xFFFFFFFFu;
+  constexpr uint32_t SPW = 32u / SDB_EXP_G;
+  unsigned long long wsum = 0;
+  for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
+    const uint32_t q = qb + lane / SDB_EXP_G;
+    const bool valid = q < r.n;
+    uint32_t a = 0, H = 0, T = 0, NT = 0;
+    if (valid) {
+      a = r.agent_idx ? r.agent_idx[q] : q;
+      const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);
+      H = h.x; T = h.y; NT = h.w;
+    }
+    const uint32_t live = T - H - NT;
+    uint32_t RO;
+    const uint32_t limit = exp_cut<MODE>(r, valid, q, l8, &RO);
+    const bool cand = valid && live && limit && (bytes || live > max_records);
+    uint2* rs = sdb_ring_of(v, a);
+    // 1. totals per level
+    uint32_t L[NL], G[NL];
+#pragma unroll
+    for (int l = 0; l < NL; ++l) { L[l] = 0; G[l] = 0; }
+    const uint32_t W1 = cand && (bytes || NL > 1) ? T - H : 0u;
+    for (uint32_t j = l8; j < W1; j += SDB_EXP_G) {
+      const uint32_t m = sdb_meta(rs[(H + j) & mask]);
+      if (m == SDB_META_TOMB) continue;
+      const uint32_t p = NL > 1 ? m >> 14 : 0u;
+#pragma unroll
+      for (int l = 0; l < NL; ++l)
+        if (p == static_cast<uint32_t>(l)) { L[l] += 1; G[l] += (m & SDB_META_GLEN_MASK) - 1u; }
+    }
+#pragma unroll
+    for (int l = 0; l < NL; ++l)
+#pragma unroll
+      for (int o = 4; o; o >>= 1) {
+        L[l] += __shfl_xor_sync(0xFFFFFFFFu, L[l], o);
+        G[l] += __shfl_xor_sync(0xFFFFFFFFu, G[l], o);
+      }
+    if (!W1) L[0] = cand ? live : 0u;            // stream order without a byte limit: the header's count
+    // suffix sums: what is left of levels >= l, and LL[l] = the records of the levels below l
+    uint32_t SL[NL], SG[NL], LL[NL];
+    SL[NL - 1] = L[NL - 1]; SG[NL - 1] = G[NL - 1];
+#pragma unroll
+    for (int l = NL - 2; l >= 0; --l) { SL[l] = SL[l + 1] + L[l]; SG[l] = SG[l + 1] + G[l]; }
+#pragma unroll
+    for (int l = 0; l < NL; ++l) LL[l] = SL[0] - SL[l];
+    // 2. select
+    const bool walk = cand && (SL[0] > max_records || SG[0] > max_gran);
+    const uint32_t W = walk ? T - H : 0u;
+    const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
+    uint32_t got = 0, nh = walk ? T : H;
+    uint32_t ri[NL], rg[NL];                     // records and granules of each level before this step
+#pragma unroll
+    for (int l = 0; l < NL; ++l) { ri[l] = 0; rg[l] = 0; }
+    for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_EXP_G * SDB_EXP_U) {
+      uint2 e[SDB_EXP_U];
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t j = j0 + u * SDB_EXP_G + l8;
+        e[u] = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+      }
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t m = sdb_meta(e[u]);
+        const bool lv = m != SDB_META_TOMB;
+        const uint32_t p = NL > 1 ? (m >> 14) & 3u : 0u;
+        const uint32_t g = lv ? (m & SDB_META_GLEN_MASK) - 1u : 0u;
+        uint32_t i = 0, pg = 0;
+#pragma unroll
+        for (int l = 0; l < NL; ++l) {
+          const bool mine = lv && p == static_cast<uint32_t>(l);
+          const uint32_t bl = (__ballot_sync(0xFFFFFFFFu, mine) >> gsh) & 0xFFu;
+          uint32_t x = mine ? g : 0u;            // inclusive scan of the level's granules over the slot's 8 lanes
+#pragma unroll
+          for (uint32_t o = 1; o < SDB_EXP_G; o <<= 1) {
+            const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o, SDB_EXP_G);
+            if (l8 >= o) x += y;
+          }
+          if (mine) { i = ri[l] + __popc(bl & below); pg = rg[l] + x - g; }
+          ri[l] += __popc(bl);
+          rg[l] += __shfl_sync(0xFFFFFFFFu, x, SDB_EXP_G - 1, SDB_EXP_G);
+        }
+        const bool drop = lv && (trim_pick<NL>(SL, p) - i > max_records || trim_pick<NL>(SG, p) - pg > max_gran);
+        const bool sel = drop && trim_pick<NL>(LL, p) + i < limit;
+        exp_retire<MODE>(r, rs, mask, e[u], H + j0 + u * SDB_EXP_G + l8, lv, sel, retire, q, RO, l8, gsh, T, got, nh);
+      }
+    }
+    exp_store<MODE>(v, r, valid, retire, l8, q, a, H, NT, got, nh, wsum);
+  }
+  exp_total<MODE>(r, lane, wsum);
+}
+
+// One mode of expiry, or of trimming when trim != nullptr ({max_records, max_gran}, ~0: no limit; r->flags picks the
+// eviction order).
+template <int MODE>
+static void launch_retire(const sdb_dev_view* v, const sdb_recv_args* r, double older_than, uint32_t all, const uint2* trim,
+                          uint32_t blocks, cudaStream_t stream) {
+  if (!trim)
+    k_expire<MODE><<<blocks, 256, 0, stream>>>(*v, *r, older_than, all);
+  else if (r->flags & SDB_RECV_PRIORITY)
+    k_trim<MODE, 4><<<blocks, 256, 0, stream>>>(*v, *r, trim->x, trim->y);
+  else
+    k_trim<MODE, 1><<<blocks, 256, 0, stream>>>(*v, *r, trim->x, trim->y);
+}
+
+// drop mode (ca == nullptr): one launch; totals[0] = records retired.  Archive mode: count, scan, select, then the compact
 // back end exactly as a compact receive runs it (totals as there).
 extern "C" cudaError_t sdb_launch_expire(const sdb_dev_view* v, const sdb_recv_args* r, double older_than, uint32_t all,
-                                         const sdb_compact_args* ca, cudaStream_t stream, int* n_launches, sdb_profiler* prof,
-                                         int sm_count) {
+                                         const uint2* trim, const sdb_compact_args* ca, cudaStream_t stream, int* n_launches,
+                                         sdb_profiler* prof, int sm_count) {
   if (r->n == 0) return cudaSuccess;
   const uint32_t n = r->n;
   const uint32_t blocks = sdb_grid(n, 32, 32 * sm_count);                    // 4 slots per warp, 8 warps per block
   const int pi = sdb_prof_begin(prof, SDB_PK_EXPIRE, stream);
   if (!ca) {
     cudaMemsetAsync(r->totals, 0, sizeof(unsigned long long), stream);
-    k_expire<SDB_EXP_DROP><<<blocks, 256, 0, stream>>>(*v, *r, older_than, all);
+    launch_retire<SDB_EXP_DROP>(v, r, older_than, all, trim, blocks, stream);
     sdb_prof_end(prof, pi, stream);
     if (n_launches) *n_launches += 1;
     return cudaGetLastError();
   }
-  k_expire<SDB_EXP_COUNT><<<blocks, 256, 0, stream>>>(*v, *r, older_than, all);
+  launch_retire<SDB_EXP_COUNT>(v, r, older_than, all, trim, blocks, stream);
   // totals[0] = matches; the cut may lower it
   const cudaError_t e = sdb_scan_u32(r->cnt, r->rec_local, r->rec_tops, n, r->totals, nullptr, stream, n_launches);
-  k_expire<SDB_EXP_SELECT><<<blocks, 256, 0, stream>>>(*v, *r, older_than, all);
+  launch_retire<SDB_EXP_SELECT>(v, r, older_than, all, trim, blocks, stream);
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += 2;
   if (e != cudaSuccess) return e;

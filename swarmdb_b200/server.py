@@ -104,6 +104,13 @@ class GroupSendIn(BaseModel):
     metadata: Optional[Dict[str, Any]] = None
 
 
+class TrimIn(BaseModel):
+    max_messages: Optional[int] = None     # messages each agent keeps (None: no count limit)
+    max_bytes: Optional[int] = None        # pending payload bytes each agent keeps, sum of pad32(len) (None: no limit)
+    by_priority: bool = False              # drop the lowest priority first (oldest first within a level)
+    agent_ids: Optional[List[str]] = None  # None: every agent
+
+
 class MessageOut(BaseModel):
     id: str
     sender_id: str
@@ -386,6 +393,17 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
         # include_device: also archive and expire the device-queued messages older than the cutoff
         return {"status": "success", "flushed_count": guarded("flush old messages",
                                                               lambda: db.flush_old_messages(older_than, include_device))}
+
+    @app.post("/admin/trim")
+    def trim(t: TrimIn, _: str = Depends(admin)):
+        # bounded queues on demand: drop what takes each agent's device queue past the caps, without delivering it
+        try:
+            n = db.trim_queues(t.max_messages, t.max_bytes, t.agent_ids, t.by_priority)
+        except ValueError as e:                   # limits outside what trim_queues accepts: the request is at fault
+            raise HTTPException(status_code=422, detail=str(e))
+        except Exception as e:
+            raise HTTPException(status_code=http.HTTP_500_INTERNAL_SERVER_ERROR, detail=f"Failed to trim queues: {e}")
+        return {"trimmed": n}
 
     @app.post("/admin/resend_failed")
     def resend_failed(_: str = Depends(admin)):

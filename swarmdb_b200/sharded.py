@@ -623,6 +623,7 @@ class ShardedSwarmsDB(SwarmsDB):
             self._fail_round(e)
             raise
         self._flush_import()
+        self._apply_queue_caps()                 # on the agents this rank owns (RECV_OWNED): no collective
         self.sync_llm_backends()
 
     # ---- one balancer for all shards (SURVEY 8e): every rank picks from its own copy of the table; the per-backend
