@@ -7,6 +7,7 @@
   k1  point-to-point enqueue kernel roofline (1M records x 256 B)
   compact  the c2 step with host buffers out: full receive format against the compact format (sdb_receive_compact)
   expire   retention on the c2 backlog (sdb_expire): drop mode at the median cutoff, SDB_EXPIRE_ALL, archive mode
+  supersede  superseding sends (sdb_supersede): the c2 backlog without and with flagged sends, deep queues, a flush;
   trim     bounded queues on the c2 backlog (sdb_trim): count cap 2, byte cap 512 B, byte cap with priority, archive mode;
            and a SwarmsDB flush of 4,096 sends with and without GpuConfig.queue_max_messages
   where    filtered receive on the c2 backlog (sdb_receive_where): header-clause and keyword PEEKs, a take of one group's
@@ -553,6 +554,162 @@ def trim(rounds=3, block=4):
     for name, v in flush_ms.items():
         out[name] = {"ms_per_flush": float(np.median(v)), "ms_blocks": v, "sends": n_sends, "agents": n_agents}
     out["flush_cap2"]["records_trimmed_total"] = trimmed_db
+    out.update(_gpu_card(0))
+    out["clocks"] = clk
+    return out
+
+
+def supersede(rounds=3, block=4):
+    """sdb_supersede in drop mode: (a) on the c2 backlog (1M agents, 65,536 group sends x 64 = 4,194,304 pending
+    records) with no flagged record, the cost every caller of the pass pays; (b) the same backlog with every send
+    flagged; (c) deep queues, 10,000 agents x 1,000 pending point-to-point records, from 100 senders x 10 versions and
+    from 1,000 distinct senders (nothing to retire); each timed call on a fresh backlog (drain + resend, untimed),
+    modes alternated in blocks.  (d) a SwarmsDB flush of 4,096 point-to-point sends over 1,024 agents with 10 % of them
+    flagged against none, alternated (queues drained after every flush, untimed)."""
+    import torch
+    import swarmdb_b200 as sdb
+    from bench import ClockSampler, Workload
+    from swarmdb_b200._native import TYPEF_SUPERSEDE, Shard
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py supersede: no CUDA device - swarmdb_b200 has no CPU fallback")
+    wl = Workload()
+    per_step = wl.S * wl.F
+    stream = torch.cuda.Stream()
+    c2 = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+               member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+               max_recv_records=1 << 16, max_recv_payload=(1 << 16) * wl.L)
+    c2.set_stream(stream.cuda_stream)
+    c2.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        c2.create_group(g, wl.members(g))
+    plain = wl.batch()
+    flagged = plain[:3] + ((np.asarray(plain[3], np.uint8) | TYPEF_SUPERSEDE),) + plain[4:]
+    # deep queues: 10 batches of 1M sends, batch k holds pending records k*100 .. k*100+99 of every agent
+    DA, DD = 10_000, 1_000
+    deep = Shard(max_agents=DA, ring_slots=1024, arena_bytes=1 << 31, max_payload_bytes=64, max_batch_sends=1 << 20,
+                 max_batch_payload=(1 << 20) * 32, max_recv_records=1 << 16, max_recv_payload=(1 << 16) * 64)
+    deep.set_stream(stream.cuda_stream)
+    deep.register(np.arange(DA, dtype=np.uint32))
+    per = DD // 10
+    recv = np.repeat(np.arange(DA, dtype=np.uint32), per)
+    lens, off = np.full(len(recv), 16, np.uint16), np.zeros(len(recv), np.uint64)     # one shared 16-B payload
+    dpay = np.full(64, 65, np.uint8)
+    typ = np.full(len(recv), TYPEF_SUPERSEDE | 6, np.uint8)
+
+    def deep_batches(distinct):
+        j = np.tile(np.arange(per, dtype=np.uint32), DA)
+        return [((j + k * per) if distinct else j) for k in range(10)]     # senders; 100 x 10 versions or 1,000
+    senders = {"deep_100x10": deep_batches(False), "deep_1000_distinct": deep_batches(True)}
+
+    def drain(sh):
+        while sh.receive_batch(None, 1 << 10, copy_out=False)[1]:
+            pass
+
+    def c2_backlog(b):
+        drain(c2)
+        c2.send_group_batch(*b)
+        c2.sync()
+
+    def deep_backlog(name):
+        drain(deep)
+        for s in senders[name]:
+            deep.send_batch(s, recv, None, typ, lens, off, dpay)
+        deep.sync()
+
+    # name: (shard, backlog, records pending)
+    cases = {"c2_unflagged": (c2, lambda: c2_backlog(plain), per_step),
+             "c2_flagged": (c2, lambda: c2_backlog(flagged), per_step),
+             "deep_100x10": (deep, lambda: deep_backlog("deep_100x10"), DA * DD),
+             "deep_1000_distinct": (deep, lambda: deep_backlog("deep_1000_distinct"), DA * DD)}
+
+    def timed(sh, make):
+        make()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        t = time.perf_counter()
+        n = sh.supersede(None, archive=False)[1]          # synchronises: it returns totals
+        wall = (time.perf_counter() - t) * 1e3
+        e1.record(stream)
+        torch.cuda.synchronize()
+        return wall, e0.elapsed_time(e1), n
+
+    res = {k: {"call_ms": [], "event_ms": []} for k in cases}
+    retired, kern = {}, {}
+    with torch.cuda.stream(stream):
+        for sh, make, _ in cases.values():              # warm-up: every shape once
+            timed(sh, make)
+        clocks = ClockSampler(0); clocks.start()
+        for _ in range(rounds):
+            for name, (sh, make, _) in cases.items():
+                for _ in range(block):
+                    wall, ev, n = timed(sh, make)
+                    res[name]["call_ms"].append(wall); res[name]["event_ms"].append(ev)
+                    retired[name] = n
+        clk = clocks.stop()
+        for name, (sh, make, _) in cases.items():
+            make()
+            sh.profile(True)
+            sh.supersede(None, archive=False)
+            prof = sh.profile_read()
+            sh.profile(False)
+            kern[name] = {k: v[0] for k, v in prof.items() if v[1]}
+    c2.close(); deep.close()
+    out = {"config": f"c2 backlog: {wl.A} agents, {per_step} pending records, {wl.L}-B payloads; deep: {DA} agents x "
+                     f"{DD} pending; {rounds} rounds of {block} calls per case, each on a fresh backlog"}
+    for name, (_, _, N) in cases.items():
+        A = wl.A if name.startswith("c2") else DA
+        n = retired[name]
+        flag = name != "c2_unflagged"
+        # algorithmic bytes: the count walk (16-B ring header per agent, 8 B per ring entry, the header's last word from
+        # one 32-B sector per record); with flagged records also the insert walk (the same, a whole sector per record,
+        # a 24-B candidate and a 32-B table slot written), the tie and verdict passes (candidate and slot read twice,
+        # a 4-B verdict word), the retire walk (header, entries, verdict words) and an 8-B tombstone per retired record
+        nbytes = 16 * A + 8 * N + 32 * N
+        if flag:
+            nbytes += (16 * A + 8 * N + 32 * N + 24 * N + 32 * N) + 2 * (24 * N + 32 * N) + 4 * N + \
+                      (16 * A + 8 * N + N // 8) + 8 * n
+        kms = kern[name].get("expire", sum(kern[name].values()))
+        out[name] = {"records_pending": N, "records_retired": n, "ms_per_call": float(np.median(res[name]["call_ms"])),
+                     "event_ms_per_call": float(np.median(res[name]["event_ms"])), "kernel_ms": kern[name],
+                     "supersede_kernel_ms": kms, "algorithmic_bytes": nbytes,
+                     "algorithmic_gb_per_s_kernel": nbytes / (kms * 1e-3) / 1e9 if kms else None,
+                     "share_of_3_35_TBps": nbytes / (kms * 1e-3) / 3.35e12 if kms else None,
+                     "call_ms_blocks": res[name]["call_ms"]}
+    # SwarmsDB flush of 4,096 point-to-point sends, 10 % flagged against none
+    import tempfile
+    n_agents, n_sends = 1024, 4096
+    rng = np.random.default_rng(5)
+    to = rng.integers(0, n_agents, n_sends).tolist()
+    flag_mask = (rng.random(n_sends) < 0.1).tolist()
+    with tempfile.TemporaryDirectory() as tmp:
+        dbs = {name: sdb.SwarmsDB(save_dir=tmp, auto_save=False,
+                                  gpu_config=sdb.GpuConfig(max_agents=n_sends, flush_threshold=n_sends + 1,
+                                                           deterministic_ids=True))
+               for name in ("flush_none_flagged", "flush_10pct_flagged")}
+        names = [f"a{i}" for i in range(n_agents)]
+        for db in dbs.values():
+            for a in names:
+                db.register_agent(a)
+        flush_ms = {name: [] for name in dbs}
+        for r in range(2 + rounds * block):
+            for name, db in (dbs.items() if r % 2 == 0 else reversed(list(dbs.items()))):
+                on = name == "flush_10pct_flagged"
+                for i, a in enumerate(to):
+                    db.send_message(names[i % n_agents], "x" * 100, receiver_id=names[a], supersede=on and flag_mask[i])
+                torch.cuda.synchronize()
+                t = time.perf_counter()
+                db.flush()
+                db.shard.sync()
+                if r >= 2:
+                    flush_ms[name].append((time.perf_counter() - t) * 1e3)
+                db.shard.receive_batch(None, 1 << 10, copy_out=False)
+                db.messages.clear(); db.agent_inbox.clear()
+        superseded_db = dbs["flush_10pct_flagged"].get_stats()["superseded"]
+        for db in dbs.values():
+            db.close()
+    for name, v in flush_ms.items():
+        out[name] = {"ms_per_flush": float(np.median(v)), "ms_blocks": v, "sends": n_sends, "agents": n_agents}
+    out["flush_10pct_flagged"]["records_superseded_total"] = superseded_db
     out.update(_gpu_card(0))
     out["clocks"] = clk
     return out

@@ -58,6 +58,7 @@ enum { SDB_TYPE_CHAT = 0, SDB_TYPE_COMMAND, SDB_TYPE_FUNCTION_CALL, SDB_TYPE_FUN
 #define SDB_TYPE_MASK 0x07u
 #define SDB_TYPEF_JSON 0x08u            /* payload content is JSON (dict/list content, M:75) */
 #define SDB_TYPEF_EXTRAS 0x10u          /* payload = u32 content_len | content | JSON extras */
+#define SDB_TYPEF_SUPERSEDE 0x20u       /* superseding: a newer flagged record with the same (sender, group, type) replaces it (sdb_supersede) */
 
 /* Replaces KafkaConfig (M:114-127) + SwarmsDB.__init__ kwargs (M:156-165) for the device side. */
 typedef struct sdb_config {
@@ -738,6 +739,46 @@ int sdb_trim(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_
              uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
              sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
              uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
+
+/* ---- superseding sends: last-value queues, conflation (RabbitMQ last-value cache, Kafka compaction, MQTT retained) ---
+ * sdb_supersede keeps, at each listed agent, only the newest pending record of each key among the records sent with
+ * SDB_TYPEF_SUPERSEDE in their type byte, and retires the others without delivering them.  The send calls do not change:
+ * the caller sets the bit in type[].  Costs one header read per live pending record when nothing is flagged.
+ *   1. Key        two pending records of one agent have the same key when both carry SDB_TYPEF_SUPERSEDE and have equal
+ *                 sender, group and type & SDB_TYPE_MASK.  The JSON and extras bits, priority, length and timestamp are
+ *                 not part of it.  Point-to-point sends and broadcast copies both have group == SDB_NO_GROUP, so for one
+ *                 sender and one type they share a key.
+ *   2. Newest     within a key the record with the largest seq is kept; a tie in seq goes to the record later in the
+ *                 ring (restoring the output of a PEEK compact receive with sdb_restore_compact makes one: restore does
+ *                 not refuse a seq that is still pending).  Ring order is not seq order once a lease sweep, redrive,
+ *                 restore or requeue put records back behind newer ones: the rule is by seq, so a redelivered stale
+ *                 version is the one that goes.  Every other record of the key is superseded; unflagged records are
+ *                 never counted or retired.
+ *   3. Scope      only pending ring records are compared, as in sdb_trim: in-flight leases and dead letters are neither
+ *                 compared nor touched, so a redelivered version can follow a newer one that was already received.
+ *                 agent_idx == NULL and SDB_RECV_OWNED as in sdb_expire; an agent listed twice or out of range is
+ *                 SDB_EINVAL.
+ *   4. Effect     that of sdb_trim: every later receive (any order, any path, digests included) delivers what it would
+ *                 have delivered had the superseded records never been enqueued.  sdb_stats does not move; in
+ *                 sdb_agent_loads `pending` and `pending_granules` fall and `received` stays.  The head and ntomb stay
+ *                 exact.  Ledger entries of retired records (sdb_lease_set_policy) are collected as expired ones.
+ *   5. Archive    as sdb_trim: the superseded records come back in the compact receive format with sdb_expire's
+ *      mode       capacity rule: agents in list order, ring order within an agent, the first agent of the output may be
+ *                 partial.  The newest record of a key is never selected, so any subset of the superseded set is safe
+ *                 to retire: calls repeated until *total_out == 0 retire exactly what one drop-mode call retires.  No
+ *                 usable output capacity: SDB_EOUTPUT.
+ *   6. Drop mode  as sdb_trim: count_out[n_agents] (nullable) and *total_out are filled, *n_sends_out and
+ *                 *payload_bytes_out read 0.
+ *   7. Flags      SDB_RECV_PEEK (dry run: select and report, retire nothing), SDB_RECV_OWNED; any other bit is SDB_EINVAL.
+ *   8. Ordering   as sdb_trim: stream-ordered, synchronising, rings only; kernels are timed under SDB_PK_EXPIRE.  A
+ *                 count pass runs first and the call ends there when no listed agent has a flagged pending record.
+ *                 Otherwise it needs a key table of 32 bytes per slot (a power of two >= 2 x the flagged records) and
+ *                 24 bytes per flagged record, kept by the handle and grown on demand; when they cannot be allocated the
+ *                 call refuses with SDB_ECAPACITY before anything is retired.  A refused call changes nothing. */
+int sdb_supersede(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t flags,
+                  uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                  sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                  uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
 
 /* ---- relocation of pinned queues: the other remedy for an agent that pins the log.  Where sdb_expire drops its records,
  * sdb_arena_relocate keeps them: it copies the live records of the agents pinning the log to the tail of the arena and

@@ -51,6 +51,7 @@ FILTER_MAX_KEYWORD = 256
 FILTER_MAX_IDS = 1 << 22
 TYPEF_JSON = 0x08
 TYPEF_EXTRAS = 0x10
+TYPEF_SUPERSEDE = 0x20
 TYPE_MASK = 0x07
 
 STATUS_NAMES = {0: "SDB_OK", -1: "SDB_EINVAL", -2: "SDB_ECUDA", -3: "SDB_ENOMEM", -4: "SDB_ERING_OVERFLOW",
@@ -167,7 +168,7 @@ class SdbRelocateSummary(C.Structure):
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_profile_read_n", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
-           "sdb_receive_batch", "sdb_receive_compact", "sdb_receive_budget", "sdb_receive_compact_budget", "sdb_restore_compact", "sdb_expire", "sdb_trim", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
+           "sdb_receive_batch", "sdb_receive_compact", "sdb_receive_budget", "sdb_receive_compact_budget", "sdb_restore_compact", "sdb_expire", "sdb_trim", "sdb_supersede", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
@@ -262,6 +263,8 @@ def load_library() -> C.CDLL:
     L.sdb_expire.argtypes = [vp, u32, vp, C.c_double, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_trim.restype = i32
     L.sdb_trim.argtypes = [vp, u32, vp, u32, u64, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    L.sdb_supersede.restype = i32
+    L.sdb_supersede.argtypes = [vp, u32, vp, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_receive_where.restype = i32
     L.sdb_receive_where.argtypes = [vp, u32, vp, u32, u32, C.POINTER(SdbFilter), vp, vp, u64, vp, u64, vp, vp]
     L.sdb_latency_server.restype = i32; L.sdb_latency_server.argtypes = [vp, i32]
@@ -903,6 +906,28 @@ class Shard:
                                      _p(pay), 0 if pay is None else pay.nbytes,
                                      C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
                                      C.cast(C.byref(pbytes), C.c_void_p)))
+        if agents is None:
+            counts = self._served_counts(counts, flags)
+        if not archive:
+            return counts, int(total.value)
+        return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
+
+    def supersede(self, agents, flags: int = 0, archive: bool = True, out_entries: Optional[np.ndarray] = None,
+                  out_sends: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+        """Keep, per agent and key (sender, group, type & TYPE_MASK) of the pending records sent with TYPEF_SUPERSEDE,
+        only the newest one (largest seq, the later in the ring on a tie) and retire the others without delivering them
+        (include/swarmdb_b200.h: sdb_supersede).  Returns trim's shapes: archive=True gives the superseded records as
+        (counts, entries, sends, payload) - loop until no entry comes back; archive=False drops them: (counts, total)."""
+        a, n, counts = self._agents_arg(agents)
+        total, n_sends, pbytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        ent = snd = pay = None
+        if archive:
+            ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
+        self._check(self._L.sdb_supersede(self._h, n, _p(a), flags, _p(counts),
+                                          _p(ent), 0 if ent is None else len(ent), _p(snd), 0 if snd is None else len(snd),
+                                          _p(pay), 0 if pay is None else pay.nbytes,
+                                          C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
+                                          C.cast(C.byref(pbytes), C.c_void_p)))
         if agents is None:
             counts = self._served_counts(counts, flags)
         if not archive:

@@ -41,7 +41,7 @@ import numpy as np
 from pydantic import BaseModel, Field
 
 from . import _native
-from ._native import (EXPIRE_ALL, FILTER_MAX_IDS, FILTER_MAX_KEYWORD, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON,
+from ._native import (EXPIRE_ALL, FILTER_MAX_IDS, FILTER_MAX_KEYWORD, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON, TYPEF_SUPERSEDE,
                       SdbError, Shard, make_filter, pad32, recv_capacity)
 
 
@@ -209,6 +209,18 @@ def _trim_limits(max_messages: Optional[int], max_bytes: Optional[int]) -> Tuple
     return max_messages or 0, max_bytes or 0
 
 
+def _check_supersede(supersede: Any) -> None:
+    if not isinstance(supersede, bool):
+        raise TypeError(f"supersede={supersede!r} is not a bool")
+
+
+def _flagged(typ, n: int) -> np.ndarray:
+    """Which of n index-level sends carry TYPEF_SUPERSEDE in their type (typ None: none)."""
+    if typ is None:
+        return np.zeros(n, bool)
+    return np.broadcast_to((np.asarray(typ, np.int64) & TYPEF_SUPERSEDE) != 0, (n,))
+
+
 def _encode_content(content: Any) -> (bytes, int):
     if isinstance(content, str):
         return content.encode("utf-8"), 0
@@ -335,6 +347,8 @@ class SwarmsDB:
                 raise ValueError(f"GpuConfig.dedup_window={g.dedup_window} must be > 0 seconds")
             self.shard.dedup_reserve(g.dedup_entries, g.dedup_window)
         self._trimmed = 0                       # records the automatic queue caps dropped (get_stats()["trimmed"])
+        self._superseded = 0                    # records superseding sends retired (get_stats()["superseded"])
+        self._supersedes = False                # a flagged record was staged, sent or restored: passes after re-enqueues
         self._reset_buffer()
         self._closed = False
         self.admin_client = _TransportAdmin(self)          # M:202-204: callers only list topics through it
@@ -356,6 +370,7 @@ class SwarmsDB:
         self._b_msgs: List[Message] = []
         self._b_key: List[Tuple[int, int]] = []          # dedup key of each send, (0, 0): none
         self._b_seq0: List[int] = []                     # first seq of each send
+        self._b_supersede: Set[int] = set()              # receivers of the buffered superseding sends
         self._b_first_seq = self._next_seq
 
     def _index(self, agent_id: str) -> int:
@@ -400,6 +415,7 @@ class SwarmsDB:
         if n == 0:
             return
         msgs = self._b_msgs
+        superseding = self._b_supersede
         keys = None                             # the keys the device used (deduplicated sends only)
         try:
             payload = np.frombuffer(bytes(self._b_payload) + b"\0" * 32, dtype=np.uint8)
@@ -447,9 +463,57 @@ class SwarmsDB:
             # ids already handed out stay used: the device counter moves up to the host's, never the other way
             self.shard.advance_seq(self._next_seq)
             self._reset_buffer()
+            if isinstance(e, RingOverflow):     # the device took the batch but some records: they may supersede
+                self._supersede_receivers(superseding)
             raise
         self._reset_buffer()
+        self._supersede_receivers(superseding)
         self._apply_queue_caps()
+
+    def _supersede_receivers(self, receivers) -> None:
+        """The pass after a send: over the receivers of its superseding sends, nothing when there were none."""
+        if receivers:
+            self._supersede_pass(np.fromiter(sorted(receivers), dtype=np.uint32, count=len(receivers)))
+
+    def _supersede_pass(self, agents: Optional[np.ndarray]) -> int:
+        """sdb_supersede over `agents` (None: every agent below the watermark) in archive mode, call after call until
+        nothing comes back.  Each retired copy that has a host record leaves its receiver's inbox and adds the receiver
+        to metadata["superseded_for"]; the record stays in `messages` with its status.  Returns the records retired."""
+        total = 0
+        while True:
+            cnt, ent, _, _ = self.shard.supersede(agents)
+            if len(ent) == 0:
+                break
+            idx = agents if agents is not None else np.arange(len(cnt), dtype=np.uint32)
+            for a, seq in zip(np.repeat(idx, cnt.astype(np.int64)).tolist(), ent["seq"].tolist()):
+                m = self.messages.get(self._make_id(int(seq)))
+                if m is None:
+                    continue
+                name = self._agent_name[a] if a < len(self._agent_name) else None
+                inbox = self.agent_inbox.get(name)
+                if inbox and m.id in inbox:
+                    inbox.remove(m.id)
+                m.metadata.setdefault("superseded_for", []).append(name)
+            total += len(ent)
+        self._superseded += total
+        return total
+
+    def _supersede_after_restore(self, flagged: bool = False) -> None:
+        """The pass over every agent after a call that put records back (flagged: those records include one)."""
+        self._supersedes = self._supersedes or bool(flagged)
+        if self._supersedes:
+            self._supersede_pass(None)
+
+    def supersede_pending(self, agent_ids: Optional[Iterable[str]] = None) -> int:
+        """Keep, per agent (default: every agent) and per (sender, group, message type), only the newest pending message
+        among those sent with supersede=True, and drop the others without delivering them.  Host records are updated as
+        after a flush: a dropped copy leaves its receiver's inbox and names it in metadata["superseded_for"].  Returns
+        the number of records dropped."""
+        agents = None if agent_ids is None else self._expire_scope(agent_ids)[0]
+        self._pre_read()
+        if agents is not None and len(agents) == 0:
+            return 0
+        return self._supersede_pass(agents)
 
     def _apply_queue_caps(self) -> None:
         """GpuConfig.queue_max_messages / queue_max_bytes: one drop-mode trim of every agent this instance serves."""
@@ -614,9 +678,13 @@ class SwarmsDB:
         visible_to: Optional[List[str]] = None,
         _group: int = NO_GROUP,
         dedup_id: Optional[str] = None,
+        supersede: bool = False,
     ) -> str:
         """dedup_id: with GpuConfig.dedup_entries, a second send of the same sender with the same dedup_id inside the
-        window is not queued; after the flush, original_id() names the message it matched."""
+        window is not queued; after the flush, original_id() names the message it matched.
+        supersede: a later superseding send of the same sender and message type to the same receiver replaces this one
+        while both are pending (a last-value queue for status reports, heartbeats, plans); each flush keeps the newest."""
+        _check_supersede(supersede)
         key = self._dedup_key(sender_id, dedup_id)
         if sender_id not in self.registered_agents:
             self.register_agent(sender_id)
@@ -662,19 +730,20 @@ class SwarmsDB:
             flags |= TYPEF_EXTRAS
         else:
             payload = body
-        type_code = _TYPE_CODE[MessageType(message_type)] | flags
+        type_code = _TYPE_CODE[MessageType(message_type)] | flags | (TYPEF_SUPERSEDE if supersede else 0)
         prio = int(MessagePriority(priority))
         sender = self._index(sender_id)
+        recips: List[int] = []
         try:
             if receiver_id is not None:
                 deliverable = (not message.visible_to) or (receiver_id in message.visible_to)    # M:579-585
                 if deliverable:
-                    self._stage(0, sender, self._index(receiver_id), prio, type_code, payload, message.timestamp, key)
+                    recips = [self._index(receiver_id)]
+                    self._stage(0, sender, recips[0], prio, type_code, payload, message.timestamp, key)
                 else:      # in the log, matched by no consumer: an empty recipient list
                     self._stage_list(sender, [], prio, type_code, payload, message.timestamp, key)
             else:
                 seen: Set[int] = set()
-                recips = []
                 for a in message.visible_to:
                     i = self._index(a)
                     if i not in seen:
@@ -686,6 +755,9 @@ class SwarmsDB:
             raise
         self._next_seq += 1
         self._b_msgs.append(message)
+        if supersede:
+            self._supersedes = True
+            self._b_supersede.update(recips)
         if dedup_id is not None:
             self._dedup_ids[message.id] = dedup_id
         message.status = MessageStatus.DELIVERED                          # delivery report, M:374-391
@@ -742,11 +814,13 @@ class SwarmsDB:
         metadata: Optional[Dict[str, Any]] = None,
         exclude_agents: Optional[List[str]] = None,
         dedup_id: Optional[str] = None,
+        supersede: bool = False,
     ) -> str:
         excluded = set(exclude_agents or [])
         visible = [a for a in self.registered_agents if a != sender_id and a not in excluded]
         return self.send_message(sender_id=sender_id, content=content, receiver_id=None, message_type=message_type,
-                                 priority=priority, metadata=metadata, visible_to=visible, dedup_id=dedup_id)
+                                 priority=priority, metadata=metadata, visible_to=visible, dedup_id=dedup_id,
+                                 supersede=supersede)
 
     # ------------------------------------------------------------------ groups
     def add_agent_group(self, group_name: str, agent_ids: List[str]) -> None:
@@ -784,7 +858,11 @@ class SwarmsDB:
         priority: MessagePriority = MessagePriority.NORMAL,
         metadata: Optional[Dict[str, Any]] = None,
         dedup_id: Optional[str] = None,
+        supersede: bool = False,
     ) -> List[str]:
+        """supersede: as in send_message, per member: the newest pending superseding send of this sender and message
+        type to the group is the one each member keeps."""
+        _check_supersede(supersede)
         key = self._dedup_key(sender_id, dedup_id)
         groups = self.metadata.get("agent_groups", {})
         if group_name not in groups:
@@ -834,8 +912,12 @@ class SwarmsDB:
             staged = True
         if staged or members:
             self._stage(1, self._index(sender_id), g, int(MessagePriority(priority)),
-                        _TYPE_CODE[MessageType(message_type)] | flags, payload, now, key)
+                        _TYPE_CODE[MessageType(message_type)] | flags | (TYPEF_SUPERSEDE if supersede else 0), payload, now,
+                        key)
             self._next_seq += len(members)
+            if supersede:
+                self._supersedes = True
+                self._b_supersede.update(self._index(a) for a in members if a != sender_id)
         if ids:
             self._after_send()
         return ids
@@ -1000,6 +1082,8 @@ class SwarmsDB:
         if not all and not blocked:
             while self._lease_deadlines and self._lease_deadlines[0] <= now:
                 heapq.heappop(self._lease_deadlines)
+        if total:
+            self._supersede_after_restore()
         return total
 
     # ------------------------------------------------------------------ dead letters (GpuConfig.lease_max_deliveries)
@@ -1059,6 +1143,7 @@ class SwarmsDB:
             for a, mid in zip(who, ids):
                 self._forget(a, [mid])
             total += n
+            self._supersede_after_restore()
 
     def _sweep_due(self, now: float) -> None:
         if self._lease_deadlines and self._lease_deadlines[0] <= now:
@@ -1268,12 +1353,25 @@ class SwarmsDB:
         self.flush()
         base = self.shard.send_batch(sender_idx, receiver_idx, prio, typ, lens, payload_off, payload, ts)
         self._next_seq = base + len(np.atleast_1d(sender_idx)); self._b_first_seq = self._next_seq
+        flagged = _flagged(typ, len(np.atleast_1d(sender_idx)))
+        if flagged.any():
+            self._supersedes = True
+            self._supersede_receivers(set(np.broadcast_to(np.asarray(receiver_idx, np.int64), flagged.shape)[flagged].tolist()))
         return base
 
     def send_to_group_batch(self, sender_idx, group_idx, prio, typ, lens, payload_off, payload, ts=None) -> int:
         self.flush()
         base = self.shard.send_group_batch(sender_idx, group_idx, prio, typ, lens, payload_off, payload, ts)
         self._next_seq = self.shard.stats()["next_seq"]; self._b_first_seq = self._next_seq
+        flagged = _flagged(typ, len(np.atleast_1d(sender_idx)))
+        if flagged.any():
+            self._supersedes = True
+            groups = set(np.broadcast_to(np.asarray(group_idx, np.int64), flagged.shape)[flagged].tolist())
+            known = [self._group_snapshot[k] for k in groups if k < len(self._group_snapshot)]
+            if len(known) == len(groups) and all(m is not None for m in known):
+                self._supersede_receivers({self._agent_idx[a] for m in known for a in m if a in self._agent_idx})
+            else:                               # a group this instance did not create: every agent
+                self._supersede_pass(None)
         return base
 
     def receive_batch(self, agent_idx=None, max_messages: int = 100, priority: Optional[bool] = None,
@@ -1306,6 +1404,7 @@ class SwarmsDB:
         ent, snd = _renumber_rows(entries, sends)
         n, seq_end = self.shard.restore_compact(agent_idx, counts, ent, snd, payload)
         self._next_seq = max(self._next_seq, seq_end); self._b_first_seq = self._next_seq
+        self._supersede_after_restore(bool(np.any(np.asarray(snd["type"]) & TYPEF_SUPERSEDE)))
         return n
 
     # ------------------------------------------------------------------ queue snapshots (restart persistence)
@@ -1557,6 +1656,7 @@ class SwarmsDB:
         self._next_seq = max(self._next_seq, seq_end); self._b_first_seq = self._next_seq
         if in_flight:
             self._load_in_flight(snap, parts)
+        self._supersede_after_restore(bool(np.any(snap["sends"]["type"] & TYPEF_SUPERSEDE)))
 
     # ------------------------------------------------------------------ LLM backends (M:1281-1325 + real balancer)
     def set_llm_load_balancing(self, enabled: bool = True) -> None:
@@ -1796,6 +1896,7 @@ class SwarmsDB:
             out["dedup"] = self.shard.dedup_stats()
         if self.gpu_config.queue_max_messages or self.gpu_config.queue_max_bytes:
             out["trimmed"] = self._trimmed                 # messages the queue caps dropped, never delivered
+        out["superseded"] = self._superseded               # records newer superseding sends replaced, never delivered
         return out
 
     def resend_failed_messages(self) -> List[str]:

@@ -143,6 +143,9 @@ struct sdb_ctx {
   unsigned long long* id_in = nullptr;                   // per-id outputs [2 x id_cap], allocated on the first call with
   uint32_t* id_out = nullptr;                            // the clause and grown on demand
   uint64_t id_cap = 0, id_slots = 0;
+  sdb_ss_slot* ss_tab = nullptr;                         // sdb_supersede: key table [ss_slots] and candidates [ss_cap],
+  sdb_ss_cand* ss_cand = nullptr;                        // allocated on the first call with a flagged record and grown on
+  uint64_t ss_slots = 0, ss_cap = 0;                     // demand
   unsigned long long* digest = nullptr;                  // [max_agents] stream digests, allocated on first use
   uint32_t* rs_agent = nullptr;                          // restore: per-agent tables [6][max_agents] + scan tops, allocated
   unsigned long long* rs_tot = nullptr;                  // on first use; totals [8]
@@ -974,7 +977,7 @@ int sdb_destroy(sdb_handle h) {
                  h->be_weight, h->be_load, h->be_scratch, h->be_logtab, h->be_req_cost, h->be_out, h->digest,
                  h->cx.table, h->cx.rec_slot, h->cx.head, h->cx.head_local, h->cx.head_tops, h->cx.gran, h->cx.gran_local,
                  h->cx.gran_tops, h->cx.totals, h->cx.entry_out, h->cx.send_out, h->cx.payload_out, h->where_bits, h->where_kw,
-                 h->id_tab, h->id_in, h->id_out,
+                 h->id_tab, h->id_in, h->id_out, h->ss_tab, h->ss_cand,
                  h->rs_agent, h->rs_tot, h->rs_sort, h->rl_bits, h->rl_cnt, h->rl_pre, h->rl_tops, h->rl_sel, h->rl_tot};
   for (void* p : dev) if (p) cudaFree(p);
   lease_free(h);
@@ -2112,6 +2115,15 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   return copy_full(h, n_agents, count_out, hdr_out, payload_out, total_out, payload_bytes_out);
 }
 
+// verdict bitmap of filtered receives and superseding, [max_agents][where_stride] words, and the keyword buffer; allocated
+// once, on first use
+static uint32_t where_stride(const sdb_ctx* h) { return (h->cfg.ring_slots + 31) / 32; }
+static int where_ensure(sdb_ctx* h) {
+  if (h->where_bits) return SDB_OK;
+  return dmalloc_set(h, {{&h->where_bits, static_cast<size_t>(h->cfg.max_agents) * where_stride(h)}, {&h->where_kw, SDB_FILTER_MAX_KEYWORD}},
+                     "filtered receive: device allocation failed");
+}
+
 // compact receive scratch and outputs, sized for max_recv_records; allocated once, on the first compact call
 static int compact_ensure(sdb_ctx* h) {
   sdb_compact_args& c = h->cx;
@@ -2228,10 +2240,43 @@ int sdb_receive_compact_budget(sdb_handle h, uint32_t n_agents, const uint32_t* 
   return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
 }
 
-// The body of sdb_expire and sdb_trim: `flags` were checked by the caller, trim == nullptr is an expiry.  Archive mode
-// takes sdb_receive_compact's capacity rule and copy-out; drop mode returns the count and the per-agent counts.
+// The first step of sdb_supersede: count the flagged pending records of r's agents (one synchronisation) and, when there
+// are any, size the key table (a power of two >= 2 x the records) and the candidate array, zero the table and fill *s.
+// s->n_cand == 0: nothing can be superseded.  Scratch that cannot be allocated refuses the call before anything retires.
+static int supersede_prepare(sdb_ctx* h, const sdb_recv_args& r, sdb_ss_args* s, int* nl) {
+  *s = sdb_ss_args{};
+  const cudaError_t e = sdb_launch_supersede(&h->view, &r, s, nullptr, h->stream, nl, &h->prof, h->sm_count);
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("supersede count launch: ") + cudaGetErrorString(e));
+  CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  h->stream_busy = false;
+  const uint64_t C = h->totals_host[TOT_RECORDS];
+  if (C == 0) return SDB_OK;
+  if (C > (1ull << 30)) return fail(h, SDB_ECAPACITY, "sdb_supersede: more than 2^30 flagged pending records");
+  uint64_t slots = 1024;
+  while (slots < 2 * C) slots <<= 1;
+  if (where_ensure(h) != SDB_OK) return fail(h, SDB_ECAPACITY, "sdb_supersede: verdict bitmap allocation failed");
+  if (slots > h->ss_slots || C > h->ss_cap) {
+    const uint64_t cap = std::max(C, h->ss_cap), sl = std::max(slots, h->ss_slots);
+    { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }   // cudaFree waits for the kernels on the device
+    for (void* p : {static_cast<void*>(h->ss_tab), static_cast<void*>(h->ss_cand)}) if (p) cudaFree(p);
+    h->ss_tab = nullptr; h->ss_cand = nullptr; h->ss_slots = h->ss_cap = 0;
+    if (dmalloc_set(h, {{&h->ss_tab, sl}, {&h->ss_cand, cap}}, "sdb_supersede: scratch allocation failed") != SDB_OK)
+      return fail(h, SDB_ECAPACITY, "sdb_supersede: no device memory for the key table of " + std::to_string(C) + " records");
+    h->ss_slots = sl; h->ss_cap = cap;
+  }
+  CUDA_TRY(h, cudaMemsetAsync(h->ss_tab, 0, slots * sizeof(sdb_ss_slot), h->stream));
+  s->tab = h->ss_tab; s->mask = static_cast<uint32_t>(slots - 1);
+  s->cand = h->ss_cand; s->n_cand = static_cast<uint32_t>(C);
+  s->bits = h->where_bits; s->stride = where_stride(h);
+  return SDB_OK;
+}
+
+// The body of sdb_expire, sdb_trim and sdb_supersede: `flags` were checked by the caller; trim == nullptr without
+// `supersede` is an expiry.  Archive mode takes sdb_receive_compact's capacity rule and copy-out; drop mode returns the
+// count and the per-agent counts.
 static int retire_call(sdb_ctx* h, uint32_t n_agents, const uint32_t* agent_idx, double older_than, const uint2* trim,
-                       uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                       bool supersede, uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
                        sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                        uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
   const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
@@ -2249,11 +2294,25 @@ static int retire_call(sdb_ctx* h, uint32_t n_agents, const uint32_t* agent_idx,
     if (rc != SDB_OK) return rc; }
   if (!archive && !count_out) r.count_out = nullptr;           // nobody reads the counts
   int nl = 0;
-  cudaError_t e = sdb_launch_expire(&h->view, &r, older_than, (flags & SDB_EXPIRE_ALL) ? 1u : 0u, trim, archive ? &h->cx : nullptr,
-                                    h->stream, &nl, &h->prof, h->sm_count);
+  cudaError_t e;
+  if (supersede) {
+    sdb_ss_args s;
+    const int rc = supersede_prepare(h, r, &s, &nl);
+    h->last_rx_valid = false; h->last_rx_compact = false;
+    if (rc != SDB_OK || s.n_cand == 0) {                        // refused, or no flagged record: nothing more to launch
+      h->launches += nl;
+      if (rc == SDB_OK && count_out) std::fill(count_out, count_out + n_agents, 0u);
+      return rc;
+    }
+    e = sdb_launch_supersede(&h->view, &r, &s, archive ? &h->cx : nullptr, h->stream, &nl, &h->prof, h->sm_count);
+  } else {
+    e = sdb_launch_expire(&h->view, &r, older_than, (flags & SDB_EXPIRE_ALL) ? 1u : 0u, trim, archive ? &h->cx : nullptr,
+                          h->stream, &nl, &h->prof, h->sm_count);
+  }
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = false;       // the receive scratch was reused: nothing left to fold
-  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string(trim ? "trim" : "expire") + " launch: " + cudaGetErrorString(e));
+  if (e != cudaSuccess)
+    return fail(h, SDB_ECUDA, std::string(supersede ? "supersede" : trim ? "trim" : "expire") + " launch: " + cudaGetErrorString(e));
   if (archive) return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
   // drop mode: the number of records retired and the counts
   CUDA_TRY(h, cudaMemcpyAsync(h->totals_host, h->rx_totals, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
@@ -2275,7 +2334,7 @@ int sdb_expire(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, doubl
   if (payload_bytes_out) *payload_bytes_out = 0;
   if (flags & ~(SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_EXPIRE_ALL))
     return fail(h, SDB_EINVAL, "sdb_expire accepts SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_EXPIRE_ALL only");
-  return retire_call(h, n_agents, agent_idx, older_than, nullptr, flags, count_out, entry_out, entry_cap, send_out, send_cap,
+  return retire_call(h, n_agents, agent_idx, older_than, nullptr, false, flags, count_out, entry_out, entry_cap, send_out, send_cap,
                      payload_out, payload_cap, total_out, n_sends_out, payload_bytes_out);
 }
 
@@ -2295,7 +2354,21 @@ int sdb_trim(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_
   const uint2 lim = make_uint2(max_records ? max_records : 0xFFFFFFFFu,
                                max_agent_bytes ? static_cast<uint32_t>(std::min<uint64_t>(max_agent_bytes / SDB_GRANULE, 0xFFFFFFFEull))
                                                : 0xFFFFFFFFu);
-  return retire_call(h, n_agents, agent_idx, 0.0, &lim, flags, count_out, entry_out, entry_cap, send_out, send_cap,
+  return retire_call(h, n_agents, agent_idx, 0.0, &lim, false, flags, count_out, entry_out, entry_cap, send_out, send_cap,
+                     payload_out, payload_cap, total_out, n_sends_out, payload_bytes_out);
+}
+
+int sdb_supersede(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t flags,
+                  uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                  sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                  uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  if (!h) return SDB_EINVAL;
+  if (total_out) *total_out = 0;
+  if (n_sends_out) *n_sends_out = 0;
+  if (payload_bytes_out) *payload_bytes_out = 0;
+  if (flags & ~(SDB_RECV_PEEK | SDB_RECV_OWNED))
+    return fail(h, SDB_EINVAL, "sdb_supersede accepts SDB_RECV_PEEK and SDB_RECV_OWNED only");
+  return retire_call(h, n_agents, agent_idx, 0.0, nullptr, true, flags, count_out, entry_out, entry_cap, send_out, send_cap,
                      payload_out, payload_cap, total_out, n_sends_out, payload_bytes_out);
 }
 
@@ -3102,12 +3175,8 @@ int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
     const int rc = out_rec_cap(h, room(hdr_out, hdr_cap), room(payload_out, payload_cap), &rec_cap);
     if (rc != SDB_OK) return rc;
   }
-  const uint32_t stride = (h->cfg.ring_slots + 31) / 32;
-  if (!h->where_bits) {
-    const int rc = dmalloc_set(h, {{&h->where_bits, static_cast<size_t>(h->cfg.max_agents) * stride}, {&h->where_kw, SDB_FILTER_MAX_KEYWORD}},
-                               "filtered receive: device allocation failed");
-    if (rc != SDB_OK) return rc;
-  }
+  const uint32_t stride = where_stride(h);
+  { const int rc = where_ensure(h); if (rc != SDB_OK) return rc; }
   sdb_recv_args r{};
   { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK), rec_cap, &r);
     if (rc != SDB_OK) return rc; }

@@ -205,6 +205,27 @@ struct __align__(16) sdb_id_slot {
   uint32_t hits, nagent;
 };
 
+// superseding (sdb_supersede): one key of the open-addressing table, {0,0} empty (a key has bit 63 of hi set), the
+// largest seq of its records and the largest ring offset among the records holding that seq
+struct __align__(16) sdb_ss_slot {
+  unsigned long long klo, khi;
+  unsigned long long seq;
+  uint32_t off, pad;
+};
+// one flagged pending record: its seq, request slot, ring offset from the head and table slot
+struct sdb_ss_cand {
+  unsigned long long seq;
+  uint32_t q, j, slot, pad;
+};
+struct sdb_ss_args {
+  sdb_ss_slot* tab;            // [mask + 1] zeroed, a power of two >= 2 x n_cand
+  uint32_t mask;
+  sdb_ss_cand* cand;           // [n_cand] in request-slot order
+  uint32_t n_cand;
+  uint32_t* bits;              // verdict bitmap, the layout of sdb_where_args::bits: bit j of agent a is superseded
+  uint32_t stride;
+};
+
 // arguments of one restore (sdb_restore_compact): the compact-format input staged in the compact receive's buffers, the
 // per-agent tables uploaded by the host, and scratch carved out of the compact receive's scratch (sdb_api.cu)
 struct sdb_restore_args {
@@ -881,6 +902,8 @@ cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaSt
                                const sdb_compact_args*, const uint2*);
 cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double, uint32_t, const uint2*, const sdb_compact_args*,
                               cudaStream_t, int*, sdb_profiler*, int);
+cudaError_t sdb_launch_supersede(const sdb_dev_view*, const sdb_recv_args*, const sdb_ss_args*, const sdb_compact_args*, cudaStream_t,
+                                 int*, sdb_profiler*, int);
 cudaError_t sdb_launch_where(const sdb_dev_view*, const sdb_recv_args*, const sdb_where_args*, int, uint32_t, cudaStream_t, int*,
                              sdb_profiler*, int);
 cudaError_t sdb_launch_id_table(const unsigned long long*, uint32_t, sdb_id_slot*, uint32_t, cudaStream_t, int*);

@@ -1593,6 +1593,249 @@ extern "C" cudaError_t sdb_launch_expire(const sdb_dev_view* v, const sdb_recv_a
 }
 
 // ------------------------------------------------------------------------------------------
+// superseding (sdb_supersede): of the pending records carrying SDB_TYPEF_SUPERSEDE, keep per key (agent, sender, group,
+// type & SDB_TYPE_MASK) the one with the largest seq, the later in the ring on a tie, and retire the others.  The flag is
+// in the header (byte 31), not in the ring meta, so the cost is the header reads, at most two per live record:
+//   k_supersede_count    k_expire's shape: cnt[q] = flagged live records (the header's last word); scan -> C
+//   (the host stops when C = 0, else sizes the table and the candidate array for C records)
+//   k_supersede_insert   the same walk: each flagged record's {seq, slot, ring offset, table slot} goes to cand[] at its
+//                        scanned position, its key into the table (128-bit CAS, linear probing), atomicMax of its seq;
+//                        the verdict words of walked slots are zeroed
+//   k_supersede_tie      per candidate: holders of the key's largest seq atomicMax their ring offset
+//   k_supersede_verdict  per candidate: superseded unless it is the key's {seq, offset}; the bit of its ring slot is
+//                        set (k_where_eval's bitmap) and cnt[q] counts it (one atomic per warp and slot)
+//   k_supersede<MODE>    k_expire's retire walk over ring entries and verdict words only: EXP_DROP, or after a scan of
+//                        cnt EXP_SELECT with its capacity cut, then the compact back end
+// Every record of a key but its newest is superseded, so any subset of them may go: the capacity cut is safe.
+// ------------------------------------------------------------------------------------------
+struct __align__(16) ss_key { unsigned long long lo, hi; };
+
+__device__ __forceinline__ uint32_t ss_hash(unsigned long long lo, unsigned long long hi) {
+  unsigned long long k = lo ^ (hi * 0x9E3779B97F4A7C15ull);
+  k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
+  return static_cast<uint32_t>(k);
+}
+
+__device__ __forceinline__ bool ss_flagged(uint32_t w7) { return ((w7 >> 24) & SDB_TYPEF_SUPERSEDE) != 0u; }
+
+__global__ void __launch_bounds__(256)
+k_supersede_count(sdb_dev_view v, sdb_recv_args r) {
+  const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_EXP_G - 1), gsh = lane & ~(SDB_EXP_G - 1);
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1;
+  constexpr uint32_t SPW = 32u / SDB_EXP_G;
+  for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
+    const uint32_t q = qb + lane / SDB_EXP_G;
+    const bool valid = q < r.n;
+    uint32_t a = 0, H = 0, T = 0, NT = 0;
+    if (valid) {
+      a = r.agent_idx ? r.agent_idx[q] : q;
+      const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);
+      H = h.x; T = h.y; NT = h.w;
+    }
+    const uint32_t W = (valid && T - H - NT) ? T - H : 0u;
+    const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
+    const uint2* rs = sdb_ring_of(v, a);
+    uint32_t got = 0;
+    for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_EXP_G * SDB_EXP_U) {
+      uint2 e[SDB_EXP_U];
+      uint32_t w7[SDB_EXP_U];
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t j = j0 + u * SDB_EXP_G + l8;
+        e[u] = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+      }
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u)               // len | prio << 16 | type << 24, one random sector each
+        w7[u] = sdb_meta(e[u]) != SDB_META_TOMB
+                    ? __ldg(reinterpret_cast<const uint32_t*>(v.arena + ((static_cast<uint64_t>(e[u].x) & v.gmask) << 5)) + 7)
+                    : 0u;
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u)
+        got += __popc((__ballot_sync(0xFFFFFFFFu, ss_flagged(w7[u])) >> gsh) & 0xFFu);
+    }
+    if (l8 == 0 && valid) r.cnt[q] = got;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_supersede_insert(sdb_dev_view v, sdb_recv_args r, sdb_ss_args s) {
+  const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_EXP_G - 1), gsh = lane & ~(SDB_EXP_G - 1);
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1;
+  constexpr uint32_t SPW = 32u / SDB_EXP_G;
+  for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
+    const uint32_t q = qb + lane / SDB_EXP_G;
+    const bool valid = q < r.n;
+    uint32_t a = 0, H = 0, T = 0, c = 0, base = 0;
+    if (valid) {
+      a = r.agent_idx ? r.agent_idx[q] : q;
+      c = r.cnt[q];
+      if (c) {
+        const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);
+        H = h.x; T = h.y;
+        base = sdb_scan_at(r.rec_local, r.rec_tops, q);
+      }
+    }
+    const uint32_t W = c ? T - H : 0u;
+    const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
+    const uint2* rs = sdb_ring_of(v, a);
+    uint32_t* bits = s.bits + static_cast<size_t>(a) * s.stride;
+    uint32_t got = 0;
+    for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_EXP_G * SDB_EXP_U) {
+      uint2 e[SDB_EXP_U];
+      uint4 lo[SDB_EXP_U], hi[SDB_EXP_U];
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t j = j0 + u * SDB_EXP_G + l8;
+        e[u] = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+      }
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {              // independent random loads, all issued before any use
+        lo[u] = hi[u] = make_uint4(0u, 0u, 0u, 0u);
+        if (sdb_meta(e[u]) != SDB_META_TOMB) {
+          const uint4* src = reinterpret_cast<const uint4*>(v.arena + ((static_cast<uint64_t>(e[u].x) & v.gmask) << 5));
+          lo[u] = __ldg(src); hi[u] = __ldg(src + 1);
+        }
+      }
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const bool fl = ss_flagged(hi[u].w);
+        const uint32_t bm = (__ballot_sync(0xFFFFFFFFu, fl) >> gsh) & 0xFFu;
+        if (fl) {
+          const unsigned long long seq = (static_cast<unsigned long long>(lo[u].y) << 32) | lo[u].x;
+          const ss_key k{a | (static_cast<unsigned long long>(hi[u].x) << 32),
+                         hi[u].z | (static_cast<unsigned long long>((hi[u].w >> 24) & SDB_TYPE_MASK) << 32) | (1ull << 63)};
+          uint32_t t = ss_hash(k.lo, k.hi) & s.mask;
+          for (;; t = (t + 1) & s.mask) {
+            const ss_key old = atomicCAS(reinterpret_cast<ss_key*>(s.tab + t), ss_key{0ull, 0ull}, k);
+            if ((old.lo == 0ull && old.hi == 0ull) || (old.lo == k.lo && old.hi == k.hi)) break;
+          }
+          atomicMax(&s.tab[t].seq, seq);
+          s.cand[base + got + __popc(bm & ((1u << l8) - 1u))] = sdb_ss_cand{seq, q, j0 + u * SDB_EXP_G + l8, t, 0u};
+        }
+        got += __popc(bm);
+      }
+      if (l8 == 0 && j0 < W) bits[j0 >> 5] = 0u;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_supersede_tie(sdb_ss_args s) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= s.n_cand) return;
+  const sdb_ss_cand c = s.cand[i];
+  if (c.seq == s.tab[c.slot].seq) atomicMax(&s.tab[c.slot].off, c.j);
+}
+
+__global__ void __launch_bounds__(256)
+k_supersede_verdict(sdb_recv_args r, sdb_ss_args s) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+  bool sup = false;
+  uint32_t q = 0xFFFFFFFFu;
+  if (i < s.n_cand) {                                         // no early return: the warp meets in the aggregation
+    const sdb_ss_cand c = s.cand[i];
+    const sdb_ss_slot t = s.tab[c.slot];
+    sup = !(c.seq == t.seq && c.j == t.off);
+    q = c.q;
+    if (sup) {
+      const uint32_t a = r.agent_idx ? r.agent_idx[q] : q;
+      atomicOr(s.bits + static_cast<size_t>(a) * s.stride + (c.j >> 5), 1u << (c.j & 31u));
+    }
+  }
+  const uint32_t b = __ballot_sync(0xFFFFFFFFu, sup) & __match_any_sync(0xFFFFFFFFu, q);
+  if (sup && lane == static_cast<uint32_t>(__ffs(b) - 1)) atomicAdd(r.cnt + q, static_cast<uint32_t>(__popc(b)));
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(256)
+k_supersede(sdb_dev_view v, sdb_recv_args r, sdb_ss_args s) {
+  const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_EXP_G - 1), gsh = lane & ~(SDB_EXP_G - 1);
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1;
+  const bool retire = !(r.flags & SDB_RECV_PEEK);
+  constexpr uint32_t SPW = 32u / SDB_EXP_G;
+  unsigned long long wsum = 0;
+  for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
+    const uint32_t q = qb + lane / SDB_EXP_G;
+    const bool valid = q < r.n;
+    uint32_t RO;
+    const uint32_t limit = exp_cut<MODE>(r, valid, q, l8, &RO);
+    const bool walk = valid && (MODE == SDB_EXP_SELECT ? limit : r.cnt[q]) != 0u;
+    uint32_t a = 0, H = 0, T = 0, NT = 0;
+    if (valid) {
+      a = r.agent_idx ? r.agent_idx[q] : q;
+      const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);
+      H = h.x; T = h.y; NT = h.w;
+    }
+    const uint32_t W = walk ? T - H : 0u;
+    const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
+    uint32_t got = 0, nh = walk ? T : H;
+    uint2* rs = sdb_ring_of(v, a);
+    const uint32_t* bits = s.bits + static_cast<size_t>(a) * s.stride;
+    for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_EXP_G * SDB_EXP_U) {
+      const uint32_t word = j0 < W ? bits[j0 >> 5] : 0u;
+      uint2 e[SDB_EXP_U];
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const uint32_t j = j0 + u * SDB_EXP_G + l8;
+        e[u] = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+      }
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_EXP_U; ++u) {
+        const bool lv = sdb_meta(e[u]) != SDB_META_TOMB;
+        const bool match = lv && ((word >> (u * SDB_EXP_G + l8)) & 1u);
+        const uint32_t bm = (__ballot_sync(0xFFFFFFFFu, match) >> gsh) & 0xFFu;
+        const bool sel = match && got + __popc(bm & ((1u << l8) - 1u)) < limit;
+        exp_retire<MODE>(r, rs, mask, e[u], H + j0 + u * SDB_EXP_G + l8, lv, sel, retire, q, RO, l8, gsh, T, got, nh);
+      }
+    }
+    exp_store<MODE>(v, r, valid, retire, l8, q, a, H, NT, got, nh, wsum);
+  }
+  exp_total<MODE>(r, lane, wsum);
+}
+
+// s->tab == nullptr: k_supersede_count and the scan, totals[0] = flagged records C.  Otherwise, with the table and the
+// candidate array sized for s->n_cand = C records: insert, tie, verdict, then drop mode (ca == nullptr, totals[0] =
+// records retired) or the select walk and the compact back end exactly as a compact receive runs it (totals as there).
+extern "C" cudaError_t sdb_launch_supersede(const sdb_dev_view* v, const sdb_recv_args* r, const sdb_ss_args* s,
+                                            const sdb_compact_args* ca, cudaStream_t stream, int* n_launches, sdb_profiler* prof,
+                                            int sm_count) {
+  if (r->n == 0) return cudaSuccess;
+  const uint32_t n = r->n;
+  const uint32_t blocks = sdb_grid(n, 32, 32 * sm_count);                    // 4 slots per warp, 8 warps per block
+  const int pi = sdb_prof_begin(prof, SDB_PK_EXPIRE, stream);
+  if (!s->tab) {
+    k_supersede_count<<<blocks, 256, 0, stream>>>(*v, *r);
+    const cudaError_t e = sdb_scan_u32(r->cnt, r->rec_local, r->rec_tops, n, r->totals, nullptr, stream, n_launches);
+    sdb_prof_end(prof, pi, stream);
+    if (n_launches) *n_launches += 1;
+    return e != cudaSuccess ? e : cudaGetLastError();
+  }
+  const uint32_t cblocks = (s->n_cand + 255u) / 256u;
+  k_supersede_insert<<<blocks, 256, 0, stream>>>(*v, *r, *s);
+  cudaMemsetAsync(r->cnt, 0, static_cast<size_t>(n) * sizeof(uint32_t), stream);   // cnt[q] = superseded records
+  k_supersede_tie<<<cblocks, 256, 0, stream>>>(*s);
+  k_supersede_verdict<<<cblocks, 256, 0, stream>>>(*r, *s);
+  if (!ca) {
+    cudaMemsetAsync(r->totals, 0, sizeof(unsigned long long), stream);
+    k_supersede<SDB_EXP_DROP><<<blocks, 256, 0, stream>>>(*v, *r, *s);
+    sdb_prof_end(prof, pi, stream);
+    if (n_launches) *n_launches += 4;
+    return cudaGetLastError();
+  }
+  // totals[0] = superseded records; the cut may lower it
+  const cudaError_t e = sdb_scan_u32(r->cnt, r->rec_local, r->rec_tops, n, r->totals, nullptr, stream, n_launches);
+  k_supersede<SDB_EXP_SELECT><<<blocks, 256, 0, stream>>>(*v, *r, *s);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += 4;
+  if (e != cudaSuccess) return e;
+  const uint64_t bound = s->n_cand < r->rec_cap ? s->n_cand : r->rec_cap;   // upper bound on the records planned
+  return launch_compact(v, r, ca, nullptr, bound, sm_count, stream, prof, n_launches);
+}
+
+// ------------------------------------------------------------------------------------------
 // filtered receive (sdb_receive_where): the predicate is evaluated once per pending record and kept as one verdict bit
 // per ring slot (f.bits, agent a, offset j from the head); the selection then reads bits and ring entries only.
 //   k_where_eval    header clauses only, k_expire's shape: 8 lanes per request slot, the ring header once, the window's

@@ -74,6 +74,7 @@ class SendIn(BaseModel):
     priority: MessagePriority = MessagePriority.NORMAL
     metadata: Optional[Dict[str, Any]] = None
     visible_to: Optional[List[str]] = None
+    supersede: bool = False                # a newer superseding send of the sender and type replaces it while pending
 
 
 class BroadcastIn(BaseModel):
@@ -82,6 +83,7 @@ class BroadcastIn(BaseModel):
     priority: MessagePriority = MessagePriority.NORMAL
     metadata: Optional[Dict[str, Any]] = None
     exclude_agents: Optional[List[str]] = None
+    supersede: bool = False
 
 
 class RegisterIn(BaseModel):
@@ -102,6 +104,7 @@ class GroupSendIn(BaseModel):
     message_type: MessageType = MessageType.CHAT
     priority: MessagePriority = MessagePriority.NORMAL
     metadata: Optional[Dict[str, Any]] = None
+    supersede: bool = False
 
 
 class TrimIn(BaseModel):
@@ -272,7 +275,7 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
         def go():
             mid = db.send_message(sender_id=who, content=body.content, receiver_id=body.receiver_id,
                                   message_type=body.message_type, priority=body.priority, metadata=body.metadata,
-                                  visible_to=body.visible_to, dedup_id=idempotency_key)
+                                  visible_to=body.visible_to, dedup_id=idempotency_key, supersede=body.supersede)
             return MessageOut.of(db.get_message(settled(mid, idempotency_key)))
         return guarded("send message", go)
 
@@ -281,7 +284,8 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
                   idempotency_key: Optional[str] = Header(None, alias="Idempotency-Key")):
         mid = guarded("broadcast message", lambda: settled(db.broadcast_message(
             sender_id=who, content=body.content, message_type=body.message_type, priority=body.priority,
-            metadata=body.metadata, exclude_agents=body.exclude_agents, dedup_id=idempotency_key), idempotency_key))
+            metadata=body.metadata, exclude_agents=body.exclude_agents, dedup_id=idempotency_key,
+            supersede=body.supersede), idempotency_key))
         return BroadcastOut(status="success", message_id=mid)
 
     @app.post("/groups", status_code=http.HTTP_201_CREATED)
@@ -295,7 +299,7 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
         def go():
             ids = db.send_to_group(sender_id=who, group_name=body.group_name, content=body.content,
                                    message_type=body.message_type, priority=body.priority, metadata=body.metadata,
-                                   dedup_id=idempotency_key)
+                                   dedup_id=idempotency_key, supersede=body.supersede)
             return [settled(mid, idempotency_key) for mid in ids]
         return GroupSendOut(status="success", message_ids=guarded("send group message", go))
 

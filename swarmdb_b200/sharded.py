@@ -597,19 +597,25 @@ class ShardedSwarmsDB(SwarmsDB):
                      visible_to=None, **kw):
         if kw.get("dedup_id") is not None:
             self._no_dedup()
+        if kw.get("supersede"):
+            self._no_supersede()
         self._require_known(sender_id, receiver_id, *(visible_to or []))
         return super().send_message(sender_id, content, receiver_id, message_type or MessageType.CHAT,
                                     priority if priority is not None else MessagePriority.NORMAL, metadata, visible_to, **kw)
 
-    def broadcast_message(self, sender_id, content, *a, dedup_id=None, **kw):
+    def broadcast_message(self, sender_id, content, *a, dedup_id=None, supersede=False, **kw):
         if dedup_id is not None:
             self._no_dedup()
+        if supersede:
+            self._no_supersede()
         return super().broadcast_message(sender_id, content, *a, **kw)
 
     def send_to_group(self, sender_id, group_name, content, message_type=None, priority=None, metadata=None,
-                      dedup_id=None):
+                      dedup_id=None, supersede=False):
         if dedup_id is not None:
             self._no_dedup()
+        if supersede:
+            self._no_supersede()
         self._require_known(sender_id)
         return super().send_to_group(sender_id, group_name, content, message_type or MessageType.CHAT,
                                      priority if priority is not None else MessagePriority.NORMAL, metadata)
@@ -756,6 +762,13 @@ class ShardedSwarmsDB(SwarmsDB):
     def _no_dedup(self):
         raise NotImplementedError("ShardedSwarmsDB does not deduplicate sends yet (GpuConfig.dedup_entries, dedup_id): "
                                   "a key must be checked on the rank that numbers the send, before the exchange")
+
+    def _no_supersede(self, *args, **kwargs):
+        raise NotImplementedError("ShardedSwarmsDB does not supersede sends yet (supersede=True, supersede_pending): a "
+                                  "rank does not know which agents other ranks' superseding sends reached, and host "
+                                  "records live on the sending rank")
+
+    supersede_pending = _no_supersede
 
     def _no_leases(self, *args, **kwargs):
         raise NotImplementedError("ShardedSwarmsDB does not lease yet: redelivered ids must stay below the composite "
