@@ -760,10 +760,18 @@ __device__ __forceinline__ void sdb_tma_load(void* smem_dst, const void* gsrc, u
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                :: "r"(sdb_smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(sdb_smem_u32(bar)) : "memory");
 }
+__device__ __forceinline__ void sdb_tma_load_pol(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+               :: "r"(sdb_smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(sdb_smem_u32(bar)), "l"(pol) : "memory");
+}
 // shared -> global bulk copy (bulk_group completion)
 __device__ __forceinline__ void sdb_tma_store(void* gdst, const void* smem_src, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
                :: "l"(gdst), "r"(sdb_smem_u32(smem_src)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void sdb_tma_store_pol(void* gdst, const void* smem_src, uint32_t bytes, uint64_t pol) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
+               :: "l"(gdst), "r"(sdb_smem_u32(smem_src)), "r"(bytes), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void sdb_tma_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>

@@ -770,6 +770,10 @@ k_recv_gather(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __restr
 // A per-lane bulk copy costs the warp ~12 issue slots (the copy engine takes its operands from uniform registers), which
 // looked like the limit with the payloads coming out of the L2.  It is not: a form with the whole warp moving the
 // payloads by 16-byte cp.async copies ran the c2 gather in the same 0.775 ms on an H100 (700 W) and was removed.
+// L2 policy: a payload shared by a group send is read once per member, at places spread over the whole receiver-ordered
+// output, so its loads are evict-last; everything the kernel touches once (plan entries, headers in, headers and
+// payloads out) is evict-first.  On an H100 (700 W) the c2 gather went from 0.782 to 0.686 ms.  Splitting the copy into
+// a header pass and a payload pass did not pay (scripts/ubench/gather_phases.cu, DESIGN §8 item 19).
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32)
 k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __restrict__ packed_inv, uint32_t slot_bytes) {
@@ -782,6 +786,7 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
   __syncwarp();
   const uint32_t gw = blockIdx.x * WARPS + warp, nw = gridDim.x * WARPS;
   uint32_t phase = 0;                                        // bit s = parity of stage s
+  const uint64_t pol = sdb_policy_evict_first(), keep = sdb_policy_evict_last();
   // per-lane state of the two stages.  The 32-byte header travels through registers (two 16-byte loads now, stored one
   // step later: the lanes' headers are consecutive in hdr_out, and sdb_st_headers swaps halves between lanes so that
   // each of the warp's two store instructions writes 512 contiguous bytes of whole sectors; stored as loaded, every
@@ -797,7 +802,7 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
     const bool have = rec < total;
     uint32_t bytes = 0; uint4 pe = make_uint4(0, 0, 0, 0);
     if (have) { pe = pe_ahead; bytes = (pe.z & 0xFFFFu) << 5; }
-    { const uint32_t ra = rec + nw * 32u; if (ra < total) pe_ahead = __ldg(r.plan + ra); }   // consumed one step later
+    { const uint32_t ra = rec + nw * 32u; if (ra < total) pe_ahead = sdb_ld_stream_pol(r.plan + ra, pol); }   // consumed one step later
     uint32_t sum = bytes;
     for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xFFFFFFFFu, sum, o);
     if (lane == 0) sdb_mbar_expect_tx(&s_bar[warp][st], sum);
@@ -805,15 +810,15 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
     uint4 ha = make_uint4(0, 0, 0, 0), hb = ha;
     if (have) {
       const uint8_t* src = v.arena + ((static_cast<uint64_t>(pe.x) & v.gmask) << 5);
-      ha = sdb_ld_stream(src); hb = sdb_ld_stream(src + 16);
-      if (bytes) sdb_tma_load(wbase + (static_cast<size_t>(st) * 32u + lane) * slot_bytes, sdb_payload_of(v, pe.x, sdb_entry_dm1(pe.z)), bytes, &s_bar[warp][st]);
+      ha = sdb_ld_stream_pol(src, pol); hb = sdb_ld_stream_pol(src + 16, pol);
+      if (bytes) sdb_tma_load_pol(wbase + (static_cast<size_t>(st) * 32u + lane) * slot_bytes, sdb_payload_of(v, pe.x, sdb_entry_dm1(pe.z)), bytes, &s_bar[warp][st], keep);
     }
     const uint64_t po = static_cast<uint64_t>(pe.y) + ((have && r.plan_tops) ? r.plan_tops[rec / SDB_SCAN_TILE] : 0u);
     if (st) { g1 = pe.z & 0xFFFFu; hv1 = have; po1 = po; ha1 = ha; hb1 = hb; }
     else { g0 = pe.z & 0xFFFFu; hv0 = have; po0 = po; ha0 = ha; hb0 = hb; }
   };
   uint32_t r0 = gw * 32u;
-  if (r0 + lane < total) pe_ahead = __ldg(r.plan + r0 + lane);
+  if (r0 + lane < total) pe_ahead = sdb_ld_stream_pol(r.plan + r0 + lane, pol);
   if (r0 < total) issue(0, r0);
   uint32_t st = 0;
   for (; r0 < total; r0 += nw * 32u, st ^= 1u) {
@@ -822,7 +827,7 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
     sdb_tma_wait_read<0>();
     __syncwarp();
     if (rn < total) issue(st ^ 1u, rn);
-    sdb_st_headers<32>(r.hdr_out + r0, sdb_sel4(st, ha1, ha0), sdb_sel4(st, hb1, hb0), st ? hv1 : hv0, lane);   // whole sectors
+    sdb_st_headers_pol<32>(r.hdr_out + r0, sdb_sel4(st, ha1, ha0), sdb_sel4(st, hb1, hb0), st ? hv1 : hv0, lane, pol);   // whole sectors
     sdb_mbar_wait_bounded(&s_bar[warp][st], (phase >> st) & 1u);
     phase ^= 1u << st;
     {
@@ -831,9 +836,9 @@ k_recv_gather_tma(sdb_dev_view v, sdb_recv_args r, const unsigned long long* __r
       // payload offsets are cumulative in record order: when all 32 payloads fill their slots exactly, the warp's output
       // is ONE contiguous run and the slots are contiguous too - one bulk store instead of 32
       if (__all_sync(0xFFFFFFFFu, hv && (g << 5) == slot_bytes)) {
-        if (lane == 0) sdb_tma_store(r.payload_out + ((st ? po1 : po0) << 5), wbase + static_cast<size_t>(st) * 32u * slot_bytes, 32u * slot_bytes);
+        if (lane == 0) sdb_tma_store_pol(r.payload_out + ((st ? po1 : po0) << 5), wbase + static_cast<size_t>(st) * 32u * slot_bytes, 32u * slot_bytes, pol);
       } else if (hv && g) {
-        sdb_tma_store(r.payload_out + ((st ? po1 : po0) << 5), wbase + (static_cast<size_t>(st) * 32u + lane) * slot_bytes, g << 5);
+        sdb_tma_store_pol(r.payload_out + ((st ? po1 : po0) << 5), wbase + (static_cast<size_t>(st) * 32u + lane) * slot_bytes, g << 5, pol);
       }
     }
     sdb_tma_commit();
