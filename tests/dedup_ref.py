@@ -49,6 +49,70 @@ def content_key(sender: int, kind: int, target: int, recipients, length: int, pr
     return lo, hi
 
 
+def content_keys(sender, kind, target, list_off, list_idx, lens, prio, typ, payload_off, payload):
+    """content_key of every send of a mixed batch as (lo, hi) uint64 arrays.  Sends with the same word layout (the same
+    len, and for a list send the same list length) share one matrix of words, so a batch of tens of thousands of sends
+    costs one numpy pass per layout instead of one call per send."""
+    sender, kind, target = (np.asarray(x, np.uint64) for x in (sender, kind, target))
+    lens, off = np.asarray(lens, np.int64), np.asarray(payload_off, np.int64)
+    lpt = lens.astype(np.uint64) | np.asarray(prio, np.uint64) << np.uint64(16) | np.asarray(typ, np.uint64) << np.uint64(24)
+    lo_, hi_ = np.zeros(len(lens), np.uint64), np.zeros(len(lens), np.uint64)
+    lb = np.zeros(len(lens), np.int64)
+    cnt = np.full(len(lens), -1, np.int64)                       # -1: not a list send
+    lst = np.flatnonzero(kind == 2)
+    if len(lst):
+        lo_off = np.asarray(list_off, np.int64)
+        lb[lst] = lo_off[target[lst].astype(np.int64)]
+        cnt[lst] = lo_off[target[lst].astype(np.int64) + 1] - lb[lst]
+    layouts, which = np.unique(np.stack([cnt, lens], 1), axis=0, return_inverse=True)
+    pay = np.asarray(payload, np.uint8)
+    for u, (c, ln) in enumerate(layouts.tolist()):
+        idx = np.flatnonzero(which.ravel() == u)
+        nr, nw = max(c, 0), (ln + 7) // 8
+        m = 3 + nr + nw
+        w = np.zeros((len(idx), m), np.uint64)
+        w[:, 0] = sender[idx] | kind[idx] << np.uint64(32)
+        w[:, 1] = np.uint64(c) if c >= 0 else target[idx]
+        if nr:
+            w[:, 2:2 + nr] = np.asarray(list_idx, np.uint64)[lb[idx][:, None] + np.arange(nr)]
+        w[:, 2 + nr] = lpt[idx]
+        if ln:
+            b = np.zeros((len(idx), nw * 8), np.uint8)
+            b[:, :ln] = pay[off[idx][:, None] + np.arange(ln)]
+            w[:, 3 + nr:] = b.view("<u8").astype(np.uint64)
+        with np.errstate(over="ignore"):
+            pos = np.arange(1, m + 1, dtype=np.uint64) * np.uint64(PHI)
+            sa = _mix64(w + np.uint64(SEED_A) + pos).sum(axis=1, dtype=np.uint64)
+            sb = _mix64(w + np.uint64(SEED_B) + pos).sum(axis=1, dtype=np.uint64)
+        lo_[idx] = _mix64(sa ^ np.uint64(m))
+        hi_[idx] = _mix64(sb ^ np.uint64((m << 32) & M64))
+    lo_[(lo_ == 0) & (hi_ == 0)] = 1
+    return lo_, hi_
+
+
+def edge_lengths(max_len: int) -> list:
+    """Payload lengths at the edges of a content key's 16-byte loads and 512-byte warp steps: 0, 1-17, every residue
+    mod 16 around the first four 512-byte boundaries, 1023-1025, 8191 and max_len."""
+    out = set(range(0, 18)) | {1023, 1024, 1025, 8191, max_len}
+    for k in range(1, 5):
+        out |= set(range(512 * k - 16, 512 * k + 17))
+    return sorted(x for x in out if x <= max_len)
+
+
+def table_mask(entries: int) -> int:
+    """Slot mask of a table reserved for `entries` keys: pow2_at_least(2 entries) - 1, at least 64 slots."""
+    p = 64
+    while p < 2 * entries:
+        p <<= 1
+    return p - 1
+
+
+def slot_hash(lo, hi) -> np.ndarray:
+    """The home slot hash of sdb_dedup.cu: mix64(lo ^ rotl(hi, 32)), before the mask."""
+    lo, hi = np.asarray(lo, np.uint64), np.asarray(hi, np.uint64)
+    return _mix64(lo ^ ((hi << np.uint64(32)) | (hi >> np.uint64(32))))
+
+
 class DedupModel:
     """The table as the host and the kernels keep it: key -> [seq, inserted_at] for every occupied slot (live,
     expired or forgotten until a rebuild drops it)."""
