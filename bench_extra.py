@@ -1547,6 +1547,125 @@ def budget(rounds=2, per_agent=2):
     return out
 
 
+def tokens(rounds=2, reps=10):
+    """Receive by token budget (sdb_receive_compact_tokens, sdb_pending_tokens).
+    c2: the c2 backlog (bench.py's step, 4,194,304 records over 1 M agents) with every send tagged (TYPEF_TOKENS,
+      counts uniform in 1..512): a token-limited PEEK (512 tokens, about half of each queue) against a budget PEEK of
+      two padded payloads (the same share by bytes); wall time per call, and the plan (recv_select) and token pre-pass
+      (recv_count) kernel times from the library profiler.  pending_tokens over the 1 M agents.
+    deep: 10,000 agents x 1,000 pending tagged records (16-byte payloads, private images), a limit near a quarter of
+      each window's tokens, in stream and priority order.
+    Algorithmic bytes of the pre-pass: a 16-B ring header per agent, 8 B per ring entry, one 32-B header sector per
+    record and one payload sector per distinct tagged payload it reads, over its kernel time, against the 3.35 TB/s
+    of NVIDIA's H100 SXM data sheet.  The c2 windows (4 records) fit one 32-entry step, which reads them all; a deep
+    stream-order walk stops at the end of the step holding the first record that does not fit; a priority-order walk
+    reads every record once for its level totals (the bytes given: the second walk over the cut level is left out,
+    so the rate is a lower bound)."""
+    import torch
+    from bench import Workload
+    from swarmdb_b200._native import RECV_PEEK, RECV_PRIORITY, Shard, pad32
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py tokens: no CUDA device - swarmdb_b200 has no CPU fallback")
+    TOK, HBM = 0x40, 3.35e12
+
+    def timed(shard, fn):
+        fn()                                                                  # warm-up
+        shard.sync()
+        shard.profile(True)
+        t = time.perf_counter()
+        for _ in range(reps):
+            r = fn()
+        shard.sync()
+        wall = (time.perf_counter() - t) * 1e3 / reps
+        prof = shard.profile_read()
+        shard.profile(False)
+        return r, {"call_ms": wall, "prepass_ms": prof["recv_count"][0] / reps, "plan_ms": prof["recv_select"][0] / reps}
+
+    def share(ms, nbytes):
+        return {"algorithmic_bytes": nbytes, "prepass_tb_s": nbytes / (ms * 1e-3) / 1e12 if ms else None,
+                "share_of_3_35_tb_s": nbytes / (ms * 1e-3) / HBM if ms else None}
+
+    out = {}
+    # ---- c2
+    wl = Workload()
+    rng = np.random.default_rng(9)
+    snd, grp, prio, typ, lens, off, pay = wl.batch()
+    pay = pay.copy()
+    pay.reshape(wl.S, wl.L)[:, :4] = rng.integers(1, 513, wl.S).astype(np.uint32).view(np.uint8).reshape(wl.S, 4)
+    typ = np.full(wl.S, TOK, np.uint8)
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    shard = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+    shard.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        shard.create_group(g, wl.members(g))
+    shard.send_group_batch(snd, grp, prio, typ, lens, off, pay)
+    shard.sync()
+    res = {"tokens": [], "budget": [], "pending_tokens": []}
+    recs = {}
+    for r in range(rounds):
+        for name in (("tokens", "budget", "pending_tokens") if r % 2 == 0 else ("pending_tokens", "budget", "tokens")):
+            if name == "tokens":
+                got, t = timed(shard, lambda: shard.receive_compact_tokens(None, 100, 512, 0, RECV_PEEK))
+            elif name == "budget":
+                got, t = timed(shard, lambda: shard.receive_compact(None, 100, RECV_PEEK, max_agent_bytes=2 * pad32(wl.L)))
+            else:
+                got, t = timed(shard, lambda: shard.pending_tokens())
+            recs[name] = len(got[1]) if name != "pending_tokens" else int(got.sum())
+            res[name].append(t)
+    shard.close()
+    nbytes = 16 * wl.A + 8 * per_step + 32 * per_step + 32 * wl.S
+    out["c2_config"] = (f"c2 backlog: {per_step} records over {wl.A} agents, {wl.L}-B payloads, every send tagged "
+                        f"(counts 1..512); token limit 512 vs byte limit {2 * pad32(wl.L)} B; PEEK compact receives, "
+                        f"{reps} per block, blocks alternated")
+    out["c2"] = {k: {"blocks": v, **{f: float(np.median([x[f] for x in v])) for f in ("call_ms", "prepass_ms", "plan_ms")},
+                     "result": recs[k]} for k, v in res.items()}
+    for k in ("tokens", "pending_tokens"):
+        out["c2"][k].update(share(out["c2"][k]["prepass_ms"], nbytes))
+
+    # ---- 10,000 agents x 1,000 pending
+    A, D, L = 10_000, 1_000, 16
+    n = A * D
+    shard = Shard(max_agents=A, ring_slots=1024, arena_bytes=1 << 30, max_payload_bytes=64, max_batch_sends=1 << 16,
+                  max_batch_payload=(1 << 16) * L, max_recv_records=1 << 22, max_recv_payload=1 << 28)
+    shard.register(np.arange(A, dtype=np.uint32))
+    B = 1 << 16
+    recv_all = np.tile(np.arange(A, dtype=np.uint32), D)
+    lens, ts = np.full(B, L, np.uint16), np.zeros(B)
+    t8 = np.full(B, TOK, np.uint8)
+    poff = np.arange(B, dtype=np.uint64) * L
+    for i in range(0, n, B):
+        m = min(B, n - i)
+        p = rng.integers(0, 256, B * L, dtype=np.uint8)
+        p.reshape(B, L)[:, :4] = rng.integers(1, 513, B).astype(np.uint32).view(np.uint8).reshape(B, 4)
+        shard.send_batch(recv_all[i:i + m] ^ 1, recv_all[i:i + m], rng.integers(0, 4, m).astype(np.uint8), t8[:m],
+                         lens[:m], poff[:m], p[:m * L], ts[:m])
+    shard.sync()
+    total = shard.pending_tokens()
+    lim = int(np.median(total)) // 4
+    deep = {}
+    for r in range(rounds):
+        for fl in ((0, RECV_PRIORITY) if r % 2 == 0 else (RECV_PRIORITY, 0)):
+            got, t = timed(shard, lambda: shard.receive_compact_tokens(None, D, lim, 0, fl | RECV_PEEK))
+            t["records"] = len(got[1])
+            # records the walk reads: the whole window (priority), or the steps up to the first one that does not fit
+            k = got[0].astype(np.int64)
+            read = n if fl else int(np.minimum(D, 32 * ((k + 32) // 32)).sum())
+            t["bytes"] = 16 * A + (8 + 32 + 32) * read
+            deep.setdefault("priority" if fl else "stream", []).append(t)
+    shard.close()
+    out["deep_config"] = (f"{A} agents x {D} pending tagged records ({L}-B payloads, counts 1..512), token limit {lim} "
+                          f"(a quarter of the median window); PEEK compact receives, {reps} per block, orders alternated")
+    out["deep"] = {k: {"blocks": v, **{f: float(np.median([x[f] for x in v])) for f in ("call_ms", "prepass_ms", "plan_ms")},
+                       "records": v[-1]["records"]} for k, v in deep.items()}
+    for k in out["deep"]:
+        out["deep"][k].update(share(out["deep"][k]["prepass_ms"], out["deep"][k]["blocks"][-1]["bytes"]))
+    out.update(_gpu_card(0))
+    return out
+
+
 def dedup(rounds=2, batch=1 << 16, n=1 << 20, L=256):
     """Deduplicated sends (sdb_send_mixed_batch_dedup) against plain sdb_send_mixed_batch of the same batches.
     send: n point-to-point sends of L bytes (one per agent), in batches of `batch`, host clock to a synchronise, each

@@ -59,6 +59,9 @@ enum { SDB_TYPE_CHAT = 0, SDB_TYPE_COMMAND, SDB_TYPE_FUNCTION_CALL, SDB_TYPE_FUN
 #define SDB_TYPEF_JSON 0x08u            /* payload content is JSON (dict/list content, M:75) */
 #define SDB_TYPEF_EXTRAS 0x10u          /* payload = u32 content_len | content | JSON extras */
 #define SDB_TYPEF_SUPERSEDE 0x20u       /* superseding: a newer flagged record with the same (sender, group, type) replaces it (sdb_supersede) */
+#define SDB_TYPEF_TOKENS 0x40u          /* payload = u32 token count (little-endian) | the payload without this flag; len counts
+                                           the 4 bytes.  The record weighs that many tokens in sdb_receive_tokens (a record
+                                           without the flag, or with len < 4, weighs 0) */
 
 /* Replaces KafkaConfig (M:114-127) + SwarmsDB.__init__ kwargs (M:156-165) for the device side. */
 typedef struct sdb_config {
@@ -320,6 +323,35 @@ int sdb_receive_compact_budget(sdb_handle h, uint32_t n_agents, const uint32_t* 
                                uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
                                sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                                uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
+/* Receive by token budget (as many pending messages as fit N tokens of a model's context): the arguments of
+ * sdb_receive_budget / sdb_receive_compact_budget plus max_agent_tokens.  A record's weight is the u32 count at the start
+ * of its payload when its type carries SDB_TYPEF_TOKENS (and len >= 4), else 0; records of unknown cost are bounded by
+ * max_agent_bytes.
+ *   1. Per-agent token take: the longest prefix of the agent's delivery order (stream order, or priority order with
+ *      SDB_RECV_PRIORITY) whose weights sum to at most max_agent_tokens (64-bit sums), or its first record alone when that
+ *      one is heavier.  In priority order that is whole levels from the top while they fit, then the arrival-order
+ *      prefix of the level where the limit falls.
+ *   2. Equivalence: the result (records, order, bytes, retirement, counters, rings and, after a full-format call,
+ *      sdb_digest_fold) is exactly what sdb_receive_budget / sdb_receive_compact_budget return when each agent's
+ *      max_messages is the smaller of max_messages and its token take.  Both takes are prefixes of one delivery order, so
+ *      the byte limit, the call's capacity and its truncation rule apply on top exactly as there.
+ *   3. max_agent_tokens == 0: no token limit; the call is sdb_receive_budget / sdb_receive_compact_budget.
+ *   4. SDB_RECV_PRIORITY, SDB_RECV_PEEK and SDB_RECV_OWNED as in the budget call; SDB_RECV_ASYNC is refused (SDB_EINVAL).
+ *      Refused calls leave every queue untouched.  The token pass is timed under SDB_PK_RECV_COUNT. */
+int sdb_receive_tokens(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                       uint64_t max_agent_bytes, uint64_t max_agent_tokens, uint32_t flags,
+                       uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
+                       uint8_t* payload_out, uint64_t payload_cap,
+                       uint64_t* total_out, uint64_t* payload_bytes_out);
+int sdb_receive_compact_tokens(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                               uint64_t max_agent_bytes, uint64_t max_agent_tokens, uint32_t flags,
+                               uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                               sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                               uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out);
+/* tokens_out[i] = the token weights (as in sdb_receive_tokens) of agent agent_idx[i]'s pending records, summed
+ * (agent_idx NULL: agents 0 .. n_agents - 1, as in sdb_agent_loads).  In-flight leases and dead letters are not pending.
+ * Synchronising; the kernel is timed under SDB_PK_RECV_COUNT. */
+int sdb_pending_tokens(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint64_t* tokens_out);
 /* Restore: put records in the compact format back on the device - a queue snapshot (a PEEK compact receive) after a
  * restart, or what a compact receive just took when its consumer failed (requeue).  Input in exactly the shape
  * sdb_receive_compact and sdb_expire's archive mode return: listed agent i owns the next count[i] entries.

@@ -52,6 +52,7 @@ FILTER_MAX_IDS = 1 << 22
 TYPEF_JSON = 0x08
 TYPEF_EXTRAS = 0x10
 TYPEF_SUPERSEDE = 0x20
+TYPEF_TOKENS = 0x40
 TYPE_MASK = 0x07
 
 STATUS_NAMES = {0: "SDB_OK", -1: "SDB_EINVAL", -2: "SDB_ECUDA", -3: "SDB_ENOMEM", -4: "SDB_ERING_OVERFLOW",
@@ -168,7 +169,7 @@ class SdbRelocateSummary(C.Structure):
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_profile_read_n", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
-           "sdb_receive_batch", "sdb_receive_compact", "sdb_receive_budget", "sdb_receive_compact_budget", "sdb_restore_compact", "sdb_expire", "sdb_trim", "sdb_supersede", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
+           "sdb_receive_batch", "sdb_receive_compact", "sdb_receive_budget", "sdb_receive_compact_budget", "sdb_receive_tokens", "sdb_receive_compact_tokens", "sdb_pending_tokens", "sdb_restore_compact", "sdb_expire", "sdb_trim", "sdb_supersede", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
@@ -240,6 +241,11 @@ def load_library() -> C.CDLL:
     L.sdb_receive_budget.argtypes = [vp, u32, vp, u32, u64, u32, vp, vp, u64, vp, u64, vp, vp]
     L.sdb_receive_compact_budget.restype = i32
     L.sdb_receive_compact_budget.argtypes = [vp, u32, vp, u32, u64, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    L.sdb_receive_tokens.restype = i32
+    L.sdb_receive_tokens.argtypes = [vp, u32, vp, u32, u64, u64, u32, vp, vp, u64, vp, u64, vp, vp]
+    L.sdb_receive_compact_tokens.restype = i32
+    L.sdb_receive_compact_tokens.argtypes = [vp, u32, vp, u32, u64, u64, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
+    L.sdb_pending_tokens.restype = i32; L.sdb_pending_tokens.argtypes = [vp, u32, vp, vp]
     L.sdb_restore_compact.restype = i32
     L.sdb_restore_compact.argtypes = [vp, u32, vp, vp, vp, u64, vp, u64, vp, u64, u32, vp, vp]
     L.sdb_lease_reserve.restype = i32; L.sdb_lease_reserve.argtypes = [vp, u64, u64]
@@ -708,6 +714,51 @@ class Shard:
         if agents is None:
             counts = self._served_counts(counts, flags)
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
+
+    def receive_tokens(self, agents, max_messages: int, max_agent_tokens: int, max_agent_bytes: int = 0, flags: int = 0,
+                       out_hdr: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+        """receive_budget by token budget (include/swarmdb_b200.h: sdb_receive_tokens): each agent's take is also cut
+        at the longest prefix of its delivery order whose token weights (the u32 count at the start of a TYPEF_TOKENS
+        payload, 0 for other records) sum to at most max_agent_tokens (0: no token limit; a heavier first record is
+        taken alone).  Returns (counts[n_agents], headers[total], payload bytes) as receive_batch does."""
+        a, n, counts = self._agents_arg(agents)
+        hdr = out_hdr if out_hdr is not None else self._grow_hdr()
+        pay = out_payload if out_payload is not None else self._grow_pay()
+        total, pbytes = C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_receive_tokens(self._h, n, _p(a), max_messages, int(max_agent_bytes), int(max_agent_tokens),
+                                               flags, _p(counts), _p(hdr), len(hdr), _p(pay), pay.nbytes,
+                                               C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(pbytes), C.c_void_p)))
+        if agents is None:
+            counts = self._served_counts(counts, flags)
+        return counts, hdr[: total.value], pay[: pbytes.value]
+
+    def receive_compact_tokens(self, agents, max_messages: int, max_agent_tokens: int, max_agent_bytes: int = 0,
+                               flags: int = 0, out_entries: Optional[np.ndarray] = None,
+                               out_sends: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None):
+        """receive_tokens' records in the compact format (sdb_receive_compact_tokens); returns what receive_compact
+        returns."""
+        a, n, counts = self._agents_arg(agents)
+        ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
+        total, n_sends, pbytes = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.sdb_receive_compact_tokens(
+            self._h, n, _p(a), max_messages, int(max_agent_bytes), int(max_agent_tokens), flags, _p(counts), _p(ent),
+            len(ent), _p(snd), len(snd), _p(pay), pay.nbytes, C.cast(C.byref(total), C.c_void_p),
+            C.cast(C.byref(n_sends), C.c_void_p), C.cast(C.byref(pbytes), C.c_void_p)))
+        if agents is None:
+            counts = self._served_counts(counts, flags)
+        return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value]
+
+    def pending_tokens(self, agents=None, n: Optional[int] = None) -> np.ndarray:
+        """uint64 per agent: the token weights of its pending records, summed (sdb_pending_tokens).  agents None: every
+        agent below the registration watermark (or the first n)."""
+        if agents is None:
+            a, cnt = None, int(n if n is not None else self.stats_n_agents())
+        else:
+            a = _arr(agents, np.uint32)
+            cnt = len(a)
+        out = np.zeros(cnt, np.uint64)
+        self._check(self._L.sdb_pending_tokens(self._h, cnt, _p(a), _p(out)))
+        return out
 
     def restore_compact(self, agents, counts, entries, sends, payload, flags: int = 0) -> Tuple[int, int]:
         """Append records in the compact receive format behind what each listed agent has pending, with their own

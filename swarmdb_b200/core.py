@@ -41,7 +41,7 @@ import numpy as np
 from pydantic import BaseModel, Field
 
 from . import _native
-from ._native import (EXPIRE_ALL, FILTER_MAX_IDS, FILTER_MAX_KEYWORD, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON, TYPEF_SUPERSEDE,
+from ._native import (EXPIRE_ALL, FILTER_MAX_IDS, FILTER_MAX_KEYWORD, NO_GROUP, RECV_PEEK, RECV_PRIORITY, TYPE_MASK, TYPEF_EXTRAS, TYPEF_JSON, TYPEF_SUPERSEDE, TYPEF_TOKENS,
                       SdbError, Shard, make_filter, pad32, recv_capacity)
 
 
@@ -225,6 +225,26 @@ def _encode_content(content: Any) -> (bytes, int):
     if isinstance(content, str):
         return content.encode("utf-8"), 0
     return json.dumps(content).encode("utf-8"), TYPEF_JSON
+
+
+def _check_token_count(n: Any) -> None:
+    if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or not 0 <= n < (1 << 32):
+        raise ValueError(f"token_count={n!r} is not an integer in [0, 2^32): the device carries it as a u32")
+
+
+def _encode_payload(body: bytes, flags: int, extras: Dict[str, Any], token_count: Optional[int]) -> Tuple[bytes, int]:
+    """Wire form of a message and its type flags: the content bytes, or with JSON extras (metadata, visibility)
+    u32 content length | content | extras (TYPEF_EXTRAS); a token count goes in front of either as a u32 (TYPEF_TOKENS),
+    where the device reads it."""
+    if extras:
+        payload = len(body).to_bytes(4, "little") + body + json.dumps(extras).encode("utf-8")
+        flags |= TYPEF_EXTRAS
+    else:
+        payload = body
+    if token_count is not None:
+        payload = int(token_count).to_bytes(4, "little") + payload
+        flags |= TYPEF_TOKENS
+    return payload, flags
 
 
 def _renumber_rows(entries, sends) -> Tuple[np.ndarray, np.ndarray]:
@@ -691,6 +711,8 @@ class SwarmsDB:
         if receiver_id is not None and receiver_id not in self.registered_agents:
             self.register_agent(receiver_id)
         token_count = self._count_tokens(content) if self.token_counter else None
+        if token_count is not None:
+            _check_token_count(token_count)
 
         seq = self._next_seq
         if not isinstance(content, (str, dict, list)):
@@ -713,7 +735,7 @@ class SwarmsDB:
             for agent_id in self.registered_agents:                      # M:461-463
                 self.agent_inbox[agent_id].append(message.id)
 
-        # wire form: content bytes (+ JSON extras for metadata / visible_to / token_count)
+        # wire form: content bytes (+ JSON extras for metadata / visible_to, + the token count)
         body, flags = _encode_content(content)
         extras: Dict[str, Any] = {}
         md = dict(message.metadata)
@@ -723,13 +745,7 @@ class SwarmsDB:
             extras["m"] = md
         if message.visible_to:
             extras.update(self._encode_visibility(message.visible_to))
-        if token_count is not None:
-            extras["t"] = token_count
-        if extras:
-            payload = len(body).to_bytes(4, "little") + body + json.dumps(extras).encode("utf-8")
-            flags |= TYPEF_EXTRAS
-        else:
-            payload = body
+        payload, flags = _encode_payload(body, flags, extras, token_count)
         type_code = _TYPE_CODE[MessageType(message_type)] | flags | (TYPEF_SUPERSEDE if supersede else 0)
         prio = int(MessagePriority(priority))
         sender = self._index(sender_id)
@@ -876,18 +892,14 @@ class SwarmsDB:
         if sender_id not in self.registered_agents:
             self.register_agent(sender_id)
         token_count = self._count_tokens(content) if self.token_counter else None
+        if token_count is not None:
+            _check_token_count(token_count)
         body, flags = _encode_content(content)
         md = {k: v for k, v in msg_metadata.items() if k != "group"}
         extras: Dict[str, Any] = {}
         if md:
             extras["m"] = md
-        if token_count is not None:
-            extras["t"] = token_count
-        if extras:
-            payload = len(body).to_bytes(4, "little") + body + json.dumps(extras).encode("utf-8")
-            flags |= TYPEF_EXTRAS
-        else:
-            payload = body
+        payload, flags = _encode_payload(body, flags, extras, token_count)
         base = self._next_seq
         now = time.time()
         mtype, mprio = MessageType(message_type), MessagePriority(priority)
@@ -924,16 +936,18 @@ class SwarmsDB:
 
     # ------------------------------------------------------------------ receive
     def receive_messages(self, agent_id: str, max_messages: int = 100, timeout: float = 1.0,
-                         max_bytes: Optional[int] = None) -> List[Message]:
+                         max_bytes: Optional[int] = None, max_tokens: Optional[int] = None) -> List[Message]:
         """Pop up to `max_messages` pending messages for `agent_id` in stream order (or priority
         order with GpuConfig.priority_dequeue).  Never blocks: `timeout` is accepted for
         compatibility (the reference spins up to `timeout` when fewer are available, M:553-556).
         max_bytes bounds the encoded payload bytes returned: the longest run of pending messages, in delivery order,
         whose encoded payloads (each rounded up to 32 bytes) fit max_bytes, or the first message alone when it is
-        larger.  A byte budget is the device's stand-in for a token budget (as many messages as fit N bytes of
-        context).  One such call returns at most GpuConfig.max_recv_records messages and max_recv_payload bytes."""
+        larger.  max_tokens bounds their token counts the same way: as many pending messages as fit max_tokens tokens
+        of a model's context, counted with the token_counter the messages were sent with (a message sent without a
+        count weighs 0, so max_bytes is what bounds those).  The two combine: the shorter run wins.  One such call
+        returns at most GpuConfig.max_recv_records messages and max_recv_payload bytes."""
         self._prepare_receive(agent_id)
-        return self._receive_local(agent_id, max_messages, max_bytes)
+        return self._receive_local(agent_id, max_messages, max_bytes, max_tokens)
 
     def _prepare_receive(self, agent_id: str) -> bool:
         """Before a receive for `agent_id`: register it if needed and push buffered sends (a sharded front-end checks
@@ -944,21 +958,30 @@ class SwarmsDB:
         self.flush()
         return True
 
-    def _receive_budget_one(self, agent_id: str, max_messages: int, max_bytes: int, flags: int):
-        """(headers, payload) of one byte-budget receive for one agent (Shard.receive_budget)."""
-        if max_bytes < 0:
+    def _receive_budget_one(self, agent_id: str, max_messages: int, max_bytes: Optional[int], flags: int,
+                            max_tokens: Optional[int] = None):
+        """(headers, payload) of one byte- and/or token-budget receive for one agent (Shard.receive_budget,
+        Shard.receive_tokens)."""
+        if max_bytes is not None and max_bytes < 0:
             raise ValueError("max_bytes must be >= 0")
+        if max_tokens is not None and not 0 < max_tokens < (1 << 64):
+            raise ValueError("max_tokens must be positive (None: no token limit)")
         k = min(max_messages, self.shard.max_recv_records)
         # the device reads 0 as "no limit"; a 1-byte limit takes the same records as a 0-byte one (sizes are multiples of 32)
-        _, hdr, pay = self.shard.receive_budget([self._index(agent_id)], k, max(int(max_bytes), 1), flags)
+        nbytes = 0 if max_bytes is None else max(int(max_bytes), 1)
+        if max_tokens is not None:
+            _, hdr, pay = self.shard.receive_tokens([self._index(agent_id)], k, int(max_tokens), nbytes, flags)
+        else:
+            _, hdr, pay = self.shard.receive_budget([self._index(agent_id)], k, nbytes, flags)
         return hdr, pay
 
-    def _receive_local(self, agent_id: str, max_messages: int, max_bytes: Optional[int] = None) -> List[Message]:
+    def _receive_local(self, agent_id: str, max_messages: int, max_bytes: Optional[int] = None,
+                       max_tokens: Optional[int] = None) -> List[Message]:
         if max_messages <= 0:
             return []
         flags = RECV_PRIORITY if self.gpu_config.priority_dequeue else 0
-        if max_bytes is not None:
-            hdr, pay = self._receive_budget_one(agent_id, max_messages, max_bytes, flags)
+        if max_bytes is not None or max_tokens is not None:
+            hdr, pay = self._receive_budget_one(agent_id, max_messages, max_bytes, flags, max_tokens)
             return self._decode(hdr, pay, agent_id)
         out: List[Message] = []
         a = self._index(agent_id)
@@ -1154,15 +1177,16 @@ class SwarmsDB:
         flushes delivered, so it overrides this with a no-op)."""
         self.flush()
 
-    def peek_messages(self, agent_id: str, max_messages: int = 100, max_bytes: Optional[int] = None) -> List[Message]:
-        """What `receive_messages` (with the same max_bytes) would return next, without consuming it (device PEEK
-        receive)."""
+    def peek_messages(self, agent_id: str, max_messages: int = 100, max_bytes: Optional[int] = None,
+                      max_tokens: Optional[int] = None) -> List[Message]:
+        """What `receive_messages` (with the same max_bytes and max_tokens) would return next, without consuming it
+        (device PEEK receive)."""
         self._pre_read()
         flags = RECV_PEEK | (RECV_PRIORITY if self.gpu_config.priority_dequeue else 0)
-        if max_bytes is not None:
+        if max_bytes is not None or max_tokens is not None:
             if max_messages <= 0:
                 return []
-            hdr, pay = self._receive_budget_one(agent_id, max_messages, max_bytes, flags)
+            hdr, pay = self._receive_budget_one(agent_id, max_messages, max_bytes, flags, max_tokens)
         else:
             hdr, pay, _ = self.shard.receive_one(self._index(agent_id), max_messages, flags)
         return self._decode(hdr, pay, agent_id, record=False, status=MessageStatus.DELIVERED)
@@ -1325,6 +1349,9 @@ class SwarmsDB:
         for k in range(n):
             blob = raw[offs[k]: offs[k] + lens[k]]
             t = types[k]
+            tokens = None
+            if t & TYPEF_TOKENS:
+                tokens, blob = int.from_bytes(blob[:4], "little"), blob[4:]
             extras: Dict[str, Any] = {}
             if t & TYPEF_EXTRAS:
                 clen = int.from_bytes(blob[:4], "little")
@@ -1342,7 +1369,7 @@ class SwarmsDB:
                 receiver_id=None if receiver == _native.NO_RECEIVER else names[receiver],
                 content=content, type=_TYPE_BY_CODE[t & TYPE_MASK], priority=MessagePriority(prios[k]),
                 timestamp=stamps[k], status=status, metadata=metadata,
-                token_count=extras.get("t") if extras else None, visible_to=self._decode_visibility(extras) if extras else [])
+                token_count=tokens if tokens is not None else (extras.get("t") if extras else None), visible_to=self._decode_visibility(extras) if extras else [])
             if record:
                 self.messages[m.id] = m                    # M:587-588
             msgs.append(m)
@@ -1375,23 +1402,31 @@ class SwarmsDB:
         return base
 
     def receive_batch(self, agent_idx=None, max_messages: int = 100, priority: Optional[bool] = None,
-                      max_bytes: Optional[int] = None, **kw):
+                      max_bytes: Optional[int] = None, max_tokens: Optional[int] = None, **kw):
         """max_bytes: each agent takes at most that many encoded payload bytes (each payload rounded up to 32 bytes; an
         oversized first message alone; 0: no per-agent limit) and the call is sized by the bytes it selects
-        (Shard.receive_budget).  None keeps the plain receive."""
+        (Shard.receive_budget).  max_tokens: each agent's take is also cut where its token counts would pass
+        max_tokens (a heavier first message alone; messages without a count weigh 0; 0: no token limit;
+        Shard.receive_tokens).  None for both keeps the plain receive."""
         self.flush()
         pr = self.gpu_config.priority_dequeue if priority is None else priority
+        if max_tokens is not None:
+            return self.shard.receive_tokens(agent_idx, max_messages, int(max_tokens), int(max_bytes or 0),
+                                             RECV_PRIORITY if pr else 0, **kw)
         if max_bytes is not None:
             return self.shard.receive_budget(agent_idx, max_messages, int(max_bytes), RECV_PRIORITY if pr else 0, **kw)
         return self.shard.receive_batch(agent_idx, max_messages, RECV_PRIORITY if pr else 0, **kw)
 
     def receive_batch_compact(self, agent_idx=None, max_messages: int = 100, priority: Optional[bool] = None,
-                              max_bytes: Optional[int] = None, **kw):
+                              max_bytes: Optional[int] = None, max_tokens: Optional[int] = None, **kw):
         """receive_batch's records in the compact format: (counts, entries, sends, payload) with each distinct
         payload once (Shard.receive_compact; _native.expand_compact gives receive_batch's (headers, payload)).
-        max_bytes as in receive_batch; bytes are counted per message, shared payloads included."""
+        max_bytes and max_tokens as in receive_batch; bytes are counted per message, shared payloads included."""
         self.flush()
         pr = self.gpu_config.priority_dequeue if priority is None else priority
+        if max_tokens is not None:
+            return self.shard.receive_compact_tokens(agent_idx, max_messages, int(max_tokens), int(max_bytes or 0),
+                                                     RECV_PRIORITY if pr else 0, **kw)
         return self.shard.receive_compact(agent_idx, max_messages, RECV_PRIORITY if pr else 0,
                                           max_agent_bytes=None if max_bytes is None else int(max_bytes), **kw)
 
@@ -2013,6 +2048,18 @@ class SwarmsDB:
         if agents is not None and len(agents) == 0:
             return 0
         return self.shard.trim(agents, *limits, flags | (RECV_PRIORITY if by_priority else 0), archive=False)[1]
+
+    def pending_tokens(self, agent_ids: Optional[Iterable[str]] = None) -> Dict[str, int]:
+        """Per agent (default: every agent this instance serves), the token counts of its device-pending messages,
+        summed; messages sent without a count weigh 0 and in-flight leases are not pending.  Unknown agents read 0."""
+        self._pre_read()
+        names = list(self._agent_name) if agent_ids is None else list(dict.fromkeys(agent_ids))
+        agents, _ = self._expire_scope(names)
+        out = dict.fromkeys(names, 0) if agent_ids is not None else {}
+        if len(agents):
+            for a, t in zip(agents.tolist(), self.shard.pending_tokens(agents).tolist()):
+                out[self._agent_name[a]] = int(t)
+        return out
 
     def _expire_device_archive(self, cutoff: float) -> List[Message]:
         """Expire the device-queued records older than the cutoff in archive mode, call after call until none is left,

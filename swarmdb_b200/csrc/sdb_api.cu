@@ -2106,7 +2106,7 @@ int sdb_receive_batch(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
   if (async && (count_out || hdr_out || payload_out)) return fail(h, SDB_EINVAL, "SDB_RECV_ASYNC takes no host output buffers");
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
-                                     nullptr, nullptr);
+                                     nullptr, nullptr, 0ull);
   h->launches += nl;
   if (!(r.flags & SDB_RECV_PRIORITY)) r.plan_tops = nullptr;       // single-pass path: plan offsets are absolute
   h->last_rx = r; h->last_rx_valid = (e == cudaSuccess); h->last_rx_compact = false;
@@ -2160,7 +2160,7 @@ int sdb_receive_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_i
     if (rc != SDB_OK) return rc; }
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
-                                     &h->cx, nullptr);
+                                     &h->cx, nullptr, 0ull);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = true;
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("compact receive launch: ") + cudaGetErrorString(e));
@@ -2182,13 +2182,16 @@ static int budget_caps(sdb_ctx* h, uint64_t rec_room, const void* payload_out, u
   return SDB_OK;
 }
 
-int sdb_receive_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint64_t max_agent_bytes,
-                       uint32_t flags, uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
-                       uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+// sdb_receive_budget and sdb_receive_tokens (max_agent_tokens 0: the budget call); `name` and `what` name the call in
+// error messages
+static int receive_budget_full(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                               uint64_t max_agent_bytes, uint64_t max_agent_tokens, uint32_t flags, uint32_t* count_out,
+                               sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out, uint64_t payload_cap,
+                               uint64_t* total_out, uint64_t* payload_bytes_out, const char* name, const char* what) {
   if (!h) return SDB_EINVAL;
   if (total_out) *total_out = 0;
   if (payload_bytes_out) *payload_bytes_out = 0;
-  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_budget returns host results: SDB_RECV_ASYNC is not accepted");
+  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, std::string(name) + " returns host results: SDB_RECV_ASYNC is not accepted");
   uint64_t rec_cap = 0;
   uint2 budget;
   { const int rc = budget_caps(h, room(hdr_out, hdr_cap), payload_out, payload_cap, max_agent_bytes, &rec_cap, &budget);
@@ -2201,23 +2204,39 @@ int sdb_receive_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_id
     if (rc != SDB_OK) return rc; }
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
-                                     nullptr, &budget);
+                                     nullptr, &budget, max_agent_tokens);
   h->launches += nl;
   r.plan_tops = nullptr;                                        // single-pass plan in both orders: offsets are absolute
   h->last_rx = r; h->last_rx_valid = (e == cudaSuccess); h->last_rx_compact = false;
-  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("budget receive launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string(what) + " launch: " + cudaGetErrorString(e));
   return copy_full(h, n_agents, count_out, hdr_out, payload_out, total_out, payload_bytes_out);
 }
 
-int sdb_receive_compact_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
-                               uint64_t max_agent_bytes, uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out,
-                               uint64_t entry_cap, sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out,
-                               uint64_t payload_cap, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+int sdb_receive_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint64_t max_agent_bytes,
+                       uint32_t flags, uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
+                       uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+  return receive_budget_full(h, n_agents, agent_idx, max_messages, max_agent_bytes, 0, flags, count_out, hdr_out, hdr_cap,
+                             payload_out, payload_cap, total_out, payload_bytes_out, "sdb_receive_budget", "budget receive");
+}
+
+int sdb_receive_tokens(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint64_t max_agent_bytes,
+                       uint64_t max_agent_tokens, uint32_t flags, uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
+                       uint8_t* payload_out, uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+  return receive_budget_full(h, n_agents, agent_idx, max_messages, max_agent_bytes, max_agent_tokens, flags, count_out, hdr_out,
+                             hdr_cap, payload_out, payload_cap, total_out, payload_bytes_out, "sdb_receive_tokens", "token receive");
+}
+
+// sdb_receive_compact_budget and sdb_receive_compact_tokens (max_agent_tokens 0: the budget call)
+static int receive_budget_compact(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                                  uint64_t max_agent_bytes, uint64_t max_agent_tokens, uint32_t flags, uint32_t* count_out,
+                                  sdb_recv_entry* entry_out, uint64_t entry_cap, sdb_recv_send* send_out, uint64_t send_cap,
+                                  uint8_t* payload_out, uint64_t payload_cap, uint64_t* total_out, uint64_t* n_sends_out,
+                                  uint64_t* payload_bytes_out, const char* name, const char* what) {
   if (!h) return SDB_EINVAL;
   if (total_out) *total_out = 0;
   if (n_sends_out) *n_sends_out = 0;
   if (payload_bytes_out) *payload_bytes_out = 0;
-  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_compact_budget returns host results: SDB_RECV_ASYNC is not accepted");
+  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, std::string(name) + " returns host results: SDB_RECV_ASYNC is not accepted");
   // bytes are counted per record, so the compact payload (one copy per distinct image) never exceeds the count
   uint64_t rec_cap = 0;
   uint2 budget;
@@ -2233,11 +2252,52 @@ int sdb_receive_compact_budget(sdb_handle h, uint32_t n_agents, const uint32_t* 
     if (rc != SDB_OK) return rc; }
   int nl = 0;
   cudaError_t e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + pad32(h->cfg.max_payload_bytes),
-                                     &h->cx, &budget);
+                                     &h->cx, &budget, max_agent_tokens);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = true;
-  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("compact budget receive launch: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string(what) + " launch: " + cudaGetErrorString(e));
   return copy_compact(h, n_agents, count_out, entry_out, send_out, payload_out, total_out, n_sends_out, payload_bytes_out);
+}
+
+int sdb_receive_compact_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                               uint64_t max_agent_bytes, uint32_t flags, uint32_t* count_out, sdb_recv_entry* entry_out,
+                               uint64_t entry_cap, sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out,
+                               uint64_t payload_cap, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out) {
+  return receive_budget_compact(h, n_agents, agent_idx, max_messages, max_agent_bytes, 0, flags, count_out, entry_out, entry_cap,
+                                send_out, send_cap, payload_out, payload_cap, total_out, n_sends_out, payload_bytes_out,
+                                "sdb_receive_compact_budget", "compact budget receive");
+}
+
+int sdb_receive_compact_tokens(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                               uint64_t max_agent_bytes, uint64_t max_agent_tokens, uint32_t flags, uint32_t* count_out,
+                               sdb_recv_entry* entry_out, uint64_t entry_cap, sdb_recv_send* send_out, uint64_t send_cap,
+                               uint8_t* payload_out, uint64_t payload_cap, uint64_t* total_out, uint64_t* n_sends_out,
+                               uint64_t* payload_bytes_out) {
+  return receive_budget_compact(h, n_agents, agent_idx, max_messages, max_agent_bytes, max_agent_tokens, flags, count_out,
+                                entry_out, entry_cap, send_out, send_cap, payload_out, payload_cap, total_out, n_sends_out,
+                                payload_bytes_out, "sdb_receive_compact_tokens", "compact token receive");
+}
+
+int sdb_pending_tokens(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint64_t* tokens_out) {
+  if (!h || (n_agents && !tokens_out)) return SDB_EINVAL;
+  if (n_agents == 0) return SDB_OK;
+  if (n_agents > h->cfg.max_agents) return fail(h, SDB_EINVAL, "n_agents > max_agents");
+  if (agent_idx)
+    for (uint32_t i = 0; i < n_agents; ++i)
+      if (agent_idx[i] >= h->cfg.max_agents) return fail(h, SDB_EINVAL, "agent index out of range");
+  sdb_recv_args r{};
+  { const int rc = recv_args(h, n_agents, agent_idx, false, 0xFFFFFFFFu, 0, 0, &r); if (rc != SDB_OK) return rc; }
+  unsigned long long* sums = nullptr;
+  CUDA_TRY(h, cudaMallocAsync(reinterpret_cast<void**>(&sums), static_cast<size_t>(n_agents) * sizeof(unsigned long long), h->stream));
+  int nl = 0;
+  cudaError_t e = sdb_launch_token_take(&h->view, &r, ~0ull, sums, h->stream, &nl, &h->prof, h->sm_count);
+  h->launches += nl;
+  if (e == cudaSuccess) e = cudaMemcpyAsync(tokens_out, sums, static_cast<size_t>(n_agents) * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaFreeAsync(sums, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("pending tokens: ") + cudaGetErrorString(e));
+  h->stream_busy = false;
+  return SDB_OK;
 }
 
 // The first step of sdb_supersede: count the flagged pending records of r's agents (one synchronisation) and, when there
@@ -2674,7 +2734,7 @@ int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_id
   int nl = 0;
   const bool ledger = L.policy && L.led_n;      // the ledger holds entries: collect before anything is retired, look up after
   cudaError_t e = ledger ? ledger_collect(h) : cudaSuccess;
-  if (e == cudaSuccess) e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx, nullptr);
+  if (e == cudaSuccess) e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx, nullptr, 0ull);
   h->last_rx_valid = false; h->last_rx_compact = true;
   if (e == cudaSuccess)
     e = sdb_launch_lease_append(&L.buf[L.cur], &L.s, &h->cx, h->rx_count, h->rx_totals, r.agent_idx, n_agents,

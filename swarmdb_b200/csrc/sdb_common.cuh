@@ -907,7 +907,9 @@ cudaError_t sdb_launch_pull(const sdb_dev_view*, const sdb_pull_view*, const sdb
                             uint32_t, uint32_t, const uint32_t*, const uint32_t*, uint64_t, int, cudaStream_t, sdb_profiler*, int*,
                             const sdb_batch_base*, uint32_t);
 cudaError_t sdb_launch_receive(const sdb_dev_view*, const sdb_recv_args*, cudaStream_t, int*, sdb_profiler*, int, uint32_t,
-                               const sdb_compact_args*, const uint2*);
+                               const sdb_compact_args*, const uint2*, unsigned long long);
+cudaError_t sdb_launch_token_take(const sdb_dev_view*, const sdb_recv_args*, unsigned long long, unsigned long long*, cudaStream_t,
+                                  int*, sdb_profiler*, int);
 cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double, uint32_t, const uint2*, const sdb_compact_args*,
                               cudaStream_t, int*, sdb_profiler*, int);
 cudaError_t sdb_launch_supersede(const sdb_dev_view*, const sdb_recv_args*, const sdb_ss_args*, const sdb_compact_args*, cudaStream_t,

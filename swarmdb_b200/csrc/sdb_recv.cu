@@ -528,15 +528,18 @@ __device__ __forceinline__ uint32_t budget_take_regs(const uint64_t (&ev)[8], ui
 }
 
 // MODE: SDB_PLAN_PLAIN (sdb_receive_batch, stream order), SDB_PLAN_BUDGET (byte budgets, stream order),
-// SDB_PLAN_BUDGET_PRIO (byte budgets, priority order: every agent is walked and selected by its warp).
-// budget = {per-agent limit, call capacity} in payload granules, read by the budget modes only.
-enum { SDB_PLAN_PLAIN = 0, SDB_PLAN_BUDGET = 1, SDB_PLAN_BUDGET_PRIO = 2 };
+// SDB_PLAN_BUDGET_PRIO (byte budgets, priority order: every agent is walked and selected by its warp),
+// SDB_PLAN_TOKENS / SDB_PLAN_TOKENS_PRIO (token budgets: the budget modes with min(max_messages, cnt[q]) records per
+// agent, cnt[q] written by k_token_take).
+// budget = {per-agent limit, call capacity} in payload granules, read by the budget and token modes only.
+enum { SDB_PLAN_PLAIN = 0, SDB_PLAN_BUDGET = 1, SDB_PLAN_BUDGET_PRIO = 2, SDB_PLAN_TOKENS = 3, SDB_PLAN_TOKENS_PRIO = 4 };
 // at most 64 registers (4 CTAs per SM, the shared-memory limit allows 5): with 80, which the compiler picks otherwise,
 // the c2 plan ran 13 % slower on an H100 (400 W power limit)
 template <int MODE>
 __global__ void __launch_bounds__(SDB_PLAN_TILE, 4)
 k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint2 budget) {
-  constexpr bool BUDGET = MODE != SDB_PLAN_PLAIN, PRIO = MODE == SDB_PLAN_BUDGET_PRIO;
+  constexpr bool BUDGET = MODE != SDB_PLAN_PLAIN, PRIO = MODE == SDB_PLAN_BUDGET_PRIO || MODE == SDB_PLAN_TOKENS_PRIO;
+  constexpr bool TOKENS = MODE == SDB_PLAN_TOKENS || MODE == SDB_PLAN_TOKENS_PRIO;
   __shared__ uint32_t s_tile;
   __shared__ unsigned long long s_wr[SDB_PLAN_WARPS], s_wg[SDB_PLAN_WARPS];
   __shared__ unsigned long long s_br, s_bg;
@@ -563,6 +566,7 @@ k_recv_plan(sdb_dev_view v, sdb_recv_args r, uint32_t tiles, uint2 budget) {
       h4 = *reinterpret_cast<const uint4*>(v.ring_hdr + a);                 // head, tail, ctail, ntomb
       head = h4.x; tail = h4.y; nt = h4.w;
       cnt = min(tail - head - nt, r.max_messages);
+      if constexpr (TOKENS) cnt = min(cnt, r.cnt[q]);                       // both takes are prefixes of one order
     }
   }
   const bool holey = cnt && (PRIO || nt != 0);      // planned by the warp (select_agent_warp)
@@ -1249,12 +1253,158 @@ extern "C" cudaError_t sdb_recv_prepare_device() {
   return cudaFuncSetAttribute(k_recv_gather_tma<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 2 * 32 * 544);
 }
 
+// ------------------------------------------------------------------------------------------
+// token budgets (sdb_receive_tokens, sdb_pending_tokens).  A record whose type byte carries SDB_TYPEF_TOKENS and whose
+// len is at least 4 weighs the little-endian u32 at the start of its payload; every other record weighs 0.
+// k_token_take<PRIO> writes each request slot's token take to cnt[q]: the longest prefix of its delivery order whose
+// token sum is <= lim, or its first record alone when that one is heavier.  Priority order takes whole levels from the
+// top while they fit, then the arrival-order prefix of the level where the limit falls (budget_take_warp's rule).
+// sums (nullable) receives the token sum of each take (lim = ~0: every pending record).
+// k_expire's shape: 8 lanes per request slot, the ring header once, the window's entries coalesced, then per live entry
+// the header's last word and the payload's first word - two independent random loads - 4 entries per lane in flight.
+// Priority order walks twice: per-level totals, then the entries of the cut level only (none when every level fits).
+// ------------------------------------------------------------------------------------------
+#define SDB_TK_G 8u      // lanes per request slot
+#define SDB_TK_U 4u      // entries per lane in flight
+
+// the token weights of one step's entries (0 where sel is false)
+__device__ __forceinline__ void tk_weights(const sdb_dev_view& v, const uint2 (&e)[SDB_TK_U], const bool (&sel)[SDB_TK_U],
+                                           uint32_t (&tk)[SDB_TK_U]) {
+  uint32_t hw[SDB_TK_U], pw[SDB_TK_U];
+#pragma unroll
+  for (uint32_t u = 0; u < SDB_TK_U; ++u) {             // all loads issued before any use
+    hw[u] = sel[u] ? __ldg(reinterpret_cast<const uint32_t*>(v.arena + ((static_cast<uint64_t>(e[u].x) & v.gmask) << 5) + 28))
+                   : 0u;                                 // len | prio << 16 | type << 24
+    pw[u] = sel[u] && (sdb_meta(e[u]) & SDB_META_GLEN_MASK) > 1u
+                ? __ldg(reinterpret_cast<const uint32_t*>(sdb_payload_of(v, e[u].x, sdb_entry_dm1(e[u].y))))
+                : 0u;
+  }
+#pragma unroll
+  for (uint32_t u = 0; u < SDB_TK_U; ++u)
+    tk[u] = (((hw[u] >> 24) & SDB_TYPEF_TOKENS) && (hw[u] & 0xFFFFu) >= 4u) ? pw[u] : 0u;
+}
+
+template <bool PRIO>
+__global__ void __launch_bounds__(256)
+k_token_take(sdb_dev_view v, sdb_recv_args r, unsigned long long lim, unsigned long long* __restrict__ sums) {
+  const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_TK_G - 1), gsh = lane & ~(SDB_TK_G - 1), below = (1u << l8) - 1u;
+  const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t mask = v.ring_slots - 1;
+  constexpr uint32_t SPW = 32u / SDB_TK_G;                      // request slots per warp
+  for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
+    const uint32_t q = qb + lane / SDB_TK_G;
+    const bool valid = q < r.n;
+    uint32_t a = 0, H = 0, T = 0, NT = 0;
+    if (valid) {
+      a = r.agent_idx ? r.agent_idx[q] : q;
+      const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);     // one address for the slot's 8 lanes
+      H = h.x; T = h.y; NT = h.w;
+    }
+    const uint32_t W = valid && T - H - NT ? T - H : 0u;
+    const uint2* rs = sdb_ring_of(v, a);
+    uint32_t take = 0, cut = 4;                                 // cut: the level where the limit falls (4: none)
+    unsigned long long tsum = 0;
+    if (PRIO) {
+      // 1. per level: live records and their tokens
+      uint32_t c[4] = {0u, 0u, 0u, 0u};
+      unsigned long long t[4] = {0ull, 0ull, 0ull, 0ull};
+      const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
+      for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_TK_G * SDB_TK_U) {
+        uint2 e[SDB_TK_U];
+        bool lv[SDB_TK_U];
+        uint32_t tk[SDB_TK_U];
+#pragma unroll
+        for (uint32_t u = 0; u < SDB_TK_U; ++u) {
+          const uint32_t j = j0 + u * SDB_TK_G + l8;
+          e[u] = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+          lv[u] = sdb_meta(e[u]) != SDB_META_TOMB;
+        }
+        tk_weights(v, e, lv, tk);
+#pragma unroll
+        for (uint32_t u = 0; u < SDB_TK_U; ++u) {
+          const uint32_t p = sdb_meta(e[u]) >> 14;
+#pragma unroll
+          for (uint32_t l = 0; l < 4; ++l)
+            if (lv[u] && p == l) { c[l] += 1; t[l] += tk[u]; }
+        }
+      }
+#pragma unroll
+      for (int l = 3; l >= 0; --l) {
+#pragma unroll
+        for (int o = 4; o; o >>= 1) {
+          c[l] += __shfl_xor_sync(0xFFFFFFFFu, c[l], o);
+          t[l] += __shfl_xor_sync(0xFFFFFFFFu, t[l], o);
+        }
+        if (cut == 4) {
+          if (tsum + t[l] <= lim) { take += c[l]; tsum += t[l]; }
+          else cut = static_cast<uint32_t>(l);
+        }
+      }
+    }
+    // 2. stream order, or the arrival-order prefix of the cut level: entry i is taken while the running sum fits (or it
+    // is the first of the delivery order); sums only grow, so the first one that does not fit ends the take
+    const uint32_t W2 = (!PRIO || cut < 4) ? W : 0u;
+    bool open = W2 != 0;
+    const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W2);
+    for (uint32_t j0 = 0; j0 < wmax && __any_sync(0xFFFFFFFFu, open); j0 += SDB_TK_G * SDB_TK_U) {
+      uint2 e[SDB_TK_U];
+      bool sel[SDB_TK_U];
+      uint32_t tk[SDB_TK_U];
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_TK_U; ++u) {
+        const uint32_t j = j0 + u * SDB_TK_G + l8;
+        e[u] = open && j < W2 ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+        sel[u] = sdb_meta(e[u]) != SDB_META_TOMB && (!PRIO || sdb_meta(e[u]) >> 14 == cut);
+      }
+      tk_weights(v, e, sel, tk);
+#pragma unroll
+      for (uint32_t u = 0; u < SDB_TK_U; ++u) {
+        const uint32_t bs = (__ballot_sync(0xFFFFFFFFu, sel[u]) >> gsh) & 0xFFu;
+        unsigned long long x = tk[u];                           // inclusive scan over the slot's 8 lanes
+#pragma unroll
+        for (uint32_t o = 1; o < SDB_TK_G; o <<= 1) {
+          const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, x, o, SDB_TK_G);
+          if (l8 >= o) x += y;
+        }
+        const bool ok = open && sel[u] && (take + __popc(bs & below) == 0 || tsum + x <= lim);
+        const uint32_t bo = (__ballot_sync(0xFFFFFFFFu, ok) >> gsh) & 0xFFu;
+        unsigned long long s = ok ? tk[u] : 0ull;
+#pragma unroll
+        for (int o = 4; o; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
+        take += __popc(bo); tsum += s;
+        if (bo != bs) open = false;                             // an entry did not fit: the take ends before it
+      }
+    }
+    if (valid && l8 == 0) {
+      r.cnt[q] = take;
+      if (sums) sums[q] = tsum;
+    }
+  }
+}
+
+// cnt[q] = the token take of each request slot under `lim` (~0: everything pending), sums[q] (nullable) its token sum
+extern "C" cudaError_t sdb_launch_token_take(const sdb_dev_view* v, const sdb_recv_args* r, unsigned long long lim,
+                                             unsigned long long* sums, cudaStream_t stream, int* n_launches,
+                                             sdb_profiler* prof, int sm_count) {
+  if (r->n == 0) return cudaSuccess;
+  const uint32_t blocks = sdb_grid(r->n, 32, 32 * sm_count);                 // 4 slots per warp, 8 warps per block
+  const int pi = sdb_prof_begin(prof, SDB_PK_RECV_COUNT, stream);
+  if (r->flags & SDB_RECV_PRIORITY)
+    k_token_take<true><<<blocks, 256, 0, stream>>>(*v, *r, lim, sums);
+  else
+    k_token_take<false><<<blocks, 256, 0, stream>>>(*v, *r, lim, sums);
+  sdb_prof_end(prof, pi, stream);
+  if (n_launches) *n_launches += 1;
+  return cudaGetLastError();
+}
+
 // ca != nullptr: a compact receive (the same plan; the compact kernels replace the gather)
 // budget != nullptr: byte budgets (sdb_receive_budget), {per-agent limit, call capacity} in payload granules; both orders
 // take the single-pass plan
+// max_tokens != 0 (with budget): token budgets (sdb_receive_tokens), k_token_take first, then the plan's token modes
 extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_args* r0, cudaStream_t stream,
                                           int* n_launches, sdb_profiler* prof, int sm_count, uint32_t max_rec_bytes,
-                                          const sdb_compact_args* ca, const uint2* budget) {
+                                          const sdb_compact_args* ca, const uint2* budget, unsigned long long max_tokens) {
   if (r0->n == 0) return cudaSuccess;
   sdb_recv_args ra = *r0;
   sdb_recv_args* r = &ra;
@@ -1267,10 +1417,18 @@ extern "C" cudaError_t sdb_launch_receive(const sdb_dev_view* v, const sdb_recv_
     // ---- stream order (and byte budgets): single-pass plan + gather
     const uint32_t tiles = (n + SDB_PLAN_TILE - 1) / SDB_PLAN_TILE;
     r->plan_tops = nullptr;
+    if (budget && max_tokens) {
+      const cudaError_t e = sdb_launch_token_take(v, r, max_tokens, nullptr, stream, n_launches, prof, sm_count);
+      if (e != cudaSuccess) return e;
+    }
     pi = sdb_prof_begin(prof, SDB_PK_RECV_SELECT, stream);
     cudaMemsetAsync(r->lb, 0, sdb_lb_words(tiles) * sizeof(unsigned long long), stream);
     if (!budget)
       k_recv_plan<SDB_PLAN_PLAIN><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, make_uint2(0u, 0u));
+    else if (max_tokens && (r->flags & SDB_RECV_PRIORITY))
+      k_recv_plan<SDB_PLAN_TOKENS_PRIO><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, *budget);
+    else if (max_tokens)
+      k_recv_plan<SDB_PLAN_TOKENS><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, *budget);
     else if (r->flags & SDB_RECV_PRIORITY)
       k_recv_plan<SDB_PLAN_BUDGET_PRIO><<<tiles, SDB_PLAN_TILE, 0, stream>>>(*v, *r, tiles, *budget);
     else
@@ -2060,10 +2218,11 @@ k_where_kw(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
         const uint32_t hw = __shfl_sync(0xFFFFFFFFu, hi.w, src);
         const uint32_t len = hw & 0xFFFFu;
         const uint8_t* p = sdb_payload_of(v, hx, sdb_entry_dm1(hy));      // shared-layout images: handle + 1 + dm1
-        uint32_t cs = 0, ce = len;
+        const uint32_t c0 = ((hw >> 24) & SDB_TYPEF_TOKENS) ? 4u : 0u;    // u32 token count first
+        uint32_t cs = c0, ce = len;
         if ((hw >> 24) & SDB_TYPEF_EXTRAS) {                               // u32 content length | content | extras
-          cs = 4;
-          ce = len < 4 ? 4u : 4u + min(__ldg(reinterpret_cast<const uint32_t*>(p)), len - 4u);
+          cs = c0 + 4u;
+          ce = len < cs ? cs : cs + min(__ldg(reinterpret_cast<const uint32_t*>(p + c0)), len - cs);
         }
         if (!where_find(p, (len + 31u) & ~31u, cs, ce, s_kw, K, icase, s_buf[warp], lane)) word &= ~(1u << src);
       }

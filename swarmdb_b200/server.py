@@ -305,9 +305,12 @@ def create_app(db: Optional[SwarmsDB] = None, settings: Optional[Settings] = Non
 
     # ---- read -------------------------------------------------------------------------------------------------
     @app.post("/agents/receive", response_model=List[MessageOut])
-    def receive(max_messages: int = 100, timeout: float = 1.0, who: str = Depends(caller)):
+    def receive(max_messages: int = 100, timeout: float = 1.0, max_tokens: Optional[int] = Query(None, ge=1, lt=1 << 64),
+                who: str = Depends(caller)):
+        # max_tokens: as many pending messages as fit that many tokens of context (SwarmsDB.receive_messages)
+        kw = {} if max_tokens is None else {"max_tokens": max_tokens}
         return [MessageOut.of(m) for m in guarded("receive messages", lambda: db.receive_messages(
-            agent_id=who, max_messages=max_messages, timeout=timeout))]
+            agent_id=who, max_messages=max_messages, timeout=timeout, **kw))]
 
     @app.get("/messages/{message_id}", response_model=MessageOut)
     def get_message(message_id: str, include_device: bool = False, who: str = Depends(caller)):

@@ -710,12 +710,13 @@ class ShardedSwarmsDB(SwarmsDB):
             raise RuntimeError("send buffer full: call flush() (collectively) more often or raise flush_threshold")
 
     # ---- local receive on the owner
-    def receive_messages(self, agent_id: str, max_messages: int = 100, timeout: float = 1.0, max_bytes: Optional[int] = None):
+    def receive_messages(self, agent_id: str, max_messages: int = 100, timeout: float = 1.0, max_bytes: Optional[int] = None,
+                         max_tokens: Optional[int] = None):
         if self.owner(agent_id) != self.rank:
             raise ValueError(f"agent {agent_id!r} lives on shard {self.owner(agent_id)}, not on rank {self.rank}")
         if agent_id not in self._agent_idx:
             return []
-        return self._receive_local(agent_id, max_messages, max_bytes)
+        return self._receive_local(agent_id, max_messages, max_bytes, max_tokens)
 
     def _prepare_receive(self, agent_id: str) -> bool:
         """receive_matching runs on the owner rank, locally (no collective), like receive_messages."""
@@ -726,12 +727,13 @@ class ShardedSwarmsDB(SwarmsDB):
     def _pre_read(self) -> None:
         return None                              # reads see what earlier collective flushes delivered
 
-    def peek_messages(self, agent_id: str, max_messages: int = 100, max_bytes: Optional[int] = None):
+    def peek_messages(self, agent_id: str, max_messages: int = 100, max_bytes: Optional[int] = None,
+                      max_tokens: Optional[int] = None):
         if self.owner(agent_id) != self.rank:
             raise ValueError(f"agent {agent_id!r} lives on shard {self.owner(agent_id)}, not on rank {self.rank}")
         if agent_id not in self._agent_idx:
             return []
-        return super().peek_messages(agent_id, max_messages, max_bytes)
+        return super().peek_messages(agent_id, max_messages, max_bytes, max_tokens)
 
     def deregister_agent(self, agent_id: str, purge: bool = False) -> None:
         """REPLICATED, like register_agent (the registry must agree on every rank); purge=True drops the agent's
