@@ -1666,6 +1666,113 @@ def tokens(rounds=2, reps=10):
     return out
 
 
+def select(rounds=2, reps=10):
+    """Filtered and leased receives by budget (sdb_receive_where_budget, sdb_receive_leased_select) on the c2 backlog
+    (bench.py's step, 4,194,304 records over 1 M agents) with every send tagged (TYPEF_TOKENS, counts uniform in
+    1..512) and a priority filter (levels 1-3):
+      where / where_tokens   a filtered PEEK, without a limit and with 512 tokens per agent; wall time per call and the
+                             take pass (recv_count) kernel time from the library profiler
+      lease / lease_tokens   a leased take of every agent (2 messages each, and 512 tokens with the filter) plus the ack
+                             of every lease it made; the backlog is sent again and drained between calls, untimed
+    Legs alternate within each round.  Algorithmic bytes of the take pass: a 16-B ring header per agent, 8 B per ring
+    entry and 4 B per 32 verdict bits, and per match one 32-B header sector and one 32-B payload sector per distinct
+    send (the c2 windows fit one 32-entry step, which reads them all), over its kernel time, against the 3.35 TB/s of
+    NVIDIA's H100 SXM data sheet."""
+    import torch
+    from bench import Workload
+    from swarmdb_b200._native import LEASE_ACK, RECV_PEEK, Shard, make_filter
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_extra.py select: no CUDA device - swarmdb_b200 has no CPU fallback")
+    TOK, HBM = 0x40, 3.35e12
+    wl = Workload()
+    rng = np.random.default_rng(9)
+    snd, grp, prio, typ, lens, off, pay = wl.batch()
+    pay = pay.copy()
+    pay.reshape(wl.S, wl.L)[:, :4] = rng.integers(1, 513, wl.S).astype(np.uint32).view(np.uint8).reshape(wl.S, 4)
+    typ = np.full(wl.S, TOK, np.uint8)
+    per_step = wl.S * wl.F
+    rec_cap = per_step + (1 << 16)
+    shard = Shard(max_agents=wl.A, ring_slots=64, arena_bytes=1 << 33, max_payload_bytes=wl.L, max_groups=1 << 14,
+                  member_pool_entries=wl.A + 1024, max_batch_sends=wl.S, max_batch_payload=wl.S * wl.L,
+                  max_recv_records=rec_cap, max_recv_payload=rec_cap * wl.L)
+    shard.register(np.arange(wl.A, dtype=np.uint32))
+    for g in range(wl.G):
+        shard.create_group(g, wl.members(g))
+    shard.lease_reserve(rec_cap, rec_cap * wl.L)
+    filt = make_filter(prios=[1, 2, 3])
+
+    def fill():
+        shard.send_group_batch(snd, grp, prio, typ, lens, off, pay)
+        shard.sync()
+
+    def drain():
+        while len(shard.receive_compact(None, 64)[1]):
+            pass
+        shard.lease_sweep(0.0)
+        shard.sync()
+
+    def peek(limit):
+        fn = lambda: shard.receive_where(None, 100, RECV_PEEK, filt, max_agent_tokens=limit)   # noqa: E731
+        fn()                                                                  # warm-up
+        shard.sync()
+        shard.profile(True)
+        t = time.perf_counter()
+        for _ in range(reps):
+            r = fn()
+        shard.sync()
+        wall = (time.perf_counter() - t) * 1e3 / reps
+        prof = shard.profile_read()
+        shard.profile(False)
+        return r, {"call_ms": wall, "take_ms": prof["recv_count"][0] / reps, "where_ms": prof["where"][0] / reps}
+
+    def lease(tokens):
+        kw = {"max_agent_tokens": 512, "filt": filt} if tokens else {}
+        calls, recs = [], 0
+        for i in range(reps + 1):                                             # the first is a warm-up
+            drain()
+            fill()
+            t = time.perf_counter()
+            cnt, ent, sends, p, base = shard.receive_leased(None, 2 if not tokens else 100, 1e18, 0, **kw)
+            shard.lease_settle(np.arange(base, base + len(ent), dtype=np.uint64), LEASE_ACK)
+            shard.sync()
+            if i:
+                calls.append((time.perf_counter() - t) * 1e3)
+            recs = len(ent)
+        drain()
+        return recs, {"take_ack_ms": float(np.median(calls))}
+
+    fill()
+    res = {"where": [], "where_tokens": [], "lease": [], "lease_tokens": []}
+    out_recs = {}
+    for r in range(rounds):
+        for name in (list(res) if r % 2 == 0 else list(res)[::-1]):
+            if name.startswith("where"):
+                got, t = peek(512 if name == "where_tokens" else 0)
+                out_recs[name] = len(got[1])
+                if name == "where_tokens":
+                    k = got[0].astype(np.int64)
+                    _, h, _ = shard.receive_where(None, 100, RECV_PEEK, filt)
+                    matches = len(h)
+                    t["bytes"] = 16 * wl.A + 8 * per_step + 4 * wl.A + 32 * matches + 32 * matches // wl.F
+                    t["matches"], t["taken"] = matches, int(k.sum())
+            else:
+                out_recs[name], t = lease(name == "lease_tokens")
+                fill()
+            res[name].append(t)
+    shard.close()
+    out = {"config": (f"c2 backlog: {per_step} records over {wl.A} agents, {wl.L}-B payloads, every send tagged "
+                      f"(counts 1..512), filter prios 1-3; token limit 512; {reps} calls per block, legs alternated")}
+    for k, v in res.items():
+        fields = [f for f in v[0] if f.endswith("_ms")]
+        out[k] = {"blocks": v, **{f: float(np.median([x[f] for x in v])) for f in fields}, "records": out_recs[k]}
+    tk = out["where_tokens"]
+    nb = tk["blocks"][-1]["bytes"]
+    tk.update({"algorithmic_bytes": nb, "take_tb_s": nb / (tk["take_ms"] * 1e-3) / 1e12 if tk["take_ms"] else None,
+               "share_of_3_35_tb_s": nb / (tk["take_ms"] * 1e-3) / HBM if tk["take_ms"] else None})
+    out.update(_gpu_card(0))
+    return out
+
+
 def dedup(rounds=2, batch=1 << 16, n=1 << 20, L=256):
     """Deduplicated sends (sdb_send_mixed_batch_dedup) against plain sdb_send_mixed_batch of the same batches.
     send: n point-to-point sends of L bytes (one per agent), in batches of `batch`, host clock to a synchronise, each

@@ -441,6 +441,28 @@ int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_id
                        double deadline, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
                        sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
                        uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out, uint64_t* lease_base_out);
+/* Leased receive by budget and filter (an agent that assembles a model's context from its queue and needs its messages
+ * back when the model call fails): sdb_receive_leased's arguments plus max_agent_bytes, max_agent_tokens and a nullable
+ * filter (sdb_receive_where's sdb_filter, declared below).
+ *   1. Take: per agent, over its pending records that match the filter (NULL: every pending record), in the call's
+ *      delivery order, the shortest of max_messages, the byte take (the longest prefix with sum(pad32(len)) <=
+ *      max_agent_bytes) and the token take (sdb_receive_tokens' weights and 64-bit sums).  A budget take is the first
+ *      record alone when that record is heavier than its limit; a limit of 0 is no limit.
+ *   2. Equivalence: the result (records, order, bytes, retirement, counters, rings, lease ids, deadlines, delivery
+ *      counts and the dead-letter ledger) is exactly sdb_receive_leased with each agent's max_messages lowered to its
+ *      take, on a queue holding only the matching records.  Capacity is sdb_receive_leased's rule (records x
+ *      pad32(max_payload_bytes), the store's free room, lead-agent truncation), not sdb_receive_budget's exact bytes.
+ *   3. Both limits 0 and a NULL filter: the call is sdb_receive_leased.
+ *   4. Flags, SDB_ECAPACITY and lease_base_out as in sdb_receive_leased; the filter's refusals as in sdb_receive_where
+ *      (its per-id outputs included).  A refused call leaves queues, store and ledger untouched.  The take pass of a
+ *      filtered call is timed under SDB_PK_RECV_COUNT. */
+struct sdb_filter;
+int sdb_receive_leased_select(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                              uint64_t max_agent_bytes, uint64_t max_agent_tokens, const struct sdb_filter* filter,
+                              uint32_t flags, double deadline, uint32_t* count_out, sdb_recv_entry* entry_out,
+                              uint64_t entry_cap, sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out,
+                              uint64_t payload_cap, uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out,
+                              uint64_t* lease_base_out);
 int sdb_lease_settle(sdb_handle h, uint64_t n, const uint64_t* lease_id, uint32_t op, double deadline, uint8_t* settled_out,
                      uint64_t* n_settled_out);
 int sdb_lease_sweep(sdb_handle h, double now, uint32_t flags, uint64_t* redelivered_out, uint64_t* blocked_out,
@@ -943,6 +965,25 @@ int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
                       const sdb_filter* filter,
                       uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
                       uint8_t* payload_out, uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out);
+/* Filtered receive by budget ("the FUNCTION_RESULT messages the coordinator sent me, up to 4k tokens"):
+ * sdb_receive_where's arguments plus max_agent_bytes and max_agent_tokens.
+ *   1. Take: per agent, over its pending records that match the filter, in the call's delivery order, the shortest of
+ *      max_messages, the byte take (the longest prefix with sum(pad32(len)) <= max_agent_bytes) and the token take
+ *      (sdb_receive_tokens' weights and 64-bit sums).  A budget take is the first match alone when that match is heavier
+ *      than its limit; a limit of 0 is no limit.  In priority order that is whole levels from the top while they fit,
+ *      then the arrival-order prefix of the level where a limit falls.
+ *   2. Equivalence: the result is exactly sdb_receive_where with each agent's max_messages lowered to its take (records,
+ *      order, bytes, retirement, counters, rings, capacity and its lead-agent rule, id_hits / id_agent, which count the
+ *      matches before the cut).  Capacity is sdb_receive_where's records x pad32(max_payload_bytes) rule.
+ *   3. Both limits 0: the call is sdb_receive_where.
+ *   4. Flags and refusals as in sdb_receive_where (SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_WHERE_DROP included).  With a
+ *      limit, a pass between the filter's evaluation and the selection walks each agent's matches and cuts its count;
+ *      it reads ring entries and verdict bits, and with a token limit the header's last word and the payload's first
+ *      word of each match.  It is timed under SDB_PK_RECV_COUNT. */
+int sdb_receive_where_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                             uint64_t max_agent_bytes, uint64_t max_agent_tokens, uint32_t flags, const sdb_filter* filter,
+                             uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
+                             uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out);
 
 /* ---- LLM backend balancer: set_llm_load_balancing / assign_llm_backend / get_llm_backend
  * (M:1281-1325).  The reference stores a flag and a dict and has NO pick algorithm

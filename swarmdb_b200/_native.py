@@ -169,12 +169,12 @@ class SdbRelocateSummary(C.Structure):
 EXPORTS = ["sdb_abi_version", "sdb_create", "sdb_destroy", "sdb_set_stream", "sdb_sync", "sdb_last_error",
            "sdb_get_stats", "sdb_debug_set_arena_pos", "sdb_advance_seq", "sdb_profile", "sdb_profile_read", "sdb_profile_read_n", "sdb_register_agents", "sdb_deregister_agents", "sdb_create_group", "sdb_send_batch",
            "sdb_send_group_batch", "sdb_send_list_batch", "sdb_send_mixed_batch", "sdb_stage_batch", "sdb_submit_staged", "sdb_free_staged",
-           "sdb_receive_batch", "sdb_receive_compact", "sdb_receive_budget", "sdb_receive_compact_budget", "sdb_receive_tokens", "sdb_receive_compact_tokens", "sdb_pending_tokens", "sdb_restore_compact", "sdb_expire", "sdb_trim", "sdb_supersede", "sdb_receive_where", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
+           "sdb_receive_batch", "sdb_receive_compact", "sdb_receive_budget", "sdb_receive_compact_budget", "sdb_receive_tokens", "sdb_receive_compact_tokens", "sdb_pending_tokens", "sdb_restore_compact", "sdb_expire", "sdb_trim", "sdb_supersede", "sdb_receive_where", "sdb_receive_where_budget", "sdb_latency_server", "sdb_last_receive_dev", "sdb_last_receive_totals",
            "sdb_digest_reset", "sdb_digest_fold", "sdb_digest_read", "sdb_wire_bytes", "sdb_set_agent_shards",
            "sdb_export_group_batch", "sdb_export_mixed_batch", "sdb_export_mixed_batch_seq", "sdb_import_wire_batches", "sdb_wire_alloc", "sdb_wire_open",
            "sdb_wire_close", "sdb_import_wire_ptrs", "sdb_wire_wait_done", "sdb_wire_publish", "sdb_import_wire_ptrs_async", "sdb_import_prefetch", "sdb_overflow_log", "sdb_set_backends", "sdb_get_backend_loads",
            "sdb_release_backends", "sdb_select_backend_batch", "sdb_agent_loads", "sdb_queue_stats",
-           "sdb_assign_agent_backends", "sdb_backend_loads_from_queues", "sdb_lease_reserve", "sdb_receive_leased",
+           "sdb_assign_agent_backends", "sdb_backend_loads_from_queues", "sdb_lease_reserve", "sdb_receive_leased", "sdb_receive_leased_select",
            "sdb_lease_settle", "sdb_lease_sweep", "sdb_lease_stats", "sdb_lease_set_policy", "sdb_lease_deliveries",
            "sdb_lease_dead_letters", "sdb_lease_policy_stats", "sdb_arena_relocate", "sdb_lease_export",
            "sdb_lease_import", "sdb_lease_ledger_export", "sdb_lease_ledger_import", "sdb_dedup_reserve",
@@ -251,6 +251,9 @@ def load_library() -> C.CDLL:
     L.sdb_lease_reserve.restype = i32; L.sdb_lease_reserve.argtypes = [vp, u64, u64]
     L.sdb_receive_leased.restype = i32
     L.sdb_receive_leased.argtypes = [vp, u32, vp, u32, u32, C.c_double, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp, vp]
+    L.sdb_receive_leased_select.restype = i32
+    L.sdb_receive_leased_select.argtypes = [vp, u32, vp, u32, u64, u64, vp, u32, C.c_double, vp, vp, u64, vp, u64, vp, u64,
+                                            vp, vp, vp, vp]
     L.sdb_lease_settle.restype = i32; L.sdb_lease_settle.argtypes = [vp, u64, vp, u32, C.c_double, vp, vp]
     L.sdb_lease_sweep.restype = i32; L.sdb_lease_sweep.argtypes = [vp, C.c_double, u32, vp, vp, vp]
     L.sdb_lease_stats.restype = i32; L.sdb_lease_stats.argtypes = [vp, C.POINTER(SdbLeaseSummary)]
@@ -273,6 +276,8 @@ def load_library() -> C.CDLL:
     L.sdb_supersede.argtypes = [vp, u32, vp, u32, vp, vp, u64, vp, u64, vp, u64, vp, vp, vp]
     L.sdb_receive_where.restype = i32
     L.sdb_receive_where.argtypes = [vp, u32, vp, u32, u32, C.POINTER(SdbFilter), vp, vp, u64, vp, u64, vp, vp]
+    L.sdb_receive_where_budget.restype = i32
+    L.sdb_receive_where_budget.argtypes = [vp, u32, vp, u32, u64, u64, u32, C.POINTER(SdbFilter), vp, vp, u64, vp, u64, vp, vp]
     L.sdb_latency_server.restype = i32; L.sdb_latency_server.argtypes = [vp, i32]
     L.sdb_last_receive_dev.restype = i32; L.sdb_last_receive_dev.argtypes = [vp, vp, vp, vp]
     L.sdb_last_receive_totals.restype = i32; L.sdb_last_receive_totals.argtypes = [vp, vp, vp]
@@ -782,16 +787,26 @@ class Shard:
 
     def receive_leased(self, agents, max_messages: int, deadline: float, flags: int = 0,
                        out_entries: Optional[np.ndarray] = None, out_sends: Optional[np.ndarray] = None,
-                       out_payload: Optional[np.ndarray] = None):
+                       out_payload: Optional[np.ndarray] = None, max_agent_bytes: int = 0, max_agent_tokens: int = 0,
+                       filt: Optional[SdbFilter] = None):
         """receive_compact's records and result, each also kept in the lease store with `deadline` until it is acked or
-        redelivered.  Returns (counts, entries, sends, payload, lease_base): entry r holds lease lease_base + r."""
+        redelivered.  Returns (counts, entries, sends, payload, lease_base): entry r holds lease lease_base + r.
+        max_agent_bytes / max_agent_tokens (0: no limit) cut each agent's take as receive_budget / receive_tokens do,
+        and `filt` (make_filter()) leases only the matching records, as receive_where takes them
+        (include/swarmdb_b200.h: sdb_receive_leased_select)."""
         a, n, counts = self._agents_arg(agents)
         ent, snd, pay = self._compact_outputs(out_entries, out_sends, out_payload)
         total, n_sends, pbytes, base = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-        self._check(self._L.sdb_receive_leased(self._h, n, _p(a), max_messages, flags, float(deadline), _p(counts), _p(ent),
-                                               len(ent), _p(snd), len(snd), _p(pay), pay.nbytes,
-                                               C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
-                                               C.cast(C.byref(pbytes), C.c_void_p), C.cast(C.byref(base), C.c_void_p)))
+        tail = (float(deadline), _p(counts), _p(ent), len(ent), _p(snd), len(snd), _p(pay), pay.nbytes,
+                C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(n_sends), C.c_void_p),
+                C.cast(C.byref(pbytes), C.c_void_p), C.cast(C.byref(base), C.c_void_p))
+        if max_agent_bytes or max_agent_tokens or filt is not None:
+            self._check(self._L.sdb_receive_leased_select(self._h, n, _p(a), max_messages, int(max_agent_bytes),
+                                                          int(max_agent_tokens),
+                                                          None if filt is None else C.cast(C.byref(filt), C.c_void_p),
+                                                          flags, *tail))
+        else:
+            self._check(self._L.sdb_receive_leased(self._h, n, _p(a), max_messages, flags, *tail))
         if agents is None:
             counts = self._served_counts(counts, flags)
         return counts, ent[: total.value], snd[: n_sends.value], pay[: pbytes.value], int(base.value)
@@ -987,14 +1002,16 @@ class Shard:
 
     def receive_where(self, agents, max_messages: int, flags: int = 0, filt: Optional[SdbFilter] = None,
                       drop: bool = False, out_hdr: Optional[np.ndarray] = None, out_payload: Optional[np.ndarray] = None,
-                      id_hits: Optional[np.ndarray] = None, id_agent: Optional[np.ndarray] = None):
+                      id_hits: Optional[np.ndarray] = None, id_agent: Optional[np.ndarray] = None,
+                      max_agent_bytes: int = 0, max_agent_tokens: int = 0):
         """Take (or with RECV_PEEK, only look at) the first max_messages pending records per agent that match `filt`
         (make_filter(); None matches every record), in delivery order (include/swarmdb_b200.h: sdb_receive_where).
         Returns receive_batch's (counts, headers, payload); what does not fit stays queued, so loop until nothing
         comes back.  drop=True retires the matches on the device without returning them: (counts, total).
         With an id clause (make_filter(ids=...)), id_hits / id_agent (u32 arrays, one per listed id) receive each id's
         matching records, counted before max_messages and the capacity cut, and the smallest agent holding one
-        (NO_RECEIVER: none)."""
+        (NO_RECEIVER: none).  max_agent_bytes / max_agent_tokens (0: no limit) also cut each agent's take of the matches
+        as receive_budget / receive_tokens cut a plain one (sdb_receive_where_budget)."""
         if filt is None:
             filt = make_filter()
         n_ids = int(filt.n_ids) if filt.fields & FILTER_IDS else 0
@@ -1010,11 +1027,14 @@ class Shard:
             hdr = out_hdr if out_hdr is not None else self._grow_hdr()
             pay = out_payload if out_payload is not None else self._grow_pay()
         filt.id_hits, filt.id_agent = _p(id_hits), _p(id_agent)
+        tail = (_p(counts), _p(hdr), 0 if hdr is None else len(hdr), _p(pay), 0 if pay is None else pay.nbytes,
+                C.cast(C.byref(total), C.c_void_p), C.cast(C.byref(pbytes), C.c_void_p))
         try:
-            self._check(self._L.sdb_receive_where(self._h, n, _p(a), max_messages, flags, C.byref(filt), _p(counts),
-                                                  _p(hdr), 0 if hdr is None else len(hdr), _p(pay),
-                                                  0 if pay is None else pay.nbytes, C.cast(C.byref(total), C.c_void_p),
-                                                  C.cast(C.byref(pbytes), C.c_void_p)))
+            if max_agent_bytes or max_agent_tokens:
+                self._check(self._L.sdb_receive_where_budget(self._h, n, _p(a), max_messages, int(max_agent_bytes),
+                                                             int(max_agent_tokens), flags, C.byref(filt), *tail))
+            else:
+                self._check(self._L.sdb_receive_where(self._h, n, _p(a), max_messages, flags, C.byref(filt), *tail))
         finally:
             filt.id_hits = filt.id_agent = None                    # the filter does not keep the caller's arrays
         if agents is None:

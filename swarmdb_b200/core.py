@@ -958,17 +958,22 @@ class SwarmsDB:
         self.flush()
         return True
 
-    def _receive_budget_one(self, agent_id: str, max_messages: int, max_bytes: Optional[int], flags: int,
-                            max_tokens: Optional[int] = None):
-        """(headers, payload) of one byte- and/or token-budget receive for one agent (Shard.receive_budget,
-        Shard.receive_tokens)."""
+    @staticmethod
+    def _budget_limits(max_bytes: Optional[int], max_tokens: Optional[int]) -> Tuple[int, int]:
+        """The device's per-agent (byte, token) limits for max_bytes / max_tokens, 0 for None (no limit)."""
         if max_bytes is not None and max_bytes < 0:
             raise ValueError("max_bytes must be >= 0")
         if max_tokens is not None and not 0 < max_tokens < (1 << 64):
             raise ValueError("max_tokens must be positive (None: no token limit)")
-        k = min(max_messages, self.shard.max_recv_records)
         # the device reads 0 as "no limit"; a 1-byte limit takes the same records as a 0-byte one (sizes are multiples of 32)
-        nbytes = 0 if max_bytes is None else max(int(max_bytes), 1)
+        return (0 if max_bytes is None else max(int(max_bytes), 1)), (0 if max_tokens is None else int(max_tokens))
+
+    def _receive_budget_one(self, agent_id: str, max_messages: int, max_bytes: Optional[int], flags: int,
+                            max_tokens: Optional[int] = None):
+        """(headers, payload) of one byte- and/or token-budget receive for one agent (Shard.receive_budget,
+        Shard.receive_tokens)."""
+        nbytes, _ = self._budget_limits(max_bytes, max_tokens)
+        k = min(max_messages, self.shard.max_recv_records)
         if max_tokens is not None:
             _, hdr, pay = self.shard.receive_tokens([self._index(agent_id)], k, int(max_tokens), nbytes, flags)
         else:
@@ -997,12 +1002,25 @@ class SwarmsDB:
         return out
 
     # ------------------------------------------------------------------ leased receive (at-least-once delivery)
-    def receive_messages_leased(self, agent_id: str, max_messages: int = 100, visibility_timeout: float = 30.0) -> List[Message]:
+    def receive_messages_leased(self, agent_id: str, max_messages: int = 100, visibility_timeout: float = 30.0,
+                                max_bytes: Optional[int] = None, max_tokens: Optional[int] = None) -> List[Message]:
         """receive_messages with at-least-once delivery: the messages read READ, and each stays owed until it is acked
         (ack_messages, mark_message_as_processed).  One not acked within `visibility_timeout` seconds goes back behind
         what the agent has pending and is delivered again, with its id (an SQS visibility timeout).  Expired leases are
-        swept back first, so they are visible to this call.  Needs GpuConfig.lease_records."""
+        swept back first, so they are visible to this call.  max_bytes and max_tokens bound the take as in
+        receive_messages (one call, at most GpuConfig.max_recv_records messages): an agent that builds a model's
+        context from its queue gets as many messages as fit, and each comes back if the model call fails.  Needs
+        GpuConfig.lease_records."""
         self._prepare_receive(agent_id)
+        return self._receive_leased_local(agent_id, max_messages, visibility_timeout, max_bytes, max_tokens)
+
+    def _receive_leased_local(self, agent_id: str, max_messages: int, visibility_timeout: float,
+                              max_bytes: Optional[int] = None, max_tokens: Optional[int] = None,
+                              filt=None) -> List[Message]:
+        """Leased receives for one agent with the bookkeeping of receive_messages_leased; with a limit one call, else
+        a loop until max_messages or nothing more.  `filt`: leases only the matching messages (Shard.receive_leased)."""
+        limited = max_bytes is not None or max_tokens is not None
+        nbytes, ntokens = self._budget_limits(max_bytes, max_tokens)
         now = time.time()
         self._sweep_due(now)
         if max_messages <= 0:
@@ -1010,11 +1028,13 @@ class SwarmsDB:
         flags = RECV_PRIORITY if self.gpu_config.priority_dequeue else 0
         a = self._index(agent_id)
         deadline = now + visibility_timeout
+        select = {} if filt is None and not limited else {"max_agent_bytes": nbytes, "max_agent_tokens": ntokens, "filt": filt}
         out: List[Message] = []
         remaining = max_messages
         while remaining > 0:
+            k = min(remaining, self.shard.max_recv_records) if limited else remaining
             try:
-                _, ent, snd, pay, base = self.shard.receive_leased([a], remaining, deadline, flags)
+                _, ent, snd, pay, base = self.shard.receive_leased([a], k, deadline, flags, **select)
             except SdbError as e:
                 if out and e.code == -6:                   # SDB_ECAPACITY
                     break                                  # the store is full: what was leased so far is returned
@@ -1027,18 +1047,25 @@ class SwarmsDB:
                 counts = self.shard.lease_deliveries(np.arange(base, base + len(ent), dtype=np.uint64)).tolist()
                 for m, c in zip(msgs, counts):
                     m.metadata["delivery_count"] = int(c)
-            for k, m in enumerate(msgs):
-                self._leases.setdefault(m.id, []).append((a, base + k))
+            for j, m in enumerate(msgs):
+                self._leases.setdefault(m.id, []).append((a, base + j))
             out += msgs
             remaining -= len(ent)
+            if limited:
+                break
         if out:
             heapq.heappush(self._lease_deadlines, deadline)
         return out
 
     def receive_batch_leased(self, agent_idx=None, max_messages: int = 100, visibility_timeout: float = 30.0,
-                             priority: Optional[bool] = None, **kw):
+                             priority: Optional[bool] = None, max_bytes: Optional[int] = None,
+                             max_tokens: Optional[int] = None, filt=None, **kw):
         """receive_batch_compact, leased (Shard.receive_leased): (counts, entries, sends, payload, lease_base); entry r
-        holds lease lease_base + r, for settle_leases.  Index-level: no host message records."""
+        holds lease lease_base + r, for settle_leases.  Index-level: no host message records.  max_bytes and
+        max_tokens bound each agent's take as in receive_batch; `filt` (make_filter()) leases only matching records."""
+        nbytes, ntokens = self._budget_limits(max_bytes, max_tokens)
+        if max_bytes is not None or max_tokens is not None or filt is not None:
+            kw.update(max_agent_bytes=nbytes, max_agent_tokens=ntokens, filt=filt)
         self.flush()
         pr = self.gpu_config.priority_dequeue if priority is None else priority
         deadline = time.time() + visibility_timeout
@@ -1225,13 +1252,19 @@ class SwarmsDB:
                          message_type: Optional[MessageType] = None, min_priority: Optional[MessagePriority] = None,
                          group_name: Optional[str] = None, after_timestamp: Optional[float] = None,
                          before_timestamp: Optional[float] = None, keyword: Optional[str] = None,
-                         case_sensitive: bool = False, message_ids: Optional[Iterable[str]] = None) -> List[Message]:
+                         case_sensitive: bool = False, message_ids: Optional[Iterable[str]] = None,
+                         max_bytes: Optional[int] = None, max_tokens: Optional[int] = None, leased: bool = False,
+                         visibility_timeout: float = 30.0) -> List[Message]:
         """A selective receive_messages: pop up to `max_messages` of the agent's pending messages that match every
         given clause, in stream order (priority order with GpuConfig.priority_dequeue), with receive_messages'
         bookkeeping; the other messages stay queued in their order.  The timestamp bounds are strict.  `keyword` must
         occur in the message content (its UTF-8 text; JSON content as json.dumps gives it), at most 256 bytes; the
         case-insensitive compare folds ASCII letters only.  `message_ids` takes those specific messages (ids this
-        instance did not issue match nothing)."""
+        instance did not issue match nothing).  max_bytes and max_tokens bound the take of the matches as in
+        receive_messages (one call, at most GpuConfig.max_recv_records messages).  leased=True takes the matches with
+        receive_messages_leased's at-least-once delivery and `visibility_timeout`."""
+        limits = self._budget_limits(max_bytes, max_tokens)
+        limited = max_bytes is not None or max_tokens is not None
         if message_ids is not None:
             message_ids = list(message_ids)
             if len(message_ids) > FILTER_MAX_IDS:
@@ -1244,9 +1277,15 @@ class SwarmsDB:
                                   before_timestamp, keyword, case_sensitive, message_ids)
         if max_messages <= 0 or filt is None:
             return []
+        if leased:
+            return self._receive_leased_local(agent_id, max_messages, visibility_timeout, max_bytes, max_tokens, filt)
         flags = RECV_PRIORITY if self.gpu_config.priority_dequeue else 0
-        out: List[Message] = []
         a = np.array([self._index(agent_id)], np.uint32)
+        if limited:
+            _, hdr, pay = self.shard.receive_where(a, min(max_messages, self.shard.max_recv_records), flags, filt,
+                                                   max_agent_bytes=limits[0], max_agent_tokens=limits[1])
+            return self._decode(hdr, pay, agent_id)
+        out: List[Message] = []
         while len(out) < max_messages:
             _, hdr, pay = self.shard.receive_where(a, max_messages - len(out), flags, filt)
             if len(hdr) == 0:

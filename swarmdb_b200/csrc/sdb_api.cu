@@ -2695,6 +2695,98 @@ int sdb_lease_reserve(sdb_handle h, uint64_t max_records, uint64_t max_payload_b
   return SDB_OK;
 }
 
+// What a filtered call reads from its sdb_filter besides the clauses: the id block and whether a keyword applies
+struct where_req {
+  uint64_t n_ids = 0;
+  uint32_t* id_hits = nullptr;
+  uint32_t* id_agent = nullptr;
+  bool use_ids = false, use_kw = false;
+};
+// A filter's refusals (sdb_receive_where's), checked before anything runs; `name` names the call in error messages
+static int where_check(sdb_ctx* h, const sdb_filter* filter, const char* name, where_req* w) {
+  constexpr uint32_t all_fields = SDB_FILTER_SENDER | SDB_FILTER_RECEIVER | SDB_FILTER_GROUP | SDB_FILTER_TYPE | SDB_FILTER_PRIO |
+                                  SDB_FILTER_TIME | SDB_FILTER_SEQ | SDB_FILTER_KEYWORD | SDB_FILTER_ICASE | SDB_FILTER_IDS;
+  constexpr uint32_t v1_bytes = offsetof(sdb_filter, n_ids);  // the struct before the id block: callers built against it
+  const std::string n(name);
+  if (!filter || (filter->struct_bytes != sizeof(sdb_filter) && filter->struct_bytes != v1_bytes))
+    return fail(h, SDB_EINVAL, n + ": struct_bytes is neither sizeof(sdb_filter) nor offsetof(sdb_filter, n_ids)");
+  if (filter->fields & ~all_fields) return fail(h, SDB_EINVAL, n + ": unknown filter fields");
+  // the id block is read only with the full struct_bytes
+  w->use_ids = (filter->fields & SDB_FILTER_IDS) != 0;
+  w->n_ids = w->use_ids ? filter->n_ids : 0;
+  w->id_hits = filter->struct_bytes == v1_bytes ? nullptr : filter->id_hits;
+  w->id_agent = filter->struct_bytes == v1_bytes ? nullptr : filter->id_agent;
+  if (w->use_ids) {
+    if (filter->struct_bytes == v1_bytes) return fail(h, SDB_EINVAL, n + ": SDB_FILTER_IDS needs struct_bytes == sizeof(sdb_filter)");
+    if (w->n_ids > SDB_FILTER_MAX_IDS) return fail(h, SDB_EINVAL, n + ": n_ids > SDB_FILTER_MAX_IDS");
+    if (!filter->ids) return fail(h, SDB_EINVAL, n + ": NULL ids (an empty set takes any other pointer)");
+  } else if (w->id_hits || w->id_agent) {
+    return fail(h, SDB_EINVAL, n + ": id_hits / id_agent without SDB_FILTER_IDS");
+  }
+  w->use_kw = (filter->fields & SDB_FILTER_KEYWORD) && filter->keyword_len;
+  if (filter->fields & SDB_FILTER_KEYWORD) {
+    if (filter->keyword_len > SDB_FILTER_MAX_KEYWORD) return fail(h, SDB_EINVAL, n + ": keyword_len > SDB_FILTER_MAX_KEYWORD");
+    if (filter->keyword_len && !filter->keyword) return fail(h, SDB_EINVAL, n + ": NULL keyword");
+  }
+  return SDB_OK;
+}
+
+// the per-id outputs before the call: no hits, no agent
+static void where_id_reset(const where_req& w) {
+  if (w.id_hits) std::fill(w.id_hits, w.id_hits + w.n_ids, 0u);
+  if (w.id_agent) std::fill(w.id_agent, w.id_agent + w.n_ids, SDB_NO_RECEIVER);
+}
+
+// After where_check: the verdict bitmap allocated, the keyword and the id table on the device, *f filled
+static int where_setup(sdb_ctx* h, const sdb_filter* filter, const where_req& w, sdb_where_args* f, int* nl) {
+  const uint32_t stride = where_stride(h);
+  { const int rc = where_ensure(h); if (rc != SDB_OK) return rc; }
+  if (w.use_kw) CUDA_TRY(h, cudaMemcpyAsync(h->where_kw, filter->keyword, filter->keyword_len, cudaMemcpyHostToDevice, h->stream));
+  const uint64_t n_ids = w.n_ids;
+  uint64_t id_slots = 64;                                     // a power of two >= 2 x n_ids (an empty table matches nothing)
+  while (id_slots < 2 * n_ids) id_slots <<= 1;
+  if (w.use_ids) {
+    if (id_slots > h->id_slots || n_ids > h->id_cap) {
+      const uint64_t cap = std::max(n_ids, h->id_cap), slots = std::max(id_slots, h->id_slots);
+      { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }   // cudaFree waits for the kernels on the device
+      for (void* p : {static_cast<void*>(h->id_tab), static_cast<void*>(h->id_in), static_cast<void*>(h->id_out)}) if (p) cudaFree(p);
+      h->id_tab = nullptr; h->id_in = nullptr; h->id_out = nullptr; h->id_cap = h->id_slots = 0;
+      const int rc = dmalloc_set(h, {{&h->id_tab, slots}, {&h->id_in, cap}, {&h->id_out, 2 * cap}},
+                                 "filtered receive: id table allocation failed");
+      if (rc != SDB_OK) return rc;
+      h->id_cap = cap; h->id_slots = slots;
+    }
+    CUDA_TRY(h, cudaMemsetAsync(h->id_tab, 0, id_slots * sizeof(sdb_id_slot), h->stream));
+    if (n_ids) CUDA_TRY(h, cudaMemcpyAsync(h->id_in, filter->ids, n_ids * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+    const cudaError_t e = sdb_launch_id_table(h->id_in, static_cast<uint32_t>(n_ids), h->id_tab, static_cast<uint32_t>(id_slots - 1),
+                                              h->stream, nl);
+    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("id table launch: ") + cudaGetErrorString(e));
+  }
+  *f = sdb_where_args{};
+  f->fields = w.use_kw ? filter->fields : (filter->fields & ~SDB_FILTER_KEYWORD);
+  f->sender = filter->sender; f->receiver = filter->receiver; f->group = filter->group;
+  f->type_mask = filter->type_mask; f->prio_mask = filter->prio_mask; f->kw_len = w.use_kw ? filter->keyword_len : 0u;
+  f->after = filter->after; f->before = filter->before; f->seq_lo = filter->seq_lo; f->seq_hi = filter->seq_hi;
+  f->kw = h->where_kw; f->bits = h->where_bits; f->stride = stride;
+  f->id_tab = h->id_tab; f->id_mask = static_cast<uint32_t>(id_slots - 1); f->id_count = (w.id_hits || w.id_agent) && n_ids ? 1u : 0u;
+  return SDB_OK;
+}
+
+// After the filtered launch: the per-id outputs read out and their copies queued (the caller's synchronisation covers them)
+static cudaError_t where_id_out(sdb_ctx* h, const where_req& w, const sdb_where_args& f, int* nl) {
+  if (!f.id_count) return cudaSuccess;
+  cudaError_t e = sdb_launch_id_out(h->id_in, static_cast<uint32_t>(w.n_ids), h->id_tab, f.id_mask, h->id_out, h->stream, nl);
+  if (e == cudaSuccess && w.id_hits)
+    e = cudaMemcpyAsync(w.id_hits, h->id_out, w.n_ids * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess && w.id_agent)
+    e = cudaMemcpyAsync(w.id_agent, h->id_out + w.n_ids, w.n_ids * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream);
+  return e;
+}
+
+// the take limits of sdb_launch_where (~0: none): sum(pad32(len)) <= max_agent_bytes in payload granules, and tokens
+static unsigned long long agent_gran_limit(uint64_t max_agent_bytes) { return max_agent_bytes ? max_agent_bytes / SDB_GRANULE : ~0ull; }
+static unsigned long long token_limit(uint64_t max_agent_tokens) { return max_agent_tokens ? max_agent_tokens : ~0ull; }
+
 // Collection pass of the redelivery ledger (stream-ordered, no synchronisation): the entries whose record is still the
 // one a sweep put back are rebuilt into the other buffer and re-indexed; led.tot[0] counts them.
 static cudaError_t ledger_collect(sdb_ctx* h) {
@@ -2706,20 +2798,29 @@ static cudaError_t ledger_collect(sdb_ctx* h) {
   return e;
 }
 
-int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
-                       double deadline, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
-                       sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
-                       uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out, uint64_t* lease_base_out) {
+// sdb_receive_leased and sdb_receive_leased_select (both limits 0 and no filter: the plain leased call); `name` names the
+// call in errors.  Without a filter the limits run the receive's budget or token plan, with a granule capacity that the
+// records capacity always reaches first; with one, the filtered pipeline with its take pass and the compact back end.
+static int receive_leased_full(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                               uint64_t max_agent_bytes, uint64_t max_agent_tokens, const sdb_filter* filter, uint32_t flags,
+                               double deadline, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                               sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                               uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out, uint64_t* lease_base_out,
+                               const char* name) {
   if (!h) return SDB_EINVAL;
   sdb_ctx::LeaseStore& L = h->lease;
+  const std::string nm(name);
   if (total_out) *total_out = 0;
   if (n_sends_out) *n_sends_out = 0;
   if (payload_bytes_out) *payload_bytes_out = 0;
   if (lease_base_out) *lease_base_out = L.next_id;
   if (flags & ~(SDB_RECV_PRIORITY | SDB_RECV_OWNED))
-    return fail(h, SDB_EINVAL, "sdb_receive_leased accepts SDB_RECV_PRIORITY and SDB_RECV_OWNED only");
-  if (!L.cap) return fail(h, SDB_EINVAL, "sdb_receive_leased: no lease store (sdb_lease_reserve)");
+    return fail(h, SDB_EINVAL, nm + " accepts SDB_RECV_PRIORITY and SDB_RECV_OWNED only");
+  if (!L.cap) return fail(h, SDB_EINVAL, nm + ": no lease store (sdb_lease_reserve)");
+  where_req w;
+  if (filter) { const int rc = where_check(h, filter, name, &w); if (rc != SDB_OK) return rc; }
   const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
+  where_id_reset(w);
   if (n_agents == 0 || max_messages == 0) return SDB_OK;
   { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
   uint64_t rec_cap = 0;
@@ -2732,9 +2833,26 @@ int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_id
   sdb_recv_args r{};
   { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & SDB_RECV_PRIORITY, rec_cap, &r); if (rc != SDB_OK) return rc; }
   int nl = 0;
+  sdb_where_args f{};
+  if (filter) { const int rc = where_setup(h, filter, w, &f, &nl); if (rc != SDB_OK) return rc; }
   const bool ledger = L.policy && L.led_n;      // the ledger holds entries: collect before anything is retired, look up after
   cudaError_t e = ledger ? ledger_collect(h) : cudaSuccess;
-  if (e == cudaSuccess) e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx, nullptr, 0ull);
+  if (e == cudaSuccess) {
+    if (filter) {
+      e = sdb_launch_where(&h->view, &r, &f, 0, 32u + P, h->stream, &nl, &h->prof, h->sm_count, &h->cx,
+                           agent_gran_limit(max_agent_bytes), token_limit(max_agent_tokens));
+      if (e == cudaSuccess) e = where_id_out(h, w, f, &nl);
+    } else if (max_agent_bytes || max_agent_tokens) {
+      // granule capacity rec_cap x P / 32: a plan within rec_cap records never reaches it, so the records capacity and
+      // its truncation rule are sdb_receive_leased's
+      const uint64_t agent_gran = agent_gran_limit(max_agent_bytes), gran_cap = rec_cap * (P / SDB_GRANULE);
+      const uint2 budget = make_uint2(static_cast<uint32_t>(std::min<uint64_t>(agent_gran, 0xFFFFFFFFull)),
+                                      static_cast<uint32_t>(std::min<uint64_t>(gran_cap, 0xFFFFFFFFull)));
+      e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx, &budget, max_agent_tokens);
+    } else {
+      e = sdb_launch_receive(&h->view, &r, h->stream, &nl, &h->prof, h->sm_count, 32u + P, &h->cx, nullptr, 0ull);
+    }
+  }
   h->last_rx_valid = false; h->last_rx_compact = true;
   if (e == cudaSuccess)
     e = sdb_launch_lease_append(&L.buf[L.cur], &L.s, &h->cx, h->rx_count, h->rx_totals, r.agent_idx, n_agents,
@@ -2756,6 +2874,25 @@ int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_id
   if (n_sends_out) *n_sends_out = n_sends;
   if (payload_bytes_out) *payload_bytes_out = pbytes;
   return SDB_OK;
+}
+
+int sdb_receive_leased(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                       double deadline, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                       sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                       uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out, uint64_t* lease_base_out) {
+  return receive_leased_full(h, n_agents, agent_idx, max_messages, 0, 0, nullptr, flags, deadline, count_out, entry_out, entry_cap,
+                             send_out, send_cap, payload_out, payload_cap, total_out, n_sends_out, payload_bytes_out,
+                             lease_base_out, "sdb_receive_leased");
+}
+
+int sdb_receive_leased_select(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                              uint64_t max_agent_bytes, uint64_t max_agent_tokens, const sdb_filter* filter, uint32_t flags,
+                              double deadline, uint32_t* count_out, sdb_recv_entry* entry_out, uint64_t entry_cap,
+                              sdb_recv_send* send_out, uint64_t send_cap, uint8_t* payload_out, uint64_t payload_cap,
+                              uint64_t* total_out, uint64_t* n_sends_out, uint64_t* payload_bytes_out, uint64_t* lease_base_out) {
+  return receive_leased_full(h, n_agents, agent_idx, max_messages, max_agent_bytes, max_agent_tokens, filter, flags, deadline,
+                             count_out, entry_out, entry_cap, send_out, send_cap, payload_out, payload_cap, total_out,
+                             n_sends_out, payload_bytes_out, lease_base_out, "sdb_receive_leased_select");
 }
 
 int sdb_lease_settle(sdb_handle h, uint64_t n, const uint64_t* lease_id, uint32_t op, double deadline, uint8_t* settled_out,
@@ -3191,43 +3328,24 @@ int sdb_lease_ledger_import(sdb_handle h, uint64_t n, const uint32_t* agent, con
   return SDB_OK;
 }
 
-int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
-                      const sdb_filter* filter, uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
-                      uint8_t* payload_out, uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+// sdb_receive_where and sdb_receive_where_budget (both limits 0: the plain filtered call); `name` names the call in errors
+static int receive_where_full(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                              uint64_t max_agent_bytes, uint64_t max_agent_tokens, uint32_t flags, const sdb_filter* filter,
+                              uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
+                              uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out, const char* name) {
   if (!h) return SDB_EINVAL;
   if (total_out) *total_out = 0;
   if (payload_bytes_out) *payload_bytes_out = 0;
-  constexpr uint32_t all_fields = SDB_FILTER_SENDER | SDB_FILTER_RECEIVER | SDB_FILTER_GROUP | SDB_FILTER_TYPE | SDB_FILTER_PRIO |
-                                  SDB_FILTER_TIME | SDB_FILTER_SEQ | SDB_FILTER_KEYWORD | SDB_FILTER_ICASE | SDB_FILTER_IDS;
-  constexpr uint32_t v1_bytes = offsetof(sdb_filter, n_ids);  // the struct before the id block: callers built against it
-  if (!filter || (filter->struct_bytes != sizeof(sdb_filter) && filter->struct_bytes != v1_bytes))
-    return fail(h, SDB_EINVAL, "sdb_receive_where: struct_bytes is neither sizeof(sdb_filter) nor offsetof(sdb_filter, n_ids)");
-  if (filter->fields & ~all_fields) return fail(h, SDB_EINVAL, "sdb_receive_where: unknown filter fields");
-  // the id block is read only with the full struct_bytes
-  const bool use_ids = (filter->fields & SDB_FILTER_IDS) != 0;
-  const uint64_t n_ids = use_ids ? filter->n_ids : 0;
-  uint32_t* const id_hits = filter->struct_bytes == v1_bytes ? nullptr : filter->id_hits;
-  uint32_t* const id_agent = filter->struct_bytes == v1_bytes ? nullptr : filter->id_agent;
-  if (use_ids) {
-    if (filter->struct_bytes == v1_bytes) return fail(h, SDB_EINVAL, "sdb_receive_where: SDB_FILTER_IDS needs struct_bytes == sizeof(sdb_filter)");
-    if (n_ids > SDB_FILTER_MAX_IDS) return fail(h, SDB_EINVAL, "sdb_receive_where: n_ids > SDB_FILTER_MAX_IDS");
-    if (!filter->ids) return fail(h, SDB_EINVAL, "sdb_receive_where: NULL ids (an empty set takes any other pointer)");
-  } else if (id_hits || id_agent) {
-    return fail(h, SDB_EINVAL, "sdb_receive_where: id_hits / id_agent without SDB_FILTER_IDS");
-  }
-  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, "sdb_receive_where returns host results: SDB_RECV_ASYNC is not accepted");
+  const std::string n(name);
+  where_req w;
+  { const int rc = where_check(h, filter, name, &w); if (rc != SDB_OK) return rc; }
+  if (flags & SDB_RECV_ASYNC) return fail(h, SDB_EINVAL, n + " returns host results: SDB_RECV_ASYNC is not accepted");
   if (flags & ~(SDB_RECV_PRIORITY | SDB_RECV_PEEK | SDB_RECV_OWNED | SDB_WHERE_DROP))
-    return fail(h, SDB_EINVAL, "sdb_receive_where accepts SDB_RECV_PRIORITY, SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_WHERE_DROP only");
-  const bool use_kw = (filter->fields & SDB_FILTER_KEYWORD) && filter->keyword_len;
-  if (filter->fields & SDB_FILTER_KEYWORD) {
-    if (filter->keyword_len > SDB_FILTER_MAX_KEYWORD) return fail(h, SDB_EINVAL, "sdb_receive_where: keyword_len > SDB_FILTER_MAX_KEYWORD");
-    if (filter->keyword_len && !filter->keyword) return fail(h, SDB_EINVAL, "sdb_receive_where: NULL keyword");
-  }
+    return fail(h, SDB_EINVAL, n + " accepts SDB_RECV_PRIORITY, SDB_RECV_PEEK, SDB_RECV_OWNED and SDB_WHERE_DROP only");
   const bool drop = (flags & SDB_WHERE_DROP) != 0;
-  if (drop && (hdr_out || payload_out)) return fail(h, SDB_EINVAL, "sdb_receive_where: drop mode takes no output buffers but count_out");
+  if (drop && (hdr_out || payload_out)) return fail(h, SDB_EINVAL, n + ": drop mode takes no output buffers but count_out");
   const bool owned = recv_agents(h, flags, agent_idx, &n_agents);
-  if (id_hits) std::fill(id_hits, id_hits + n_ids, 0u);
-  if (id_agent) std::fill(id_agent, id_agent + n_ids, SDB_NO_RECEIVER);
+  where_id_reset(w);
   if (n_agents == 0 || max_messages == 0) return SDB_OK;
   { const int rc = check_recv_agents(h, n_agents, agent_idx); if (rc != SDB_OK) return rc; }
   uint64_t rec_cap = ~0ull;
@@ -3235,51 +3353,35 @@ int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx
     const int rc = out_rec_cap(h, room(hdr_out, hdr_cap), room(payload_out, payload_cap), &rec_cap);
     if (rc != SDB_OK) return rc;
   }
-  const uint32_t stride = where_stride(h);
-  { const int rc = where_ensure(h); if (rc != SDB_OK) return rc; }
   sdb_recv_args r{};
   { const int rc = recv_args(h, n_agents, agent_idx, owned, max_messages, flags & (SDB_RECV_PRIORITY | SDB_RECV_PEEK), rec_cap, &r);
     if (rc != SDB_OK) return rc; }
-  if (use_kw) CUDA_TRY(h, cudaMemcpyAsync(h->where_kw, filter->keyword, filter->keyword_len, cudaMemcpyHostToDevice, h->stream));
-  uint64_t id_slots = 64;                                     // a power of two >= 2 x n_ids (an empty table matches nothing)
-  while (id_slots < 2 * n_ids) id_slots <<= 1;
   int nl = 0;
-  if (use_ids) {
-    if (id_slots > h->id_slots || n_ids > h->id_cap) {
-      const uint64_t cap = std::max(n_ids, h->id_cap), slots = std::max(id_slots, h->id_slots);
-      { const int rc = ls_stop(h); if (rc != SDB_OK) return rc; }   // cudaFree waits for the kernels on the device
-      for (void* p : {static_cast<void*>(h->id_tab), static_cast<void*>(h->id_in), static_cast<void*>(h->id_out)}) if (p) cudaFree(p);
-      h->id_tab = nullptr; h->id_in = nullptr; h->id_out = nullptr; h->id_cap = h->id_slots = 0;
-      const int rc = dmalloc_set(h, {{&h->id_tab, slots}, {&h->id_in, cap}, {&h->id_out, 2 * cap}},
-                                 "filtered receive: id table allocation failed");
-      if (rc != SDB_OK) return rc;
-      h->id_cap = cap; h->id_slots = slots;
-    }
-    CUDA_TRY(h, cudaMemsetAsync(h->id_tab, 0, id_slots * sizeof(sdb_id_slot), h->stream));
-    if (n_ids) CUDA_TRY(h, cudaMemcpyAsync(h->id_in, filter->ids, n_ids * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
-    const cudaError_t e = sdb_launch_id_table(h->id_in, static_cast<uint32_t>(n_ids), h->id_tab, static_cast<uint32_t>(id_slots - 1),
-                                              h->stream, &nl);
-    if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("id table launch: ") + cudaGetErrorString(e));
-  }
-  sdb_where_args f{};
-  f.fields = use_kw ? filter->fields : (filter->fields & ~SDB_FILTER_KEYWORD);
-  f.sender = filter->sender; f.receiver = filter->receiver; f.group = filter->group;
-  f.type_mask = filter->type_mask; f.prio_mask = filter->prio_mask; f.kw_len = use_kw ? filter->keyword_len : 0u;
-  f.after = filter->after; f.before = filter->before; f.seq_lo = filter->seq_lo; f.seq_hi = filter->seq_hi;
-  f.kw = h->where_kw; f.bits = h->where_bits; f.stride = stride;
-  f.id_tab = h->id_tab; f.id_mask = static_cast<uint32_t>(id_slots - 1); f.id_count = (id_hits || id_agent) && n_ids ? 1u : 0u;
+  sdb_where_args f;
+  { const int rc = where_setup(h, filter, w, &f, &nl); if (rc != SDB_OK) return rc; }
   cudaError_t e = sdb_launch_where(&h->view, &r, &f, drop ? 1 : 0, 32u + pad32(h->cfg.max_payload_bytes), h->stream, &nl,
-                                   &h->prof, h->sm_count);
-  if (e == cudaSuccess && f.id_count)
-    e = sdb_launch_id_out(h->id_in, static_cast<uint32_t>(n_ids), h->id_tab, f.id_mask, h->id_out, h->stream, &nl);
+                                   &h->prof, h->sm_count, nullptr, agent_gran_limit(max_agent_bytes), token_limit(max_agent_tokens));
+  if (e == cudaSuccess) e = where_id_out(h, w, f, &nl);
   h->launches += nl;
   h->last_rx_valid = false; h->last_rx_compact = false;       // no full receive to fold: the plan belongs to a filtered call
   if (e != cudaSuccess) return fail(h, SDB_ECUDA, std::string("filtered receive launch: ") + cudaGetErrorString(e));
-  if (id_hits && f.id_count) CUDA_TRY(h, cudaMemcpyAsync(id_hits, h->id_out, n_ids * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-  if (id_agent && f.id_count)
-    CUDA_TRY(h, cudaMemcpyAsync(id_agent, h->id_out + n_ids, n_ids * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   // drop mode has no output buffers, and its payload byte count stays 0; the synchronisation covers the id outputs
   return copy_full(h, n_agents, count_out, hdr_out, payload_out, total_out, drop ? nullptr : payload_bytes_out);
+}
+
+int sdb_receive_where(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages, uint32_t flags,
+                      const sdb_filter* filter, uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap,
+                      uint8_t* payload_out, uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+  return receive_where_full(h, n_agents, agent_idx, max_messages, 0, 0, flags, filter, count_out, hdr_out, hdr_cap, payload_out,
+                            payload_cap, total_out, payload_bytes_out, "sdb_receive_where");
+}
+
+int sdb_receive_where_budget(sdb_handle h, uint32_t n_agents, const uint32_t* agent_idx, uint32_t max_messages,
+                             uint64_t max_agent_bytes, uint64_t max_agent_tokens, uint32_t flags, const sdb_filter* filter,
+                             uint32_t* count_out, sdb_msg_header* hdr_out, uint64_t hdr_cap, uint8_t* payload_out,
+                             uint64_t payload_cap, uint64_t* total_out, uint64_t* payload_bytes_out) {
+  return receive_where_full(h, n_agents, agent_idx, max_messages, max_agent_bytes, max_agent_tokens, flags, filter, count_out,
+                            hdr_out, hdr_cap, payload_out, payload_cap, total_out, payload_bytes_out, "sdb_receive_where_budget");
 }
 
 int sdb_last_receive_dev(sdb_handle h, const uint32_t** count_dev, const sdb_msg_header** hdr_dev, const uint8_t** payload_dev) {

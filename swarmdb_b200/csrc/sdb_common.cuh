@@ -915,7 +915,7 @@ cudaError_t sdb_launch_expire(const sdb_dev_view*, const sdb_recv_args*, double,
 cudaError_t sdb_launch_supersede(const sdb_dev_view*, const sdb_recv_args*, const sdb_ss_args*, const sdb_compact_args*, cudaStream_t,
                                  int*, sdb_profiler*, int);
 cudaError_t sdb_launch_where(const sdb_dev_view*, const sdb_recv_args*, const sdb_where_args*, int, uint32_t, cudaStream_t, int*,
-                             sdb_profiler*, int);
+                             sdb_profiler*, int, const sdb_compact_args*, unsigned long long, unsigned long long);
 cudaError_t sdb_launch_id_table(const unsigned long long*, uint32_t, sdb_id_slot*, uint32_t, cudaStream_t, int*);
 cudaError_t sdb_launch_id_out(const unsigned long long*, uint32_t, const sdb_id_slot*, uint32_t, uint32_t*, cudaStream_t, int*);
 cudaError_t sdb_recv_prepare_device();

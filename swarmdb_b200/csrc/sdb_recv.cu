@@ -1284,48 +1284,62 @@ __device__ __forceinline__ void tk_weights(const sdb_dev_view& v, const uint2 (&
     tk[u] = (((hw[u] >> 24) & SDB_TYPEF_TOKENS) && (hw[u] & 0xFFFFu) >= 4u) ? pw[u] : 0u;
 }
 
-template <bool PRIO>
-__global__ void __launch_bounds__(256)
-k_token_take(sdb_dev_view v, sdb_recv_args r, unsigned long long lim, unsigned long long* __restrict__ sums) {
+// The walk of k_token_take and, with SEL, of k_where_take.  SEL: only the entries whose verdict bit is set (bits: the
+// agent's row of f.bits) are walked, the take is also cut where their payload granules would pass glim, and
+// cnt[q] = min(cnt[q], take) (cnt[q] as the where eval left it); the walk stops once the take reaches cnt[q].  lim and
+// glim are ~0 for no limit; with lim = ~0 under SEL no payload word is read.
+template <bool PRIO, bool SEL>
+__device__ __forceinline__ void token_take_walk(const sdb_dev_view& v, const sdb_recv_args& r, unsigned long long lim,
+                                                unsigned long long* __restrict__ sums, const uint32_t* __restrict__ fbits,
+                                                uint32_t stride, unsigned long long glim) {
   const uint32_t lane = threadIdx.x & 31, l8 = lane & (SDB_TK_G - 1), gsh = lane & ~(SDB_TK_G - 1), below = (1u << l8) - 1u;
   const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
   const uint32_t mask = v.ring_slots - 1;
+  const bool tok = !SEL || lim != ~0ull;                        // token weights are read
   constexpr uint32_t SPW = 32u / SDB_TK_G;                      // request slots per warp
   for (uint32_t qb = gw * SPW; qb < r.n; qb += nw * SPW) {      // warp-uniform
     const uint32_t q = qb + lane / SDB_TK_G;
     const bool valid = q < r.n;
-    uint32_t a = 0, H = 0, T = 0, NT = 0;
+    uint32_t a = 0, H = 0, T = 0, NT = 0, cin = 0;
     if (valid) {
       a = r.agent_idx ? r.agent_idx[q] : q;
       const uint4 h = *reinterpret_cast<const uint4*>(v.ring_hdr + a);     // one address for the slot's 8 lanes
       H = h.x; T = h.y; NT = h.w;
+      if (SEL) cin = r.cnt[q];
     }
-    const uint32_t W = valid && T - H - NT ? T - H : 0u;
+    const uint32_t W = valid && T - H - NT && (!SEL || cin) ? T - H : 0u;
     const uint2* rs = sdb_ring_of(v, a);
+    const uint32_t* bits = SEL ? fbits + static_cast<size_t>(a) * stride : nullptr;
     uint32_t take = 0, cut = 4;                                 // cut: the level where the limit falls (4: none)
-    unsigned long long tsum = 0;
+    unsigned long long tsum = 0, gsum = 0;
     if (PRIO) {
-      // 1. per level: live records and their tokens
+      // 1. per level: live records and their tokens (and, SEL, granules)
       uint32_t c[4] = {0u, 0u, 0u, 0u};
-      unsigned long long t[4] = {0ull, 0ull, 0ull, 0ull};
+      unsigned long long t[4] = {0ull, 0ull, 0ull, 0ull}, gs[4] = {0ull, 0ull, 0ull, 0ull};
       const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W);
       for (uint32_t j0 = 0; j0 < wmax; j0 += SDB_TK_G * SDB_TK_U) {
+        const uint32_t word = SEL && j0 < W ? bits[j0 >> 5] : 0u;
         uint2 e[SDB_TK_U];
-        bool lv[SDB_TK_U];
+        bool lv[SDB_TK_U], lt[SDB_TK_U];
         uint32_t tk[SDB_TK_U];
 #pragma unroll
         for (uint32_t u = 0; u < SDB_TK_U; ++u) {
           const uint32_t j = j0 + u * SDB_TK_G + l8;
-          e[u] = j < W ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+          const bool in = j < W && (!SEL || ((word >> (u * SDB_TK_G + l8)) & 1u));
+          e[u] = in ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
           lv[u] = sdb_meta(e[u]) != SDB_META_TOMB;
+          lt[u] = lv[u] && tok;
         }
-        tk_weights(v, e, lv, tk);
+        tk_weights(v, e, lt, tk);
 #pragma unroll
         for (uint32_t u = 0; u < SDB_TK_U; ++u) {
           const uint32_t p = sdb_meta(e[u]) >> 14;
 #pragma unroll
           for (uint32_t l = 0; l < 4; ++l)
-            if (lv[u] && p == l) { c[l] += 1; t[l] += tk[u]; }
+            if (lv[u] && p == l) {
+              c[l] += 1; t[l] += tk[u];
+              if (SEL) gs[l] += (sdb_meta(e[u]) & SDB_META_GLEN_MASK) - 1u;
+            }
         }
       }
 #pragma unroll
@@ -1334,52 +1348,81 @@ k_token_take(sdb_dev_view v, sdb_recv_args r, unsigned long long lim, unsigned l
         for (int o = 4; o; o >>= 1) {
           c[l] += __shfl_xor_sync(0xFFFFFFFFu, c[l], o);
           t[l] += __shfl_xor_sync(0xFFFFFFFFu, t[l], o);
+          if (SEL) gs[l] += __shfl_xor_sync(0xFFFFFFFFu, gs[l], o);
         }
         if (cut == 4) {
-          if (tsum + t[l] <= lim) { take += c[l]; tsum += t[l]; }
+          if (tsum + t[l] <= lim && (!SEL || gsum + gs[l] <= glim)) { take += c[l]; tsum += t[l]; gsum += gs[l]; }
           else cut = static_cast<uint32_t>(l);
         }
       }
     }
-    // 2. stream order, or the arrival-order prefix of the cut level: entry i is taken while the running sum fits (or it
+    // 2. stream order, or the arrival-order prefix of the cut level: entry i is taken while the running sums fit (or it
     // is the first of the delivery order); sums only grow, so the first one that does not fit ends the take
     const uint32_t W2 = (!PRIO || cut < 4) ? W : 0u;
-    bool open = W2 != 0;
+    bool open = W2 != 0 && (!SEL || take < cin);
     const uint32_t wmax = __reduce_max_sync(0xFFFFFFFFu, W2);
     for (uint32_t j0 = 0; j0 < wmax && __any_sync(0xFFFFFFFFu, open); j0 += SDB_TK_G * SDB_TK_U) {
+      const uint32_t word = SEL && open && j0 < W2 ? bits[j0 >> 5] : 0u;
       uint2 e[SDB_TK_U];
-      bool sel[SDB_TK_U];
+      bool sel[SDB_TK_U], st[SDB_TK_U];
       uint32_t tk[SDB_TK_U];
 #pragma unroll
       for (uint32_t u = 0; u < SDB_TK_U; ++u) {
         const uint32_t j = j0 + u * SDB_TK_G + l8;
-        e[u] = open && j < W2 ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
+        const bool in = open && j < W2 && (!SEL || ((word >> (u * SDB_TK_G + l8)) & 1u));
+        e[u] = in ? rs[(H + j) & mask] : make_uint2(0u, SDB_META_TOMB);
         sel[u] = sdb_meta(e[u]) != SDB_META_TOMB && (!PRIO || sdb_meta(e[u]) >> 14 == cut);
+        st[u] = sel[u] && tok;
       }
-      tk_weights(v, e, sel, tk);
+      tk_weights(v, e, st, tk);
 #pragma unroll
       for (uint32_t u = 0; u < SDB_TK_U; ++u) {
         const uint32_t bs = (__ballot_sync(0xFFFFFFFFu, sel[u]) >> gsh) & 0xFFu;
-        unsigned long long x = tk[u];                           // inclusive scan over the slot's 8 lanes
+        const unsigned long long g = SEL && sel[u] ? (sdb_meta(e[u]) & SDB_META_GLEN_MASK) - 1u : 0u;
+        unsigned long long x = tk[u], xg = g;                   // inclusive scans over the slot's 8 lanes
 #pragma unroll
         for (uint32_t o = 1; o < SDB_TK_G; o <<= 1) {
           const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, x, o, SDB_TK_G);
           if (l8 >= o) x += y;
+          if (SEL) {
+            const unsigned long long yg = __shfl_up_sync(0xFFFFFFFFu, xg, o, SDB_TK_G);
+            if (l8 >= o) xg += yg;
+          }
         }
-        const bool ok = open && sel[u] && (take + __popc(bs & below) == 0 || tsum + x <= lim);
+        const bool ok = open && sel[u] && (take + __popc(bs & below) == 0 ||
+                                           (tsum + x <= lim && (!SEL || gsum + xg <= glim)));
         const uint32_t bo = (__ballot_sync(0xFFFFFFFFu, ok) >> gsh) & 0xFFu;
-        unsigned long long s = ok ? tk[u] : 0ull;
+        unsigned long long s = ok ? tk[u] : 0ull, sg = ok ? g : 0ull;
 #pragma unroll
-        for (int o = 4; o; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
-        take += __popc(bo); tsum += s;
+        for (int o = 4; o; o >>= 1) {
+          s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
+          if (SEL) sg += __shfl_xor_sync(0xFFFFFFFFu, sg, o);
+        }
+        take += __popc(bo); tsum += s; gsum += sg;
         if (bo != bs) open = false;                             // an entry did not fit: the take ends before it
       }
+      if (SEL && take >= cin) open = false;                     // max_messages (or the matches) reached
     }
     if (valid && l8 == 0) {
-      r.cnt[q] = take;
+      r.cnt[q] = SEL ? min(cin, take) : take;
       if (sums) sums[q] = tsum;
     }
   }
+}
+
+template <bool PRIO>
+__global__ void __launch_bounds__(256)
+k_token_take(sdb_dev_view v, sdb_recv_args r, unsigned long long lim, unsigned long long* __restrict__ sums) {
+  token_take_walk<PRIO, false>(v, r, lim, sums, nullptr, 0u, ~0ull);
+}
+
+// filtered take (sdb_receive_where_budget, sdb_receive_leased_select): between the where eval and the count scan,
+// cnt[q] = min(cnt[q], the take of the matching records under the token limit lim and the granule limit glim)
+template <bool PRIO>
+__global__ void __launch_bounds__(256)
+k_where_take(sdb_dev_view v, sdb_recv_args r, const uint32_t* __restrict__ bits, uint32_t stride, unsigned long long lim,
+             unsigned long long glim) {
+  token_take_walk<PRIO, true>(v, r, lim, nullptr, bits, stride, glim);
 }
 
 // cnt[q] = the token take of each request slot under `lim` (~0: everything pending), sums[q] (nullable) its token sum
@@ -2328,10 +2371,13 @@ k_where_select(sdb_dev_view v, sdb_recv_args r, sdb_where_args f) {
 }
 
 // drop mode: eval + select, totals[0] = records selected.  Take mode: eval, scan, select, plan scan, then the receive
-// gather exactly as the priority pipeline runs it (totals[0] records, totals[1] payload granules)
+// gather exactly as the priority pipeline runs it (totals[0] records, totals[1] payload granules), or with ca the compact
+// back end.  glim / tlim (~0: no limit): per-agent limits on the matches' payload granules and token weights; either one
+// set runs k_where_take between the eval and the rest (timed under SDB_PK_RECV_COUNT too)
 extern "C" cudaError_t sdb_launch_where(const sdb_dev_view* v, const sdb_recv_args* r, const sdb_where_args* f, int drop,
                                         uint32_t max_rec_bytes, cudaStream_t stream, int* n_launches, sdb_profiler* prof,
-                                        int sm_count) {
+                                        int sm_count, const sdb_compact_args* ca, unsigned long long glim,
+                                        unsigned long long tlim) {
   if (r->n == 0) return cudaSuccess;
   const uint32_t n = r->n;
   const uint32_t blocks = sdb_grid(n, 32, 32 * sm_count);                    // 4 slots per warp, 8 warps per block
@@ -2340,6 +2386,15 @@ extern "C" cudaError_t sdb_launch_where(const sdb_dev_view* v, const sdb_recv_ar
     k_where_kw<<<sdb_grid(n, 8, 8 * sm_count), 256, 0, stream>>>(*v, *r, *f);   // a warp per slot, 8 warps per block
   } else {
     k_where_eval<<<blocks, 256, 0, stream>>>(*v, *r, *f);
+  }
+  if (glim != ~0ull || tlim != ~0ull) {
+    const int pt = sdb_prof_begin(prof, SDB_PK_RECV_COUNT, stream);
+    if (r->flags & SDB_RECV_PRIORITY)
+      k_where_take<true><<<blocks, 256, 0, stream>>>(*v, *r, f->bits, f->stride, tlim, glim);
+    else
+      k_where_take<false><<<blocks, 256, 0, stream>>>(*v, *r, f->bits, f->stride, tlim, glim);
+    sdb_prof_end(prof, pt, stream);
+    if (n_launches) *n_launches += 1;
   }
   if (drop) {
     cudaMemsetAsync(r->totals, 0, 2 * sizeof(unsigned long long), stream);
@@ -2359,6 +2414,7 @@ extern "C" cudaError_t sdb_launch_where(const sdb_dev_view* v, const sdb_recv_ar
   sdb_prof_end(prof, pi, stream);
   if (n_launches) *n_launches += 4;
   if (e != cudaSuccess) return e;
+  if (ca) return launch_compact(v, r, ca, nullptr, bound, sm_count, stream, prof, n_launches);
   return launch_gather(v, r, nullptr, bound, max_rec_bytes, sm_count, stream, prof, n_launches);
 }
 

@@ -777,6 +777,12 @@ class ShardedSwarmsDB(SwarmsDB):
                                   "sequence numbers of later rounds (see requeue_batch_compact)")
 
     receive_messages_leased = receive_batch_leased = settle_leases = _no_leases
+
+    def receive_matching(self, agent_id: str, max_messages: int = 100, *, leased: bool = False, **kw):
+        """SwarmsDB.receive_matching on the owner rank; leased=True is refused like every lease call."""
+        if leased:
+            self._no_leases()
+        return super().receive_matching(agent_id, max_messages, **kw)
     ack_messages = nack_messages = extend_leases = redeliver_expired = _no_leases
     dead_letters = redrive_dead_letters = _no_leases
 
